@@ -1235,6 +1235,21 @@ int pt_batch_stats(pt_batch* b, uint64_t out[4]) {
     return PT_OK;
 }
 
+#ifdef PT_PHASE_CLOCKS
+// Profiling build only (make PHASE_CLOCKS=1): the warp kernel's per-phase cycle sums on the current device, summed over
+// its warps since the last reset: out[0..8] = log start, A+B, C, D, E, F, G, I, round wait; out[9] = logs merged.
+int pt_phase_clocks(uint64_t out[ptk::kNumPhases + 1], int reset) {
+    if (!out) return PT_ERR_INVALID;
+    PT_CUDA(cudaDeviceSynchronize());
+    PT_CUDA(cudaMemcpyFromSymbol(out, ptk::ptk_phase_clk, sizeof(ptk::ptk_phase_clk)));
+    if (reset) {
+        static const unsigned long long zero[ptk::kNumPhases + 1] = {};
+        PT_CUDA(cudaMemcpyToSymbol(ptk::ptk_phase_clk, zero, sizeof(zero)));
+    }
+    return PT_OK;
+}
+#endif
+
 int pt_batch_set_comment_pool(pt_batch* b, uint64_t entries) {
     if (!b) return PT_ERR_INVALID;
     PT_CUDA(cudaSetDevice(b->device));

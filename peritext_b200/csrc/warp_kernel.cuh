@@ -77,12 +77,32 @@ __device__ __forceinline__ void wfill(T* p, uint32_t count, T v, uint32_t lane) 
     for (uint32_t i = lane; i < nvec; i += 32) d[i] = q;
 }
 
+// Per-phase cycle profile (build with `make PHASE_CLOCKS=1`; tools/phase_profile.py reads it through pt_phase_clocks).
+// Every warp sums clock64() deltas per phase in registers and adds them to ptk_phase_clk when it exits; the default build
+// contains none of it.
+#ifdef PT_PHASE_CLOCKS
+enum : int { kPhStart, kPhAB, kPhC, kPhD, kPhE, kPhF, kPhG, kPhI, kPhRound, kNumPhases };
+__device__ unsigned long long ptk_phase_clk[kNumPhases + 1];   // cycles per phase summed over warps, then the logs merged
+struct PhaseClock {
+    long long t;
+    unsigned long long c[kNumPhases], logs;
+    __device__ __forceinline__ void mark(int k) { const long long now = clock64(); c[k] += (unsigned long long)(now - t); t = now; }
+};
+#define PT_PHASE(k) pclk.mark(k)
+#define PT_PHASE_PARAM , PhaseClock& pclk
+#define PT_PHASE_ARG , pclk
+#else
+#define PT_PHASE(k) ((void)0)
+#define PT_PHASE_PARAM
+#define PT_PHASE_ARG
+#endif
+
 // id-table forms of the warp kernel (one kernel instantiation each; the host sorts the logs into the launches)
 constexpr int kIdDirect = 0, kIdCompact = 1, kIdPacked3 = 2;
 
 // returns 0: done (result header written), 1: defer to the block kernel.  IDM selects the id-table form (below).
 template <int IDM>
-__device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const uint32_t li, const uint32_t slice_base, const uint32_t slice_bytes, const uint32_t li_next, PhaseSync ps) {
+__device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const uint32_t li, const uint32_t slice_base, const uint32_t slice_bytes, const uint32_t li_next, PhaseSync ps PT_PHASE_PARAM) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t lt = (1u << lane) - 1u;
 
@@ -173,6 +193,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         const char* insb = reinterpret_cast<const char*>(ins);
         const uint32_t insBytes = n * 16u;
         if (lane * 128u + 1024u < insBytes) prefetch_l2(insb + 1024u + lane * 128u);          // trips 2 .. 9
+        PT_PHASE(kPhStart);
 #pragma unroll 2
         for (uint32_t base = 0; base < n; base += 32) {
             const uint32_t i = base + lane;
@@ -260,6 +281,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     if (compact && nOv > kOvMax) { ps.leave(); return 1; }                                    // too many concurrent-counter inserts for the compact table
     st = __reduce_or_sync(kFull, st);
     if (st) { bail(31u - __clz(st)); ps.leave(); return 0; }
+    PT_PHASE(kPhAB);
 
     // ---- C: runs, bit-parallel: head = insert & (!chain-link | predecessor has another child); visible = insert & !deleted
     uint32_t M, nvis, N = 0;
@@ -277,12 +299,17 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t pc = __popc(head) | (__popc(vis) << 16);
             const uint32_t inc = warp_incl_scan(pc, lane), ex = inc - pc, tot = __shfl_sync(kFull, inc, 31);
             if (w < NWr) WI[w] = make_uint4(insW, head, vis, (carryH + (ex & 0xFFFFu)) | ((carryV + (ex >> 16)) << 16));
+            // phase D reads every run head's record again: the 128-byte lines that hold heads go to L2 now, all at once
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++)
+                if ((head >> (8u * k)) & 0xFFu) prefetch_l2(ins + w * 32u + 8u * k);
             carryH += tot & 0xFFFFu; carryV += tot >> 16;
             N += __reduce_add_sync(kFull, (uint32_t)__popc(insW));
         }
         M = carryH; nvis = carryV;
     }
     __syncwarp();
+    PT_PHASE(kPhC);
 
     auto runOf = [&](uint32_t i) -> uint32_t {
         const uint4 q = WI[i >> 5];
@@ -294,10 +321,6 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     };
 
     if ((P.warp_flags & 2u) && li_next != 0xFFFFFFFFu && lane == 0) prefetch_l2(P.desc + li_next);   // read in phase F
-    if (m) {       // the first 6 trips of mark records (needed in phase G) start their way to L2 now
-        const uint32_t pfb = min(m * 32u, 6u * 1024u);
-        for (uint32_t o = lane * 128u; o < pfb; o += 32u * 128u) prefetch_l2(reinterpret_cast<const char*>(mk) + o);
-    }
     // ---- D: run tree; E: Euler tour + splitter list ranking of the VISIBLE weights ------------------------------------------
     const uint32_t E = 2 * (M + 1), END = (E + 7u) & ~7u;          // END: terminator id, a multiple of 8 like every splitter node
     if (END + 1 >= 0xFFFFu) { ps.leave(); return 1; }
@@ -340,12 +363,12 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t r = rb + lane;
             if (r < M) {
                 const uint32_t i = HV[r], w = i >> 5, b = i & 31;
+                const uint4 rec = ld_rec(ins + i);                 // issued before the run-end scan: its latency overlaps the scan
                 const uint4 q0 = WI[w];
                 uint32_t stop = (q0.y | ~q0.x) & ~(0xFFFFFFFFu >> (31 - b));
                 uint32_t ww = w;
                 while (!stop) { ww++; const uint2 q1 = *reinterpret_cast<const uint2*>(&WI[ww]); stop = q1.y | ~q1.x; }   // pad word: insert bits == 0 -> stops
                 const uint32_t end = ww * 32 + (__ffs(stop) - 1);
-                const uint4 rec = ld_rec(ins + i);
                 const uint32_t key = keyOf(rec.x, rec.z & 0xFFFFu);
                 const uint32_t p = rec.y == 0 ? n : lookup(rec.y, rec.z >> 16);
                 const uint32_t q = p == n ? M : runOf(p);
@@ -405,6 +428,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             }
             __syncwarp();
         }
+        PT_PHASE(kPhD);
 #pragma unroll 1
         for (uint32_t rb = 0; rb <= M; rb += 32) {                 // enter(r): first child, else exit(r)
             const uint32_t r = rb + lane;
@@ -462,6 +486,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     }
     A.used = markD;                                                // release the run-tree temporaries
     ps.pass();                                                     // (4) sequence ranked
+    PT_PHASE(kPhE);
 
     // ---- F: per-element visible rank table + text out (visible index = prefix count of non-deleted elements,
     // micromerge.ts:747-750).  EV[i] = visible elements before insert record i in the sequence | visible << 15: every mark
@@ -498,6 +523,13 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         for (uint32_t l = lane; l < lines; l += 32) prefetch_l2(p0 + ((size_t)l << 7));
     }
 
+    // the first 6 trips of mark records -> L2 now, just before G: prefetched right after C, most lines were evicted from L2
+    // (thousands of logs in flight stream through it) before G read them (DESIGN.md §4.1)
+    if (m) {
+        const uint32_t pfb = min(m * 32u, 6u * 1024u);
+        for (uint32_t o = lane * 128u; o < pfb; o += 32u * 128u) prefetch_l2(reinterpret_cast<const char*>(mk) + o);
+    }
+    PT_PHASE(kPhF);
     uint32_t nS = 0, nC = 0;
     uint4* Sv = nullptr;                                           // survivors: {va | vb << 16, priority:16 | kind << 16, attr, -}
     uint16_t* CIdx = nullptr;                                      // surviving comment ops (indices into Sv), arrival order
@@ -580,6 +612,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     }
 
     ps.pass();                                                     // (5) marks resolved
+    PT_PHASE(kPhG);
     unsigned long long pool_base = 0;
     if (nvis == 0) nspans = 0;
     else if (nS == 0) {
@@ -862,6 +895,10 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         r.digest[0] = d0 + t; r.digest[1] = d1 ^ pt_term_hi(t);
         *res = r;
     }
+    PT_PHASE(kPhI);
+#ifdef PT_PHASE_CLOCKS
+    pclk.logs++;
+#endif
     ps.leave();
     return 0;
 }
@@ -884,6 +921,10 @@ __global__ void __launch_bounds__(WARPS * 32, (32 / WARPS) > 0 ? (32 / WARPS) : 
     PhaseSync ps; ps.on = phased ? 1u : 0u; ps.nthreads = WARPS * 32; ps.next = kFirstPhaseBar; ps.skip = (P.warp_flags >> 8) & 0xFu;
     uint32_t nextb = 0, nextb2 = 0, par = 0;   // phased: the CTA's next two rounds (held by thread 0)
     uint32_t w = 0, wend = 0, wn = 0;      // free: this warp's current grab [w, wend) and the next one
+#ifdef PT_PHASE_CLOCKS
+    PhaseClock pclk{};
+    pclk.t = clock64();
+#endif
     if (phased) { if (threadIdx.x == 0) { nextb = atomicAdd(P.work_counter, (uint32_t)WARPS); nextb2 = atomicAdd(P.work_counter, (uint32_t)WARPS); } }
     else {
         if (lane == 0) { w = atomicAdd(P.work_counter, kWarpGrab); wn = atomicAdd(P.work_counter, kWarpGrab); }
@@ -913,11 +954,12 @@ __global__ void __launch_bounds__(WARPS * 32, (32 / WARPS) > 0 ? (32 / WARPS) : 
             x = w++;
             xn = w < wend ? w : wn;
         }
+        PT_PHASE(kPhRound);
         if (x < n_work) {
             const uint32_t li = P.order[x];
             if (P.admit && P.admit[li]) { ps.leave(); continue; }      // rejected by the admission pre-pass
             const uint32_t li_next = ((P.warp_flags & 2u) && xn < n_work) ? P.order[xn] : 0xFFFFFFFFu;
-            const int rc = warp_merge_one_log<IDM>(P, li, base, slice, li_next, ps);   // the host put the log in the right launch
+            const int rc = warp_merge_one_log<IDM>(P, li, base, slice, li_next, ps PT_PHASE_ARG);   // the host put the log in the right launch
             __syncwarp();
             if (rc) { if (lane == 0) P.retry_list[atomicAdd(P.retry_count, 1u)] = li; deferred++; } else done++;
         } else ps.leave();
@@ -925,6 +967,10 @@ __global__ void __launch_bounds__(WARPS * 32, (32 / WARPS) > 0 ? (32 / WARPS) : 
     if (lane == 0) {
         if (done) atomicAdd(&P.stats[0], (unsigned long long)done);
         if (deferred) atomicAdd(&P.stats[2], (unsigned long long)deferred);
+#ifdef PT_PHASE_CLOCKS
+        for (int k = 0; k < kNumPhases; k++) atomicAdd(&ptk_phase_clk[k], pclk.c[k]);
+        atomicAdd(&ptk_phase_clk[kNumPhases], pclk.logs);
+#endif
     }
 }
 
