@@ -131,6 +131,9 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     auto keyOf = [&](uint32_t ctr, uint32_t actor) -> uint32_t { return (ctr - 1u) * R + actor; };
     auto badId = [&](uint32_t ctr, uint32_t actor) -> bool { return ctr - 1u >= C || actor >= R; };
     auto fail = [&](uint32_t code) { st |= 1u << code; };
+    // a duplicate insert opId sets bit 0 (no status has code 0): it is reported as PT_LOG_BAD_OPID only when the record pass
+    // found no other failure — the block and team kernels count duplicates only after their record pass (DESIGN.md §2)
+    auto failDup = [&]() { st |= 1u; };
     auto bail = [&](uint32_t code) { if (lane == 0) { pt_log_result r{}; r.status = code; *res = r; } };
 
     // ---- id table: opId -> insert record index ------------------------------------------------------------------------------
@@ -217,15 +220,15 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             if (isIns) {
                 if (packed) {
                     const uint32_t sh = 10u * actor;
-                    if ((atomicOr(&T32[ctr - 1u], (i + 1u) << sh) >> sh) & 1023u) fail(PT_LOG_BAD_OPID);   // two inserts with one opId
+                    if ((atomicOr(&T32[ctr - 1u], (i + 1u) << sh) >> sh) & 1023u) failDup();   // two inserts with one opId
                 } else if (!compact) {
-                    if (T[key] != kNone16) fail(PT_LOG_BAD_OPID);      // two inserts with one opId (earlier trip)
+                    if (T[key] != kNone16) failDup();                  // two inserts with one opId (earlier trip)
                     T[key] = (uint16_t)i;
                 } else {
                     mine = (actor << 11) | i;
                     const uint32_t e = T[ctr - 1u];
                     if (e == kNone16) { T[ctr - 1u] = (uint16_t)mine; wrote = true; }
-                    else if ((e >> 11) == actor) fail(PT_LOG_BAD_OPID);
+                    else if ((e >> 11) == actor) failDup();
                     else toOv = true;
                 }
             }
@@ -241,11 +244,11 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             if (lane == 0) *reinterpret_cast<uint2*>(&WI[base >> 5]) = make_uint2(insW, candW);
             __syncwarp();                                          // the trip's ids are in T
             if (IDM == kIdDirect) {
-                if (isIns && T[key] != (uint16_t)i) fail(PT_LOG_BAD_OPID);   // two inserts with one opId (same trip)
+                if (isIns && T[key] != (uint16_t)i) failDup();               // two inserts with one opId (same trip)
             } else if (compact) {
                 if (wrote) {                                       // same counter twice in one trip: one lane owns the slot
                     const uint32_t e2 = T[ctr - 1u];
-                    if (e2 != mine) { if ((e2 >> 11) == actor) fail(PT_LOG_BAD_OPID); else toOv = true; }
+                    if (e2 != mine) { if ((e2 >> 11) == actor) failDup(); else toOv = true; }
                 }
                 const uint32_t ovW = __ballot_sync(kFull, toOv);
                 if (ovW) {
@@ -255,7 +258,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                         for (uint32_t h = ovHash(key);; h = (h + 1u) & (kOvSlots - 1u)) {
                             const uint32_t old = atomicCAS(&OV[h], kOvEmpty, val);
                             if (old == kOvEmpty) break;
-                            if ((old >> 16) == key) { fail(PT_LOG_BAD_OPID); break; }
+                            if ((old >> 16) == key) { failDup(); break; }
                         }
                     }
                     __syncwarp();
@@ -280,7 +283,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     ps.pass();                                                     // (2) end of the record pass
     if (compact && nOv > kOvMax) { ps.leave(); return 1; }                                    // too many concurrent-counter inserts for the compact table
     st = __reduce_or_sync(kFull, st);
-    if (st) { bail(31u - __clz(st)); ps.leave(); return 0; }
+    if (st) { bail(st > 1u ? 31u - __clz(st) : PT_LOG_BAD_OPID); ps.leave(); return 0; }
     PT_PHASE(kPhAB);
 
     // ---- C: runs, bit-parallel: head = insert & (!chain-link | predecessor has another child); visible = insert & !deleted
