@@ -366,6 +366,28 @@ typedef struct pt_elem_query { uint32_t log; uint32_t index; uint32_t flags; uin
 #define PT_ELEM_NOT_FOUND 0xFFFFFFFFu
 int pt_batch_query_elements(pt_batch*, const pt_elem_query* queries, uint32_t n, uint32_t* record_index_out);
 
+/* Batched elemId -> position resolution, the inverse of the query above: findListElement (src/micromerge.ts:731-755) on the
+ * materialised documents, whose `.visible` is resolveCursor's answer (:475-477).  Same preconditions as
+ * pt_batch_query_elements (PT_FLAG_EMIT_SEQUENCE and a completed merge, else PT_ERR_STATE); synchronises.
+ * Query k names the element of log `log` whose insert op has the opId (ctr, actor) in the PACKED id space (actor rank; the
+ * dense counter rank where the packer re-ranked sparse counters).  An opId that no INSERT record of the log carries is not
+ * found: opIds of delete and mark ops (not list elements), ctr 0 (HEAD), ctr > max_ctr, actor >= n_actors.  Not found means
+ * index = record = PT_ELEM_NOT_FOUND and visible = 0; a log index >= n_logs or a log whose status is not PT_LOG_OK also sets
+ * PT_ELEM_LOG_FAILED (the reference would have thrown before such a document existed).
+ * One warp per query on the device: a coalesced scan of the log's ins/del records for the insert, then of its element
+ * sequence for the position, counting the visible elements before it. */
+typedef struct pt_elem_ref { uint32_t log; uint32_t ctr; uint16_t actor; uint16_t reserved0; uint32_t reserved1; } pt_elem_ref;   /* 16 B */
+typedef struct pt_elem_pos {
+    uint32_t index;    /* position in the element sequence incl. tombstones (the reference's metadata index)           */
+    uint32_t visible;  /* non-deleted elements before it (resolveCursor's answer)                                     */
+    uint32_t record;   /* its insert record in the log's ins/del records (what pt_batch_query_elements returns)       */
+    uint32_t flags;    /* PT_ELEM_DELETED, PT_ELEM_AFTER_DEFINED (the sequence's bit 30), PT_ELEM_LOG_FAILED          */
+} pt_elem_pos;     /* 16 B */
+#define PT_ELEM_DELETED 1u
+#define PT_ELEM_AFTER_DEFINED 2u
+#define PT_ELEM_LOG_FAILED 4u
+int pt_batch_find_elements(pt_batch*, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out);
+
 /* Copy only the per-log result headers (status, counts, digest). Synchronises the stream. */
 int pt_batch_download_results(pt_batch*, pt_log_result* out, uint32_t n_logs);
 

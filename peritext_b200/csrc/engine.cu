@@ -368,6 +368,60 @@ __global__ void query_elements_kernel(const pt_elem_query* __restrict__ q, uint3
     }
 }
 
+// ---- batched findListElement (reference src/micromerge.ts:731-755; resolveCursor :475 = .visible) -------------------------
+// One warp per query, the inverse of query_elements_kernel.  Stage 1 finds the element's insert record: the log's ins/del
+// records 32 per trip (coalesced 16-byte loads), first ballot hit (a log that merged OK has no duplicate insert opIds).
+// Stage 2 finds the sequence word that names that record, 32 words per trip, and counts the visible elements before it:
+// the running popcount of the live ballot plus the live lanes below the matching one.  O(n_insdel + n_elems) reads per
+// query, like the reference's linear scan.
+__global__ void find_elements_kernel(const pt_elem_ref* __restrict__ q, uint32_t n, const pt_log_desc* __restrict__ desc,
+                                     const pt_insdel_rec* __restrict__ insdel, const pt_log_result* __restrict__ res,
+                                     const uint64_t* __restrict__ seq_off, const uint32_t* __restrict__ seq, uint32_t n_logs,
+                                     pt_elem_pos* __restrict__ out) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t k = warp; k < n; k += nwarps) {
+        const uint4 Q = __ldg(reinterpret_cast<const uint4*>(q + k));
+        const uint32_t log = Q.x, ctr = Q.y, actor = Q.z & 0xFFFFu;
+        uint4 ans = make_uint4(PT_ELEM_NOT_FOUND, 0u, PT_ELEM_NOT_FOUND, 0u);      // index, visible, record, flags
+        if (log >= n_logs || res[log].status != PT_LOG_OK) {
+            ans.w = PT_ELEM_LOG_FAILED;
+        } else if (ctr != 0) {
+            const pt_log_desc D = desc[log];
+            const uint4* r = reinterpret_cast<const uint4*>(insdel + D.insdel_off);
+            uint32_t rec = PT_ELEM_NOT_FOUND;
+            for (uint32_t b = 0; b < D.n_insdel; b += 32) {
+                bool hit = false;
+                if (b + lane < D.n_insdel) {
+                    const uint4 w = __ldg(r + b + lane);
+                    hit = w.x == ctr && (w.z & 0xFFFFu) == actor && PT_PAYLOAD_KIND(w.w) == PT_KIND_INSERT;
+                }
+                const uint32_t bal = __ballot_sync(0xffffffffu, hit);
+                if (bal) { rec = b + __ffs(bal) - 1; break; }
+            }
+            if (rec != PT_ELEM_NOT_FOUND) {
+                const uint32_t N = res[log].n_elems;
+                const uint32_t* s = seq + seq_off[log];
+                uint32_t seen = 0;
+                for (uint32_t b = 0; b < N; b += 32) {
+                    const bool valid = b + lane < N;
+                    const uint32_t e = valid ? s[b + lane] : 0u;
+                    const uint32_t live = __ballot_sync(0xffffffffu, valid && !(e >> 31));
+                    const uint32_t match = __ballot_sync(0xffffffffu, valid && (e & 0x3FFFFFFFu) == rec);
+                    if (match) {
+                        const uint32_t m = __ffs(match) - 1;
+                        const uint32_t em = __shfl_sync(0xffffffffu, e, m);
+                        ans = make_uint4(b + m, seen + __popc(live & ((1u << m) - 1u)), rec,
+                                         ((em >> 31) ? PT_ELEM_DELETED : 0u) | (((em >> 30) & 1u) ? PT_ELEM_AFTER_DEFINED : 0u));
+                        break;
+                    }
+                    seen += __popc(live);
+                }
+            }
+        }
+        if (lane == 0) reinterpret_cast<uint4*>(out)[k] = ans;
+    }
+}
+
 }  // namespace
 
 struct pt_batch {
@@ -1208,6 +1262,31 @@ int pt_batch_query_elements(pt_batch* b, const pt_elem_query* queries, uint32_t 
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
     dq.release(); da.release();
     if (e != cudaSuccess) { g_last_error = std::string("pt_batch_query_elements: ") + cudaGetErrorString(e); return PT_ERR_CUDA; }
+    return PT_OK;
+}
+
+int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out) {
+    if (!b || (n && (!refs || !out))) return PT_ERR_INVALID;
+    if (!b->merged) { g_last_error = "find before merge"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
+    if (!n) return PT_OK;
+    PT_CUDA(cudaSetDevice(b->device));
+    DevBuf dq, da;
+    int rc;
+    if ((rc = dq.reserve((size_t)n * sizeof(pt_elem_ref))) || (rc = da.reserve((size_t)n * sizeof(pt_elem_pos)))) { dq.release(); da.release(); return rc; }
+    cudaError_t e = cudaMemcpyAsync(dq.p, refs, (size_t)n * sizeof(pt_elem_ref), cudaMemcpyHostToDevice, b->stream);
+    if (e == cudaSuccess) {
+        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+        find_elements_kernel<<<grid, threads, 0, b->stream>>>((const pt_elem_ref*)dq.p, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel,
+                                                             (const pt_log_result*)b->d_results.p, (const uint64_t*)b->d_text_off.p,
+                                                             (const uint32_t*)b->d_seq.p, b->n_logs, (pt_elem_pos*)da.p);
+        e = cudaGetLastError();
+        b->launches++;
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * sizeof(pt_elem_pos), cudaMemcpyDeviceToHost, b->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
+    dq.release(); da.release();
+    if (e != cudaSuccess) { g_last_error = std::string("pt_batch_find_elements: ") + cudaGetErrorString(e); return PT_ERR_CUDA; }
     return PT_OK;
 }
 

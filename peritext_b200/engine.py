@@ -11,7 +11,8 @@ import os
 
 import numpy as np
 
-from .packing import (CDESC_DT, CHANGE_DT, DEP_DT, DESC_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT, ChangeTable, MergedBatch, PackedBatch)
+from .packing import (CDESC_DT, CHANGE_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT,
+                      ChangeTable, MergedBatch, PackedBatch, elem_refs)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
@@ -20,7 +21,7 @@ _lib = None
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
            "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
-           "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_query_elements", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
+           "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_query_elements", "pt_batch_find_elements", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
 
 
 class EngineError(RuntimeError):
@@ -155,6 +156,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_download_patches.argtypes = [vp, vp]
     L.pt_batch_set_patch_pool.argtypes = [vp, u64]
     L.pt_batch_query_elements.argtypes = [vp, vp, u32, vp]
+    L.pt_batch_find_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_destroy.argtypes = [vp]; L.pt_batch_destroy.restype = None
     L.pt_strerror.argtypes = [ctypes.c_int]; L.pt_strerror.restype = ctypes.c_char_p
     L.pt_last_error.restype = ctypes.c_char_p
@@ -325,6 +327,29 @@ class BatchEngine:
         q["flags"] = np.asarray(look_after_tombstones, dtype=np.uint32) if not np.isscalar(look_after_tombstones) else (1 if look_after_tombstones else 0)
         out = np.zeros(len(q), np.uint32)
         _check(self._L.pt_batch_query_elements(self._h, q.ctypes.data, len(q), out.ctypes.data), "pt_batch_query_elements")
+        return out
+
+    def find_elements(self, logs, ctrs, actors) -> np.ndarray:
+        """Batched findListElement on the device (reference src/micromerge.ts:731-755): for query k the element of log
+        `logs[k]` whose insert has the packed opId (`ctrs[k]`, `actors[k]`) (see ``packing.elem_refs``).  Returns ELEM_POS_DT
+        rows: `index` in the element sequence incl. tombstones, `visible` = non-deleted elements before it (resolveCursor),
+        `record` = its insert record in the log, `flags` = ELEM_DELETED | ELEM_AFTER_DEFINED | ELEM_LOG_FAILED;
+        index = record = ELEM_NOT_FOUND where no insert of the log has that opId.  Needs emit_sequence and a completed merge."""
+        q = np.zeros(len(logs), ELEM_REF_DT)
+        q["log"], q["ctr"], q["actor"] = logs, ctrs, actors
+        out = np.zeros(len(q), ELEM_POS_DT)
+        _check(self._L.pt_batch_find_elements(self._h, q.ctypes.data, len(q), out.ctypes.data), "pt_batch_find_elements")
+        return out
+
+    def resolve_cursors(self, batch: PackedBatch, logs, elem_ids) -> np.ndarray:
+        """resolveCursor (reference src/micromerge.ts:475-477) for many documents in one device pass: the number of visible
+        elements before the element `elem_ids[k]` ("ctr@actor") of the merged log `logs[k]` of `batch` (the batch of the
+        last merge), or -1 where the reference throws "List element not found"."""
+        refs, ok = elem_refs(batch, logs, elem_ids)
+        out = np.full(len(refs), -1, np.int64)
+        if ok.any():
+            pos = self.find_elements(refs["log"][ok], refs["ctr"][ok], refs["actor"][ok])
+            out[ok] = np.where(pos["index"] != ELEM_NOT_FOUND, pos["visible"].astype(np.int64), -1)
         return out
 
     def set_comment_pool(self, entries: int):

@@ -32,13 +32,18 @@ SPAN_DT = np.dtype([("start", "<u4"), ("flags", "<u4"), ("link_attr", "<u4"), ("
 CHANGE_DT = np.dtype([("seq", "<u4"), ("actor", "<u2"), ("n_deps", "<u2"), ("dep_off", "<u4"), ("n_ops", "<u4")])
 DEP_DT = np.dtype([("seq", "<u4"), ("actor", "<u2"), ("reserved", "<u2")])
 CDESC_DT = np.dtype([("change_off", "<u8"), ("dep_off", "<u8"), ("n_changes", "<u4"), ("n_deps", "<u4")])
+ELEM_REF_DT = np.dtype([("log", "<u4"), ("ctr", "<u4"), ("actor", "<u2"), ("reserved0", "<u2"), ("reserved1", "<u4")])
+ELEM_POS_DT = np.dtype([("index", "<u4"), ("visible", "<u4"), ("record", "<u4"), ("flags", "<u4")])
 assert CHANGE_DT.itemsize == 16 and DEP_DT.itemsize == 8 and CDESC_DT.itemsize == 24
+assert ELEM_REF_DT.itemsize == 16 and ELEM_POS_DT.itemsize == 16
 assert INSDEL_DT.itemsize == 16 and MARK_DT.itemsize == 32 and DESC_DT.itemsize == 32
 assert RESULT_DT.itemsize == 32 and SPAN_DT.itemsize == 16
 
 KIND_INSERT, KIND_DELETE = 0, 1
 TOKEN_POOLED = 0x20000000
 ATTR_NONE = 0xFFFFFFFF
+ELEM_NOT_FOUND = 0xFFFFFFFF
+ELEM_DELETED, ELEM_AFTER_DEFINED, ELEM_LOG_FAILED = 1, 2, 4      # pt_elem_pos.flags
 MARK_TYPES = ["strong", "em", "comment", "link"]  # ALL_MARKS order, reference src/schema.ts:125
 BOUND_TYPES = ["before", "after", "startOfText", "endOfText"]
 SPAN_STRONG, SPAN_EM, SPAN_LINK, SPAN_COMMENT = 1, 2, 4, 8
@@ -337,6 +342,49 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
         table = ChangeTable(cdesc, crecs, cdeps)
     return PackedBatch(desc, insdel, marks, values, link_attrs, [comment_objs[c] for c in comment_sorted], other_attrs,
                        log_actors=[sorted(b.actors, key=js_key) for b in builders], log_counters=counters, changes=table)
+
+
+def elem_refs(batch: PackedBatch, logs: Sequence[int], elem_ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
+    """elemIds ``"ctr@actor"`` of the logs ``logs[k]`` -> packed ids for ``pt_batch_find_elements``: (ELEM_REF_DT array,
+    bool mask of the ids that can exist in their log).  The actor becomes its rank in ``batch.log_actors[log]``; the counter
+    its dense rank in ``batch.log_counters[log]`` where the packer re-ranked sparse counters.  Masked (and not to be sent to
+    the device; their rows hold ctr 0): a log index outside the batch, ``"_head"`` or a malformed id, an actor the log never
+    saw, a counter missing from the log's re-rank table or beyond 32 bits.  Batches from ``pack_logs`` and
+    ``pack_logs_native`` carry the same tables, so both give the same refs."""
+    n = len(elem_ids)
+    refs = np.zeros(n, ELEM_REF_DT)
+    ok = np.zeros(n, bool)
+    logs = np.asarray(logs, dtype=np.int64)
+    if logs.shape != (n,):
+        raise ValueError("logs and elem_ids must have the same length")
+    refs["log"] = np.clip(logs, 0, 0xFFFFFFFF)
+    ranks: dict[int, dict[str, int]] = {}
+    for k in range(n):
+        i = int(logs[k])
+        if i < 0 or i >= batch.n_logs or i >= len(batch.log_actors):
+            continue
+        m = _OPID_RE.match(elem_ids[k]) if isinstance(elem_ids[k], str) else None
+        if m is None:
+            continue
+        ctr = int(m.group(1))
+        rank = ranks.get(i)
+        if rank is None:
+            rank = ranks[i] = {a: r for r, a in enumerate(batch.log_actors[i])}
+        a = rank.get(m.group(2))
+        if a is None:
+            continue
+        cmap = batch.log_counters[i] if i < len(batch.log_counters) else None
+        if cmap is not None:
+            c = int(np.searchsorted(cmap, ctr)) if ctr < 2 ** 64 else len(cmap)
+            if c >= len(cmap) or int(cmap[c]) != ctr:
+                continue
+            ctr = c
+        if ctr > 0xFFFFFFFF:
+            continue
+        refs["ctr"][k] = ctr
+        refs["actor"][k] = a
+        ok[k] = True
+    return refs, ok
 
 
 # ------------------------------------------------------------------------------------------------------------------
