@@ -52,17 +52,17 @@ def check(engine, docs, logs):
         assert decode_spans(batch, got, i) == docs[i].getTextWithFormatting()
 
 
-def test_typing_backwards_all_children_of_head(engine):
+def typing_backwards_session():
     docs, logs, q, do = session(2)
     for k in range(300):
         do(k % 2, [dict(action="insert", index=0, values=[chr(97 + k % 26)])])
         if k % 50 == 49:
             sync_all(docs, logs, q)
     sync_all(docs, logs, q)
-    check(engine, docs, logs)
+    return docs, logs
 
 
-def test_one_character_changes_and_interleaved_actors(engine):
+def interleaved_actors_session():
     docs, logs, q, do = session(3)
     rng = random.Random(1)
     for k in range(240):
@@ -72,19 +72,19 @@ def test_one_character_changes_and_interleaved_actors(engine):
         if rng.random() < 0.2:
             sync_all(docs, logs, q)
     sync_all(docs, logs, q)
-    check(engine, docs, logs)
+    return docs, logs
 
 
-def test_eight_actors_insert_at_one_position(engine):
-    docs, logs, q, do = session(8, "xy")
+def one_position_session(n_actors):
+    docs, logs, q, do = session(n_actors, "xy")
     for rnd in range(6):
-        for a in range(8):
-            do(a, [dict(action="insert", index=1, values=list("%d%d" % (a, rnd)))])
+        for a in range(n_actors):
+            do(a, [dict(action="insert", index=1, values=list("%x%d" % (a, rnd)))])
         sync_all(docs, logs, q)
-    check(engine, docs, logs)
+    return docs, logs
 
 
-def test_delete_everything_then_retype(engine):
+def delete_retype_session():
     docs, logs, q, do = session(2, "hello world")
     do(0, [dict(action="addMark", startIndex=0, endIndex=11, markType="strong")])
     sync_all(docs, logs, q)
@@ -94,10 +94,10 @@ def test_delete_everything_then_retype(engine):
     do(1, [dict(action="insert", index=0, values=list("again"))])
     do(0, [dict(action="delete", index=0, count=len(docs[0].root["text"]))])
     sync_all(docs, logs, q)
-    check(engine, docs, logs)
+    return docs, logs
 
 
-def test_identical_nested_and_repeated_marks(engine):
+def repeated_marks_session():
     docs, logs, q, do = session(3, "The Peritext editor is a rich text CRDT")
     for k in range(40):
         a = k % 3
@@ -109,13 +109,10 @@ def test_identical_nested_and_repeated_marks(engine):
         if k % 5 == 4:
             sync_all(docs, logs, q)     # add/remove of one id only race inside a sync window of <= 5 steps per actor
     sync_all(docs, logs, q)
-    # concurrent add/remove of ONE comment id is arrival-order dependent in the reference itself (SURVEY.md §9.3 Q4): the
-    # engine folds comment ops in each replica's own arrival order, so every replica matches the oracle exactly — all
-    # arrays, spans and comment lists included — even where the replicas do not agree with each other
-    check(engine, docs, logs)
+    return docs, logs
 
 
-def test_nested_and_identical_ranges_without_comment_race(engine):
+def nested_ranges_session():
     docs, logs, q, do = session(3, "The Peritext editor is a rich text CRDT")
     for k in range(30):
         a = k % 3
@@ -128,6 +125,46 @@ def test_nested_and_identical_ranges_without_comment_race(engine):
         if k % 5 == 4:
             sync_all(docs, logs, q)
     sync_all(docs, logs, q)
+    return docs, logs
+
+
+# every session above, by name: (docs, logs) with logs[r] = the changes replica r applied, in arrival order
+SESSIONS = {
+    "typing-backwards": typing_backwards_session,
+    "interleaved-actors": interleaved_actors_session,
+    "eight-actors-one-position": lambda: one_position_session(8),
+    "delete-retype": delete_retype_session,
+    "repeated-marks": repeated_marks_session,
+    "nested-ranges": nested_ranges_session,
+    "twelve-actors-one-position": lambda: one_position_session(12),
+}
+
+
+def test_typing_backwards_all_children_of_head(engine):
+    check(engine, *typing_backwards_session())
+
+
+def test_one_character_changes_and_interleaved_actors(engine):
+    check(engine, *interleaved_actors_session())
+
+
+def test_eight_actors_insert_at_one_position(engine):
+    check(engine, *one_position_session(8))
+
+
+def test_delete_everything_then_retype(engine):
+    check(engine, *delete_retype_session())
+
+
+def test_identical_nested_and_repeated_marks(engine):
+    # concurrent add/remove of ONE comment id is arrival-order dependent in the reference itself (SURVEY.md §9.3 Q4): the
+    # engine folds comment ops in each replica's own arrival order, so every replica matches the oracle exactly — all
+    # arrays, spans and comment lists included — even where the replicas do not agree with each other
+    check(engine, *repeated_marks_session())
+
+
+def test_nested_and_identical_ranges_without_comment_race(engine):
+    docs, logs = nested_ranges_session()
     check(engine, docs, logs)
     spans = [d.getTextWithFormatting() for d in docs]
     assert spans[0] == spans[1] == spans[2]       # no same-id race: the replicas converge
@@ -136,11 +173,7 @@ def test_nested_and_identical_ranges_without_comment_race(engine):
 def test_many_actors_share_counters_compact_table_overflows(engine):
     # 12 replicas insert concurrently at one position, round after round: every counter value is used by 12 inserts, far more
     # than the warp kernel's overflow table for its compact id table holds -> the log is deferred on the device; same results
-    docs, logs, q, do = session(12, "xy")
-    for rnd in range(6):
-        for a in range(12):
-            do(a, [dict(action="insert", index=1, values=list("%x%d" % (a, rnd)))])
-        sync_all(docs, logs, q)
+    docs, logs = one_position_session(12)
     check(engine, docs, logs)
     spans = [d.getTextWithFormatting() for d in docs]
     assert all(s == spans[0] for s in spans)
