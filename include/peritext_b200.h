@@ -388,6 +388,37 @@ typedef struct pt_elem_pos {
 #define PT_ELEM_LOG_FAILED 4u
 int pt_batch_find_elements(pt_batch*, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out);
 
+/* getTextWithFormatting's return value (FormatSpanWithText[], src/peritext.ts:35-38, 337-455) of every merged log as UTF-8
+ * JSON text, rendered on the device.  Log i's text is bytes[off[i] .. off[i+1]):
+ *   [{"marks":M,"text":T},...]      one object per span, keys sorted; no visible text gives []
+ *   M = {"comment":[C,...],"em":{"active":true},"link":L,"strong":{"active":true}}, only the marks present ({} for none);
+ *       the comment list follows the span's comment pool order (ascending rank = sortBy id), and is [] for a span whose
+ *       PT_SPAN_COMMENT is set with zero ids (quirk Q3)
+ *   T = the span's text (the concatenation of its element values, in UTF-16 code units) as JSON.stringify writes a string:
+ *       \" \\ \b \t \n \f \r, \u00xx (lowercase) for the other units below U+0020, raw UTF-8 for everything else (U+007F,
+ *       U+2028, U+2029, / included); a high surrogate immediately followed by a low surrogate in the same span is one 4-byte
+ *       character, also when the halves come from different elements; any other surrogate unit is \udxxx (lowercase)
+ *   C, L = the fragments of the caller's pools for the comment rank / link attr id, copied verbatim, except that the 3-byte
+ *       encoding of a lone surrogate (ED A0..BF xx) becomes \udxxx; so the output is always valid UTF-8
+ * A log whose status is not PT_LOG_OK renders as zero bytes; a log that merged is at least "[]".
+ * Pools: data + byte offsets [count + 1] each, the layouts of pt_ingest_pool's kinds PT_POOL_VALUES (UTF-16LE values),
+ * PT_POOL_LINK_ATTRS and PT_POOL_COMMENT_ATTRS (canonical JSON), so a C caller passes those three straight through.  A pool
+ * with count 0 may have null pointers.
+ * Preconditions of pt_batch_download (a completed merge, else PT_ERR_STATE); PT_FLAG_EMIT_SEQUENCE is not needed.  Null pools
+ * or out: PT_ERR_INVALID.  A log that merged and names a value index, link id or comment rank >= its pool's count:
+ * PT_ERR_INVALID, pt_last_error names the first such entry (lowest log, then value / link / comment, then lowest index), no
+ * view.  n_logs == 0: PT_OK with off[0] = 0, nothing launched.
+ * Synchronises.  The view is engine-owned pinned memory, valid until the next render, upload or destroy on the handle; the
+ * pt_spans_view / pt_patch_view of the same merge stay valid and unchanged, and rendering again gives identical bytes.
+ * Device: a size pass and a write pass, one warp per log, 32 elements of a span per trip. */
+typedef struct pt_json_pools {          /* layouts = pt_ingest_pool's kinds 0, 1, 3: data + byte offsets [count + 1] */
+    const uint8_t* values;   const uint64_t* values_off;   uint64_t n_values;    /* UTF-16LE element values (PT_POOL_VALUES)   */
+    const uint8_t* links;    const uint64_t* links_off;    uint64_t n_links;     /* JSON fragment per link attr id              */
+    const uint8_t* comments; const uint64_t* comments_off; uint64_t n_comments;  /* JSON fragment per comment rank              */
+} pt_json_pools;
+typedef struct pt_json_view { uint32_t n_logs; const uint64_t* off; /* [n_logs + 1] */ const char* bytes; uint64_t n_bytes; } pt_json_view;
+int pt_batch_render_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
+
 /* Copy only the per-log result headers (status, counts, digest). Synchronises the stream. */
 int pt_batch_download_results(pt_batch*, pt_log_result* out, uint32_t n_logs);
 

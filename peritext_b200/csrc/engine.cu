@@ -16,6 +16,7 @@
 #include "warp_kernel.cuh"
 #include "patch_kernel.cuh"
 #include "team_kernel.cuh"
+#include "render_kernel.cuh"
 
 namespace {
 
@@ -177,12 +178,25 @@ __global__ void expand_mark_c16_kernel(const pt_mark_c16* __restrict__ in, pt_ma
 // tokens, min(n_insdel, 2 n_mark + 1) spans), typically a few percent full (c4: 5 visible characters per 500-record log).
 // Before the device -> host copy the used prefixes are packed back to back: exclusive scan of (n_visible, n_spans) over
 // the logs (block sums -> one-block scan -> offsets), then one warp per log copies its tokens and spans.
+// The scan kernels take the per-log counts from a source functor: two channels (a, c) per log.  The JSON render
+// (render_kernel.cuh) scans its per-log byte counts through the same kernels, on channel a only.
 constexpr uint32_t kScanBlock = 1024;
-__global__ void out_block_sums_kernel(const pt_log_result* __restrict__ res, uint32_t n, unsigned long long* __restrict__ bsum) {
+struct MergedCounts {      // (n_visible, n_spans) of the logs that merged, 0 for the others
+    const pt_log_result* __restrict__ res;
+    __device__ void operator()(uint32_t i, unsigned long long& a, unsigned long long& c) const {
+        if (res[i].status == 0) { a = res[i].n_visible; c = res[i].n_spans; }
+    }
+};
+struct PlainCounts {       // a u64 count per log on channel a
+    const unsigned long long* __restrict__ cnt;
+    __device__ void operator()(uint32_t i, unsigned long long& a, unsigned long long&) const { a = cnt[i]; }
+};
+template <class Src>
+__global__ void out_block_sums_kernel(Src src, uint32_t n, unsigned long long* __restrict__ bsum) {
     __shared__ unsigned long long sa[32], sb[32];
     const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long a = 0, c = 0;
-    if (i < n && res[i].status == 0) { a = res[i].n_visible; c = res[i].n_spans; }
+    if (i < n) src(i, a, c);
     for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
     if (lane == 0) { sa[warp] = a; sb[warp] = c; }
     __syncthreads();
@@ -226,12 +240,13 @@ __global__ void out_scan_blocks_kernel(unsigned long long* bsum, uint32_t nb) { 
     }
     if (threadIdx.x == 0) { bsum[2 * nb] = ca; bsum[2 * nb + 1] = cb; }
 }
-__global__ void out_offsets_kernel(const pt_log_result* __restrict__ res, uint32_t n, const unsigned long long* __restrict__ bsum, uint32_t nb,
+template <class Src>   // soff may be null (one-channel sources)
+__global__ void out_offsets_kernel(Src src, uint32_t n, const unsigned long long* __restrict__ bsum, uint32_t nb,
                                    unsigned long long* __restrict__ toff, unsigned long long* __restrict__ soff) {
     __shared__ unsigned long long wa[32], wb[32];
     const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long va = 0, vb = 0;
-    if (i < n && res[i].status == 0) { va = res[i].n_visible; vb = res[i].n_spans; }
+    if (i < n) src(i, va, vb);
     unsigned long long a = va, c = vb;
     for (int o = 1; o < 32; o <<= 1) {
         const unsigned long long ya = __shfl_up_sync(0xffffffffu, a, o), yb = __shfl_up_sync(0xffffffffu, c, o);
@@ -249,8 +264,8 @@ __global__ void out_offsets_kernel(const pt_log_result* __restrict__ res, uint32
         wa[lane] = x - x0; wb[lane] = y - y0;
     }
     __syncthreads();
-    if (i < n) { toff[i] = bsum[2 * blockIdx.x] + wa[warp] + a - va; soff[i] = bsum[2 * blockIdx.x + 1] + wb[warp] + c - vb; }
-    if (i == 0) { toff[n] = bsum[2 * nb]; soff[n] = bsum[2 * nb + 1]; }
+    if (i < n) { toff[i] = bsum[2 * blockIdx.x] + wa[warp] + a - va; if (soff) soff[i] = bsum[2 * blockIdx.x + 1] + wb[warp] + c - vb; }
+    if (i == 0) { toff[n] = bsum[2 * nb]; if (soff) soff[n] = bsum[2 * nb + 1]; }
 }
 __global__ void out_gather_kernel(const pt_log_result* __restrict__ res, uint32_t n, const uint64_t* __restrict__ cap_toff, const uint64_t* __restrict__ cap_soff,
                                   const unsigned long long* __restrict__ toff, const unsigned long long* __restrict__ soff,
@@ -450,6 +465,9 @@ struct pt_batch {
     DevBuf d_cdesc, d_changes, d_deps, d_admit;           // admission pre-pass (optional change table)
     DevBuf d_patch_recs, d_patch_items, d_patch_status;   // PT_FLAG_EMIT_PATCHES
     HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc;
+    DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // pt_batch_render_json: the caller's pools,
+    DevBuf d_jsize, d_jbsum, d_joff, d_jmiss, d_jbytes;                 // per-log sizes, scan, offsets, missing-entry key, output
+    HostBuf h_joff, h_jbytes, h_jmisc;
     uint64_t patch_cap = 0;
     uint32_t patch_smem = 0;
     bool have_changes = false;
@@ -1151,9 +1169,9 @@ int pt_batch_download_begin(pt_batch* b) {
         const pt_log_result* res = (const pt_log_result*)b->d_results.p;
         unsigned long long* bsum = (unsigned long long*)b->d_bsum.p;
         unsigned long long *toff = (unsigned long long*)b->d_ctoff.p, *soff = (unsigned long long*)b->d_csoff.p;
-        out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(res, (uint32_t)n, bsum);
+        out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(MergedCounts{res}, (uint32_t)n, bsum);
         out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
-        out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(res, (uint32_t)n, bsum, nb, toff, soff);
+        out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(MergedCounts{res}, (uint32_t)n, bsum, nb, toff, soff);
         const uint32_t gthreads = 256, ggrid = (uint32_t)std::min<uint64_t>((n * 32 + gthreads - 1) / gthreads, (uint64_t)b->num_sms * 16);
         out_gather_kernel<<<ggrid, gthreads, 0, b->stream>>>(res, (uint32_t)n, (const uint64_t*)b->d_text_off.p, (const uint64_t*)b->d_span_off.p, toff, soff,
                                                            (const uint32_t*)b->d_text.p, (const pt_span*)b->d_spans.p, (uint32_t*)b->d_ctext.p, (pt_span*)b->d_cspans.p);
@@ -1290,6 +1308,82 @@ int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_
     return PT_OK;
 }
 
+// JSON render (render_kernel.cuh): upload the pools, size pass, scan of the sizes through the download path's scan kernels,
+// read back the total and the missing-entry key (one sync), size the output exactly, write pass, copy back.
+int pt_batch_render_json(pt_batch* b, const pt_json_pools* pools, pt_json_view* out) {
+    if (!b || !pools || !out) return PT_ERR_INVALID;
+    if (!b->merged) { g_last_error = "render before merge"; return PT_ERR_STATE; }
+    struct Pool { const uint8_t* data; const uint64_t* off; uint64_t count; DevBuf* dd; DevBuf* doff; const char* name; };
+    const Pool ps[3] = {{pools->values, pools->values_off, pools->n_values, &b->d_jval, &b->d_jvoff, "values"},
+                        {pools->links, pools->links_off, pools->n_links, &b->d_jlink, &b->d_jloff, "links"},
+                        {pools->comments, pools->comments_off, pools->n_comments, &b->d_jcom, &b->d_jcoff, "comments"}};
+    for (const Pool& p : ps) {
+        if (p.count && (!p.data || !p.off)) { g_last_error = std::string("pt_batch_render_json: null ") + p.name + " pool with a nonzero count"; return PT_ERR_INVALID; }
+        for (uint64_t k = 0; k < p.count; k++)
+            if (p.off[k + 1] < p.off[k]) { g_last_error = std::string("pt_batch_render_json: ") + p.name + " offsets decrease"; return PT_ERR_INVALID; }
+    }
+    PT_CUDA(cudaSetDevice(b->device));
+    int rc;
+    const uint32_t n = b->n_logs;
+    if ((rc = b->h_joff.reserve(((size_t)n + 1) * 8)) || (rc = b->h_jbytes.reserve(1)) || (rc = b->h_jmisc.reserve(16))) return rc;
+    uint64_t* hoff = (uint64_t*)b->h_joff.p;
+    if (!n) {
+        hoff[0] = 0;
+        *out = pt_json_view{0, hoff, (const char*)b->h_jbytes.p, 0};
+        return PT_OK;
+    }
+    ptr::JsonPools P{};
+    const uint8_t** pdata[3] = {&P.val, &P.link, &P.com};
+    const uint64_t** poff[3] = {&P.voff, &P.loff, &P.coff};
+    uint64_t* pcount[3] = {&P.nval, &P.nlink, &P.ncom};
+    for (int k = 0; k < 3; k++) {
+        const Pool& p = ps[k];
+        const uint64_t lo = p.count ? p.off[0] : 0, hi = p.count ? p.off[p.count] : 0;     // entries address data[lo, hi)
+        if ((rc = p.dd->reserve(std::max<uint64_t>(1, hi))) || (rc = p.doff->reserve((p.count + 1) * 8))) return rc;
+        if (hi > lo) PT_CUDA(cudaMemcpyAsync((uint8_t*)p.dd->p + lo, p.data + lo, hi - lo, cudaMemcpyHostToDevice, b->stream));
+        if (p.count) PT_CUDA(cudaMemcpyAsync(p.doff->p, p.off, (p.count + 1) * 8, cudaMemcpyHostToDevice, b->stream));
+        *pdata[k] = (const uint8_t*)p.dd->p; *poff[k] = (const uint64_t*)p.doff->p; *pcount[k] = p.count;
+    }
+    const uint32_t nb = (n + kScanBlock - 1) / kScanBlock;
+    if ((rc = b->d_jsize.reserve((size_t)n * 8)) || (rc = b->d_jbsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = b->d_joff.reserve(((size_t)n + 1) * 8)) ||
+        (rc = b->d_jmiss.reserve(8))) return rc;
+    unsigned long long *sizes = (unsigned long long*)b->d_jsize.p, *bsum = (unsigned long long*)b->d_jbsum.p, *doff = (unsigned long long*)b->d_joff.p,
+                       *miss = (unsigned long long*)b->d_jmiss.p;
+    const pt_log_result* res = (const pt_log_result*)b->d_results.p;
+    const uint64_t *toff = (const uint64_t*)b->d_text_off.p, *soff = (const uint64_t*)b->d_span_off.p;
+    const uint32_t* text = (const uint32_t*)b->d_text.p;
+    const pt_span* spans = (const pt_span*)b->d_spans.p;
+    const uint32_t* cpool = (const uint32_t*)b->d_pool.p;
+    const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+    PT_CUDA(cudaMemsetAsync(miss, 0xFF, 8, b->stream));
+    ptr::json_size_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, sizes, miss);
+    out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum);
+    out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
+    out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum, nb, doff, (unsigned long long*)nullptr);
+    PT_CUDA(cudaGetLastError());
+    b->launches += 4;
+    uint64_t* hm = (uint64_t*)b->h_jmisc.p;
+    PT_CUDA(cudaMemcpyAsync(hm, doff + n, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(hm + 1, miss, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    const uint64_t total = hm[0], key = hm[1];
+    if (key != ~0ull) {
+        static const char* kinds[3] = {"value", "link", "comment"};
+        g_last_error = "pt_batch_render_json: log " + std::to_string(key >> 34) + " names " + kinds[(key >> 32) & 3] + " pool entry " +
+                       std::to_string(key & 0xFFFFFFFFull) + ", which the caller's pools do not hold";
+        return PT_ERR_INVALID;
+    }
+    if ((rc = b->d_jbytes.reserve(std::max<uint64_t>(1, total))) || (rc = b->h_jbytes.reserve(std::max<uint64_t>(1, total)))) return rc;
+    ptr::json_write_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, doff, (uint8_t*)b->d_jbytes.p);
+    PT_CUDA(cudaGetLastError());
+    b->launches++;
+    PT_CUDA(cudaMemcpyAsync(hoff, doff, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
+    if (total) PT_CUDA(cudaMemcpyAsync(b->h_jbytes.p, b->d_jbytes.p, total, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    *out = pt_json_view{n, hoff, (const char*)b->h_jbytes.p, total};
+    return PT_OK;
+}
+
 int pt_batch_device_results(pt_batch* b, void** dev_ptr, uint32_t* n_logs) {
     if (!b || !dev_ptr) return PT_ERR_INVALID;
     if (!b->have_batch) return PT_ERR_STATE;
@@ -1351,8 +1445,10 @@ void pt_batch_destroy(pt_batch* b) {
     for (DevBuf* d : {&b->d_desc, &b->d_insdel, &b->d_marks, &b->d_order, &b->d_counters, &b->d_results, &b->d_text_off,
                       &b->d_span_off, &b->d_text, &b->d_spans, &b->d_pool, &b->d_slab, &b->d_retry, &b->d_seq,
                       &b->d_runs, &b->d_tokens, &b->d_run_off, &b->d_tok_off, &b->d_cins, &b->d_cmarks, &b->d_bsum, &b->d_ctoff, &b->d_csoff, &b->d_ctext, &b->d_cspans,
-                      &b->d_cdesc, &b->d_changes, &b->d_deps, &b->d_admit, &b->d_patch_recs, &b->d_patch_items, &b->d_patch_status}) d->release();
-    for (HostBuf* h : {&b->h_patch_recs, &b->h_patch_items, &b->h_patch_status, &b->h_patch_misc}) h->release();
+                      &b->d_cdesc, &b->d_changes, &b->d_deps, &b->d_admit, &b->d_patch_recs, &b->d_patch_items, &b->d_patch_status,
+                      &b->d_jval, &b->d_jvoff, &b->d_jlink, &b->d_jloff, &b->d_jcom, &b->d_jcoff, &b->d_jsize, &b->d_jbsum, &b->d_joff,
+                      &b->d_jmiss, &b->d_jbytes}) d->release();
+    for (HostBuf* h : {&b->h_patch_recs, &b->h_patch_items, &b->h_patch_status, &b->h_patch_misc, &b->h_joff, &b->h_jbytes, &b->h_jmisc}) h->release();
     for (HostBuf* h : {&b->h_stage, &b->h_results, &b->h_text, &b->h_spans, &b->h_pool, &b->h_misc, &b->h_seq, &b->h_ctoff, &b->h_csoff}) h->release();
     if (b->side) cudaStreamDestroy(b->side);
     if (b->ev_fork) cudaEventDestroy(b->ev_fork);

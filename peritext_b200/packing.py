@@ -457,6 +457,29 @@ def decode_spans(batch: PackedBatch, merged: MergedBatch, i: int) -> list[dict]:
     return out
 
 
+def _pool(items: Sequence[bytes]) -> tuple[np.ndarray, np.ndarray]:
+    off = np.zeros(len(items) + 1, np.uint64)
+    if items:
+        off[1:] = np.cumsum([len(b) for b in items], dtype=np.uint64)
+    return np.frombuffer(b"".join(items), np.uint8).copy(), off
+
+
+def json_pools(batch: PackedBatch) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The string pools ``pt_batch_render_json`` reads, built from a PackedBatch: (values, values_off, links, links_off,
+    comments, comments_off), each data as uint8 plus uint64 byte offsets [count + 1].  Values are UTF-16LE; link attrs and
+    comment attrs are their canonical JSON (``canon``) in UTF-8, the form ``pt_ingest_pool`` kinds 1 and 3 hold; lone
+    surrogates pass through in their 3-byte encoding, which the render writes as ``\\udxxx``."""
+    try:
+        n_comments = len(batch.comment_ids)
+    except TypeError:
+        raise ValueError("json_pools: batch.comment_ids has no length (a generated workload's synthetic comment ids): "
+                         "attach a list of the comment attrs objects in rank order first") from None
+    vals = _pool([v.encode("utf-16-le", "surrogatepass") for v in batch.values])
+    links = _pool([canon(a).encode("utf-8", "surrogatepass") for a in batch.link_attrs])
+    comments = _pool([canon(batch.comment_ids[k]).encode("utf-8", "surrogatepass") for k in range(n_comments)])
+    return vals + links + comments
+
+
 class RangeError(Exception):
     """JS RangeError equivalents (reference src/micromerge.ts:503, 507, 539, 752)."""
 
