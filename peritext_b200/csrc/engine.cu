@@ -1,15 +1,16 @@
 // engine.cu — C-ABI of the batch CRDT-merge engine (include/peritext_b200.h) over the sm_90a kernels.
 //
-// Host responsibilities (all per batch, none per op): size the output regions from the descriptors, bin the logs
-// by size (block size + shared-memory budget per bin), order each bin largest-first for the persistent-CTA work
-// queue, launch, and move results.  There is NO CPU fallback: without a CUDA device every entry point fails.
+// Host responsibilities (all per batch, none per op): plan the batch (plan.h: each log's kernel and bin, the order of
+// the persistent-CTA work queues, output capacities), launch from the plan, and move results.  There is NO CPU
+// fallback: without a CUDA device every entry point fails.
 #include <algorithm>
 #include <atomic>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "merge_kernel.cuh"
@@ -17,6 +18,7 @@
 #include "patch_kernel.cuh"
 #include "team_kernel.cuh"
 #include "render_kernel.cuh"
+#include "plan.h"
 
 namespace {
 
@@ -31,79 +33,41 @@ thread_local std::string g_last_error;
         }                                                                                               \
     } while (0)
 
-struct DevBuf {
+// Device memory, or pinned host memory, that grows on demand and is freed with its owner.
+template <bool kPinned>
+struct Buf {
     void* p = nullptr; size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    void release() { if (p) { if (kPinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
     int reserve(size_t bytes) {
         if (bytes <= cap) return PT_OK;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
+        release();
         size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) { g_last_error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return PT_ERR_NOMEM; }
+        cudaError_t e = kPinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want);
+        if (e != cudaSuccess) { g_last_error = std::string(kPinned ? "cudaMallocHost: " : "cudaMalloc: ") + cudaGetErrorString(e); return PT_ERR_NOMEM; }
         cap = want; return PT_OK;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
-struct HostBuf {   // pinned
-    void* p = nullptr; size_t cap = 0;
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return PT_OK;
-        if (p) cudaFreeHost(p);
-        p = nullptr; cap = 0;
-        size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMallocHost(&p, want);
-        if (e != cudaSuccess) { g_last_error = std::string("cudaMallocHost: ") + cudaGetErrorString(e); return PT_ERR_NOMEM; }
-        cap = want; return PT_OK;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+using DevBuf = Buf<false>;
+using HostBuf = Buf<true>;
+
+using ptp::kNumBins;
+using ptp::kCtaBins;
+
+// The device counter block of a batch, zeroed before every merge; the kernels get pointers to its fields.
+struct DevCounters {
+    unsigned long long stats[3];          // BatchParams::stats: logs finished shared-only, on the spill path, deferred
+    unsigned long long comment_used;      // comment-pool cursor: counts past the capacity, so it ends as the batch's demand
+    unsigned long long patch_items;       // patch-item cursor, likewise
+    uint32_t slab[2];                     // next free spill-slab slot: the last bin's own launch, its retry launch
+    uint32_t packed3, compact, direct, team;   // work-queue heads of bin 0's launches
+    uint32_t head[kNumBins];              // work-queue heads of the CTA bins' own lists ([0] unused)
+    uint32_t retry_head[kNumBins];        // work-queue heads of the CTA bins' retry launches ([0] unused)
+    uint32_t deferred[kNumBins];          // logs deferred into bin k, appended to list k of d_retry ([0] unused)
 };
-
-constexpr int kNumBins = 5;
-struct BinCfg { uint32_t max_recs; int block; uint32_t smem; int ctas_per_sm; };
-// shared memory per SM: 228 KB, 1 KB reserved per resident CTA, 227 KB max per CTA.
-// Bin 0 is the WARP-PER-LOG kernel (warp_kernel.cuh): block = warps per CTA * 32, smem = bytes PER WARP; a log it cannot
-// finish is deferred on the device to bin 1.  Bins 1..4 are the CTA-per-log kernel (merge_kernel.cuh).
-BinCfg kBins[kNumBins] = {
-    {2048u, 8 * 32, 7136u, 4},
-    {1536u, 128, 31u * 1024u, 7},
-    {4096u, 256, 74u * 1024u, 3},
-    {12288u, 512, 112u * 1024u, 2},
-    {0xFFFFFFFFu, 1024, 226u * 1024u, 1},
-};
-constexpr int kTeamWarps = 8;                 // team kernel (team_kernel.cuh): 8 warps per log, 4 logs per SM
-constexpr uint32_t kTeamSmem = 55u * 1024u;
-bool g_team_bin = true;
-bool g_warp_bin = true, g_warp_force = false;   // force: skip the host-side footprint estimate (tests of the device-side deferral)
-
-inline size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
-
-// Worst-case arena bytes of one log: an upper bound on the sum of every Arena::alloc in merge_one_log with
-// M <= N <= n, S <= 2m+2, nvis <= n, Mc <= m, nspans <= 2m+1 (released arrays are counted too).
-size_t arena_worst_bytes(uint64_t n, uint64_t m, uint64_t KS) {
-    const size_t I = (n < 32000 && m < 32000) ? 2 : 4;
-    size_t b = 0;
-    auto A = [&](uint64_t count, size_t sz) { b += al16((size_t)count * sz); };
-    const uint64_t NWr = (n + 31) / 32 + 1;
-    A(KS, I); A(NWr, 4); A(NWr, 4); A(NWr, 4); A(NWr, I); A(NWr, I);               // T InsBits HeadBits VisBits HeadPre VisPre
-    A(NWr * 32 + 32, 1); A(NWr * 32 + 32, 1);                                      // Other Del
-    A(2 * n + 3, 8); A((2 * n + 9) / 8 + 3, 8); A((2 * n + 9) / 8 + 3, 8);         // Node Sub Sub2
-    A(n + 1, I); A(n + 2, 4); A(n + 2, 4); A(n + 1, I); A(n + 1, 4); A(n + 2, I);  // RunHead PosBase VisBase Prun Key GrpOff
-    A(n + 1, I); A(n + 1, I); A(n + 1, I);                                         // Unsorted Sorted SPos
-    A(n / 33 + 2, I); A(KS / 32 + 2, 4); A(KS / 32 + 2, I);                        // BigList GBits GPre
-    if (m) {
-        const uint64_t KW = KS / 32 + 2, S = 2 * m + 2, Mc = m, nsp = 2 * m + 1, NWp = (n + 32) / 32 + 1;
-        A(KW + 1, 4); A(KW + 1, I); for (int k = 0; k < 6; k++) A(m + 1, I);       // KBits KPre ByRank MRank IvA IvB IvVA IvVB
-        A(m + 1, 1); A(m + 1, 4); A(m + 1, 4);                                     // MKind MAttr CompactC
-        A(NWp + 1, 4); A(NWp + 1, I);                                              // BndBits SegPre
-        A(2 * S + 2, 4); A(S + 1, 4); A(S + 1, 4); A(S + 2, 4);                    // Tree SegFlags SegLink CDiff
-        A(n / 32 + 3, 4); A(Mc + 1, 4); A(Mc + 1, I); A(Mc + 1, I); A(Mc + 1, I);  // CHead CId CK CG0 CGn
-        A(2 * Mc + 1, I); A(2 * Mc + 1, I);                                        // PcA PcB
-        A(4 * Mc + 8, 4); A(4 * Mc + 9, 4); A(4 * Mc + 9, I); A(Mc + 1, I);        // HTab HCnt HOff CSlot
-        A(n + 1, I); A(n / 32 + 2, 4); A(n / 32 + 2, I);                           // VisSeg HeadB HeadP
-        A(nsp + 1, I); A(nsp + 1, 4); A(nsp + 1, 4); A(nsp + 1, 4);                // SpanStart SpanCC SpanCO SpanCur
-    }
-    return b + 256;
-}
 
 // Expands run-compressed ins/del streams into pt_insdel_rec records (one warp per log, lanes over the runs; a run's
 // records are written by its lane — runs are short, and the expanded array is consumed from L2/HBM by the merge kernel).
@@ -445,19 +409,11 @@ struct pt_batch {
     int num_sms = 0;
     pt_limits limits{};
     // batch
-    bool have_batch = false, merged = false, adopted = false;
+    bool have_batch = false, merged = false;
     uint32_t n_logs = 0;
-    uint64_t n_insdel = 0, n_mark = 0, n_text = 0, n_span = 0, pool_cap = 0;
+    uint64_t n_insdel = 0, n_mark = 0;
     std::vector<pt_log_desc> h_desc;
-    std::vector<uint64_t> h_text_off, h_span_off;
-    std::vector<uint32_t> h_order;
-    uint32_t bin_first[kNumBins + 1] = {0};
-    uint32_t warp_packed = 0;               // bin 0: the first warp_packed logs use the packed3 id table (3 actors, <= 1022 records)
-    uint32_t warp_compact = 0;              // bin 0: the next warp_compact logs use the compact id table
-    uint32_t team_count = 0;                // bin 0: the last team_count logs run on the team kernel
-    uint32_t n_spill = 0, slab_slots = 0;   // logs that can spill / slab slots allocated
-    size_t bin_slab[kNumBins] = {0};
-    size_t retry_slab = 0;
+    ptp::Plan plan;
     // device
     DevBuf d_runs, d_tokens, d_run_off, d_tok_off, d_cins, d_cmarks;
     DevBuf d_desc, d_insdel, d_marks, d_order, d_counters, d_results, d_text_off, d_span_off, d_text, d_spans, d_pool, d_slab, d_retry, d_seq;
@@ -469,7 +425,6 @@ struct pt_batch {
     DevBuf d_jsize, d_jbsum, d_joff, d_jmiss, d_jbytes;                 // per-log sizes, scan, offsets, missing-entry key, output
     HostBuf h_joff, h_jbytes, h_jmisc;
     uint64_t patch_cap = 0;
-    uint32_t patch_smem = 0;
     bool have_changes = false;
     uint32_t adm_maxR = 1;
     const pt_insdel_rec* dp_insdel = nullptr;
@@ -490,161 +445,36 @@ struct pt_batch {
 
 namespace {
 
-// PT_BINS="max_recs:block:smem_kb:ctas_per_sm,..." (4 entries, ascending; last max_recs ignored) overrides the CTA-per-log bins;
-// PT_WARP="max_recs:warps_per_cta:slice_kb:ctas_per_sm" overrides the warp-per-log bin, PT_WARP=0 disables it (tuning)
-const BinCfg kDefaultBins[kNumBins] = {kBins[0], kBins[1], kBins[2], kBins[3], kBins[4]};
-void load_bins_from_env() {
-    // re-read whenever the variables change (tests flip PT_WARP between uploads to cross-check the two kernels)
-    static std::string last = "\x01";
-    const char* we = getenv("PT_WARP"); const char* be = getenv("PT_BINS"); const char* fe = getenv("PT_WARP_FORCE"); const char* te0 = getenv("PT_TEAM");
-    const std::string cur = std::string(we ? we : "") + "|" + (be ? be : "") + "|" + (fe ? fe : "") + "|" + (te0 ? te0 : "");
-    if (cur == last) return;
-    last = cur;
-    for (int i = 0; i < kNumBins; i++) kBins[i] = kDefaultBins[i];
-    g_warp_bin = true; g_warp_force = fe && atoi(fe) != 0;
-    { const char* te = getenv("PT_TEAM"); g_team_bin = !(te && atoi(te) == 0); }
-    if (const char* w = getenv("PT_WARP")) {
-        unsigned long a, wp, sl, ct;
-        if (sscanf(w, "%lu:%lu:%lu:%lu", &a, &wp, &sl, &ct) == 4 && (wp == 2 || wp == 4 || wp == 6 || wp == 8 || wp == 12 || wp == 16)) {
-            if (sl < 256) sl *= 1024;                    // slice: KB, or bytes when >= 256
-            sl &= ~(unsigned long)15;
-            if (sl * wp <= 227 * 1024) kBins[0] = BinCfg{(uint32_t)a, (int)wp * 32, (uint32_t)sl, (int)ct};
-        }
-        else if (atoi(w) == 0) { g_warp_bin = false; g_team_bin = false; }      // PT_WARP=0: CTA-per-log kernels only
-    }
-    const char* e = getenv("PT_BINS");
-    if (!e) return;
-    BinCfg tmp[kNumBins];
-    int k = 1;
-    const char* p = e;
-    while (k < kNumBins && *p) {
-        unsigned long a, bl, sm, ct; int used = 0;
-        if (sscanf(p, "%lu:%lu:%lu:%lu%n", &a, &bl, &sm, &ct, &used) != 4) return;
-        if (bl != 32 && bl != 64 && bl != 128 && bl != 256 && bl != 512 && bl != 1024) return;
-        tmp[k++] = BinCfg{(uint32_t)a, (int)bl, (uint32_t)(sm * 1024), (int)ct};
-        p += used; if (*p == ',') p++;
-    }
-    if (k != kNumBins) return;
-    tmp[kNumBins - 1].max_recs = 0xFFFFFFFFu;
-    for (int i = 1; i < kNumBins; i++) kBins[i] = tmp[i];
-}
+DevCounters* counters(const pt_batch* b) { return (DevCounters*)b->d_counters.p; }
 
-int plan_batch(pt_batch* b, const pt_packed_ops* ops) {
-    load_bins_from_env();
-    b->n_logs = ops->n_logs;
-    b->n_insdel = ops->n_insdel_total;
-    b->n_mark = ops->n_mark_total;
-    b->h_desc.assign(ops->logs, ops->logs + ops->n_logs);
-    b->h_text_off.resize(b->n_logs); b->h_span_off.resize(b->n_logs);
-    uint64_t to = 0, so = 0, ncomment_bound = 0;
-    uint32_t n_packed = 0, n_compact = 0, n_team = 0, n_spill = 0;
-    std::vector<uint8_t> is_team(ops->n_logs, 0);
-    std::vector<uint32_t> bins[kNumBins];
-    for (int k = 0; k < kNumBins; k++) b->bin_slab[k] = 0;
-    for (uint32_t i = 0; i < b->n_logs; i++) {
-        const pt_log_desc& L = b->h_desc[i];
-        if (L.insdel_off + L.n_insdel > b->n_insdel || L.mark_off + L.n_mark > b->n_mark) { g_last_error = "log descriptor out of range"; return PT_ERR_INVALID; }
-        b->h_text_off[i] = to; b->h_span_off[i] = so;
-        to += L.n_insdel;
-        so += std::min<uint64_t>(L.n_insdel, 2ull * L.n_mark + 1);
-        ncomment_bound += L.n_mark;
-        uint64_t recs = (uint64_t)L.n_insdel + L.n_mark;
-        uint64_t KS = (uint64_t)L.max_ctr * (L.n_actors ? L.n_actors : 1);
-        int bin = 1; while (recs > kBins[bin].max_recs) bin++;
-        // typical shared-memory need (runs ~ n/6, segments ~ min(2m, n/2)); a wrong guess only costs a device-side deferral
-        {
-            const uint64_t I = (L.n_insdel < 32000 && L.n_mark < 32000) ? 2 : 4, n_ = L.n_insdel, m_ = L.n_mark;
-            // id table + bitmaps / run offsets (~1.4 B per record) + the larger of the run-tree temporaries (~5 B per record
-            // for typing-heavy logs) and the mark tables (per-op arrays + ~18 B per elementary segment)
-            const uint64_t seg = std::min<uint64_t>(2 * m_ + 2, n_ / 2 + 2);
-            const uint64_t typical = KS * I + (14 * n_) / 10 + std::max<uint64_t>(5 * n_, m_ ? m_ * (6 * I + 13) + 18 * seg : 0) + 2048;
-            while (bin < kNumBins - 1 && typical > kBins[bin].smem) bin++;
-        }
-        // short logs: one warp per log (16-bit keys and indices).  Footprint estimate: id table (compact form with >= 3
-        // actors: one slot per counter + overflow) + bitmaps + run-tree temporaries for ~ n/3 runs; a low guess only costs
-        // a device-side deferral
-        if (g_warp_bin && !(b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && recs <= kBins[0].max_recs && KS < 0xFFFFull) {
-            const uint64_t R_ = L.n_actors ? L.n_actors : 1, n_ = L.n_insdel;
-            const bool packed3 = R_ == 3 && n_ <= 1022;
-            const uint64_t idbytes = packed3 ? 4ull * L.max_ctr : (R_ >= 3 && R_ <= 30 && n_ <= 2046) ? 2ull * L.max_ctr + 512 : 2 * KS;
-            // packed3 (three concurrent replicas): per-word state 16 B per 32 records, ~14 B per run for ~ n/4 runs, key bitmap + prefix
-            const uint64_t rest = packed3 ? n_ / 2 + 32 + 14 * (n_ / 4) + (KS / 32 + 2) * 6 + 512 : n_ / 2 + 16 * n_ / 3 + 1024;
-            if (g_warp_force || idbytes + rest <= kBins[0].smem) bin = 0;
-        }
-        if (bin == 0) {   // bin 0's warp launches: packed3 id table (3 actors) / compact (>= 3 actors) / direct
-            const uint64_t R_ = L.n_actors ? L.n_actors : 1;
-            if (R_ == 3 && L.n_insdel <= 1022) n_packed++;
-            else if (R_ >= 3 && R_ <= 30 && L.n_insdel <= 2046) n_compact++;
-        } else if (g_team_bin && !(b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && L.n_mark == 0 && KS < 0xFFFFull && L.n_insdel < 0xFFFFu &&
-                   (3ull * L.n_insdel) / 4 + 2 * KS + 2ull * L.n_insdel + 1024 <= kTeamSmem) {
-            // medium logs without mark ops: a team of 8 warps per log, 4 logs per SM (team_kernel.cuh); rides in bin 0's list
-            bin = 0; is_team[i] = 1; n_team++;
-        }
-        bins[bin].push_back(i);
-        if (KS > 0x7FFFFFFFull) { g_last_error = "max_ctr * n_actors too large; re-rank counters densely on the host"; return PT_ERR_INVALID; }
-        {   // only a log whose worst-case working set exceeds the largest shared-memory budget can ever spill to the global slab
-            const size_t worst = arena_worst_bytes(L.n_insdel, L.n_mark, KS);
-            if (worst > kBins[kNumBins - 1].smem) { b->bin_slab[kNumBins - 1] = std::max(b->bin_slab[kNumBins - 1], worst); n_spill++; }
-        }
-    }
-    b->n_text = to; b->n_span = so;
-    // default pool: 4 entries per mark op (+slack) fits the generated workloads (c3, the densest, needs < 2); a batch that needs
-    // more reports its exact demand and merges again (BatchEngine.run), so the pool need not be sized for the worst case
-    b->pool_cap = b->limits.comment_pool_entries ? b->limits.comment_pool_entries : 4ull * ncomment_bound + 1024;
-    b->h_order.clear();
-    for (int k = 0; k < kNumBins; k++) {
-        b->bin_first[k] = (uint32_t)b->h_order.size();
-        auto& v = bins[k];
-        // bin 0's list: [warp kernel, packed3 id table | compact id table | direct id table | team kernel]
-        auto cat = [&](uint32_t x) { if (is_team[x]) return 3; const pt_log_desc& D = b->h_desc[x]; const uint32_t R_ = D.n_actors ? D.n_actors : 1;
-                                     return (R_ == 3 && D.n_insdel <= 1022) ? 0 : (R_ >= 3 && R_ <= 30 && D.n_insdel <= 2046) ? 1 : 2; };
-        std::stable_sort(v.begin(), v.end(), [&](uint32_t x, uint32_t y) {
-            if (k == 0) { const int cx = cat(x), cy = cat(y); if (cx != cy) return cx < cy; }
-            return (uint64_t)b->h_desc[x].n_insdel + b->h_desc[x].n_mark > (uint64_t)b->h_desc[y].n_insdel + b->h_desc[y].n_mark; });
-        b->h_order.insert(b->h_order.end(), v.begin(), v.end());
-    }
-    b->bin_first[kNumBins] = (uint32_t)b->h_order.size();
-    b->warp_packed = n_packed; b->warp_compact = n_compact; b->team_count = n_team; b->n_spill = n_spill;
-    return PT_OK;
+// The launch sequence, or a pointer or capacity baked into it, changed: capture it again at the next repeated merge.
+void drop_graph(pt_batch* b) {
+    if (b->graph_exec) cudaGraphExecDestroy(b->graph_exec);
+    b->graph_exec = nullptr; b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0;
 }
 
 int alloc_and_upload_plan(pt_batch* b) {
     int rc;
     const size_t n = b->n_logs;
+    const ptp::Plan& pl = b->plan;
     if ((rc = b->d_desc.reserve(std::max<size_t>(1, n) * sizeof(pt_log_desc)))) return rc;
     if ((rc = b->d_order.reserve(std::max<size_t>(1, n) * 4))) return rc;
-    if ((rc = b->d_counters.reserve(256))) return rc;   // [0,64) stats | [64,72) pool cursor | [128,176) work/deferral counters
+    if ((rc = b->d_counters.reserve(sizeof(DevCounters)))) return rc;
     if ((rc = b->d_results.reserve(std::max<size_t>(1, n) * sizeof(pt_log_result)))) return rc;
     if ((rc = b->d_text_off.reserve(std::max<size_t>(1, n) * 8))) return rc;
     if ((rc = b->d_span_off.reserve(std::max<size_t>(1, n) * 8))) return rc;
-    if ((rc = b->d_text.reserve(std::max<uint64_t>(1, b->n_text) * 4))) return rc;
-    if ((b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && (rc = b->d_seq.reserve(std::max<uint64_t>(1, b->n_text) * 4))) return rc;
-    if ((rc = b->d_spans.reserve(std::max<uint64_t>(1, b->n_span) * sizeof(pt_span)))) return rc;
-    if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, b->pool_cap) * 4))) return rc;
+    if ((rc = b->d_text.reserve(std::max<uint64_t>(1, pl.n_text) * 4))) return rc;
+    if ((b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && (rc = b->d_seq.reserve(std::max<uint64_t>(1, pl.n_text) * 4))) return rc;
+    if ((rc = b->d_spans.reserve(std::max<uint64_t>(1, pl.n_span) * sizeof(pt_span)))) return rc;
+    if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, pl.pool_cap) * 4))) return rc;
     if ((rc = b->d_retry.reserve(std::max<size_t>(1, n) * 4 * kNumBins + 16))) return rc;
     if (b->limits.flags & PT_FLAG_EMIT_PATCHES) {
         b->patch_cap = b->limits.patch_pool_items ? b->limits.patch_pool_items : 4ull * (b->n_insdel + b->n_mark) + 1024;
         if ((rc = b->d_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
         if ((rc = b->d_patch_items.reserve(std::max<uint64_t>(1, b->patch_cap) * sizeof(pt_patch_item)))) return rc;
         if ((rc = b->d_patch_status.reserve(std::max<size_t>(1, n) * 4))) return rc;
-        // one warp per CTA; shared memory = the largest footprint among the logs, capped (larger logs are left to the host)
-        uint64_t need_max = 4096;
-        for (uint32_t i = 0; i < b->n_logs; i++) {
-            const pt_log_desc& L = b->h_desc[i];
-            const uint64_t KS = (uint64_t)L.max_ctr * (L.n_actors ? L.n_actors : 1);
-            const uint64_t need = ((KS * 2 + 15) & ~15ull) + 3 * (((uint64_t)L.n_insdel * 2 + 15) & ~15ull) / 1 + (((uint64_t)L.n_insdel * 4 + 15) & ~15ull) +
-                                  6 * (((uint64_t)L.n_mark * 4 + 15) & ~15ull) + (((uint64_t)L.n_mark * 2 + 15) & ~15ull) + 256;
-            if (need <= 200 * 1024) need_max = std::max(need_max, need);
-        }
-        b->patch_smem = (uint32_t)((need_max + 1023) & ~1023ull);
     }
-    // spill slab: one slot per CTA that can ever spill = min(logs that can spill, CTAs of the last bin); a batch with one huge
-    // log no longer multiplies its worst case by the whole grid
-    const size_t slab_max = b->bin_slab[kNumBins - 1];
-    b->slab_slots = (uint32_t)std::min<size_t>(b->n_spill, (size_t)b->num_sms * kBins[kNumBins - 1].ctas_per_sm);
-    const size_t slab_total = (size_t)b->slab_slots * slab_max;
-    b->retry_slab = slab_max;
-    if ((rc = b->d_slab.reserve(std::max<size_t>(slab_total, 16)))) return rc;
+    if ((rc = b->d_slab.reserve(std::max<size_t>((size_t)pl.slab_slots * pl.slab_bytes, 16)))) return rc;
     // stage the small host-derived arrays through pinned memory
     size_t stage = n * (sizeof(pt_log_desc) + 4 + 8 + 8) + 64;
     if ((rc = b->h_stage.reserve(stage))) return rc;
@@ -652,37 +482,36 @@ int alloc_and_upload_plan(pt_batch* b) {
     if (n) {
         memcpy(s, b->h_desc.data(), n * sizeof(pt_log_desc));
         PT_CUDA(cudaMemcpyAsync(b->d_desc.p, s, n * sizeof(pt_log_desc), cudaMemcpyHostToDevice, b->stream)); s += n * sizeof(pt_log_desc);
-        memcpy(s, b->h_order.data(), n * 4);
+        memcpy(s, pl.order.data(), n * 4);
         PT_CUDA(cudaMemcpyAsync(b->d_order.p, s, n * 4, cudaMemcpyHostToDevice, b->stream)); s += n * 4;
-        memcpy(s, b->h_text_off.data(), n * 8);
+        memcpy(s, pl.text_off.data(), n * 8);
         PT_CUDA(cudaMemcpyAsync(b->d_text_off.p, s, n * 8, cudaMemcpyHostToDevice, b->stream)); s += n * 8;
-        memcpy(s, b->h_span_off.data(), n * 8);
+        memcpy(s, pl.span_off.data(), n * 8);
         PT_CUDA(cudaMemcpyAsync(b->d_span_off.p, s, n * 8, cudaMemcpyHostToDevice, b->stream)); s += n * 8;
     }
     return PT_OK;
 }
 
-// counters: [0,kNumBins) work-queue heads of the bins' own lists, [kNumBins, 2k) heads of the retry launches,
-// [2k, 3k) number of logs deferred INTO bin k (list k of d_retry)
+// Bin k's own list (retry = false), or the logs deferred into it (retry = true: list k of d_retry, its length on the device).
 template <int BLOCK>
 int launch_bin_t(pt_batch* b, int k, ptk::BatchParams P, bool retry) {
-    const BinCfg& cfg = kBins[k];
-    uint32_t cnt = retry ? b->n_logs : b->bin_first[k + 1] - b->bin_first[k];
+    const ptp::BinCfg& cfg = kCtaBins[k];
+    uint32_t cnt = retry ? b->n_logs : b->plan.bin_first[k + 1] - b->plan.bin_first[k];
     uint32_t grid = (uint32_t)std::min<size_t>(cnt, (size_t)b->num_sms * cfg.ctas_per_sm);
-    uint32_t* counters = (uint32_t*)((char*)b->d_counters.p + 128);
+    DevCounters* c = counters(b);
     uint32_t* lists = (uint32_t*)b->d_retry.p;
     if (retry) {
-        P.order = lists + (size_t)k * b->n_logs; P.n_work = 0; P.n_work_dev = counters + 2 * kNumBins + k;
-        P.work_counter = counters + kNumBins + k;
+        P.order = lists + (size_t)k * b->n_logs; P.n_work = 0; P.n_work_dev = &c->deferred[k];
+        P.work_counter = &c->retry_head[k];
     } else {
-        P.order = (const uint32_t*)b->d_order.p + b->bin_first[k]; P.n_work = cnt; P.n_work_dev = nullptr;
-        P.work_counter = counters + k;
+        P.order = (const uint32_t*)b->d_order.p + b->plan.bin_first[k]; P.n_work = cnt; P.n_work_dev = nullptr;
+        P.work_counter = &c->head[k];
     }
     const bool last = k == kNumBins - 1;
-    P.slab_bytes = last ? b->retry_slab : 0;
-    if (retry) P.slab_counter += 1;      // the two launches of the last bin run one after the other: each counts its slots from zero
+    P.slab_bytes = last ? b->plan.slab_bytes : 0;
+    P.slab_counter = &c->slab[retry ? 1 : 0];   // the two launches of the last bin run one after the other: each counts its slots from zero
     P.retry_list = last ? nullptr : lists + (size_t)(k + 1) * b->n_logs;
-    P.retry_count = last ? nullptr : counters + 2 * kNumBins + (k + 1);
+    P.retry_count = last ? nullptr : &c->deferred[k + 1];
     P.smem_arena_bytes = cfg.smem;
     PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_kernel<BLOCK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem));
     ptk::merge_logs_kernel<BLOCK><<<grid, BLOCK, cfg.smem, b->launch_stream>>>(P);
@@ -690,19 +519,18 @@ int launch_bin_t(pt_batch* b, int k, ptk::BatchParams P, bool retry) {
     b->launches++;
     return PT_OK;
 }
+// cnt logs of bin 0's list from position first, on one id-table form of the warp kernel
 template <int WARPS, int IDM>
-int launch_warp_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t cnt, uint32_t counter_slot) {
+int launch_warp_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t cnt, uint32_t* head) {
     if (!cnt) return PT_OK;
-    const BinCfg& cfg = kBins[0];
+    const ptp::BinCfg& cfg = b->plan.cfg.warp;
     const uint32_t per_cta = WARPS * ptk::kWarpGrab;
     const uint32_t grid = (uint32_t)std::min<size_t>((cnt + per_cta - 1) / per_cta, (size_t)b->num_sms * cfg.ctas_per_sm);
-    uint32_t* counters = (uint32_t*)((char*)b->d_counters.p + 128);
-    uint32_t* lists = (uint32_t*)b->d_retry.p;
-    P.order = (const uint32_t*)b->d_order.p + b->bin_first[0] + first; P.n_work = cnt; P.n_work_dev = nullptr;
-    P.work_counter = counters + counter_slot;
+    P.order = (const uint32_t*)b->d_order.p + b->plan.bin_first[0] + first; P.n_work = cnt; P.n_work_dev = nullptr;
+    P.work_counter = head;
     P.slab_bytes = 0;
-    P.retry_list = lists + (size_t)1 * b->n_logs;        // deferrals go to the first CTA-per-log bin
-    P.retry_count = counters + 2 * kNumBins + 1;
+    P.retry_list = (uint32_t*)b->d_retry.p + (size_t)1 * b->n_logs;   // deferrals go to the first CTA-per-log bin
+    P.retry_count = &counters(b)->deferred[1];
     P.smem_arena_bytes = cfg.smem;                       // per warp
     const int smem = (int)(cfg.smem * WARPS);
     PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_warp_kernel<WARPS, IDM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -714,50 +542,103 @@ int launch_warp_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t 
 int launch_team_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t cnt) {
     if (!cnt) return PT_OK;
     const uint32_t grid = (uint32_t)std::min<size_t>(cnt, (size_t)b->num_sms * 4);
-    uint32_t* counters = (uint32_t*)((char*)b->d_counters.p + 128);
-    uint32_t* lists = (uint32_t*)b->d_retry.p;
-    P.order = (const uint32_t*)b->d_order.p + b->bin_first[0] + first; P.n_work = cnt; P.n_work_dev = nullptr;
-    P.work_counter = counters + 3 * kNumBins + 1;
+    P.order = (const uint32_t*)b->d_order.p + b->plan.bin_first[0] + first; P.n_work = cnt; P.n_work_dev = nullptr;
+    P.work_counter = &counters(b)->team;
     P.slab_bytes = 0;
-    P.retry_list = lists + (size_t)3 * b->n_logs;        // a log that does not fit goes to the 512-thread CTA bin (and on from there)
-    P.retry_count = counters + 2 * kNumBins + 3;
-    P.smem_arena_bytes = kTeamSmem;
-    PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_team_kernel<kTeamWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTeamSmem));
-    ptk::merge_logs_team_kernel<kTeamWarps><<<grid, kTeamWarps * 32, kTeamSmem, b->launch_stream>>>(P);
+    P.retry_list = (uint32_t*)b->d_retry.p + (size_t)3 * b->n_logs;   // a log that does not fit goes to the 512-thread CTA bin (and on from there)
+    P.retry_count = &counters(b)->deferred[3];
+    P.smem_arena_bytes = ptp::kTeamSmem;
+    PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_team_kernel<ptp::kTeamWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ptp::kTeamSmem));
+    ptk::merge_logs_team_kernel<ptp::kTeamWarps><<<grid, ptp::kTeamWarps * 32, ptp::kTeamSmem, b->launch_stream>>>(P);
     PT_CUDA(cudaGetLastError());
     b->launches++;
     return PT_OK;
 }
+// bin 0's list, in route order: the warp kernel with the packed3, compact and direct id tables, then the team kernel
 template <int WARPS>
 int launch_warp_bin_t(pt_batch* b, const ptk::BatchParams& P) {
-    const uint32_t cnt = b->bin_first[1] - b->bin_first[0] - b->team_count;
-    const uint32_t np = b->warp_packed, nc = b->warp_compact;
-    int rc = launch_warp_range<WARPS, ptk::kIdPacked3>(b, P, 0, np, 3 * kNumBins + 2);
-    if (rc) return rc;
-    if ((rc = launch_warp_range<WARPS, ptk::kIdCompact>(b, P, np, nc, 0))) return rc;
-    if ((rc = launch_warp_range<WARPS, ptk::kIdDirect>(b, P, np + nc, cnt - np - nc, 3 * kNumBins))) return rc;
-    return launch_team_range(b, P, cnt, b->team_count);
+    const uint32_t np = b->plan.n_route[ptp::kPacked3], nc = b->plan.n_route[ptp::kCompact], nd = b->plan.n_route[ptp::kDirect];
+    DevCounters* c = counters(b);
+    int rc;
+    if ((rc = launch_warp_range<WARPS, ptk::kIdPacked3>(b, P, 0, np, &c->packed3))) return rc;
+    if ((rc = launch_warp_range<WARPS, ptk::kIdCompact>(b, P, np, nc, &c->compact))) return rc;
+    if ((rc = launch_warp_range<WARPS, ptk::kIdDirect>(b, P, np + nc, nd, &c->direct))) return rc;
+    return launch_team_range(b, P, np + nc + nd, b->plan.n_route[ptp::kTeam]);
 }
 int launch_bin(pt_batch* b, int k, const ptk::BatchParams& P, bool retry) {
-    if (!retry && b->bin_first[k + 1] == b->bin_first[k]) return PT_OK;
+    if (!retry && b->plan.bin_first[k + 1] == b->plan.bin_first[k]) return PT_OK;
     if (k == 0) {
-        switch (kBins[0].block / 32) {
+        switch (b->plan.cfg.warp.block / 32) {      // RouteConfig accepts 2, 4 or 8 warps per CTA
             case 2: return launch_warp_bin_t<2>(b, P);
             case 4: return launch_warp_bin_t<4>(b, P);
-            case 6: return launch_warp_bin_t<6>(b, P);
-            case 8: return launch_warp_bin_t<8>(b, P);
-            case 12: return launch_warp_bin_t<12>(b, P);
-            default: return launch_warp_bin_t<16>(b, P);
+            default: return launch_warp_bin_t<8>(b, P);
         }
     }
-    switch (kBins[k].block) {
-        case 32: return launch_bin_t<32>(b, k, P, retry);
-        case 64: return launch_bin_t<64>(b, k, P, retry);
-        case 128: return launch_bin_t<128>(b, k, P, retry);
-        case 256: return launch_bin_t<256>(b, k, P, retry);
-        case 512: return launch_bin_t<512>(b, k, P, retry);
-        default: return launch_bin_t<1024>(b, k, P, retry);
+    switch (k) {
+        case 1: return launch_bin_t<kCtaBins[1].block>(b, k, P, retry);
+        case 2: return launch_bin_t<kCtaBins[2].block>(b, k, P, retry);
+        case 3: return launch_bin_t<kCtaBins[3].block>(b, k, P, retry);
+        default: return launch_bin_t<kCtaBins[4].block>(b, k, P, retry);
     }
+}
+
+// Shared start of every upload: the staging buffer and the device arrays of the previous batch are reused, so wait for
+// it; then plan the new batch and allocate for it (own_records: the engine keeps its own copy of the records).
+int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    b->have_batch = false; b->merged = false; b->dl_begun = false; b->have_changes = false;
+    drop_graph(b);
+    b->n_logs = ops.n_logs; b->n_insdel = ops.n_insdel_total; b->n_mark = ops.n_mark_total;
+    b->h_desc.assign(ops.logs, ops.logs + ops.n_logs);
+    if (const char* err = ptp::make_plan(ops, b->limits, b->num_sms, b->plan)) { g_last_error = err; return PT_ERR_INVALID; }
+    int rc;
+    if ((rc = alloc_and_upload_plan(b))) return rc;
+    if (own_records) {
+        if ((rc = b->d_insdel.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_rec)))) return rc;
+        if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
+    }
+    return PT_OK;
+}
+
+// Shared finish: the records the merge reads, and a wait for the copies when one of the caller's sources (pointer, bytes
+// read) is pageable, because such a buffer may be freed on return (pinned ones stay asynchronous).
+int finish_upload(pt_batch* b, const void* insdel, const void* marks, std::initializer_list<std::pair<const void*, uint64_t>> sources) {
+    bool pageable = false;
+    for (const auto& s : sources) {
+        if (!s.second) continue;
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, s.first) != cudaSuccess) { cudaGetLastError(); pageable = true; }
+        else if (a.type != cudaMemoryTypeHost) pageable = true;
+    }
+    if (pageable) PT_CUDA(cudaStreamSynchronize(b->stream));
+    b->dp_insdel = (const pt_insdel_rec*)insdel; b->dp_marks = (const pt_mark_rec*)marks;
+    b->have_batch = true;
+    return PT_OK;
+}
+
+// pt_batch_query_elements / pt_batch_find_elements: n queries up, one warp per query, n answers back.
+template <class Q, class A, class Launch>
+int run_queries(pt_batch* b, const char* fn, const char* verb, const Q* queries, uint32_t n, A* out, Launch launch) {
+    if (!b || (n && (!queries || !out))) return PT_ERR_INVALID;
+    if (!b->merged) { g_last_error = std::string(verb) + " before merge"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
+    if (!n) return PT_OK;
+    PT_CUDA(cudaSetDevice(b->device));
+    DevBuf dq, da;
+    int rc;
+    if ((rc = dq.reserve((size_t)n * sizeof(Q))) || (rc = da.reserve((size_t)n * sizeof(A)))) return rc;
+    cudaError_t e = cudaMemcpyAsync(dq.p, queries, (size_t)n * sizeof(Q), cudaMemcpyHostToDevice, b->stream);
+    if (e == cudaSuccess) {
+        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+        launch(grid, threads, (const Q*)dq.p, (A*)da.p);
+        e = cudaGetLastError();
+        b->launches++;
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * sizeof(A), cudaMemcpyDeviceToHost, b->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
+    if (e != cudaSuccess) { g_last_error = std::string(fn) + ": " + cudaGetErrorString(e); return PT_ERR_CUDA; }
+    return PT_OK;
 }
 
 }  // namespace
@@ -791,53 +672,21 @@ int pt_batch_create(int device, const pt_limits* limits, void* cuda_stream, pt_b
     return PT_OK;
 }
 
-static int upload_common(pt_batch* b, const pt_packed_ops* ops, bool adopt) {
+int pt_batch_upload(pt_batch* b, const pt_packed_ops* ops) {
     if (!b || !ops || (ops->n_logs && !ops->logs)) return PT_ERR_INVALID;
-    PT_CUDA(cudaSetDevice(b->device));
-    PT_CUDA(cudaStreamSynchronize(b->stream));            // the staging buffer and the device arrays of the previous batch are reused
-    b->have_batch = false; b->merged = false;
-    if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }
-    b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0; b->dl_begun = false; b->have_changes = false;
-    int rc = plan_batch(b, ops);
+    int rc = begin_upload(b, *ops, true);
     if (rc) return rc;
-    if ((rc = alloc_and_upload_plan(b))) return rc;
-    if (adopt) {
-        b->dp_insdel = ops->insdel; b->dp_marks = ops->marks; b->adopted = true;
-    } else {
-        if ((rc = b->d_insdel.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_rec)))) return rc;
-        if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
-        if (b->n_insdel) PT_CUDA(cudaMemcpyAsync(b->d_insdel.p, ops->insdel, b->n_insdel * sizeof(pt_insdel_rec), cudaMemcpyHostToDevice, b->stream));
-        if (b->n_mark) PT_CUDA(cudaMemcpyAsync(b->d_marks.p, ops->marks, b->n_mark * sizeof(pt_mark_rec), cudaMemcpyHostToDevice, b->stream));
-        b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p; b->adopted = false;
-        // pageable caller buffers may be freed on return: finish the copies now (pinned ones stay asynchronous)
-        auto pinned = [](const void* p) {
-            cudaPointerAttributes a;
-            if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-            return a.type == cudaMemoryTypeHost;
-        };
-        if (!((b->n_insdel == 0 || pinned(ops->insdel)) && (b->n_mark == 0 || pinned(ops->marks)))) PT_CUDA(cudaStreamSynchronize(b->stream));
-    }
-    b->have_batch = true;
-    return PT_OK;
+    if (b->n_insdel) PT_CUDA(cudaMemcpyAsync(b->d_insdel.p, ops->insdel, b->n_insdel * sizeof(pt_insdel_rec), cudaMemcpyHostToDevice, b->stream));
+    if (b->n_mark) PT_CUDA(cudaMemcpyAsync(b->d_marks.p, ops->marks, b->n_mark * sizeof(pt_mark_rec), cudaMemcpyHostToDevice, b->stream));
+    return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{ops->insdel, b->n_insdel}, {ops->marks, b->n_mark}});
 }
-
-int pt_batch_upload(pt_batch* b, const pt_packed_ops* ops) { return upload_common(b, ops, false); }
 
 int pt_batch_upload_runs(pt_batch* b, const pt_packed_runs* rr) {
     if (!b || !rr || (rr->n_logs && (!rr->logs || !rr->run_off || !rr->tok_off))) return PT_ERR_INVALID;
-    PT_CUDA(cudaSetDevice(b->device));
-    PT_CUDA(cudaStreamSynchronize(b->stream));            // the staging buffer and the device arrays of the previous batch are reused
-    b->have_batch = false; b->merged = false;
-    if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }
-    b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0; b->dl_begun = false; b->have_changes = false;
-    pt_packed_ops ops{rr->n_logs, rr->logs, nullptr, rr->n_insdel_total, nullptr, rr->n_mark_total};
-    int rc = plan_batch(b, &ops);
+    int rc = begin_upload(b, pt_packed_ops{rr->n_logs, rr->logs, nullptr, rr->n_insdel_total, nullptr, rr->n_mark_total}, true);
     if (rc) return rc;
-    if ((rc = alloc_and_upload_plan(b))) return rc;
     const size_t nl = rr->n_logs;
     const uint64_t n_runs = nl ? rr->run_off[nl] : 0, n_tok = nl ? rr->tok_off[nl] : 0;
-    if ((rc = b->d_insdel.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_rec)))) return rc;
-    if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
     if ((rc = b->d_runs.reserve(std::max<uint64_t>(1, n_runs) * sizeof(pt_run_rec)))) return rc;
     if ((rc = b->d_tokens.reserve(std::max<uint64_t>(1, n_tok) * 4))) return rc;
     if ((rc = b->d_run_off.reserve((nl + 1) * 8))) return rc;
@@ -858,16 +707,7 @@ int pt_batch_upload_runs(pt_batch* b, const pt_packed_runs* rr) {
         PT_CUDA(cudaGetLastError());
         b->launches++;
     }
-    b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p; b->adopted = false;
-    auto pinned = [](const void* p) {
-        cudaPointerAttributes a;
-        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-        return a.type == cudaMemoryTypeHost;
-    };
-    if (!((n_runs == 0 || pinned(rr->runs)) && (n_tok == 0 || pinned(rr->tokens)) && (b->n_mark == 0 || pinned(rr->marks)) && (nl == 0 || (pinned(rr->run_off) && pinned(rr->tok_off)))))
-        PT_CUDA(cudaStreamSynchronize(b->stream));
-    b->have_batch = true;
-    return PT_OK;
+    return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{rr->runs, n_runs}, {rr->tokens, n_tok}, {rr->marks, b->n_mark}, {rr->run_off, nl}, {rr->tok_off, nl}});
 }
 
 int pt_compress_runs(const pt_packed_ops* ops, uint64_t* run_off, uint64_t* tok_off, pt_run_rec* runs, uint32_t* tokens,
@@ -900,7 +740,12 @@ int pt_compress_runs(const pt_packed_ops* ops, uint64_t* run_off, uint64_t* tok_
     if (n_tokens_out) *n_tokens_out = nt;
     return PT_OK;
 }
-int pt_batch_adopt_device(pt_batch* b, const pt_packed_ops* ops) { return upload_common(b, ops, true); }
+int pt_batch_adopt_device(pt_batch* b, const pt_packed_ops* ops) {
+    if (!b || !ops || (ops->n_logs && !ops->logs)) return PT_ERR_INVALID;
+    int rc = begin_upload(b, *ops, false);
+    if (rc) return rc;
+    return finish_upload(b, ops->insdel, ops->marks, {});
+}
 
 int pt_compact_ops(const pt_packed_ops* ops, pt_insdel_c8* io, pt_mark_c16* mo, int threads) {
     if (!ops || (ops->n_insdel_total && !io) || (ops->n_mark_total && !mo)) return PT_ERR_INVALID;
@@ -939,17 +784,8 @@ int pt_compact_ops(const pt_packed_ops* ops, pt_insdel_c8* io, pt_mark_c16* mo, 
 
 int pt_batch_upload_compact(pt_batch* b, const pt_packed_compact* cc) {
     if (!b || !cc || (cc->n_logs && !cc->logs)) return PT_ERR_INVALID;
-    PT_CUDA(cudaSetDevice(b->device));
-    PT_CUDA(cudaStreamSynchronize(b->stream));
-    b->have_batch = false; b->merged = false;
-    if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }
-    b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0; b->dl_begun = false; b->have_changes = false;
-    pt_packed_ops ops{cc->n_logs, cc->logs, nullptr, cc->n_insdel_total, nullptr, cc->n_mark_total};
-    int rc = plan_batch(b, &ops);
+    int rc = begin_upload(b, pt_packed_ops{cc->n_logs, cc->logs, nullptr, cc->n_insdel_total, nullptr, cc->n_mark_total}, true);
     if (rc) return rc;
-    if ((rc = alloc_and_upload_plan(b))) return rc;
-    if ((rc = b->d_insdel.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_rec)))) return rc;
-    if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
     if ((rc = b->d_cins.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_c8)))) return rc;
     if ((rc = b->d_cmarks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_c16)))) return rc;
     const uint32_t threads = 256, gmax = (uint32_t)b->num_sms * 16;
@@ -966,15 +802,7 @@ int pt_batch_upload_compact(pt_batch* b, const pt_packed_compact* cc) {
         b->launches++;
     }
     PT_CUDA(cudaGetLastError());
-    b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p; b->adopted = false;
-    auto pinned = [](const void* p) {
-        cudaPointerAttributes a;
-        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-        return a.type == cudaMemoryTypeHost;
-    };
-    if (!((b->n_insdel == 0 || pinned(cc->insdel)) && (b->n_mark == 0 || pinned(cc->marks)))) PT_CUDA(cudaStreamSynchronize(b->stream));
-    b->have_batch = true;
-    return PT_OK;
+    return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{cc->insdel, b->n_insdel}, {cc->marks, b->n_mark}});
 }
 
 int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
@@ -1001,24 +829,24 @@ int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
     if (t->n_deps_total) PT_CUDA(cudaMemcpyAsync(b->d_deps.p, t->deps, t->n_deps_total * sizeof(pt_dep_rec), cudaMemcpyHostToDevice, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));            // the caller's arrays may be freed on return
     b->adm_maxR = maxR; b->have_changes = true;
-    if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }   // the launch sequence changes
-    b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0;
+    drop_graph(b);                                       // the launch sequence changes
     return PT_OK;
 }
 
 static int enqueue_merge(pt_batch* b) {
-    PT_CUDA(cudaMemsetAsync(b->d_counters.p, 0, 256, b->stream));   // stats, pool cursor and queue counters in one shot
+    DevCounters* c = counters(b);
+    PT_CUDA(cudaMemsetAsync(c, 0, sizeof(DevCounters), b->stream));   // stats, cursors and queue heads in one shot
     ptk::BatchParams P{};
     P.desc = (const pt_log_desc*)b->d_desc.p;
     P.insdel = b->dp_insdel; P.marks = b->dp_marks;
     P.results = (pt_log_result*)b->d_results.p;
     P.text_off = (const uint64_t*)b->d_text_off.p; P.span_off = (const uint64_t*)b->d_span_off.p;
     P.text = (uint32_t*)b->d_text.p; P.spans = (pt_span*)b->d_spans.p;
-    P.comment_pool = (uint32_t*)b->d_pool.p; P.comment_used = (unsigned long long*)((char*)b->d_counters.p + 64); P.comment_cap = b->pool_cap;
+    P.comment_pool = (uint32_t*)b->d_pool.p; P.comment_used = &c->comment_used; P.comment_cap = b->plan.pool_cap;
     P.slab = (char*)b->d_slab.p;
-    P.slab_counter = (uint32_t*)((char*)b->d_counters.p + 96); P.slab_slots = b->slab_slots;
+    P.slab_counter = c->slab; P.slab_slots = b->plan.slab_slots;
     P.seq = (b->limits.flags & PT_FLAG_EMIT_SEQUENCE) ? (uint32_t*)b->d_seq.p : nullptr;
-    P.stats = (unsigned long long*)b->d_counters.p;
+    P.stats = c->stats;
     P.admit = nullptr;
     if (b->have_changes && b->n_logs) {
         // admission pre-pass: 4 warps per CTA while the per-actor tables fit, else one warp with up to 200 KB
@@ -1042,7 +870,8 @@ static int enqueue_merge(pt_batch* b) {
     // The CTA-per-log bins' own lists do not depend on the warp / team kernels: when both exist they are launched on a side
     // stream (fork / join, also inside the captured graph) and fill the SMs the warp kernel's tail leaves idle.  The deferral
     // launches come after the join, in ascending bin order.
-    const bool have0 = b->bin_first[1] > b->bin_first[0], haveBlocks = b->bin_first[kNumBins] > b->bin_first[1];
+    const uint32_t* bin_first = b->plan.bin_first;
+    const bool have0 = bin_first[1] > bin_first[0], haveBlocks = bin_first[kNumBins] > bin_first[1];
     const bool fork = have0 && haveBlocks && b->side != nullptr;
     if (fork) {
         PT_CUDA(cudaEventRecord(b->ev_fork, b->stream));
@@ -1061,20 +890,20 @@ static int enqueue_merge(pt_batch* b) {
         for (int k = 0; k < kNumBins; k++) {
             if ((rc = launch_bin(b, k, P, false))) return rc;
             if (k > 0 && lower && (rc = launch_bin(b, k, P, true))) return rc;
-            lower = lower || b->bin_first[k + 1] > b->bin_first[k];
+            lower = lower || bin_first[k + 1] > bin_first[k];
         }
     }
     if ((b->limits.flags & PT_FLAG_EMIT_PATCHES) && b->n_logs) {
         ptk::PatchParams Q{};
         Q.desc = P.desc; Q.insdel = P.insdel; Q.marks = P.marks; Q.results = P.results; Q.text_off = P.text_off; Q.seq = P.seq;
-        Q.n_logs = b->n_logs; Q.smem_bytes = b->patch_smem;
+        Q.n_logs = b->n_logs; Q.smem_bytes = b->plan.patch_smem;
         Q.recs = (pt_patch_rec*)b->d_patch_recs.p; Q.items = (pt_patch_item*)b->d_patch_items.p;
-        Q.item_cursor = (unsigned long long*)((char*)b->d_counters.p + 80); Q.item_cap = b->patch_cap;
+        Q.item_cursor = &c->patch_items; Q.item_cap = b->patch_cap;
         Q.status = (uint32_t*)b->d_patch_status.p;
-        PT_CUDA(cudaFuncSetAttribute(ptk::patch_logs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->patch_smem));
-        const uint32_t per_sm = std::max<uint32_t>(1, std::min<uint32_t>(32, (227u * 1024u) / (b->patch_smem + 1024u)));
+        PT_CUDA(cudaFuncSetAttribute(ptk::patch_logs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->plan.patch_smem));
+        const uint32_t per_sm = std::max<uint32_t>(1, std::min<uint32_t>(32, (227u * 1024u) / (b->plan.patch_smem + 1024u)));
         const uint32_t grid = (uint32_t)std::min<uint64_t>(b->n_logs, (uint64_t)b->num_sms * per_sm);
-        ptk::patch_logs_kernel<<<grid, 32, b->patch_smem, b->stream>>>(Q);
+        ptk::patch_logs_kernel<<<grid, 32, b->plan.patch_smem, b->stream>>>(Q);
         PT_CUDA(cudaGetLastError());
         b->launches++;
     }
@@ -1089,8 +918,7 @@ int pt_batch_merge(pt_batch* b) {
     // stream, where the launches are simply enqueued directly).
     if (!b->graph_tried && b->merges_since_upload >= 1) {   // a batch merged more than once: replay its launch sequence as a graph
         b->graph_tried = true;
-        const char* eg = getenv("PT_GRAPH");
-        if (b->stream != nullptr && !(eg && atoi(eg) == 0)) {
+        if (b->stream != nullptr) {
             const uint64_t l0 = b->launches;
             if (cudaStreamBeginCapture(b->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
                 int rc = enqueue_merge(b);
@@ -1162,9 +990,9 @@ int pt_batch_download_begin(pt_batch* b) {
     if ((rc = b->d_ctoff.reserve((n + 1) * 8))) return rc;
     if ((rc = b->d_csoff.reserve((n + 1) * 8))) return rc;
     // packed outputs can never exceed the capacities; sized once per batch
-    if ((rc = b->d_ctext.reserve(std::max<uint64_t>(1, b->n_text) * 4))) return rc;
-    if ((rc = b->d_cspans.reserve(std::max<uint64_t>(1, b->n_span) * sizeof(pt_span)))) return rc;
-    PT_CUDA(cudaMemcpyAsync(b->h_misc.p, (char*)b->d_counters.p + 64, 8, cudaMemcpyDeviceToHost, b->stream));   // pool cursor = the batch's demand
+    if ((rc = b->d_ctext.reserve(std::max<uint64_t>(1, b->plan.n_text) * 4))) return rc;
+    if ((rc = b->d_cspans.reserve(std::max<uint64_t>(1, b->plan.n_span) * sizeof(pt_span)))) return rc;
+    PT_CUDA(cudaMemcpyAsync(b->h_misc.p, &counters(b)->comment_used, 8, cudaMemcpyDeviceToHost, b->stream));   // pool cursor = the batch's demand
     if (n) {
         const pt_log_result* res = (const pt_log_result*)b->d_results.p;
         unsigned long long* bsum = (unsigned long long*)b->d_bsum.p;
@@ -1184,8 +1012,8 @@ int pt_batch_download_begin(pt_batch* b) {
         ((uint64_t*)b->h_ctoff.p)[0] = 0; ((uint64_t*)b->h_csoff.p)[0] = 0;
     }
     if (b->limits.flags & PT_FLAG_EMIT_SEQUENCE) {
-        if ((rc = b->h_seq.reserve(std::max<uint64_t>(1, b->n_text) * 4))) return rc;
-        if (b->n_text) PT_CUDA(cudaMemcpyAsync(b->h_seq.p, b->d_seq.p, b->n_text * 4, cudaMemcpyDeviceToHost, b->stream));
+        if ((rc = b->h_seq.reserve(std::max<uint64_t>(1, b->plan.n_text) * 4))) return rc;
+        if (b->plan.n_text) PT_CUDA(cudaMemcpyAsync(b->h_seq.p, b->d_seq.p, b->plan.n_text * 4, cudaMemcpyDeviceToHost, b->stream));
     }
     b->dl_begun = true;
     return PT_OK;
@@ -1200,7 +1028,7 @@ int pt_batch_download(pt_batch* b, pt_spans_view* out) {
     const bool want_seq = (b->limits.flags & PT_FLAG_EMIT_SEQUENCE) != 0;
     const size_t n = b->n_logs;
     const uint64_t demand = *(unsigned long long*)b->h_misc.p;
-    const uint64_t used = std::min<uint64_t>(demand, b->pool_cap);
+    const uint64_t used = std::min<uint64_t>(demand, b->plan.pool_cap);
     const uint64_t n_ctext = ((const uint64_t*)b->h_ctoff.p)[n], n_cspan = ((const uint64_t*)b->h_csoff.p)[n];
     b->pool_used_host = used;
     if ((rc = b->h_pool.reserve(std::max<uint64_t>(1, used) * 4))) return rc;
@@ -1219,7 +1047,7 @@ int pt_batch_download(pt_batch* b, pt_spans_view* out) {
     out->comment_pool = (const uint32_t*)b->h_pool.p;
     out->comment_pool_used = used;
     out->seq = want_seq ? (const uint32_t*)b->h_seq.p : nullptr;
-    out->seq_off = want_seq ? b->h_text_off.data() : nullptr;
+    out->seq_off = want_seq ? b->plan.text_off.data() : nullptr;
     out->comment_pool_needed = demand;                  // the cursor counts past the capacity
     return PT_OK;
 }
@@ -1232,7 +1060,7 @@ int pt_batch_download_patches(pt_batch* b, pt_patch_view* out) {
     if ((rc = b->h_patch_misc.reserve(16))) return rc;
     if ((rc = b->h_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
     if ((rc = b->h_patch_status.reserve(std::max<size_t>(1, b->n_logs) * 4))) return rc;
-    PT_CUDA(cudaMemcpyAsync(b->h_patch_misc.p, (char*)b->d_counters.p + 80, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(b->h_patch_misc.p, &counters(b)->patch_items, 8, cudaMemcpyDeviceToHost, b->stream));
     if (b->n_insdel) PT_CUDA(cudaMemcpyAsync(b->h_patch_recs.p, b->d_patch_recs.p, b->n_insdel * sizeof(pt_patch_rec), cudaMemcpyDeviceToHost, b->stream));
     if (b->n_logs) PT_CUDA(cudaMemcpyAsync(b->h_patch_status.p, b->d_patch_status.p, (size_t)b->n_logs * 4, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
@@ -1253,59 +1081,23 @@ int pt_batch_set_patch_pool(pt_batch* b, uint64_t items) {
         b->patch_cap = items;
         int rc;
         if ((rc = b->d_patch_items.reserve(b->patch_cap * sizeof(pt_patch_item)))) return rc;
-        if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }
-        b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0;
+        drop_graph(b);                                   // the item pool pointer / capacity are baked in
     }
     return PT_OK;
 }
 
 int pt_batch_query_elements(pt_batch* b, const pt_elem_query* queries, uint32_t n, uint32_t* out) {
-    if (!b || (n && (!queries || !out))) return PT_ERR_INVALID;
-    if (!b->merged) { g_last_error = "query before merge"; return PT_ERR_STATE; }
-    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
-    if (!n) return PT_OK;
-    PT_CUDA(cudaSetDevice(b->device));
-    DevBuf dq, da;
-    int rc;
-    if ((rc = dq.reserve((size_t)n * sizeof(pt_elem_query))) || (rc = da.reserve((size_t)n * 4))) { dq.release(); da.release(); return rc; }
-    cudaError_t e = cudaMemcpyAsync(dq.p, queries, (size_t)n * sizeof(pt_elem_query), cudaMemcpyHostToDevice, b->stream);
-    if (e == cudaSuccess) {
-        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-        query_elements_kernel<<<grid, threads, 0, b->stream>>>((const pt_elem_query*)dq.p, n, (const pt_log_result*)b->d_results.p,
-                                                              (const uint64_t*)b->d_text_off.p, (const uint32_t*)b->d_seq.p, b->n_logs, (uint32_t*)da.p);
-        e = cudaGetLastError();
-        b->launches++;
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
-    dq.release(); da.release();
-    if (e != cudaSuccess) { g_last_error = std::string("pt_batch_query_elements: ") + cudaGetErrorString(e); return PT_ERR_CUDA; }
-    return PT_OK;
+    return run_queries(b, "pt_batch_query_elements", "query", queries, n, out, [&](uint32_t grid, uint32_t threads, const pt_elem_query* dq, uint32_t* da) {
+        query_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_result*)b->d_results.p, (const uint64_t*)b->d_text_off.p,
+                                                              (const uint32_t*)b->d_seq.p, b->n_logs, da);
+    });
 }
 
 int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out) {
-    if (!b || (n && (!refs || !out))) return PT_ERR_INVALID;
-    if (!b->merged) { g_last_error = "find before merge"; return PT_ERR_STATE; }
-    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
-    if (!n) return PT_OK;
-    PT_CUDA(cudaSetDevice(b->device));
-    DevBuf dq, da;
-    int rc;
-    if ((rc = dq.reserve((size_t)n * sizeof(pt_elem_ref))) || (rc = da.reserve((size_t)n * sizeof(pt_elem_pos)))) { dq.release(); da.release(); return rc; }
-    cudaError_t e = cudaMemcpyAsync(dq.p, refs, (size_t)n * sizeof(pt_elem_ref), cudaMemcpyHostToDevice, b->stream);
-    if (e == cudaSuccess) {
-        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-        find_elements_kernel<<<grid, threads, 0, b->stream>>>((const pt_elem_ref*)dq.p, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel,
-                                                             (const pt_log_result*)b->d_results.p, (const uint64_t*)b->d_text_off.p,
-                                                             (const uint32_t*)b->d_seq.p, b->n_logs, (pt_elem_pos*)da.p);
-        e = cudaGetLastError();
-        b->launches++;
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * sizeof(pt_elem_pos), cudaMemcpyDeviceToHost, b->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
-    dq.release(); da.release();
-    if (e != cudaSuccess) { g_last_error = std::string("pt_batch_find_elements: ") + cudaGetErrorString(e); return PT_ERR_CUDA; }
-    return PT_OK;
+    return run_queries(b, "pt_batch_find_elements", "find", refs, n, out, [&](uint32_t grid, uint32_t threads, const pt_elem_ref* dq, pt_elem_pos* da) {
+        find_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel, (const pt_log_result*)b->d_results.p,
+                                                             (const uint64_t*)b->d_text_off.p, (const uint32_t*)b->d_seq.p, b->n_logs, da);
+    });
 }
 
 // JSON render (render_kernel.cuh): upload the pools, size pass, scan of the sizes through the download path's scan kernels,
@@ -1397,14 +1189,11 @@ uint64_t pt_batch_launch_count(const pt_batch* b) { return b ? b->launches : 0; 
 int pt_batch_stats(pt_batch* b, uint64_t out[4]) {
     if (!b || !out) return PT_ERR_INVALID;
     if (!b->merged) return PT_ERR_STATE;
-    unsigned long long h[8] = {0};
-    PT_CUDA(cudaMemcpyAsync(h, b->d_counters.p, 32, cudaMemcpyDeviceToHost, b->stream));
+    DevCounters h;
+    PT_CUDA(cudaMemcpyAsync(&h, b->d_counters.p, sizeof(h), cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
-    for (int i = 0; i < 3; i++) out[i] = h[i];
-    out[3] = 0;
-    PT_CUDA(cudaMemcpyAsync(h, (char*)b->d_counters.p + 64, 8, cudaMemcpyDeviceToHost, b->stream));
-    PT_CUDA(cudaStreamSynchronize(b->stream));
-    out[3] = h[0];                                       // comment-pool entries the batch needs
+    for (int i = 0; i < 3; i++) out[i] = h.stats[i];
+    out[3] = h.comment_used;                             // comment-pool entries the batch needs
     return PT_OK;
 }
 
@@ -1429,11 +1218,10 @@ int pt_batch_set_comment_pool(pt_batch* b, uint64_t entries) {
     PT_CUDA(cudaStreamSynchronize(b->stream));
     b->limits.comment_pool_entries = entries;
     if (b->have_batch && entries) {
-        b->pool_cap = entries;
+        b->plan.pool_cap = entries;
         int rc;
-        if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, b->pool_cap) * 4))) return rc;
-        if (b->graph_exec) { cudaGraphExecDestroy(b->graph_exec); b->graph_exec = nullptr; }   // the pool pointer / capacity are baked in
-        b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0;
+        if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, b->plan.pool_cap) * 4))) return rc;
+        drop_graph(b);                                   // the pool pointer / capacity are baked in
     }
     return PT_OK;
 }
@@ -1442,20 +1230,12 @@ void pt_batch_destroy(pt_batch* b) {
     if (!b) return;
     cudaSetDevice(b->device);
     cudaStreamSynchronize(b->stream);
-    for (DevBuf* d : {&b->d_desc, &b->d_insdel, &b->d_marks, &b->d_order, &b->d_counters, &b->d_results, &b->d_text_off,
-                      &b->d_span_off, &b->d_text, &b->d_spans, &b->d_pool, &b->d_slab, &b->d_retry, &b->d_seq,
-                      &b->d_runs, &b->d_tokens, &b->d_run_off, &b->d_tok_off, &b->d_cins, &b->d_cmarks, &b->d_bsum, &b->d_ctoff, &b->d_csoff, &b->d_ctext, &b->d_cspans,
-                      &b->d_cdesc, &b->d_changes, &b->d_deps, &b->d_admit, &b->d_patch_recs, &b->d_patch_items, &b->d_patch_status,
-                      &b->d_jval, &b->d_jvoff, &b->d_jlink, &b->d_jloff, &b->d_jcom, &b->d_jcoff, &b->d_jsize, &b->d_jbsum, &b->d_joff,
-                      &b->d_jmiss, &b->d_jbytes}) d->release();
-    for (HostBuf* h : {&b->h_patch_recs, &b->h_patch_items, &b->h_patch_status, &b->h_patch_misc, &b->h_joff, &b->h_jbytes, &b->h_jmisc}) h->release();
-    for (HostBuf* h : {&b->h_stage, &b->h_results, &b->h_text, &b->h_spans, &b->h_pool, &b->h_misc, &b->h_seq, &b->h_ctoff, &b->h_csoff}) h->release();
     if (b->side) cudaStreamDestroy(b->side);
     if (b->ev_fork) cudaEventDestroy(b->ev_fork);
     if (b->ev_join) cudaEventDestroy(b->ev_join);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->graph_exec) cudaGraphExecDestroy(b->graph_exec);
+    drop_graph(b);
     delete b;
 }
 

@@ -6,15 +6,35 @@
 * run_concurrent    — testConcurrentWrites, reference test/micromerge.ts:46-86
 
 They are written against the reference's `Micromerge` class surface, so they drive either the CPU oracle
-(`oracle.oracle.Micromerge`) or the engine facade (`peritext_b200.Micromerge`) unchanged.
+(`oracle.oracle.Micromerge`) or the engine facade (`peritext_b200.Micromerge`) unchanged.  `environ` sets the engine's
+kernel-selection variables around a block.
 """
 from __future__ import annotations
 
 import copy
 import json
 import os
+from contextlib import contextmanager
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+@contextmanager
+def environ(env):
+    """Sets the variables of `env` (None: unset) for the block, then restores their earlier values."""
+    old = {k: os.environ.get(k) for k in env}
+
+    def apply(values):
+        for k, v in values.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+    try:
+        apply(env)
+        yield
+    finally:
+        apply(old)
 
 
 def load_kats():

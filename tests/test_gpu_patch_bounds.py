@@ -3,7 +3,7 @@ arrival-dependent corners, against the oracle's `applyChange` return values.
 
 The kernel runs one warp per log over 16-bit shared-memory tables.  Two guards decide whether a log is computed:
 * the key space: `max_ctr * n_actors >= 0xFFFF` is not computed (the id table holds 16-bit keys);
-* shared memory: the host sizes the launch (`alloc_and_upload_plan`, engine.cu) by the largest HOST estimate among the
+* shared memory: the host sizes the launch (`Plan::patch_smem`, plan.cpp) by the largest HOST estimate among the
   logs that is <= 200 KB, rounded up to 1 KB; the kernel compares its own, smaller, footprint `need` with that size.
 So a log too large to be computed alone may be computed next to a log that raised the launch's shared memory: its status
 depends on the batch.  `expected_patch_status` restates both sides.  The `n >= 0xFFFF` / `m >= 0xFFFF` guards cannot be
@@ -35,7 +35,7 @@ ATTR_NONE = 0xFFFFFFFF
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# The status mirror: restates the host budget (engine.cu alloc_and_upload_plan) and the kernel's check (patch_kernel.cuh)
+# The status mirror: restates the host budget (plan.cpp make_plan) and the kernel's check (patch_kernel.cuh)
 # ------------------------------------------------------------------------------------------------------------------
 def _a16(x):
     return (x + 15) & ~15

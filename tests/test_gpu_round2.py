@@ -2,8 +2,6 @@
 CTA-per-log kernel; the reference's arrival-dependent corners (mark boundaries inserted later, quirk Q4); comment-pool
 exhaustion; and the big shapes the round-1 review found untested: one true-shape c5 document (>100K characters, 10K dense
 marks: u32 indices, global-slab spill, every mark phase) and a marks-heavy log of more than 32000 records."""
-import os
-
 import numpy as np
 import pytest
 
@@ -11,7 +9,7 @@ from oracle.oracle import Micromerge as O
 from oracle.packed import replay_packed
 from peritext_b200 import workload
 from peritext_b200.packing import decode_spans, pack_logs
-from tests.harness import generateDocs
+from tests.harness import environ, generateDocs
 from tests.test_semantic_corners import noncausal_logs, q4_logs
 
 pytestmark = pytest.mark.gpu
@@ -77,23 +75,11 @@ def test_comment_pool_exhaustion_is_reported_and_one_retry_succeeds(engine):
 
 def run_with(env, batch, force=False):
     from peritext_b200.engine import BatchEngine
-    old = os.environ.get("PT_WARP")
-    try:
-        os.environ["PT_WARP_FORCE"] = "1" if force else "0"
-        if env is None:
-            os.environ.pop("PT_WARP", None)
-        else:
-            os.environ["PT_WARP"] = env
+    with environ({"PT_WARP": env, "PT_WARP_FORCE": "1" if force else "0"}):
         e = BatchEngine(0)
         e.upload(batch); e.merge(); out = e.download(); st = e.stats()
         e.close()
         return out, st
-    finally:
-        os.environ.pop("PT_WARP_FORCE", None)
-        if old is None:
-            os.environ.pop("PT_WARP", None)
-        else:
-            os.environ["PT_WARP"] = old
 
 
 @pytest.mark.parametrize("cfg,n_docs,ops", [("c4", 400, 1000), ("c3", 60, 1000), ("c2", 60, 1500), ("c4", 50, 1900)])
