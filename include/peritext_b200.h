@@ -419,6 +419,33 @@ typedef struct pt_json_pools {          /* layouts = pt_ingest_pool's kinds 0, 1
 typedef struct pt_json_view { uint32_t n_logs; const uint64_t* off; /* [n_logs + 1] */ const char* bytes; uint64_t n_bytes; } pt_json_view;
 int pt_batch_render_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
 
+/* PT_FLAG_EMIT_PATCHES: the Patch[] return values of Micromerge.applyChange (src/micromerge.ts:25-31, 659-703;
+ * src/peritext.ts:175-281) of every log of the last merge as UTF-8 JSON text, rendered on the device from the patch stream
+ * (pt_patch_view).  Log i's text is bytes[off[i] .. off[i+1]).  A log whose merge status is PT_LOG_OK and whose patch status
+ * is 0 renders as one array with one inner array per list op of the log, in arrival order (mark record k comes right before
+ * ins/del record arrival_k), holding the patches that op's applyChange returned; keys sorted; a log without list ops is []:
+ *   insert     [{"action":"insert","index":I,"marks":M,"path":["text"],"values":[V]}]
+ *              I = index & 0x7FFFFFFF; M = the marks object of pt_batch_render_json built from the record's flags /
+ *              link_attr and its comment ids (ascending rank); V = the element's value alone as JSON.stringify writes a string
+ *              (the span render's rules; surrogate halves pair only inside one value)
+ *   delete     [{"action":"delete","count":1,"index":I,"path":["text"]}] if bit 31 of index is set, else []
+ *   mark op    [{"action":A,"attrs":F,"endIndex":b,"markType":T,"path":["text"],"startIndex":a},...] its mark patches in
+ *              ascending startIndex; A addMark / removeMark; T strong / em / comment / link; "attrs" only for addMark of a link
+ *              (links pool fragment of attr) or a comment (comments pool fragment of the rank); no patches gives []
+ * A log whose merge status is not 0 or whose patch status is 1 renders as zero bytes (pt_log_result.status /
+ * pt_patch_view.status say why).  The ROOT makeList patch is not part of the output.  Where ops naming one comment id carry
+ * different attrs objects, F and C are the first-seen attrs of the id (the span render's corner).
+ * Pools and missing-entry errors as pt_batch_render_json.  Null arguments: PT_ERR_INVALID.  No completed merge, a handle
+ * created without PT_FLAG_EMIT_PATCHES, or an item demand of the last merge above the patch pool's capacity (pt_last_error
+ * gives the needed count: pt_batch_set_patch_pool and merge again), or a pt_batch_set_patch_pool since the last merge:
+ * PT_ERR_STATE.  n_logs == 0: PT_OK with off[0] = 0.
+ * Synchronises.  The view is engine-owned pinned memory of its own, valid until the next pt_batch_render_patches_json,
+ * upload or destroy; a pt_batch_render_json view, the pt_spans_view and the pt_patch_view stay valid and unchanged.  The bytes
+ * do not depend on the order of the item pool.
+ * Device: the item pool ordered by owner and key (count, scan, scatter, rank), then a size pass and a write pass, one warp
+ * per log and one lane per op. */
+int pt_batch_render_patches_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
+
 /* Copy only the per-log result headers (status, counts, digest). Synchronises the stream. */
 int pt_batch_download_results(pt_batch*, pt_log_result* out, uint32_t n_logs);
 

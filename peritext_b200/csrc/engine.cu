@@ -18,6 +18,7 @@
 #include "patch_kernel.cuh"
 #include "team_kernel.cuh"
 #include "render_kernel.cuh"
+#include "patch_json_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -56,6 +57,13 @@ using HostBuf = Buf<true>;
 
 using ptp::kNumBins;
 using ptp::kCtaBins;
+
+// One JSON render's buffers: per-log sizes, scan, offsets, missing-entry key and output on the device; the view's offsets
+// and bytes and the read-back of the total in pinned memory.
+struct JsonBufs {
+    DevBuf size, bsum, off, miss, bytes;
+    HostBuf hoff, hbytes, hmisc;
+};
 
 // The device counter block of a batch, zeroed before every merge; the kernels get pointers to its fields.
 struct DevCounters {
@@ -410,6 +418,7 @@ struct pt_batch {
     pt_limits limits{};
     // batch
     bool have_batch = false, merged = false;
+    bool patch_pool_changed = false;   // pt_batch_set_patch_pool replaced the item pool after the last merge
     uint32_t n_logs = 0;
     uint64_t n_insdel = 0, n_mark = 0;
     std::vector<pt_log_desc> h_desc;
@@ -421,9 +430,9 @@ struct pt_batch {
     DevBuf d_cdesc, d_changes, d_deps, d_admit;           // admission pre-pass (optional change table)
     DevBuf d_patch_recs, d_patch_items, d_patch_status;   // PT_FLAG_EMIT_PATCHES
     HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc;
-    DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // pt_batch_render_json: the caller's pools,
-    DevBuf d_jsize, d_jbsum, d_joff, d_jmiss, d_jbytes;                 // per-log sizes, scan, offsets, missing-entry key, output
-    HostBuf h_joff, h_jbytes, h_jmisc;
+    DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // both JSON renders: the caller's pools
+    JsonBufs spans_json, patches_json;                                  // each render's own scratch and view
+    DevBuf d_picnt, d_piseg, d_pibsum, d_pitmp, d_pisorted;             // pt_batch_render_patches_json: the ordered patch items
     uint64_t patch_cap = 0;
     bool have_changes = false;
     uint32_t adm_maxR = 1;
@@ -638,6 +647,88 @@ int run_queries(pt_batch* b, const char* fn, const char* verb, const Q* queries,
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * sizeof(A), cudaMemcpyDeviceToHost, b->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
     if (e != cudaSuccess) { g_last_error = std::string(fn) + ": " + cudaGetErrorString(e); return PT_ERR_CUDA; }
+    return PT_OK;
+}
+
+}  // namespace
+
+namespace {
+
+// The caller's pools of both JSON renders: checked on the host, then (for a batch with logs) copied into the handle's device
+// buffers and described for the kernels in *P.
+int load_json_pools(pt_batch* b, const pt_json_pools* pools, const char* fn, ptr::JsonPools* P) {
+    struct Pool { const uint8_t* data; const uint64_t* off; uint64_t count; DevBuf* dd; DevBuf* doff; const char* name; };
+    const Pool ps[3] = {{pools->values, pools->values_off, pools->n_values, &b->d_jval, &b->d_jvoff, "values"},
+                        {pools->links, pools->links_off, pools->n_links, &b->d_jlink, &b->d_jloff, "links"},
+                        {pools->comments, pools->comments_off, pools->n_comments, &b->d_jcom, &b->d_jcoff, "comments"}};
+    for (const Pool& p : ps) {
+        if (p.count && (!p.data || !p.off)) { g_last_error = std::string(fn) + ": null " + p.name + " pool with a nonzero count"; return PT_ERR_INVALID; }
+        for (uint64_t k = 0; k < p.count; k++)
+            if (p.off[k + 1] < p.off[k]) { g_last_error = std::string(fn) + ": " + p.name + " offsets decrease"; return PT_ERR_INVALID; }
+    }
+    PT_CUDA(cudaSetDevice(b->device));
+    if (!b->n_logs) return PT_OK;
+    const uint8_t** pdata[3] = {&P->val, &P->link, &P->com};
+    const uint64_t** poff[3] = {&P->voff, &P->loff, &P->coff};
+    uint64_t* pcount[3] = {&P->nval, &P->nlink, &P->ncom};
+    int rc;
+    for (int k = 0; k < 3; k++) {
+        const Pool& p = ps[k];
+        const uint64_t lo = p.count ? p.off[0] : 0, hi = p.count ? p.off[p.count] : 0;     // entries address data[lo, hi)
+        if ((rc = p.dd->reserve(std::max<uint64_t>(1, hi))) || (rc = p.doff->reserve((p.count + 1) * 8))) return rc;
+        if (hi > lo) PT_CUDA(cudaMemcpyAsync((uint8_t*)p.dd->p + lo, p.data + lo, hi - lo, cudaMemcpyHostToDevice, b->stream));
+        if (p.count) PT_CUDA(cudaMemcpyAsync(p.doff->p, p.off, (p.count + 1) * 8, cudaMemcpyHostToDevice, b->stream));
+        *pdata[k] = (const uint8_t*)p.dd->p; *poff[k] = (const uint64_t*)p.doff->p; *pcount[k] = p.count;
+    }
+    return PT_OK;
+}
+
+// Both renders after their pools are loaded: size pass (size(grid, threads, sizes, miss)), scan of the sizes through the
+// download path's scan kernels, read-back of the total and the missing-entry key (one sync), an output of exactly that size,
+// write pass (write(grid, threads, off, bytes)), copy back into J's pinned view.
+template <class Size, class Write>
+int render_passes(pt_batch* b, const char* fn, JsonBufs& J, Size size, Write write, pt_json_view* out) {
+    int rc;
+    const uint32_t n = b->n_logs;
+    if ((rc = J.hoff.reserve(((size_t)n + 1) * 8)) || (rc = J.hbytes.reserve(1)) || (rc = J.hmisc.reserve(16))) return rc;
+    uint64_t* hoff = (uint64_t*)J.hoff.p;
+    if (!n) {
+        hoff[0] = 0;
+        *out = pt_json_view{0, hoff, (const char*)J.hbytes.p, 0};
+        return PT_OK;
+    }
+    const uint32_t nb = (n + kScanBlock - 1) / kScanBlock;
+    if ((rc = J.size.reserve((size_t)n * 8)) || (rc = J.bsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = J.off.reserve(((size_t)n + 1) * 8)) ||
+        (rc = J.miss.reserve(8))) return rc;
+    unsigned long long *sizes = (unsigned long long*)J.size.p, *bsum = (unsigned long long*)J.bsum.p, *doff = (unsigned long long*)J.off.p,
+                       *miss = (unsigned long long*)J.miss.p;
+    const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+    PT_CUDA(cudaMemsetAsync(miss, 0xFF, 8, b->stream));
+    size(grid, threads, sizes, miss);
+    out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum);
+    out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
+    out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum, nb, doff, (unsigned long long*)nullptr);
+    PT_CUDA(cudaGetLastError());
+    b->launches += 4;
+    uint64_t* hm = (uint64_t*)J.hmisc.p;
+    PT_CUDA(cudaMemcpyAsync(hm, doff + n, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(hm + 1, miss, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    const uint64_t total = hm[0], key = hm[1];
+    if (key != ~0ull) {
+        static const char* kinds[3] = {"value", "link", "comment"};
+        g_last_error = std::string(fn) + ": log " + std::to_string(key >> 34) + " names " + kinds[(key >> 32) & 3] + " pool entry " +
+                       std::to_string(key & 0xFFFFFFFFull) + ", which the caller's pools do not hold";
+        return PT_ERR_INVALID;
+    }
+    if ((rc = J.bytes.reserve(std::max<uint64_t>(1, total))) || (rc = J.hbytes.reserve(std::max<uint64_t>(1, total)))) return rc;
+    write(grid, threads, (const unsigned long long*)doff, (uint8_t*)J.bytes.p);
+    PT_CUDA(cudaGetLastError());
+    b->launches++;
+    PT_CUDA(cudaMemcpyAsync(hoff, doff, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
+    if (total) PT_CUDA(cudaMemcpyAsync(J.hbytes.p, J.bytes.p, total, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    *out = pt_json_view{n, hoff, (const char*)J.hbytes.p, total};
     return PT_OK;
 }
 
@@ -942,7 +1033,7 @@ int pt_batch_merge(pt_batch* b) {
         if (rc) return rc;
     }
     PT_CUDA(cudaEventRecord(b->ev1, b->stream));
-    b->merged = true; b->merges_since_upload++; b->dl_begun = false;
+    b->merged = true; b->merges_since_upload++; b->dl_begun = false; b->patch_pool_changed = false;
     return PT_OK;
 }
 
@@ -1079,6 +1170,7 @@ int pt_batch_set_patch_pool(pt_batch* b, uint64_t items) {
     b->limits.patch_pool_items = (uint32_t)items;
     if (b->have_batch && items && (b->limits.flags & PT_FLAG_EMIT_PATCHES)) {
         b->patch_cap = items;
+        b->patch_pool_changed = b->merged;
         int rc;
         if ((rc = b->d_patch_items.reserve(b->patch_cap * sizeof(pt_patch_item)))) return rc;
         drop_graph(b);                                   // the item pool pointer / capacity are baked in
@@ -1100,80 +1192,89 @@ int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_
     });
 }
 
-// JSON render (render_kernel.cuh): upload the pools, size pass, scan of the sizes through the download path's scan kernels,
-// read back the total and the missing-entry key (one sync), size the output exactly, write pass, copy back.
+// JSON render of the spans (render_kernel.cuh).
 int pt_batch_render_json(pt_batch* b, const pt_json_pools* pools, pt_json_view* out) {
     if (!b || !pools || !out) return PT_ERR_INVALID;
     if (!b->merged) { g_last_error = "render before merge"; return PT_ERR_STATE; }
-    struct Pool { const uint8_t* data; const uint64_t* off; uint64_t count; DevBuf* dd; DevBuf* doff; const char* name; };
-    const Pool ps[3] = {{pools->values, pools->values_off, pools->n_values, &b->d_jval, &b->d_jvoff, "values"},
-                        {pools->links, pools->links_off, pools->n_links, &b->d_jlink, &b->d_jloff, "links"},
-                        {pools->comments, pools->comments_off, pools->n_comments, &b->d_jcom, &b->d_jcoff, "comments"}};
-    for (const Pool& p : ps) {
-        if (p.count && (!p.data || !p.off)) { g_last_error = std::string("pt_batch_render_json: null ") + p.name + " pool with a nonzero count"; return PT_ERR_INVALID; }
-        for (uint64_t k = 0; k < p.count; k++)
-            if (p.off[k + 1] < p.off[k]) { g_last_error = std::string("pt_batch_render_json: ") + p.name + " offsets decrease"; return PT_ERR_INVALID; }
-    }
-    PT_CUDA(cudaSetDevice(b->device));
-    int rc;
-    const uint32_t n = b->n_logs;
-    if ((rc = b->h_joff.reserve(((size_t)n + 1) * 8)) || (rc = b->h_jbytes.reserve(1)) || (rc = b->h_jmisc.reserve(16))) return rc;
-    uint64_t* hoff = (uint64_t*)b->h_joff.p;
-    if (!n) {
-        hoff[0] = 0;
-        *out = pt_json_view{0, hoff, (const char*)b->h_jbytes.p, 0};
-        return PT_OK;
-    }
     ptr::JsonPools P{};
-    const uint8_t** pdata[3] = {&P.val, &P.link, &P.com};
-    const uint64_t** poff[3] = {&P.voff, &P.loff, &P.coff};
-    uint64_t* pcount[3] = {&P.nval, &P.nlink, &P.ncom};
-    for (int k = 0; k < 3; k++) {
-        const Pool& p = ps[k];
-        const uint64_t lo = p.count ? p.off[0] : 0, hi = p.count ? p.off[p.count] : 0;     // entries address data[lo, hi)
-        if ((rc = p.dd->reserve(std::max<uint64_t>(1, hi))) || (rc = p.doff->reserve((p.count + 1) * 8))) return rc;
-        if (hi > lo) PT_CUDA(cudaMemcpyAsync((uint8_t*)p.dd->p + lo, p.data + lo, hi - lo, cudaMemcpyHostToDevice, b->stream));
-        if (p.count) PT_CUDA(cudaMemcpyAsync(p.doff->p, p.off, (p.count + 1) * 8, cudaMemcpyHostToDevice, b->stream));
-        *pdata[k] = (const uint8_t*)p.dd->p; *poff[k] = (const uint64_t*)p.doff->p; *pcount[k] = p.count;
-    }
-    const uint32_t nb = (n + kScanBlock - 1) / kScanBlock;
-    if ((rc = b->d_jsize.reserve((size_t)n * 8)) || (rc = b->d_jbsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = b->d_joff.reserve(((size_t)n + 1) * 8)) ||
-        (rc = b->d_jmiss.reserve(8))) return rc;
-    unsigned long long *sizes = (unsigned long long*)b->d_jsize.p, *bsum = (unsigned long long*)b->d_jbsum.p, *doff = (unsigned long long*)b->d_joff.p,
-                       *miss = (unsigned long long*)b->d_jmiss.p;
+    int rc;
+    if ((rc = load_json_pools(b, pools, "pt_batch_render_json", &P))) return rc;
     const pt_log_result* res = (const pt_log_result*)b->d_results.p;
     const uint64_t *toff = (const uint64_t*)b->d_text_off.p, *soff = (const uint64_t*)b->d_span_off.p;
     const uint32_t* text = (const uint32_t*)b->d_text.p;
     const pt_span* spans = (const pt_span*)b->d_spans.p;
     const uint32_t* cpool = (const uint32_t*)b->d_pool.p;
-    const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-    PT_CUDA(cudaMemsetAsync(miss, 0xFF, 8, b->stream));
-    ptr::json_size_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, sizes, miss);
-    out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum);
-    out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
-    out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum, nb, doff, (unsigned long long*)nullptr);
-    PT_CUDA(cudaGetLastError());
-    b->launches += 4;
-    uint64_t* hm = (uint64_t*)b->h_jmisc.p;
-    PT_CUDA(cudaMemcpyAsync(hm, doff + n, 8, cudaMemcpyDeviceToHost, b->stream));
-    PT_CUDA(cudaMemcpyAsync(hm + 1, miss, 8, cudaMemcpyDeviceToHost, b->stream));
-    PT_CUDA(cudaStreamSynchronize(b->stream));
-    const uint64_t total = hm[0], key = hm[1];
-    if (key != ~0ull) {
-        static const char* kinds[3] = {"value", "link", "comment"};
-        g_last_error = "pt_batch_render_json: log " + std::to_string(key >> 34) + " names " + kinds[(key >> 32) & 3] + " pool entry " +
-                       std::to_string(key & 0xFFFFFFFFull) + ", which the caller's pools do not hold";
-        return PT_ERR_INVALID;
+    const uint32_t n = b->n_logs;
+    return render_passes(b, "pt_batch_render_json", b->spans_json,
+        [&](uint32_t grid, uint32_t threads, unsigned long long* sizes, unsigned long long* miss) {
+            ptr::json_size_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, sizes, miss);
+        },
+        [&](uint32_t grid, uint32_t threads, const unsigned long long* off, uint8_t* bytes) {
+            ptr::json_write_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, off, bytes);
+        }, out);
+}
+
+// JSON render of the Patch stream (patch_json_kernel.cuh): check the item demand, order the item pool by owner and key
+// (count, scan, scatter, rank), then the same passes as the span render.
+int pt_batch_render_patches_json(pt_batch* b, const pt_json_pools* pools, pt_json_view* out) {
+    static const char* fn = "pt_batch_render_patches_json";
+    if (!b || !pools || !out) return PT_ERR_INVALID;
+    if (!b->merged) { g_last_error = "render before merge"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_PATCHES)) { g_last_error = "the handle was created without PT_FLAG_EMIT_PATCHES"; return PT_ERR_STATE; }
+    if (b->patch_pool_changed) { g_last_error = std::string(fn) + ": the patch pool was replaced after the last merge; merge again"; return PT_ERR_STATE; }
+    ptr::JsonPools P{};
+    int rc;
+    if ((rc = load_json_pools(b, pools, fn, &P))) return rc;
+    const uint32_t n = b->n_logs;
+    ptr::PatchJsonIn I{};
+    if (n) {
+        if ((rc = b->h_patch_misc.reserve(16))) return rc;
+        PT_CUDA(cudaMemcpyAsync(b->h_patch_misc.p, &counters(b)->patch_items, 8, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+        const uint64_t items = *(unsigned long long*)b->h_patch_misc.p, owners = b->n_insdel + b->n_mark;
+        if (items > b->patch_cap) {
+            g_last_error = std::string(fn) + ": the last merge needs " + std::to_string(items) + " patch items and the pool holds " +
+                           std::to_string(b->patch_cap) + "; call pt_batch_set_patch_pool(" + std::to_string(items) + ") and merge again";
+            return PT_ERR_STATE;
+        }
+        if (owners >= 0xFFFFFFFFull) { g_last_error = std::string(fn) + ": more than 2^32 - 2 op records"; return PT_ERR_INVALID; }
+        const uint32_t no = (uint32_t)owners, nb = (no + kScanBlock - 1) / kScanBlock;
+        if ((rc = b->d_picnt.reserve(std::max<uint64_t>(1, owners) * 8)) || (rc = b->d_piseg.reserve((owners + 1) * 8)) ||
+            (rc = b->d_pibsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = b->d_pitmp.reserve(std::max<uint64_t>(1, items) * sizeof(pt_patch_item))) ||
+            (rc = b->d_pisorted.reserve(std::max<uint64_t>(1, items) * sizeof(uint2)))) return rc;
+        unsigned long long *cnt = (unsigned long long*)b->d_picnt.p, *seg = (unsigned long long*)b->d_piseg.p, *bsum = (unsigned long long*)b->d_pibsum.p;
+        const pt_log_desc* desc = (const pt_log_desc*)b->d_desc.p;
+        const pt_patch_item* pool = (const pt_patch_item*)b->d_patch_items.p;
+        pt_patch_item* tmp = (pt_patch_item*)b->d_pitmp.p;
+        uint2* sorted = (uint2*)b->d_pisorted.p;
+        if (no) {
+            const uint32_t threads = 256, grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + threads - 1) / threads, (uint64_t)b->num_sms * 16));
+            PT_CUDA(cudaMemsetAsync(cnt, 0, owners * 8, b->stream));
+            if (items) ptr::pitem_count_kernel<<<grid, threads, 0, b->stream>>>(pool, items, desc, b->n_insdel, cnt);
+            out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{cnt}, no, bsum);
+            out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
+            out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{cnt}, no, bsum, nb, seg, (unsigned long long*)nullptr);
+            b->launches += 3;
+            if (items) {
+                ptr::pitem_scatter_kernel<<<grid, threads, 0, b->stream>>>(pool, items, desc, b->n_insdel, cnt, seg, tmp);
+                ptr::pitem_rank_kernel<<<grid, threads, 0, b->stream>>>(tmp, items, desc, b->n_insdel, seg, sorted);
+                b->launches += 3;
+            }
+            PT_CUDA(cudaGetLastError());
+        } else {
+            PT_CUDA(cudaMemsetAsync(seg, 0, 8, b->stream));
+        }
+        I.desc = desc; I.insdel = b->dp_insdel; I.marks = b->dp_marks; I.res = (const pt_log_result*)b->d_results.p;
+        I.recs = (const pt_patch_rec*)b->d_patch_recs.p; I.pstatus = (const uint32_t*)b->d_patch_status.p;
+        I.seg = seg; I.items = sorted; I.n_insdel = b->n_insdel;
     }
-    if ((rc = b->d_jbytes.reserve(std::max<uint64_t>(1, total))) || (rc = b->h_jbytes.reserve(std::max<uint64_t>(1, total)))) return rc;
-    ptr::json_write_kernel<<<grid, threads, 0, b->stream>>>(res, n, toff, soff, text, spans, cpool, P, doff, (uint8_t*)b->d_jbytes.p);
-    PT_CUDA(cudaGetLastError());
-    b->launches++;
-    PT_CUDA(cudaMemcpyAsync(hoff, doff, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
-    if (total) PT_CUDA(cudaMemcpyAsync(b->h_jbytes.p, b->d_jbytes.p, total, cudaMemcpyDeviceToHost, b->stream));
-    PT_CUDA(cudaStreamSynchronize(b->stream));
-    *out = pt_json_view{n, hoff, (const char*)b->h_jbytes.p, total};
-    return PT_OK;
+    return render_passes(b, fn, b->patches_json,
+        [&](uint32_t grid, uint32_t threads, unsigned long long* sizes, unsigned long long* miss) {
+            ptr::patches_json_size_kernel<<<grid, threads, 0, b->stream>>>(I, n, P, sizes, miss);
+        },
+        [&](uint32_t grid, uint32_t threads, const unsigned long long* off, uint8_t* bytes) {
+            ptr::patches_json_write_kernel<<<grid, threads, 0, b->stream>>>(I, n, P, off, bytes);
+        }, out);
 }
 
 int pt_batch_device_results(pt_batch* b, void** dev_ptr, uint32_t* n_logs) {

@@ -120,23 +120,36 @@ template <bool W> __device__ __forceinline__ void emit_lit(uint8_t* d, uint64_t&
 }
 #define PTR_LIT(W, d, pos, s, lane) emit_lit<W>(d, pos, s, (uint32_t)(sizeof(s) - 1), lane)
 
-// A pool fragment, 32 bytes per trip: verbatim, except that the 3-byte encoding of a lone surrogate becomes \udxxx.
+// The one rule for pool fragments: byte k of f[0, len) is written verbatim (1 byte), except that the 3-byte encoding of a
+// lone surrogate becomes \udxxx: its lead byte writes the 6-byte escape of unit *cu, its two continuation bytes nothing.
+__device__ __forceinline__ uint32_t frag_byte(const uint8_t* f, uint64_t k, uint64_t len, uint32_t& cu) {
+    const uint8_t x = f[k];
+    if (x == 0xEDu && k + 2 < len && (f[k + 1] & 0xE0u) == 0xA0u) { cu = 0xD000u | ((f[k + 1] & 0x3Fu) << 6) | (f[k + 2] & 0x3Fu); return 6; }
+    const bool cont = (k >= 1 && f[k - 1] == 0xEDu && (x & 0xE0u) == 0xA0u && k + 1 < len) ||
+                      (k >= 2 && f[k - 2] == 0xEDu && (f[k - 1] & 0xE0u) == 0xA0u);
+    return cont ? 0u : 1u;
+}
+template <bool W> __device__ __forceinline__ void frag_put(const uint8_t* f, uint64_t k, uint32_t c, uint32_t cu, uint8_t* o) {
+    if (W && c) { if (c == 6) put_u_escape<true>(o, cu); else o[0] = f[k]; }
+}
+
+// A pool fragment, 32 bytes per trip (warp-collective).
 template <bool W> __device__ __forceinline__ void frag_out(const uint8_t* f, uint64_t len, uint8_t* d, uint64_t& pos, uint32_t lane) {
     for (uint64_t b = 0; b < len; b += 32) {
         const uint64_t k = b + lane;
-        uint32_t c = 0, cu = 0; uint8_t x = 0; bool lead = false;
-        if (k < len) {
-            x = f[k];
-            lead = x == 0xEDu && k + 2 < len && (f[k + 1] & 0xE0u) == 0xA0u;
-            const bool cont = (k >= 1 && f[k - 1] == 0xEDu && (x & 0xE0u) == 0xA0u && k + 1 < len) ||
-                              (k >= 2 && f[k - 2] == 0xEDu && (f[k - 1] & 0xE0u) == 0xA0u);
-            c = lead ? 6u : cont ? 0u : 1u;
-            if (lead) cu = 0xD000u | ((f[k + 1] & 0x3Fu) << 6) | (f[k + 2] & 0x3Fu);
-        }
+        uint32_t c = 0, cu = 0;
+        if (k < len) c = frag_byte(f, k, len, cu);
         const uint32_t incl = warp_incl_scan(c, lane);
-        if (W && c) { uint8_t* o = d + pos + incl - c; if (lead) put_u_escape<true>(o, cu); else o[0] = x; }
+        frag_put<W>(f, k, c, cu, d + pos + incl - c);
         pos += __shfl_sync(kFull, incl, 31);
     }
+}
+
+// A pool fragment copied by one lane; returns its byte count.
+template <bool W> __device__ __forceinline__ uint32_t frag_copy(const uint8_t* f, uint64_t len, uint8_t* d) {
+    uint32_t n = 0;
+    for (uint64_t k = 0; k < len; k++) { uint32_t cu = 0; const uint32_t c = frag_byte(f, k, len, cu); frag_put<W>(f, k, c, cu, d + n); n += c; }
+    return n;
 }
 
 // Log `log`'s JSON at d (W) or its byte count (!W).  Warp-collective; every lane returns the same count.

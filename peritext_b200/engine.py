@@ -22,7 +22,7 @@ EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_com
            "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_query_elements", "pt_batch_find_elements",
-           "pt_batch_render_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
+           "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
 
 
 class EngineError(RuntimeError):
@@ -169,6 +169,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_query_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_find_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_render_json.argtypes = [vp, vp, vp]
+    L.pt_batch_render_patches_json.argtypes = [vp, vp, vp]
     L.pt_batch_destroy.argtypes = [vp]; L.pt_batch_destroy.restype = None
     L.pt_strerror.argtypes = [ctypes.c_int]; L.pt_strerror.restype = ctypes.c_char_p
     L.pt_last_error.restype = ctypes.c_char_p
@@ -364,11 +365,7 @@ class BatchEngine:
             out[ok] = np.where(pos["index"] != ELEM_NOT_FOUND, pos["visible"].astype(np.int64), -1)
         return out
 
-    def render_json(self, batch: PackedBatch, pools=None) -> tuple[np.ndarray, np.ndarray]:
-        """getTextWithFormatting's return value of every log of the last merge as UTF-8 JSON text, rendered on the device
-        (pt_batch_render_json): (uint8 bytes, uint64 offsets [n_logs + 1]); log i is bytes[off[i]:off[i+1]], empty for a log
-        that did not merge.  `pools` = (values, values_off, links, links_off, comments, comments_off), default
-        ``packing.json_pools(batch)`` of the merged batch."""
+    def _render(self, entry: str, batch: PackedBatch, pools) -> tuple[np.ndarray, np.ndarray]:
         from .packing import json_pools
         p = json_pools(batch) if pools is None else pools
         arrs = [np.ascontiguousarray(a, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, a in enumerate(p)]
@@ -376,16 +373,37 @@ class BatchEngine:
         st = _JsonPools(ptr(arrs[0]), ptr(arrs[1]), max(0, len(arrs[1]) - 1), ptr(arrs[2]), ptr(arrs[3]), max(0, len(arrs[3]) - 1),
                         ptr(arrs[4]), ptr(arrs[5]), max(0, len(arrs[5]) - 1))
         v = _JsonView()
-        _check(self._L.pt_batch_render_json(self._h, ctypes.byref(st), ctypes.byref(v)), "pt_batch_render_json")
+        _check(getattr(self._L, entry)(self._h, ctypes.byref(st), ctypes.byref(v)), entry)
         off = np.frombuffer((ctypes.c_char * ((v.n_logs + 1) * 8)).from_address(v.off), np.uint64).copy()
         data = np.frombuffer((ctypes.c_char * v.n_bytes).from_address(v.bytes), np.uint8).copy() if v.n_bytes else np.zeros(0, np.uint8)
         return data, off
 
-    def render_json_list(self, batch: PackedBatch, pools=None) -> list[bytes]:
-        """``render_json`` as one bytes object per log."""
-        data, off = self.render_json(batch, pools)
+    @staticmethod
+    def _split(data: np.ndarray, off: np.ndarray) -> list[bytes]:
         raw = data.tobytes()
         return [raw[int(off[i]): int(off[i + 1])] for i in range(len(off) - 1)]
+
+    def render_json(self, batch: PackedBatch, pools=None) -> tuple[np.ndarray, np.ndarray]:
+        """getTextWithFormatting's return value of every log of the last merge as UTF-8 JSON text, rendered on the device
+        (pt_batch_render_json): (uint8 bytes, uint64 offsets [n_logs + 1]); log i is bytes[off[i]:off[i+1]], empty for a log
+        that did not merge.  `pools` = (values, values_off, links, links_off, comments, comments_off), default
+        ``packing.json_pools(batch)`` of the merged batch."""
+        return self._render("pt_batch_render_json", batch, pools)
+
+    def render_json_list(self, batch: PackedBatch, pools=None) -> list[bytes]:
+        """``render_json`` as one bytes object per log."""
+        return self._split(*self.render_json(batch, pools))
+
+    def render_patches_json(self, batch: PackedBatch, pools=None) -> tuple[np.ndarray, np.ndarray]:
+        """The Patch[] that applyChange returned for every list op of every log of the last merge, as UTF-8 JSON text rendered
+        on the device (pt_batch_render_patches_json; needs emit_patches): (uint8 bytes, uint64 offsets [n_logs + 1]); log i is
+        bytes[off[i]:off[i+1]], one inner array per list op in arrival order, empty for a log that did not merge or whose
+        patches were not computed on the device.  `pools` as for ``render_json``."""
+        return self._render("pt_batch_render_patches_json", batch, pools)
+
+    def render_patches_json_list(self, batch: PackedBatch, pools=None) -> list[bytes]:
+        """``render_patches_json`` as one bytes object per log."""
+        return self._split(*self.render_patches_json(batch, pools))
 
     def set_comment_pool(self, entries: int):
         _check(self._L.pt_batch_set_comment_pool(self._h, int(entries)), "pt_batch_set_comment_pool")
