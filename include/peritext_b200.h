@@ -157,7 +157,10 @@ typedef struct pt_change_table {
  * Compact wire format (optional, for the host -> device leg): the same records in half the bytes.
  * Usable for a log with max_ctr < 65536, n_insdel < 65536 and n_actors <= 16 (any document the
  * benchmark shapes produce); value tokens must fit 22 bits (any Unicode code point, or a value-pool
- * index < 2^21).  Records keep their positions (the descriptors are those of the expanded layout);
+ * index < 2^21).  Every record field must fit its compact width on its own, whatever the descriptor
+ * says: ctr, ref_ctr, start_ctr, end_ctr and arrival < 65536; actor, ref_actor, start_actor and
+ * end_actor < 16; mark kind < 8 and bounds < 16.  pt_compact_ops refuses a batch with any other
+ * record (naming the field), so a faulty record is never truncated into a valid one.  Records keep their positions (the descriptors are those of the expanded layout);
  * pt_batch_upload_compact expands them to pt_insdel_rec / pt_mark_rec on the device, elementwise.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct pt_insdel_c8 {   /* 8 B */
@@ -311,7 +314,9 @@ int pt_batch_create(int device, const pt_limits* limits, void* cuda_stream, pt_b
 int pt_batch_upload(pt_batch*, const pt_packed_ops* host_ops);
 
 /* Same as pt_batch_upload for the run-compressed form: copies runs / tokens / marks host -> device and expands the runs
- * to pt_insdel_rec records on the device (one small kernel).  Typically 2-3x fewer bytes over PCIe. */
+ * to pt_insdel_rec records on the device (one small kernel).  Typically 2-3x fewer bytes over PCIe.  The run table is
+ * checked on the host first (PT_ERR_INVALID, nothing copied): run_off / tok_off start at 0 and never decrease, every count
+ * is >= 1, and per log the counts sum to n_insdel and the insert counts to the log's token span. */
 int pt_batch_upload_runs(pt_batch*, const pt_packed_runs* host_runs);
 
 /* Host helper: compress a packed batch into runs.  Call once with runs == NULL / tokens == NULL to get the counts
@@ -326,7 +331,8 @@ int pt_compress_runs(const pt_packed_ops* ops, uint64_t* run_off, uint64_t* tok_
 int pt_batch_upload_changes(pt_batch*, const pt_change_table* host_changes);
 
 /* Host helper (multithreaded): convert a packed batch to the compact wire format into caller-provided arrays of
- * n_insdel_total / n_mark_total entries.  PT_ERR_INVALID (nothing useful written) if some log is not representable. */
+ * n_insdel_total / n_mark_total entries.  PT_ERR_INVALID (nothing useful written) if some log or record is not
+ * representable (the rules above the compact records). */
 int pt_compact_ops(const pt_packed_ops* ops, pt_insdel_c8* insdel_out, pt_mark_c16* marks_out, int threads /* 0 = all cores */);
 
 /* Same as pt_batch_upload for the compact form: half the bytes over PCIe, expanded on the device (two elementwise kernels). */

@@ -772,8 +772,33 @@ int pt_batch_upload(pt_batch* b, const pt_packed_ops* ops) {
     return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{ops->insdel, b->n_insdel}, {ops->marks, b->n_mark}});
 }
 
+// The run table as expand_runs_kernel reads it: each log's runs expand to exactly its descriptor's n_insdel records and
+// consume exactly its slice of the token stream, so the expansion stays inside the log's records (make_plan checks the
+// descriptors themselves).  Returns the problem, or null.
+static const char* check_run_table(const pt_packed_runs& rr) {
+    const uint32_t nl = rr.n_logs;
+    if (!nl) return nullptr;
+    if (rr.run_off[0] != 0 || rr.tok_off[0] != 0) return "run table: run_off[0] and tok_off[0] must be 0";
+    for (uint32_t i = 0; i < nl; i++)
+        if (rr.run_off[i + 1] < rr.run_off[i] || rr.tok_off[i + 1] < rr.tok_off[i]) return "run table: run_off / tok_off decrease";
+    if ((rr.run_off[nl] && !rr.runs) || (rr.tok_off[nl] && !rr.tokens) || (rr.n_mark_total && !rr.marks)) return "run table: null array with a nonzero count";
+    for (uint32_t i = 0; i < nl; i++) {
+        uint64_t recs = 0, toks = 0;
+        for (uint64_t r = rr.run_off[i]; r < rr.run_off[i + 1]; r++) {
+            const uint32_t cnt = rr.runs[r].kind_count & 0x3FFFFFFFu, kind = rr.runs[r].kind_count >> 30;   // a 2-bit kind is always <= 3
+            if (!cnt) return "run table: a run with count 0";
+            recs += cnt;
+            if (kind == PT_KIND_INSERT) toks += cnt;
+        }
+        if (recs != rr.logs[i].n_insdel) return "run table: a log's run counts do not sum to its n_insdel";
+        if (toks != rr.tok_off[i + 1] - rr.tok_off[i]) return "run table: a log's insert runs do not match its token count";
+    }
+    return nullptr;
+}
+
 int pt_batch_upload_runs(pt_batch* b, const pt_packed_runs* rr) {
     if (!b || !rr || (rr->n_logs && (!rr->logs || !rr->run_off || !rr->tok_off))) return PT_ERR_INVALID;
+    if (const char* err = check_run_table(*rr)) { g_last_error = err; return PT_ERR_INVALID; }
     int rc = begin_upload(b, pt_packed_ops{rr->n_logs, rr->logs, nullptr, rr->n_insdel_total, nullptr, rr->n_mark_total}, true);
     if (rc) return rc;
     const size_t nl = rr->n_logs;
@@ -844,32 +869,51 @@ int pt_compact_ops(const pt_packed_ops* ops, pt_insdel_c8* io, pt_mark_c16* mo, 
         const pt_log_desc& L = ops->logs[i];
         if (L.max_ctr >= 65536u || L.n_insdel >= 65536u || L.n_actors > 16u) { g_last_error = "log not representable in the compact wire format"; return PT_ERR_INVALID; }
     }
+    // Every field is checked against its compact width: a record that names a counter or actor outside the log's bounds
+    // (a faulty log) would otherwise be truncated into a valid-looking one and merge where the plain form reports it.
+    static const char* const kField[] = {"value token", "insert/delete ctr", "insert/delete ref_ctr", "insert/delete actor",
+                                          "insert/delete ref_actor", "mark ctr", "mark start_ctr", "mark end_ctr", "mark arrival",
+                                          "mark actor", "mark start_actor", "mark end_actor", "mark kind", "mark bounds"};
     int T = threads > 0 ? threads : (int)std::max(1u, std::thread::hardware_concurrency());
-    std::atomic<int> bad{0};
+    std::atomic<uint32_t> bad{0};      // bit f: some record's field kField[f] does not fit
     auto work = [&](int t) {
+        // OR of every record's value per field: a field fits iff its OR does (widths are powers of two)
+        uint32_t o_val = 0, o_ctr = 0, o_ref = 0, o_act = 0, o_ref_act = 0;
         const uint64_t n = ops->n_insdel_total, a = n * t / T, b2 = n * (t + 1) / T;
         for (uint64_t k = a; k < b2; k++) {
             const pt_insdel_rec& r = ops->insdel[k];
             const uint32_t tok = PT_PAYLOAD_TOKEN(r.payload), val = tok & (PT_TOKEN_POOLED - 1);
-            if (val >= 0x200000u) bad = 1;
+            o_val |= val; o_ctr |= r.ctr; o_ref |= r.ref_ctr; o_act |= r.actor; o_ref_act |= r.ref_actor;
             pt_insdel_c8 o; o.ctr = (uint16_t)r.ctr; o.ref_ctr = (uint16_t)r.ref_ctr;
             o.w = (r.actor & 0xFu) | ((r.ref_actor & 0xFu) << 4) | (PT_PAYLOAD_KIND(r.payload) << 8) | (((tok & PT_TOKEN_POOLED ? 0x200000u : 0u) | (val & 0x1FFFFFu)) << 10);
             io[k] = o;
         }
+        uint32_t m_ctr = 0, m_start = 0, m_end = 0, m_arr = 0, m_act = 0, m_sact = 0, m_eact = 0, m_kind = 0, m_bounds = 0;
         const uint64_t m = ops->n_mark_total, c = m * t / T, d = m * (t + 1) / T;
         for (uint64_t k = c; k < d; k++) {
             const pt_mark_rec& r = ops->marks[k];
-            if (r.arrival >= 65536u) bad = 1;
+            m_ctr |= r.ctr; m_start |= r.start_ctr; m_end |= r.end_ctr; m_arr |= r.arrival;
+            m_act |= r.actor; m_sact |= r.start_actor; m_eact |= r.end_actor; m_kind |= r.kind; m_bounds |= r.bounds;
             pt_mark_c16 o; o.ctr = (uint16_t)r.ctr; o.start_ctr = (uint16_t)r.start_ctr; o.end_ctr = (uint16_t)r.end_ctr; o.arrival = (uint16_t)r.arrival; o.attr = r.attr;
             o.w = (r.actor & 0xFu) | ((r.start_actor & 0xFu) << 4) | ((r.end_actor & 0xFu) << 8) | ((r.kind & 7u) << 12) | ((r.bounds & 0xFu) << 15);
             mo[k] = o;
         }
+        const uint32_t mask = (o_val >= 0x200000u) | (o_ctr >= 65536u) << 1 | (o_ref >= 65536u) << 2 | (o_act >= 16u) << 3 | (o_ref_act >= 16u) << 4 |
+                              (m_ctr >= 65536u) << 5 | (m_start >= 65536u) << 6 | (m_end >= 65536u) << 7 | (m_arr >= 65536u) << 8 |
+                              (m_act >= 16u) << 9 | (m_sact >= 16u) << 10 | (m_eact >= 16u) << 11 | (m_kind >= 8u) << 12 | (m_bounds >= 16u) << 13;
+        if (mask) bad.fetch_or(mask);
     };
     std::vector<std::thread> th;
     for (int t = 1; t < T; t++) th.emplace_back(work, t);
     work(0);
     for (auto& x : th) x.join();
-    if (bad) { g_last_error = "value token or arrival index not representable in the compact wire format"; return PT_ERR_INVALID; }
+    if (const uint32_t m = bad.load()) {
+        std::string names;
+        for (uint32_t f = 0; f < sizeof(kField) / sizeof(kField[0]); f++)
+            if (m >> f & 1u) names += (names.empty() ? "" : ", ") + std::string(kField[f]);
+        g_last_error = "not representable in the compact wire format: " + names;
+        return PT_ERR_INVALID;
+    }
     return PT_OK;
 }
 

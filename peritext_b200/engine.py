@@ -49,9 +49,10 @@ class PackedRuns:
     """Run-compressed wire form of a PackedBatch (include/peritext_b200.h pt_packed_runs): typing runs and consecutive
     deletes collapse to one 16-byte run record (+ 4 bytes per inserted value)."""
 
-    def __init__(self, desc, run_off, tok_off, runs, tokens, marks, n_insdel_total):
+    def __init__(self, desc, run_off, tok_off, runs, tokens, marks, n_insdel_total, changes: ChangeTable | None = None):
         self.desc, self.run_off, self.tok_off, self.runs, self.tokens, self.marks = desc, run_off, tok_off, runs, tokens, marks
         self.n_insdel_total = int(n_insdel_total)
+        self.changes = changes        # the batch's change table (admission pre-pass), if it has one
 
     @property
     def n_logs(self) -> int:
@@ -72,7 +73,8 @@ class PackedRuns:
             d["insdel_off"] -= i0; d["mark_off"] -= m0
         else:
             i0 = i1 = m0 = m1 = 0
-        return PackedRuns(d, ro - ro[0], to - to[0], self.runs[r0:r1], self.tokens[t0:t1], self.marks[m0:m1], i1 - i0)
+        return PackedRuns(d, ro - ro[0], to - to[0], self.runs[r0:r1], self.tokens[t0:t1], self.marks[m0:m1], i1 - i0,
+                          self.changes.slice_logs(a, b) if self.changes is not None else None)
 
 
 def compress_runs(batch: PackedBatch, pin=None) -> PackedRuns:
@@ -89,7 +91,8 @@ def compress_runs(batch: PackedBatch, pin=None) -> PackedRuns:
     alloc = pin or (lambda a: a)
     runs = alloc(np.zeros(max(1, nr.value), RUN_DT)); tokens = alloc(np.zeros(max(1, nt.value), np.uint32))
     _check(L.pt_compress_runs(ctypes.byref(ops), run_off.ctypes.data, tok_off.ctypes.data, runs.ctypes.data, tokens.ctypes.data, ctypes.byref(nr), ctypes.byref(nt)), "pt_compress_runs")
-    return PackedRuns(desc, alloc(run_off), alloc(tok_off), runs[: nr.value], tokens[: nt.value], alloc(marks) if pin else marks, len(insdel))
+    return PackedRuns(desc, alloc(run_off), alloc(tok_off), runs[: nr.value], tokens[: nt.value], alloc(marks) if pin else marks, len(insdel),
+                      batch.changes)
 
 
 class _ChangeTable(ctypes.Structure):
@@ -197,7 +200,13 @@ class BatchEngine:
         lim = _Limits(comment_pool_entries, flags, 0, (ctypes.c_uint32 * 4)())
         _check(L.pt_batch_create(device, ctypes.byref(lim), ctypes.c_void_p(stream or 0), ctypes.byref(self._h)), "pt_batch_create")
         self._keep = None
-        self.n_logs = 0
+        self._uploaded(np.zeros(0, DESC_DT), 0)
+
+    def _uploaded(self, desc, n_insdel_total):
+        """Record the shape of the batch just uploaded, in whichever form: what the downloads size their views by."""
+        self.n_logs = len(desc)
+        self._n_insdel = int(n_insdel_total)                                 # patch records: one per ins/del record
+        self._n_seq = int(desc["n_insdel"].astype(np.uint64).sum())          # element sequences: the capacity layout
 
     def _ops_struct(self, desc, insdel_ptr, n_insdel, marks_ptr, n_mark):
         return _PackedOps(len(desc), desc.ctypes.data, insdel_ptr, n_insdel, marks_ptr, n_mark)
@@ -208,8 +217,7 @@ class BatchEngine:
         marks = np.ascontiguousarray(batch.marks)
         ops = self._ops_struct(desc, insdel.ctypes.data, len(insdel), marks.ctypes.data, len(marks))
         _check(self._L.pt_batch_upload(self._h, ctypes.byref(ops)), "pt_batch_upload")
-        self.n_logs = len(desc)
-        self._n_insdel = len(insdel)
+        self._uploaded(desc, len(insdel))
 
     def upload_changes(self, table: ChangeTable):
         """Attach the batch's change table: the next merge runs the admission pre-pass (seq / deps checks of
@@ -232,8 +240,7 @@ class BatchEngine:
         cc = _PackedOps(len(desc), desc.ctypes.data, cins.ctypes.data, len(insdel), cmarks.ctypes.data, len(marks))     # same field layout as pt_packed_compact
         self._keep = (desc, cins, cmarks)
         _check(self._L.pt_batch_upload_compact(self._h, ctypes.byref(cc)), "pt_batch_upload_compact")
-        self.n_logs = len(desc)
-        self._n_insdel = len(insdel)
+        self._uploaded(desc, len(insdel))
 
     def upload_runs(self, r: PackedRuns):
         desc = np.ascontiguousarray(r.desc)
@@ -241,14 +248,14 @@ class BatchEngine:
                          r.tokens.ctypes.data if len(r.tokens) else 0, r.marks.ctypes.data if len(r.marks) else 0, r.n_insdel_total, len(r.marks))
         self._keep = (desc, r)
         _check(self._L.pt_batch_upload_runs(self._h, ctypes.byref(st)), "pt_batch_upload_runs")
-        self.n_logs = len(desc)
+        self._uploaded(desc, r.n_insdel_total)
 
     def adopt_device(self, desc: np.ndarray, insdel_dev_ptr: int, n_insdel: int, marks_dev_ptr: int, n_mark: int):
         """Use op arrays already resident in device memory (e.g. ``tensor.data_ptr()``); caller keeps them alive."""
         desc = np.ascontiguousarray(desc)
         ops = self._ops_struct(desc, insdel_dev_ptr, n_insdel, marks_dev_ptr, n_mark)
         _check(self._L.pt_batch_adopt_device(self._h, ctypes.byref(ops)), "pt_batch_adopt_device")
-        self.n_logs = len(desc)
+        self._uploaded(desc, n_insdel)
 
     def merge(self):
         _check(self._L.pt_batch_merge(self._h), "pt_batch_merge")
@@ -300,7 +307,7 @@ class BatchEngine:
         span_off = arr(v.span_off, n + 1, np.uint64)
         n_text, n_span = int(text_off[-1]), int(span_off[-1])
         seq_off = arr(v.seq_off, n, np.uint64) if (n and v.seq) else None
-        n_seq = (int(seq_off[-1]) + int(results[-1]["n_elems"])) if seq_off is not None else 0
+        n_seq = self._n_seq if seq_off is not None else 0      # (a failed log's n_elems is no element count)
         self.comment_pool_needed = int(v.comment_pool_needed)
         self.comment_pool_used = int(v.comment_pool_used)
         return MergedBatch(results, text_off, span_off, arr(v.text, n_text, np.uint32), arr(v.spans, n_span, SPAN_DT),
@@ -415,10 +422,15 @@ class BatchEngine:
         self.upload(batch)
         if getattr(batch, "changes", None) is not None:
             self.upload_changes(batch.changes)
-        self.merge(); out = self.download()
+        self.merge()
+        return self._download_with_pool_retry()
+
+    def _download_with_pool_retry(self, copy: bool = True) -> MergedBatch:
+        """download, and if some log overflowed the comment pool (status 4), one re-merge with a pool of the reported demand."""
+        out = self.download(copy=copy)
         if len(out.results) and (out.results["status"] == 4).any() and self.comment_pool_needed > self.comment_pool_used:
             self.set_comment_pool(self.comment_pool_needed + 16)
-            self.merge(); out = self.download()
+            self.merge(); out = self.download(copy=copy)
         return out
 
     def close(self):
@@ -460,7 +472,8 @@ class PipelinedEngine:
     def run(self, batch, copy: bool = False, compact: bool = False, threads: int = 0) -> list[MergedBatch]:
         """`batch`: a PackedBatch, or a PackedRuns (run-compressed upload).  `compact`: convert every chunk to the compact wire
         format on the host (multithreaded, inside this call) and upload half the bytes; chunk k+1's conversion overlaps
-        chunk k's transfer."""
+        chunk k's transfer.  Like ``BatchEngine.run``, each chunk's change table is attached (admission) and a chunk whose
+        comments overflow the default pool is merged once more with a pool of its reported demand."""
         n = batch.n_logs
         # cut by records, not by log count, so the chunks carry similar work
         w = np.cumsum(batch.desc["n_insdel"].astype(np.int64) + 2 * batch.desc["n_mark"].astype(np.int64))
@@ -476,8 +489,10 @@ class PipelinedEngine:
                 e.upload_compact(sb, ci, cm, threads)
             else:
                 e.upload(sb)
+            if sb.changes is not None:
+                e.upload_changes(sb.changes)
             e.merge(); e.download_begin()
-        return [e.download(copy=copy) for e in used]
+        return [e._download_with_pool_retry(copy=copy) for e in used]
 
     def close(self):
         for e in self.engines:

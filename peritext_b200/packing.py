@@ -101,14 +101,16 @@ class PackedBatch:
     def slice_logs(self, a: int, b: int) -> "PackedBatch":
         """Logs [a, b) as VIEWS of this batch's arrays (no copy: pinned host memory stays pinned); offsets re-based."""
         d = self.desc[a:b].copy()
+        changes = self.changes.slice_logs(a, b) if self.changes is not None else None
         if len(d) == 0:
-            return PackedBatch(d, self.insdel[:0], self.marks[:0], self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta))
+            return PackedBatch(d, self.insdel[:0], self.marks[:0], self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta),
+                               changes=changes)
         i0, m0 = int(d[0]["insdel_off"]), int(d[0]["mark_off"])
         i1 = int(d[-1]["insdel_off"]) + int(d[-1]["n_insdel"]); m1 = int(d[-1]["mark_off"]) + int(d[-1]["n_mark"])
         d["insdel_off"] -= i0; d["mark_off"] -= m0
         return PackedBatch(d, self.insdel[i0:i1], self.marks[m0:m1], self.values, self.link_attrs, self.comment_ids, self.other_attrs,
                            dict(self.meta), self.log_actors[a:b] if self.log_actors else [],
-                           self.log_counters[a:b] if self.log_counters else [])
+                           self.log_counters[a:b] if self.log_counters else [], changes)
 
     def select(self, idx: Sequence[int]) -> "PackedBatch":
         """Sub-batch with the given logs (re-based offsets); pools are shared."""
@@ -124,7 +126,8 @@ class PackedBatch:
             io += len(a); mo += len(b)
         ins = np.concatenate(ins_parts) if ins_parts else np.zeros(0, INSDEL_DT)
         mk = np.concatenate(mk_parts) if mk_parts else np.zeros(0, MARK_DT)
-        return PackedBatch(desc, ins, mk, self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta))
+        return PackedBatch(desc, ins, mk, self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta),
+                           changes=self.changes.select(idx) if self.changes is not None else None)
 
     def algorithmic_bytes(self, results: np.ndarray | None = None) -> int:
         """SURVEY.md §8(d): 16 B per ins/del + 32 B per mark read; 4 B per visible element, 16 B per span and
@@ -142,6 +145,28 @@ class ChangeTable:
     desc: np.ndarray      # CDESC_DT [n_logs]
     changes: np.ndarray   # CHANGE_DT
     deps: np.ndarray      # DEP_DT
+
+    def slice_logs(self, a: int, b: int) -> "ChangeTable":
+        """Logs [a, b) as views of the change and dep arrays; offsets re-based (a change's dep_off is relative to its log)."""
+        d = self.desc[a:b].copy()
+        if len(d) == 0:
+            return ChangeTable(d, self.changes[:0], self.deps[:0])
+        c0, p0 = int(d[0]["change_off"]), int(d[0]["dep_off"])
+        c1 = int(d[-1]["change_off"]) + int(d[-1]["n_changes"]); p1 = int(d[-1]["dep_off"]) + int(d[-1]["n_deps"])
+        d["change_off"] -= c0; d["dep_off"] -= p0
+        return ChangeTable(d, self.changes[c0:c1], self.deps[p0:p1])
+
+    def select(self, idx: Sequence[int]) -> "ChangeTable":
+        """The tables of the given logs, in that order (copies; offsets re-based)."""
+        parts = [self.slice_logs(i, i + 1) for i in idx]
+        desc = np.zeros(len(parts), CDESC_DT)
+        co = do = 0
+        for k, t in enumerate(parts):
+            desc[k] = t.desc[0]
+            desc[k]["change_off"] = co; desc[k]["dep_off"] = do
+            co += len(t.changes); do += len(t.deps)
+        return ChangeTable(desc, np.concatenate([t.changes for t in parts] + [self.changes[:0]]),
+                           np.concatenate([t.deps for t in parts] + [self.deps[:0]]))
 
 
 class _LogBuilder:
