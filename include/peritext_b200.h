@@ -342,6 +342,62 @@ int pt_batch_upload_compact(pt_batch*, const pt_packed_compact* host_compact);
  * caller, e.g. torch tensors); only the descriptors are read on the host. */
 int pt_batch_adopt_device(pt_batch*, const pt_packed_ops* host_desc_device_arrays);
 
+/* ------------------------------------------------------------------------------------------------
+ * Append: extend every log of the resident batch with new records on the device, so that a re-merge after a few new
+ * changes (Micromerge.applyChange on a document that already exists, src/micromerge.ts:499) uploads only what is new.
+ * After a successful append the handle holds exactly the batch an upload of the concatenated logs would hold: logs
+ * contiguous and in order, each with its old records first and then its delta records; the same descriptors, plan and
+ * change table.
+ *
+ * Three packed id spaces carry an ORDER, and new changes can move every existing id in them: the per-log actor rank
+ * (a new actor that sorts before the old ones), the per-log dense counter rank (where the packer re-ranked sparse
+ * counters; a log can also switch between dense and plain counters as it grows) and the per-batch comment rank.  The
+ * remap says how the resident records' ids move; value-pool indices and link attr ids carry no order and never move.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_append_remap {      /* NULL pointer = identity everywhere */
+    const uint64_t* actor_off;        /* [n_logs + 1] or NULL: log i's map is actor_map[actor_off[i] .. actor_off[i+1]),
+                                         old rank -> new rank; empty = identity, else exactly the log's old n_actors
+                                         entries, strictly increasing                                                   */
+    const uint16_t* actor_map;
+    const uint64_t* ctr_off;          /* [n_logs + 1] or NULL: log i's map is ctr_map[ctr_off[i] .. ctr_off[i+1]), old
+                                         ctr -> new ctr; empty = identity, else at least old max_ctr + 1 entries (more
+                                         where a record names a counter past max_ctr, e.g. a mark boundary on an element
+                                         inserted later), entry 0 = 0 (HEAD), strictly increasing over the entries that are not
+                                         0xFFFFFFFF; 0xFFFFFFFF marks an old counter that no record of the log names
+                                         (a plain log turning dense: the dense ranks leave no room for unused values)   */
+    const uint32_t* ctr_map;
+    const uint32_t* comment_map;      /* old comment rank -> new rank, n_comment_map entries, strictly increasing;
+                                         NULL = identity                                                                */
+    uint64_t n_comment_map;
+} pt_append_remap;
+
+/* Append `delta` to the resident batch.  The delta has the batch's n_logs; descriptor i indexes the delta's own arrays and
+ * counts only log i's NEW records (zero is allowed); its n_actors / max_ctr are the log's values AFTER the append.  Delta
+ * records are already in the new id space.  A delta mark's arrival counts the ins/del records of the whole log, so it lies
+ * in [old n_insdel, old n_insdel + delta n_insdel].  delta_changes is the change table of the new changes (NULL iff the
+ * handle has no change table); a delta change record's dep_off is relative to its delta log's deps (the engine rebases it).
+ * Resident records: actor ranks go through the log's actor map, counters (ctr, ref_ctr, start_ctr, end_ctr) through its
+ * counter map, and the attr of a comment mark through the comment map.  An id whose counter is 0 (HEAD, start / end of
+ * text) keeps its actor field.  A resident value outside its map's domain (actor >= old n_actors, ctr > old max_ctr) or
+ * mapped to 0xFFFFFFFF becomes 0xFFFF / 0xFFFFFFFF, so a faulty log still fails at merge; identity maps copy verbatim.  The
+ * change table is concatenated per log, and the old change and dep records' actor ranks go through the actor maps.
+ * Refused before anything changes (PT_ERR_INVALID, pt_last_error names the problem): n_logs differs; a map has the wrong
+ * length or is not strictly increasing; ctr_map[0] != 0; a mapped old bound (identity included; for the counter map, the
+ * image of the old max_ctr) exceeds the new n_actors / max_ctr; a delta descriptor or arrival is out of range; a log would exceed 2^32 - 1 records; a change table on one side
+ * only.  No batch: PT_ERR_STATE.  The device refuses too: a resident comment rank (other than PT_ATTR_NONE) outside
+ * comment_map gives PT_ERR_INVALID with the batch untouched, because the splice writes new record buffers and only a
+ * successful one replaces the old.
+ * On success: the batch is re-planned like an upload (routes, capacities and the patch kernel's shared memory can change),
+ * there is no merge (views of the last merge are invalid, as after an upload), comment-pool and patch-pool settings persist
+ * as across uploads, and the records are engine-owned, also after pt_batch_adopt_device (whose arrays it only reads).
+ * Synchronises; the caller's arrays may be freed on return.
+ * Device: one warp per log (up to 64 for a log with many records) copies the old records with coalesced 16-byte accesses,
+ * applying the log's maps (a log with identity maps is a straight copy), then the delta records; a second warp-per-log
+ * kernel splices the change and dep tables.  Peak device memory during the call: old + delta + new records (and change
+ * tables).  The delta, remap and change-table copies on the device are freed on return; the handle keeps only the new
+ * batch. */
+int pt_batch_append(pt_batch*, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* delta_changes);
+
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */
 int pt_batch_merge(pt_batch*);

@@ -19,6 +19,7 @@
 #include "team_kernel.cuh"
 #include "render_kernel.cuh"
 #include "patch_json_kernel.cuh"
+#include "append_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -43,6 +44,7 @@ struct Buf {
     Buf& operator=(const Buf&) = delete;
     ~Buf() { release(); }
     void release() { if (p) { if (kPinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
+    void swap(Buf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
     int reserve(size_t bytes) {
         if (bytes <= cap) return PT_OK;
         release();
@@ -428,6 +430,8 @@ struct pt_batch {
     DevBuf d_desc, d_insdel, d_marks, d_order, d_counters, d_results, d_text_off, d_span_off, d_text, d_spans, d_pool, d_slab, d_retry, d_seq;
     DevBuf d_bsum, d_ctoff, d_csoff, d_ctext, d_cspans;   // download path: packed outputs + their offsets ([n_logs + 1])
     DevBuf d_cdesc, d_changes, d_deps, d_admit;           // admission pre-pass (optional change table)
+    std::vector<pt_change_desc> h_cdesc;                 // its descriptors, and its totals
+    uint64_t n_changes = 0, n_deps = 0;
     DevBuf d_patch_recs, d_patch_items, d_patch_status;   // PT_FLAG_EMIT_PATCHES
     HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc;
     DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // both JSON renders: the caller's pools
@@ -591,16 +595,13 @@ int launch_bin(pt_batch* b, int k, const ptk::BatchParams& P, bool retry) {
     }
 }
 
-// Shared start of every upload: the staging buffer and the device arrays of the previous batch are reused, so wait for
-// it; then plan the new batch and allocate for it (own_records: the engine keeps its own copy of the records).
-int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
-    PT_CUDA(cudaSetDevice(b->device));
-    PT_CUDA(cudaStreamSynchronize(b->stream));
-    b->have_batch = false; b->merged = false; b->dl_begun = false; b->have_changes = false;
-    drop_graph(b);
+// Makes `plan` (made by ptp::make_plan from `ops`) the handle's batch: its shape, descriptors, per-log arrays and output
+// buffers (own_records: the engine keeps its own copy of the records and allocates for them).  Every upload and
+// pt_batch_append end their planning here.
+int install_plan(pt_batch* b, const pt_packed_ops& ops, ptp::Plan&& plan, bool own_records) {
     b->n_logs = ops.n_logs; b->n_insdel = ops.n_insdel_total; b->n_mark = ops.n_mark_total;
     b->h_desc.assign(ops.logs, ops.logs + ops.n_logs);
-    if (const char* err = ptp::make_plan(ops, b->limits, b->num_sms, b->plan)) { g_last_error = err; return PT_ERR_INVALID; }
+    b->plan = std::move(plan);
     int rc;
     if ((rc = alloc_and_upload_plan(b))) return rc;
     if (own_records) {
@@ -608,6 +609,18 @@ int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
         if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
     }
     return PT_OK;
+}
+
+// Shared start of every upload: the staging buffer and the device arrays of the previous batch are reused, so wait for
+// it; then plan the new batch and allocate for it.
+int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    b->have_batch = false; b->merged = false; b->dl_begun = false; b->have_changes = false;
+    drop_graph(b);
+    ptp::Plan plan;
+    if (const char* err = ptp::make_plan(ops, b->limits, b->num_sms, plan)) { g_last_error = err; return PT_ERR_INVALID; }
+    return install_plan(b, ops, std::move(plan), own_records);
 }
 
 // Shared finish: the records the merge reads, and a wait for the copies when one of the caller's sources (pointer, bytes
@@ -963,8 +976,183 @@ int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
     if (t->n_changes_total) PT_CUDA(cudaMemcpyAsync(b->d_changes.p, t->changes, t->n_changes_total * sizeof(pt_change_rec), cudaMemcpyHostToDevice, b->stream));
     if (t->n_deps_total) PT_CUDA(cudaMemcpyAsync(b->d_deps.p, t->deps, t->n_deps_total * sizeof(pt_dep_rec), cudaMemcpyHostToDevice, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));            // the caller's arrays may be freed on return
+    b->h_cdesc.assign(t->logs, t->logs + n); b->n_changes = t->n_changes_total; b->n_deps = t->n_deps_total;
     b->adm_maxR = maxR; b->have_changes = true;
     drop_graph(b);                                       // the launch sequence changes
+    return PT_OK;
+}
+
+// Host checks of a delta and its remap against the resident batch (include/peritext_b200.h, pt_batch_append); on success
+// nd / ncd hold the descriptors of the concatenated batch and its change table.  Returns the problem, or an empty string.
+static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, const pt_append_remap& R, const pt_change_table* dch,
+                                std::vector<pt_log_desc>& nd, std::vector<pt_change_desc>& ncd, uint32_t& maxR) {
+    const uint32_t n = b->n_logs;
+    auto at = [](uint32_t i) { return "log " + std::to_string(i) + ": "; };
+    if (delta.n_logs != n) return "the delta has " + std::to_string(delta.n_logs) + " logs and the batch " + std::to_string(n);
+    if ((dch != nullptr) != b->have_changes)
+        return b->have_changes ? "the batch has a change table and the delta none" : "the delta has a change table and the batch none";
+    if ((delta.n_insdel_total && !delta.insdel) || (delta.n_mark_total && !delta.marks)) return "null delta records with a nonzero count";
+    if ((R.actor_off && R.actor_off[n] > R.actor_off[0] && !R.actor_map) || (R.ctr_off && R.ctr_off[n] > R.ctr_off[0] && !R.ctr_map) ||
+        (R.n_comment_map && !R.comment_map)) return "null map with a nonzero length";
+    for (uint64_t k = 1; R.comment_map && k < R.n_comment_map; k++)
+        if (R.comment_map[k] <= R.comment_map[k - 1]) return "comment_map is not strictly increasing";
+    nd.resize(n);
+    uint64_t io = 0, mo = 0;
+    maxR = 1;
+    for (uint32_t i = 0; i < n; i++) {
+        const pt_log_desc &O = b->h_desc[i], &D = delta.logs[i];
+        if (D.insdel_off + D.n_insdel > delta.n_insdel_total || D.mark_off + D.n_mark > delta.n_mark_total) return at(i) + "delta descriptor out of range";
+        if ((uint64_t)O.n_insdel + D.n_insdel > 0xFFFFFFFFull || (uint64_t)O.n_mark + D.n_mark > 0xFFFFFFFFull) return at(i) + "more than 2^32 - 1 records";
+        const uint64_t na = R.actor_off ? R.actor_off[i + 1] - R.actor_off[i] : 0, nc = R.ctr_off ? R.ctr_off[i + 1] - R.ctr_off[i] : 0;
+        if (R.actor_off && R.actor_off[i + 1] < R.actor_off[i]) return "actor_off decreases";
+        if (R.ctr_off && R.ctr_off[i + 1] < R.ctr_off[i]) return "ctr_off decreases";
+        if (na) {
+            const uint16_t* a = R.actor_map + R.actor_off[i];
+            if (na != O.n_actors) return at(i) + "the actor map has " + std::to_string(na) + " entries and the log had " + std::to_string(O.n_actors) + " actors";
+            for (uint64_t k = 1; k < na; k++) if (a[k] <= a[k - 1]) return at(i) + "the actor map is not strictly increasing";
+            if (a[na - 1] >= D.n_actors) return at(i) + "the actor map names a rank >= the new n_actors";
+        } else if (O.n_actors > D.n_actors) {
+            return at(i) + "the new n_actors is below the old (identity actor map)";
+        }
+        if (nc) {
+            const uint32_t* c = R.ctr_map + R.ctr_off[i];
+            if (nc <= (uint64_t)O.max_ctr) return at(i) + "the counter map has " + std::to_string(nc) + " entries and the log's old max_ctr is " + std::to_string(O.max_ctr);
+            if (c[0] != 0) return at(i) + "ctr_map[0] is not 0";
+            uint32_t last = 0, bound = 0;         // bound: the image of the old max_ctr (the last mapped entry up to it)
+            for (uint64_t k = 1; k < nc; k++) {
+                if (c[k] == 0xFFFFFFFFu) continue;
+                if (c[k] <= last) return at(i) + "the counter map is not strictly increasing";
+                last = c[k];
+                if (k <= O.max_ctr) bound = c[k];
+            }
+            if (bound > D.max_ctr) return at(i) + "the counter map sends the old max_ctr past the new max_ctr";
+        } else if (O.max_ctr > D.max_ctr) {
+            return at(i) + "the new max_ctr is below the old (identity counter map)";
+        }
+        for (uint32_t k = 0; k < D.n_mark; k++) {
+            const uint32_t a = delta.marks[D.mark_off + k].arrival;
+            if (a < O.n_insdel || a > (uint64_t)O.n_insdel + D.n_insdel) return at(i) + "delta mark " + std::to_string(k) + " has arrival " + std::to_string(a) +
+                                                                                 " outside [" + std::to_string(O.n_insdel) + ", " + std::to_string((uint64_t)O.n_insdel + D.n_insdel) + "]";
+        }
+        nd[i] = pt_log_desc{io, mo, O.n_insdel + D.n_insdel, O.n_mark + D.n_mark, D.n_actors, D.max_ctr};
+        io += nd[i].n_insdel; mo += nd[i].n_mark;
+        maxR = std::max<uint32_t>(maxR, D.n_actors);
+    }
+    if (dch) {
+        if (dch->n_logs != n || (n && !dch->logs)) return "the delta's change table does not match the batch";
+        if ((dch->n_changes_total && !dch->changes) || (dch->n_deps_total && !dch->deps)) return "null delta change records with a nonzero count";
+        if ((size_t)2 * maxR * 4 > 200 * 1024) return "more than 25600 actors in one log: not supported by the admission pre-pass";
+        ncd.resize(n);
+        uint64_t co = 0, po = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            const pt_change_desc &O = b->h_cdesc[i], &D = dch->logs[i];
+            if (D.change_off + D.n_changes > dch->n_changes_total || D.dep_off + D.n_deps > dch->n_deps_total) return at(i) + "delta change descriptor out of range";
+            if ((uint64_t)O.n_changes + D.n_changes > 0xFFFFFFFFull || (uint64_t)O.n_deps + D.n_deps > 0xFFFFFFFFull) return at(i) + "more than 2^32 - 1 changes or deps";
+            ncd[i] = pt_change_desc{co, po, O.n_changes + D.n_changes, O.n_deps + D.n_deps};
+            co += ncd[i].n_changes; po += ncd[i].n_deps;
+        }
+    }
+    return std::string();
+}
+
+int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* dch) {
+    if (!b || !delta || (delta->n_logs && !delta->logs)) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_append before pt_batch_upload"; return PT_ERR_STATE; }
+    const pt_append_remap R = remap ? *remap : pt_append_remap{};
+    std::vector<pt_log_desc> nd;
+    std::vector<pt_change_desc> ncd;
+    uint32_t maxR = 1;
+    std::string err = check_append(b, *delta, R, dch, nd, ncd, maxR);
+    const uint32_t n = b->n_logs;
+    const bool sized = err.empty() && n;                      // nd is filled only when the checks passed
+    const uint64_t n_ins = sized ? nd[n - 1].insdel_off + nd[n - 1].n_insdel : 0, n_mk = sized ? nd[n - 1].mark_off + nd[n - 1].n_mark : 0;
+    const pt_packed_ops ops{n, nd.data(), nullptr, n_ins, nullptr, n_mk};
+    ptp::Plan plan;
+    if (err.empty()) if (const char* e = ptp::make_plan(ops, b->limits, b->num_sms, plan)) err = e;
+    if (!err.empty()) { g_last_error = "pt_batch_append: " + err; return PT_ERR_INVALID; }
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge and downloads of the resident batch are done
+    // The delta and the remap go to the device; the splice writes NEW buffers, so the resident batch stays intact until the
+    // device has accepted every record.
+    int rc;
+    const size_t dsz = std::max<size_t>(1, n) * sizeof(pt_log_desc);
+    DevBuf ndesc, nins, nmarks, ncdesc, nch, ndp;              // the new batch's descriptors, records and change table
+    DevBuf ddesc, dins, dmarks, dcdesc, dchg, ddep, amap[5], abad;   // the delta, its remap and the refusal flag: freed on return
+    if ((rc = ddesc.reserve(dsz)) || (rc = ndesc.reserve(dsz)) || (rc = abad.reserve(4)) ||
+        (rc = dins.reserve(std::max<uint64_t>(1, delta->n_insdel_total) * sizeof(pt_insdel_rec))) ||
+        (rc = dmarks.reserve(std::max<uint64_t>(1, delta->n_mark_total) * sizeof(pt_mark_rec))) ||
+        (rc = nins.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = nmarks.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec)))) return rc;
+    auto h2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
+    PT_CUDA(h2d(ddesc.p, delta->logs, (size_t)n * sizeof(pt_log_desc)));
+    PT_CUDA(h2d(ndesc.p, nd.data(), (size_t)n * sizeof(pt_log_desc)));
+    PT_CUDA(h2d(dins.p, delta->insdel, delta->n_insdel_total * sizeof(pt_insdel_rec)));
+    PT_CUDA(h2d(dmarks.p, delta->marks, delta->n_mark_total * sizeof(pt_mark_rec)));
+    pta::Remap DR{};
+    const void* hsrc[5] = {R.actor_off, R.actor_map, R.ctr_off, R.ctr_map, R.comment_map};
+    const size_t hbytes[5] = {R.actor_off ? ((size_t)n + 1) * 8 : 0, R.actor_off ? (size_t)R.actor_off[n] * 2 : 0,
+                              R.ctr_off ? ((size_t)n + 1) * 8 : 0, R.ctr_off ? (size_t)R.ctr_off[n] * 4 : 0, R.comment_map ? (size_t)R.n_comment_map * 4 : 0};
+    const void* dptr[5] = {};
+    for (int k = 0; k < 5; k++) {
+        if (!hsrc[k]) continue;
+        if ((rc = amap[k].reserve(std::max<size_t>(16, hbytes[k])))) return rc;
+        PT_CUDA(h2d(amap[k].p, hsrc[k], hbytes[k]));
+        dptr[k] = amap[k].p;
+    }
+    DR.actor_off = (const unsigned long long*)dptr[0]; DR.actor_map = (const uint16_t*)dptr[1];
+    DR.ctr_off = (const unsigned long long*)dptr[2]; DR.ctr_map = (const uint32_t*)dptr[3];
+    DR.comment_map = (const uint32_t*)dptr[4]; DR.n_comment = R.comment_map ? R.n_comment_map : 0;
+    PT_CUDA(cudaMemsetAsync(abad.p, 0, 4, b->stream));
+    const uint32_t threads = 128, grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16));
+    if (n) {
+        // a log with many records gets up to 64 warps, one per slice (8 K records per slice): few huge logs (c5) must not
+        // leave the copy to a handful of warps
+        uint64_t most = 0;
+        for (uint32_t i = 0; i < n; i++) most = std::max<uint64_t>(most, (uint64_t)nd[i].n_insdel + 2ull * nd[i].n_mark);
+        const uint32_t slices = (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, most / 8192));
+        const dim3 rgrid(std::max<uint32_t>(1, std::min<uint32_t>(grid, (uint32_t)b->num_sms * 16 / slices)), slices);
+        pta::splice_records_kernel<<<rgrid, threads, 0, b->stream>>>((const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, n, DR,
+                                                                    b->dp_insdel, b->dp_marks, (const pt_insdel_rec*)dins.p, (const pt_mark_rec*)dmarks.p,
+                                                                    (pt_insdel_rec*)nins.p, (pt_mark_rec*)nmarks.p, (uint32_t*)abad.p);
+        PT_CUDA(cudaGetLastError());
+        b->launches++;
+    }
+    uint64_t n_ch = 0, n_dp = 0;
+    if (dch) {
+        n_ch = n ? ncd[n - 1].change_off + ncd[n - 1].n_changes : 0; n_dp = n ? ncd[n - 1].dep_off + ncd[n - 1].n_deps : 0;
+        const size_t csz = std::max<size_t>(1, n) * sizeof(pt_change_desc);
+        if ((rc = dcdesc.reserve(csz)) || (rc = ncdesc.reserve(csz)) ||
+            (rc = dchg.reserve(std::max<uint64_t>(1, dch->n_changes_total) * sizeof(pt_change_rec))) ||
+            (rc = ddep.reserve(std::max<uint64_t>(1, dch->n_deps_total) * sizeof(pt_dep_rec))) ||
+            (rc = nch.reserve(std::max<uint64_t>(1, n_ch) * sizeof(pt_change_rec))) || (rc = ndp.reserve(std::max<uint64_t>(1, n_dp) * sizeof(pt_dep_rec)))) return rc;
+        PT_CUDA(h2d(dcdesc.p, dch->logs, (size_t)n * sizeof(pt_change_desc)));
+        PT_CUDA(h2d(ncdesc.p, ncd.data(), (size_t)n * sizeof(pt_change_desc)));
+        PT_CUDA(h2d(dchg.p, dch->changes, dch->n_changes_total * sizeof(pt_change_rec)));
+        PT_CUDA(h2d(ddep.p, dch->deps, dch->n_deps_total * sizeof(pt_dep_rec)));
+        if (n) {
+            pta::splice_changes_kernel<<<grid, threads, 0, b->stream>>>((const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p,
+                                                                        n, DR, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p,
+                                                                        (const pt_change_rec*)dchg.p, (const pt_dep_rec*)ddep.p,
+                                                                        (pt_change_rec*)nch.p, (pt_dep_rec*)ndp.p);
+            PT_CUDA(cudaGetLastError());
+            b->launches++;
+        }
+    }
+    uint32_t bad = 0;
+    PT_CUDA(cudaMemcpyAsync(&bad, abad.p, 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // also: the caller's arrays may be freed on return
+    if (bad) { g_last_error = "pt_batch_append: a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
+    // Accepted: the new records and change table replace the old ones (freed with the locals), and the batch is re-planned.
+    b->have_batch = false; b->merged = false; b->dl_begun = false;
+    drop_graph(b);
+    b->d_insdel.swap(nins); b->d_marks.swap(nmarks);
+    if (dch) {
+        b->d_cdesc.swap(ncdesc); b->d_changes.swap(nch); b->d_deps.swap(ndp);
+        b->h_cdesc = std::move(ncd); b->n_changes = n_ch; b->n_deps = n_dp; b->adm_maxR = maxR;
+    }
+    if ((rc = install_plan(b, ops, std::move(plan), true))) return rc;
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p;
+    b->have_batch = true;
     return PT_OK;
 }
 

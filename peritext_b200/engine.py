@@ -12,14 +12,14 @@ import os
 import numpy as np
 
 from .packing import (CDESC_DT, CHANGE_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT,
-                      ChangeTable, MergedBatch, PackedBatch, elem_refs)
+                      AppendRemap, ChangeTable, MergedBatch, PackedBatch, elem_refs)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
 _lib = None
 
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
-           "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
+           "pt_batch_append", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_query_elements", "pt_batch_find_elements",
            "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
@@ -100,6 +100,17 @@ class _ChangeTable(ctypes.Structure):
                 ("deps", ctypes.c_void_p), ("n_deps_total", ctypes.c_uint64)]
 
 
+class _AppendRemap(ctypes.Structure):
+    _fields_ = [("actor_off", ctypes.c_void_p), ("actor_map", ctypes.c_void_p), ("ctr_off", ctypes.c_void_p), ("ctr_map", ctypes.c_void_p),
+                ("comment_map", ctypes.c_void_p), ("n_comment_map", ctypes.c_uint64)]
+
+
+def _change_struct(table: ChangeTable):
+    """(pt_change_table, the contiguous arrays it points into)."""
+    d, c, p = np.ascontiguousarray(table.desc), np.ascontiguousarray(table.changes), np.ascontiguousarray(table.deps)
+    return _ChangeTable(len(d), d.ctypes.data, c.ctypes.data if len(c) else 0, len(c), p.ctypes.data if len(p) else 0, len(p)), (d, c, p)
+
+
 class _SpansView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("results", ctypes.c_void_p), ("text_off", ctypes.c_void_p),
                 ("span_off", ctypes.c_void_p), ("text", ctypes.c_void_p), ("spans", ctypes.c_void_p),
@@ -149,6 +160,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_upload_runs.argtypes = [vp, vp]
     L.pt_compress_runs.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(u64), ctypes.POINTER(u64)]
     L.pt_batch_upload_changes.argtypes = [vp, vp]
+    L.pt_batch_append.argtypes = [vp, vp, vp, vp]
     L.pt_compact_ops.argtypes = [vp, vp, vp, ctypes.c_int]
     L.pt_batch_upload_compact.argtypes = [vp, vp]
     L.pt_ingest_create.argtypes = [ctypes.POINTER(vp)]
@@ -222,9 +234,27 @@ class BatchEngine:
     def upload_changes(self, table: ChangeTable):
         """Attach the batch's change table: the next merge runs the admission pre-pass (seq / deps checks of
         Micromerge.applyChange, reference src/micromerge.ts:501-509) and rejected logs report status 6 / 7."""
-        d, c, p = np.ascontiguousarray(table.desc), np.ascontiguousarray(table.changes), np.ascontiguousarray(table.deps)
-        t = _ChangeTable(len(d), d.ctypes.data, c.ctypes.data if len(c) else 0, len(c), p.ctypes.data if len(p) else 0, len(p))
+        t, _keep = _change_struct(table)
         _check(self._L.pt_batch_upload_changes(self._h, ctypes.byref(t)), "pt_batch_upload_changes")
+
+    def append(self, delta: PackedBatch, remap: AppendRemap | None = None, changes: ChangeTable | None = None):
+        """Extend every log of the resident batch with the delta's records on the device (pt_batch_append): afterwards the
+        handle holds what an upload of ``packing.apply_append(batch, delta, remap)`` would hold, and needs a merge.  `delta`
+        and `remap` come from ``packing.pack_append``; `changes` is the delta's change table (default ``delta.changes``),
+        required exactly when the resident batch has one.  Works after every upload form and after an earlier append."""
+        r = remap or AppendRemap()
+        desc = np.ascontiguousarray(delta.desc)
+        insdel = np.ascontiguousarray(delta.insdel); marks = np.ascontiguousarray(delta.marks)
+        ops = self._ops_struct(desc, insdel.ctypes.data if len(insdel) else 0, len(insdel), marks.ctypes.data if len(marks) else 0, len(marks))
+        arrs = [None if a is None else np.ascontiguousarray(a, dtype=dt)
+                for a, dt in ((r.actor_off, np.uint64), (r.actor_map, np.uint16), (r.ctr_off, np.uint64), (r.ctr_map, np.uint32), (r.comment_map, np.uint32))]
+        ptr = lambda a: None if a is None else a.ctypes.data
+        st = _AppendRemap(*[ptr(a) for a in arrs], 0 if arrs[4] is None else len(arrs[4]))
+        table = delta.changes if changes is None else changes
+        ct = _change_struct(table) if table is not None else None
+        _check(self._L.pt_batch_append(self._h, ctypes.byref(ops), ctypes.byref(st), ctypes.byref(ct[0]) if ct else None), "pt_batch_append")
+        self._n_insdel += len(insdel)
+        self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion

@@ -84,6 +84,7 @@ class PackedBatch:
     log_actors: list[list[str]] = field(default_factory=list)   # per log: actor rank -> actorId
     log_counters: list = field(default_factory=list)            # per log: None, or dense counter rank -> original counter
     changes: Any = None                                         # optional ChangeTable (admission pre-pass)
+    log_lists: list = field(default_factory=list)               # per log: the object id of the text list that was packed
 
     @property
     def n_logs(self) -> int:
@@ -104,16 +105,16 @@ class PackedBatch:
         changes = self.changes.slice_logs(a, b) if self.changes is not None else None
         if len(d) == 0:
             return PackedBatch(d, self.insdel[:0], self.marks[:0], self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta),
-                               changes=changes)
+                               changes=changes, log_lists=self.log_lists[a:b] if self.log_lists else [])
         i0, m0 = int(d[0]["insdel_off"]), int(d[0]["mark_off"])
         i1 = int(d[-1]["insdel_off"]) + int(d[-1]["n_insdel"]); m1 = int(d[-1]["mark_off"]) + int(d[-1]["n_mark"])
         d["insdel_off"] -= i0; d["mark_off"] -= m0
         return PackedBatch(d, self.insdel[i0:i1], self.marks[m0:m1], self.values, self.link_attrs, self.comment_ids, self.other_attrs,
                            dict(self.meta), self.log_actors[a:b] if self.log_actors else [],
-                           self.log_counters[a:b] if self.log_counters else [], changes)
+                           self.log_counters[a:b] if self.log_counters else [], changes, self.log_lists[a:b] if self.log_lists else [])
 
     def select(self, idx: Sequence[int]) -> "PackedBatch":
-        """Sub-batch with the given logs (re-based offsets); pools are shared."""
+        """Sub-batch with the given logs (re-based offsets); pools are shared, per-log tables follow their logs."""
         idx = list(idx)
         ins_parts, mk_parts = [], []
         desc = np.zeros(len(idx), DESC_DT)
@@ -126,8 +127,10 @@ class PackedBatch:
             io += len(a); mo += len(b)
         ins = np.concatenate(ins_parts) if ins_parts else np.zeros(0, INSDEL_DT)
         mk = np.concatenate(mk_parts) if mk_parts else np.zeros(0, MARK_DT)
+        pick = lambda t: [t[i] for i in idx] if t else []
         return PackedBatch(desc, ins, mk, self.values, self.link_attrs, self.comment_ids, self.other_attrs, dict(self.meta),
-                           changes=self.changes.select(idx) if self.changes is not None else None)
+                           pick(self.log_actors), pick(self.log_counters), self.changes.select(idx) if self.changes is not None else None,
+                           pick(self.log_lists))
 
     def algorithmic_bytes(self, results: np.ndarray | None = None) -> int:
         """SURVEY.md §8(d): 16 B per ins/del + 32 B per mark read; 4 B per visible element, 16 B per span and
@@ -202,6 +205,157 @@ def _root_text_list(changes: Iterable[dict]) -> str | None:
     return children.get("text")
 
 
+class _Pools:
+    """A batch's interned strings: the value pool, link attrs, comment attrs (the first-seen attrs object per comment id)
+    and other attrs.  Known entries keep their index; new ones get the next."""
+
+    def __init__(self, values=(), link_attrs=(), comment_attrs=(), other_attrs=()):
+        self.values = list(values)
+        self.value_index = {v: i for i, v in enumerate(self.values)}
+        self.link_attrs = list(link_attrs)
+        self.link_index = {canon(a): i for i, a in enumerate(self.link_attrs)}
+        self.comment_objs: dict[str, Any] = {a["id"]: a for a in comment_attrs}
+        self.other_attrs = list(other_attrs)
+        self.other_index = {canon(a): i for i, a in enumerate(self.other_attrs)}
+
+    def token_of(self, v: Any) -> int:
+        """Element value -> 30-bit token: the code point of a one-code-point string, else a value-pool reference
+        (an element may hold a multi-character string, reference test/micromerge.ts:202)."""
+        if not isinstance(v, str):
+            raise TypeError("Expected value inserted into text to be a string")   # src/micromerge.ts:654-656
+        if len(v) == 1:
+            return ord(v)
+        if v not in self.value_index:
+            self.value_index[v] = len(self.values)
+            self.values.append(v)
+        return TOKEN_POOLED | self.value_index[v]
+
+
+def _collect_log(changes: Iterable[dict], lid: str | None, with_changes: bool, pools: _Pools) -> _LogBuilder:
+    """One log's ops that target list `lid` (arrival order), with their ids still as strings; see ``pack_logs``."""
+    b = _LogBuilder()
+    for ch in changes:
+        if with_changes:
+            b.actors.add(ch["actor"])
+            deps = list((ch.get("deps") or {}).items())
+            for a, _ in deps:
+                b.actors.add(a)
+            b.changes.append([ch["actor"], int(ch["seq"]), [(a, int(v)) for a, v in deps], 0])
+        for op in ch["ops"]:
+            if lid is None or op.get("obj") != lid:
+                continue
+            if with_changes:
+                b.changes[-1][3] += 1
+            ctr, actor = parse_op_id(op["opId"])
+            b.actors.add(actor)
+            b.max_ctr = max(b.max_ctr, ctr)
+            act = op["action"]
+            if act in ("addMark", "removeMark"):
+                mt = MARK_TYPES.index(op["markType"])
+                bounds = []
+                for side in ("start", "end"):
+                    bd = op[side]
+                    t = BOUND_TYPES.index(bd["type"])
+                    if t <= 1:
+                        ec, ea = parse_op_id(bd["elemId"])
+                        b.actors.add(ea)
+                    else:
+                        ec, ea = 0, None
+                    bounds.append((t, ec, ea))
+                attrs = op.get("attrs")
+                attr_ref = None
+                if attrs is not None:
+                    if mt == 3:
+                        k = canon(attrs)
+                        if k not in pools.link_index:
+                            pools.link_index[k] = len(pools.link_attrs)
+                            pools.link_attrs.append(attrs)
+                        attr_ref = ("link", pools.link_index[k])
+                    elif mt == 2:
+                        cid = attrs["id"]
+                        pools.comment_objs.setdefault(cid, attrs)
+                        attr_ref = ("comment", cid)
+                    else:
+                        k = canon(attrs)
+                        if k != '{"active":true}':
+                            if k not in pools.other_index:
+                                pools.other_index[k] = len(pools.other_attrs)
+                                pools.other_attrs.append(attrs)
+                            attr_ref = ("other", pools.other_index[k])
+                elif mt == 2:
+                    raise ValueError("comment mark without attrs")
+                b.marks.append((ctr, actor, act == "addMark", mt, bounds[0], bounds[1], attr_ref, len(b.insdel)))
+            elif act == "set" and op.get("insert"):
+                ref = op.get("elemId")
+                if ref in (None, "_head"):
+                    rc, ra = 0, None
+                else:
+                    rc, ra = parse_op_id(ref)
+                    b.actors.add(ra)
+                b.insdel.append((ctr, actor, rc, ra, KIND_INSERT, pools.token_of(op.get("value"))))
+            elif act == "del" and op.get("key") is None:
+                ref = op.get("elemId")
+                if ref in (None, "_head"):
+                    raise ValueError("List element not found: _head")
+                rc, ra = parse_op_id(ref)
+                b.actors.add(ra)
+                b.insdel.append((ctr, actor, rc, ra, KIND_DELETE, 0))
+            else:
+                raise NotImplementedError(f"{act} on a list")                   # src/micromerge.ts:567
+    return b
+
+
+def _used_counters(b: _LogBuilder) -> set[int]:
+    """Every counter a log's ops name (opIds, references, mark boundaries), HEAD excluded."""
+    used = {c for (c, _a, rc, _ra, _k, _t) in b.insdel for c in (c, rc)} | {c for mk_ in b.marks for c in (mk_[0], mk_[4][1], mk_[5][1])}
+    used.discard(0)
+    return used
+
+
+def _wants_dense(max_ctr: int, n_ops: int) -> bool:
+    """Sparse counters (a peer may choose any startOp, reference src/micromerge.ts:511): the engine's id table is
+    direct-addressed by (ctr, actor), so counters far beyond the op count are re-ranked densely.  Only the ORDER of
+    counters matters to compareOpIds, and the dense rank preserves it."""
+    return max_ctr > 2 * n_ops + 16
+
+
+def _emit_log(b: _LogBuilder, rank: dict, dc, comment_rank: dict, insdel: np.ndarray, io: int, marks: np.ndarray, mo: int,
+              arrival_base: int = 0) -> None:
+    """Writes one log's records at insdel[io:] / marks[mo:] in the packed id space (`rank`: actor ranks, `dc`: counters)."""
+    for k, (ctr, actor, rc, ra, kind, tok) in enumerate(b.insdel):
+        insdel[io + k] = (dc(ctr), dc(rc), rank[actor], rank[ra] if ra is not None else 0, (kind << 30) | tok)
+    for k, (ctr, actor, add, mt, sb, eb, attr_ref, arrival) in enumerate(b.marks):
+        if attr_ref is None:
+            attr = ATTR_NONE
+        elif attr_ref[0] == "comment":
+            attr = comment_rank[attr_ref[1]]
+        elif attr_ref[0] == "link":
+            attr = attr_ref[1]
+        else:
+            attr = ATTR_NONE  # non-default strong/em attrs are not representable on the device path
+            raise NotImplementedError("strong/em marks with custom attrs")
+        marks[mo + k] = (dc(ctr), rank[actor], (0 if add else 1) | (mt << 1), sb[0] | (eb[0] << 2),
+                         dc(sb[1]), dc(eb[1]), rank[sb[2]] if sb[2] is not None else 0,
+                         rank[eb[2]] if eb[2] is not None else 0, attr, arrival_base + arrival, 0)
+
+
+def _change_table(builders: Sequence[_LogBuilder], ranks: Sequence[dict]) -> ChangeTable:
+    cdesc = np.zeros(len(builders), CDESC_DT)
+    crecs = np.zeros(sum(len(b.changes) for b in builders), CHANGE_DT)
+    cdeps = np.zeros(sum(len(c[2]) for b in builders for c in b.changes), DEP_DT)
+    co = do = 0
+    for li, b in enumerate(builders):
+        rank = ranks[li]
+        nd = 0
+        cdesc[li]["change_off"] = co; cdesc[li]["dep_off"] = do; cdesc[li]["n_changes"] = len(b.changes)
+        for (actor, seq, deps, n_ops) in b.changes:
+            crecs[co] = (seq, rank[actor], len(deps), nd, n_ops); co += 1
+            for a, v in deps:
+                cdeps[do] = (v, rank[a], 0); do += 1; nd += 1
+        cdesc[li]["n_deps"] = nd
+    return ChangeTable(cdesc, crecs, cdeps)
+
+
 def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] | None = None, with_changes: bool = False) -> PackedBatch:
     """Pack ``logs[i]`` = the Change objects one replica applied, in arrival order.
 
@@ -209,101 +363,15 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
     packed.  ``list_ids[i]`` overrides the list object id (default: what ``["text"]`` resolves to).  ``with_changes``
     also builds the per-change admission table (then the change / deps actors take part in the log's actor ranking).
     The native, multithreaded equivalent over JSON text is ``pack_logs_native`` (csrc/ingest.cpp)."""
+    pools = _Pools()
     builders: list[_LogBuilder] = []
-    values: list[str] = []
-    value_index: dict[str, int] = {}
-    link_attrs: list[Any] = []
-    link_index: dict[str, int] = {}
-    comment_objs: dict[str, Any] = {}
-    other_attrs: list[Any] = []
-    other_index: dict[str, int] = {}
-
-    def token_of(v: Any) -> int:
-        """Element value -> 30-bit token: the code point of a one-code-point string, else a value-pool reference
-        (an element may hold a multi-character string, reference test/micromerge.ts:202)."""
-        if not isinstance(v, str):
-            raise TypeError("Expected value inserted into text to be a string")   # src/micromerge.ts:654-656
-        if len(v) == 1:
-            return ord(v)
-        if v not in value_index:
-            value_index[v] = len(values)
-            values.append(v)
-        return TOKEN_POOLED | value_index[v]
-
+    lids: list[str | None] = []
     for li, changes in enumerate(logs):
-        b = _LogBuilder()
         lid = list_ids[li] if list_ids is not None and list_ids[li] is not None else _root_text_list(changes)
-        for ch in changes:
-            if with_changes:
-                b.actors.add(ch["actor"])
-                deps = list((ch.get("deps") or {}).items())
-                for a, _ in deps:
-                    b.actors.add(a)
-                b.changes.append([ch["actor"], int(ch["seq"]), [(a, int(v)) for a, v in deps], 0])
-            for op in ch["ops"]:
-                if lid is None or op.get("obj") != lid:
-                    continue
-                if with_changes:
-                    b.changes[-1][3] += 1
-                ctr, actor = parse_op_id(op["opId"])
-                b.actors.add(actor)
-                b.max_ctr = max(b.max_ctr, ctr)
-                act = op["action"]
-                if act in ("addMark", "removeMark"):
-                    mt = MARK_TYPES.index(op["markType"])
-                    bounds = []
-                    for side in ("start", "end"):
-                        bd = op[side]
-                        t = BOUND_TYPES.index(bd["type"])
-                        if t <= 1:
-                            ec, ea = parse_op_id(bd["elemId"])
-                            b.actors.add(ea)
-                        else:
-                            ec, ea = 0, None
-                        bounds.append((t, ec, ea))
-                    attrs = op.get("attrs")
-                    attr_ref = None
-                    if attrs is not None:
-                        if mt == 3:
-                            k = canon(attrs)
-                            if k not in link_index:
-                                link_index[k] = len(link_attrs)
-                                link_attrs.append(attrs)
-                            attr_ref = ("link", link_index[k])
-                        elif mt == 2:
-                            cid = attrs["id"]
-                            comment_objs.setdefault(cid, attrs)
-                            attr_ref = ("comment", cid)
-                        else:
-                            k = canon(attrs)
-                            if k != '{"active":true}':
-                                if k not in other_index:
-                                    other_index[k] = len(other_attrs)
-                                    other_attrs.append(attrs)
-                                attr_ref = ("other", other_index[k])
-                    elif mt == 2:
-                        raise ValueError("comment mark without attrs")
-                    b.marks.append((ctr, actor, act == "addMark", mt, bounds[0], bounds[1], attr_ref, len(b.insdel)))
-                elif act == "set" and op.get("insert"):
-                    ref = op.get("elemId")
-                    if ref in (None, "_head"):
-                        rc, ra = 0, None
-                    else:
-                        rc, ra = parse_op_id(ref)
-                        b.actors.add(ra)
-                    b.insdel.append((ctr, actor, rc, ra, KIND_INSERT, token_of(op.get("value"))))
-                elif act == "del" and op.get("key") is None:
-                    ref = op.get("elemId")
-                    if ref in (None, "_head"):
-                        raise ValueError("List element not found: _head")
-                    rc, ra = parse_op_id(ref)
-                    b.actors.add(ra)
-                    b.insdel.append((ctr, actor, rc, ra, KIND_DELETE, 0))
-                else:
-                    raise NotImplementedError(f"{act} on a list")                   # src/micromerge.ts:567
-        builders.append(b)
+        lids.append(lid)
+        builders.append(_collect_log(changes, lid, with_changes, pools))
 
-    comment_sorted = sorted(comment_objs, key=js_key)       # sortBy(..., c => c.id), src/peritext.ts:318
+    comment_sorted = sorted(pools.comment_objs, key=js_key)       # sortBy(..., c => c.id), src/peritext.ts:318
     comment_rank = {cid: i for i, cid in enumerate(comment_sorted)}
 
     n_ins = sum(len(b.insdel) for b in builders)
@@ -313,19 +381,16 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
     marks = np.zeros(n_mk, MARK_DT)
     io = mo = 0
     counters: list = []      # per log: None, or dense counter rank -> original counter
+    ranks: list[dict] = []
     for li, b in enumerate(builders):
         ranked = sorted(b.actors, key=js_key)
         rank = {a: i for i, a in enumerate(ranked)}
+        ranks.append(rank)
         if len(ranked) > 0xFFFF:
             raise ValueError("more than 65535 actors in one log")
-        # Sparse counters (a peer may choose any startOp, reference src/micromerge.ts:511): the engine's id table is
-        # direct-addressed by (ctr, actor), so counters far beyond the op count are re-ranked densely.  Only the ORDER
-        # of counters matters to compareOpIds, and the dense rank preserves it.
         dense = None
-        if b.max_ctr > 2 * (len(b.insdel) + len(b.marks)) + 16:
-            used = {c for (c, _a, rc, _ra, _k, _t) in b.insdel for c in (c, rc)} | {c for mk_ in b.marks for c in (mk_[0], mk_[4][1], mk_[5][1])}
-            used.discard(0)
-            order = sorted(used)
+        if _wants_dense(b.max_ctr, len(b.insdel) + len(b.marks)):
+            order = sorted(_used_counters(b))
             dense = {c: i + 1 for i, c in enumerate(order)}
             dense[0] = 0
             counters.append(np.array([0] + order, dtype=np.uint64))
@@ -333,40 +398,284 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
             counters.append(None)
         dc = (lambda c: dense[c]) if dense is not None else (lambda c: c)
         desc[li] = (io, mo, len(b.insdel), len(b.marks), max(1, len(ranked)), dc(b.max_ctr) if dense is not None else b.max_ctr)
-        for k, (ctr, actor, rc, ra, kind, tok) in enumerate(b.insdel):
-            insdel[io + k] = (dc(ctr), dc(rc), rank[actor], rank[ra] if ra is not None else 0, (kind << 30) | tok)
-        for k, (ctr, actor, add, mt, sb, eb, attr_ref, arrival) in enumerate(b.marks):
-            if attr_ref is None:
-                attr = ATTR_NONE
-            elif attr_ref[0] == "comment":
-                attr = comment_rank[attr_ref[1]]
-            elif attr_ref[0] == "link":
-                attr = attr_ref[1]
-            else:
-                attr = ATTR_NONE  # non-default strong/em attrs are not representable on the device path
-                raise NotImplementedError("strong/em marks with custom attrs")
-            marks[mo + k] = (dc(ctr), rank[actor], (0 if add else 1) | (mt << 1), sb[0] | (eb[0] << 2),
-                             dc(sb[1]), dc(eb[1]), rank[sb[2]] if sb[2] is not None else 0,
-                             rank[eb[2]] if eb[2] is not None else 0, attr, arrival, 0)
+        _emit_log(b, rank, dc, comment_rank, insdel, io, marks, mo)
         io += len(b.insdel); mo += len(b.marks)
-    table = None
-    if with_changes:
-        cdesc = np.zeros(len(builders), CDESC_DT)
-        crecs = np.zeros(sum(len(b.changes) for b in builders), CHANGE_DT)
-        cdeps = np.zeros(sum(len(c[2]) for b in builders for c in b.changes), DEP_DT)
-        co = do = 0
-        for li, b in enumerate(builders):
-            rank = {a: i for i, a in enumerate(sorted(b.actors, key=js_key))}
-            nd = 0
-            cdesc[li]["change_off"] = co; cdesc[li]["dep_off"] = do; cdesc[li]["n_changes"] = len(b.changes)
-            for (actor, seq, deps, n_ops) in b.changes:
-                crecs[co] = (seq, rank[actor], len(deps), nd, n_ops); co += 1
-                for a, v in deps:
-                    cdeps[do] = (v, rank[a], 0); do += 1; nd += 1
-            cdesc[li]["n_deps"] = nd
-        table = ChangeTable(cdesc, crecs, cdeps)
-    return PackedBatch(desc, insdel, marks, values, link_attrs, [comment_objs[c] for c in comment_sorted], other_attrs,
-                       log_actors=[sorted(b.actors, key=js_key) for b in builders], log_counters=counters, changes=table)
+    table = _change_table(builders, ranks) if with_changes else None
+    return PackedBatch(desc, insdel, marks, pools.values, pools.link_attrs, [pools.comment_objs[c] for c in comment_sorted], pools.other_attrs,
+                       log_actors=[sorted(b.actors, key=js_key) for b in builders], log_counters=counters, changes=table, log_lists=lids)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Append (include/peritext_b200.h pt_batch_append)
+# ------------------------------------------------------------------------------------------------------------------
+CTR_UNUSED = 0xFFFFFFFF      # a counter-map entry for an old counter that no record of the log names
+
+
+@dataclass
+class AppendRemap:
+    """How the resident records' ids move when a batch grows (pt_append_remap); None = identity.  Log i's actor map is
+    actor_map[actor_off[i]:actor_off[i+1]] (old rank -> new rank; empty = identity), its counter map likewise (old ctr ->
+    new ctr, entry 0 = 0; CTR_UNUSED for an old counter no record names); comment_map: old comment rank -> new rank."""
+    actor_off: np.ndarray | None = None      # u64 [n_logs + 1]
+    actor_map: np.ndarray | None = None      # u16
+    ctr_off: np.ndarray | None = None        # u64 [n_logs + 1]
+    ctr_map: np.ndarray | None = None        # u32
+    comment_map: np.ndarray | None = None    # u32
+
+
+def _flat_maps(maps: Sequence[Sequence[int] | None], dtype) -> tuple[np.ndarray | None, np.ndarray | None]:
+    """Per-log maps (None = identity) -> (offsets [n + 1], concatenated map), or (None, None) if every map is the identity."""
+    if all(m is None for m in maps):
+        return None, None
+    off = np.zeros(len(maps) + 1, np.uint64)
+    off[1:] = np.cumsum([0 if m is None else len(m) for m in maps])
+    flat = [x for m in maps if m is not None for x in m]
+    return off, np.array(flat, dtype)
+
+
+def pack_append(prev: PackedBatch, new_logs: Sequence[Sequence[dict]], *, with_changes: bool = False,
+                list_ids: Sequence[str | None] | None = None) -> tuple[PackedBatch, AppendRemap]:
+    """The delta and remap of ``pt_batch_append`` that extend every log of ``prev`` (a ``pack_logs`` batch) with the Change
+    objects ``new_logs[i]``, so that ``apply_append(prev, delta, remap)`` is ``pack_logs`` of the concatenated logs.
+
+    Everything about the old logs comes from ``prev``: actors from ``log_actors``, used counters from ``log_counters`` (or
+    from the records where a log was not re-ranked), comment ids from ``comment_ids``, pools from ``values`` /
+    ``link_attrs``, the text list from ``log_lists`` (or ``list_ids``; a log with old records and neither raises ValueError,
+    since the new changes alone rarely name the list).  ``pack_logs``'s rules apply to the FULL log: the actor set (with the
+    change and dep actors when ``with_changes``, which must match how ``prev`` was packed), the dense-counter rule, the
+    batch-wide comment order.  Known strings keep their pool index and new ones get the next, so the result names the same
+    strings as ``pack_logs`` of the full logs, maybe at other indices; a known comment id keeps its first-seen attrs.  A log's
+    counter map covers every counter its old records name, except, where a plain log turns dense, counters beyond
+    2 x (old max_ctr + old records) + 16, which only a reference to an element far past the log's opIds can name: those become
+    0xFFFFFFFF where ``pack_logs`` would rank them.
+    The delta carries the new pools, ``log_actors``, ``log_counters`` and ``log_lists``, and the change table of the new
+    changes."""
+    n = prev.n_logs
+    if len(new_logs) != n:
+        raise ValueError(f"pack_append: {len(new_logs)} new logs for a batch of {n}")
+    if with_changes != (prev.changes is not None):
+        raise ValueError("pack_append: with_changes must match whether prev has a change table")
+    if len(prev.log_actors) != n:
+        raise ValueError("pack_append: prev carries no log_actors (pack it with pack_logs)")
+    pools = _Pools(prev.values, prev.link_attrs, prev.comment_ids, prev.other_attrs)
+    builders, lids = [], []
+    for i, changes in enumerate(new_logs):
+        old_recs = int(prev.desc[i]["n_insdel"]) + int(prev.desc[i]["n_mark"])
+        if list_ids is not None and list_ids[i] is not None:
+            lid = list_ids[i]
+        elif i < len(prev.log_lists) and prev.log_lists[i] is not None:
+            lid = prev.log_lists[i]
+        elif old_recs and i >= len(prev.log_lists):
+            raise ValueError(f"pack_append: log {i} has records but prev does not record its text list (a batch from "
+                             "pack_logs_native or built by hand): pass list_ids")
+        else:
+            lid = _root_text_list(changes)       # the old log has no text list: the new changes may create it
+        lids.append(lid)
+        builders.append(_collect_log(changes, lid, with_changes, pools))
+    old_cids = [a["id"] for a in prev.comment_ids]
+    comment_sorted = sorted(pools.comment_objs, key=js_key)
+    comment_rank = {cid: i for i, cid in enumerate(comment_sorted)}
+    cmap = [comment_rank[c] for c in old_cids]
+
+    desc = np.zeros(n, DESC_DT)
+    insdel = np.zeros(sum(len(b.insdel) for b in builders), INSDEL_DT)
+    marks = np.zeros(sum(len(b.marks) for b in builders), MARK_DT)
+    io = mo = 0
+    actor_maps, ctr_maps, log_actors, counters, ranks = [], [], [], [], []
+    for i, b in enumerate(builders):
+        d = prev.desc[i]
+        old_actors = list(prev.log_actors[i])
+        ranked = sorted(set(old_actors) | b.actors, key=js_key)
+        if len(ranked) > 0xFFFF:
+            raise ValueError("more than 65535 actors in one log")
+        rank = {a: r for r, a in enumerate(ranked)}
+        ranks.append(rank); log_actors.append(ranked)
+        amap = [rank[a] for a in old_actors]
+        actor_maps.append(amap if amap != list(range(len(amap))) else None)
+        old_dense = prev.log_counters[i] if i < len(prev.log_counters) else None
+        old_max_ctr = int(d["max_ctr"])
+        full_max = max(int(old_dense[old_max_ctr]) if old_dense is not None else old_max_ctr, b.max_ctr)
+        full_ops = int(d["n_insdel"]) + int(d["n_mark"]) + len(b.insdel) + len(b.marks)
+        if _wants_dense(full_max, full_ops):
+            if old_dense is not None:
+                old_used = set(int(c) for c in old_dense[1:])
+            else:
+                ins, mk = prev.log_slice(i)
+                old_used = set(np.concatenate([ins["ctr"], ins["ref_ctr"], mk["ctr"], mk["start_ctr"], mk["end_ctr"]]).astype(np.int64).tolist())
+                old_used.discard(0)
+            order = sorted(old_used | _used_counters(b))
+            dense = {c: k + 1 for k, c in enumerate(order)}
+            dense[0] = 0
+            counters.append(np.array([0] + order, dtype=np.uint64))
+            dc = dense.__getitem__
+            new_max = dense[full_max]
+            if old_dense is not None:
+                cm = [dense[int(c)] for c in old_dense]
+            else:
+                # the domain: every counter the old records name (a mark boundary may name an element inserted later), up
+                # to a bound that keeps a reference far past the log's opIds from sizing the map
+                cap = 2 * (old_max_ctr + int(d["n_insdel"]) + int(d["n_mark"])) + 16
+                hi = max([old_max_ctr] + [c for c in old_used if c <= cap])
+                cm = [dense.get(c, CTR_UNUSED) for c in range(hi + 1)]
+        else:
+            counters.append(None)
+            dc = (lambda c: c)
+            new_max = full_max
+            cm = [int(c) for c in old_dense] if old_dense is not None else None
+        ctr_maps.append(cm if cm is not None and cm != list(range(len(cm))) else None)
+        desc[i] = (io, mo, len(b.insdel), len(b.marks), max(1, len(ranked)), new_max)
+        _emit_log(b, rank, dc, comment_rank, insdel, io, marks, mo, arrival_base=int(d["n_insdel"]))
+        io += len(b.insdel); mo += len(b.marks)
+    aoff, amaps = _flat_maps(actor_maps, np.uint16)
+    coff, cmaps = _flat_maps(ctr_maps, np.uint32)
+    remap = AppendRemap(aoff, amaps, coff, cmaps, np.array(cmap, np.uint32) if cmap != list(range(len(cmap))) else None)
+    delta = PackedBatch(desc, insdel, marks, pools.values, pools.link_attrs, [pools.comment_objs[c] for c in comment_sorted], pools.other_attrs,
+                        dict(prev.meta), log_actors, counters, _change_table(builders, ranks) if with_changes else None, lids)
+    return delta, remap
+
+
+def split_records(batch: PackedBatch, cuts) -> tuple[PackedBatch, PackedBatch]:
+    """(prefix, delta) of a record-level batch: log i keeps its first cuts[i] ins/del records and the marks that arrived
+    before them (marks must be in arrival order), the rest is the delta of ``pt_batch_append`` with identity maps.  Both
+    keep the log's n_actors / max_ctr.  For benchmarks and tests that grow generated workloads; vectorised."""
+    d = batch.desc
+    n_mk = d["n_mark"].astype(np.int64)
+    cuts = np.minimum(np.asarray(cuts, np.int64), d["n_insdel"].astype(np.int64))
+    li = np.repeat(np.arange(batch.n_logs), n_mk)
+    keep = batch.marks["arrival"][_ranges(d["mark_off"], n_mk)].astype(np.int64) < cuts[li]
+    m_pre = np.bincount(li[keep], minlength=batch.n_logs).astype(np.int64)
+    first_mk = np.concatenate([[0], np.cumsum(n_mk)[:-1]]).astype(np.int64)
+    if not (keep == (np.arange(len(li)) - first_mk[li] < m_pre[li])).all():
+        raise ValueError("split_records: a log's marks are not in arrival order")
+
+    def part(first_ins, cnt_ins, first_m, cnt_m):
+        desc = np.zeros(batch.n_logs, DESC_DT)
+        desc["n_insdel"], desc["n_mark"] = cnt_ins, cnt_m
+        desc["insdel_off"], desc["mark_off"] = _excl_scan(cnt_ins), _excl_scan(cnt_m)
+        desc["n_actors"], desc["max_ctr"] = d["n_actors"], d["max_ctr"]
+        return PackedBatch(desc, batch.insdel[_ranges(d["insdel_off"].astype(np.int64) + first_ins, cnt_ins)],
+                           batch.marks[_ranges(d["mark_off"].astype(np.int64) + first_m, cnt_m)], batch.values, batch.link_attrs,
+                           batch.comment_ids, batch.other_attrs)
+    return (part(np.zeros_like(cuts), cuts, np.zeros_like(m_pre), m_pre),
+            part(cuts, d["n_insdel"].astype(np.int64) - cuts, m_pre, n_mk - m_pre))
+
+
+def _ranges(off: np.ndarray, cnt: np.ndarray) -> np.ndarray:
+    """Indices [off[i], off[i] + cnt[i]) of every i, concatenated."""
+    cnt = np.asarray(cnt, np.int64)
+    if int(cnt.sum()) == 0:
+        return np.zeros(0, np.int64)
+    first = np.concatenate([[0], np.cumsum(cnt)[:-1]])
+    return np.repeat(np.asarray(off, np.int64) - first, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
+
+
+def _excl_scan(x: np.ndarray) -> np.ndarray:
+    x = np.asarray(x, np.uint64)
+    out = np.zeros(len(x), np.uint64)
+    if len(x):
+        out[1:] = np.cumsum(x)[:-1]
+    return out
+
+
+def _through(vals: np.ndarray, log: np.ndarray, off: np.ndarray | None, m: np.ndarray | None, fill: int) -> np.ndarray:
+    """vals[k] through the map of log log[k] (m[off[l]:off[l+1]], empty = identity); outside the map's domain -> fill."""
+    vals = np.asarray(vals, np.int64)
+    if off is None or len(vals) == 0:
+        return vals
+    off = np.asarray(off, np.int64)
+    ln = (off[1:] - off[:-1])[log]
+    out = vals.copy()
+    mapped = ln > 0
+    inside = mapped & (vals < ln)
+    out[mapped & ~inside] = fill
+    out[inside] = np.asarray(m, np.int64)[(off[:-1][log] + vals)[inside]]
+    return out
+
+
+def apply_append(prev: PackedBatch, delta: PackedBatch, remap: AppendRemap | None = None) -> PackedBatch:
+    """The readable host specification of ``pt_batch_append``'s splice: the batch the handle holds after appending
+    ``delta`` with ``remap`` to ``prev``.  Logs are contiguous and in order, each with its old records (ids through the
+    log's maps) and then its delta records.  An id whose counter is 0 (HEAD, a text boundary) keeps its actor field; a value
+    outside its map's domain, or mapped to CTR_UNUSED, becomes 0xFFFF / 0xFFFFFFFF.  A comment mark's rank goes through the
+    comment map (PT_ATTR_NONE stays); a rank outside it raises ValueError, as the device refuses it.  The change table is
+    concatenated per log with old actor ranks mapped and the delta's dep_off rebased.  Pools, ``log_actors``,
+    ``log_counters`` and ``log_lists`` are the delta's."""
+    r = remap or AppendRemap()
+    n = prev.n_logs
+    if delta.n_logs != n:
+        raise ValueError(f"apply_append: the delta has {delta.n_logs} logs and the batch {n}")
+    od, dd = prev.desc, delta.desc
+    desc = np.zeros(n, DESC_DT)
+    desc["n_insdel"] = od["n_insdel"].astype(np.uint64) + dd["n_insdel"]
+    desc["n_mark"] = od["n_mark"].astype(np.uint64) + dd["n_mark"]
+    desc["insdel_off"] = _excl_scan(desc["n_insdel"]); desc["mark_off"] = _excl_scan(desc["n_mark"])
+    desc["n_actors"] = dd["n_actors"]; desc["max_ctr"] = dd["max_ctr"]
+    logs = np.arange(n)
+
+    def splice(recs, drecs, off_f, cnt_f, dt, remap_fn):
+        out = np.zeros(int(desc[cnt_f].astype(np.int64).sum()), dt)
+        o = recs[_ranges(od[off_f], od[cnt_f])].copy()
+        remap_fn(o, np.repeat(logs, od[cnt_f].astype(np.int64)))
+        out[_ranges(desc[off_f], od[cnt_f])] = o
+        out[_ranges(desc[off_f].astype(np.int64) + od[cnt_f], dd[cnt_f])] = drecs[_ranges(dd[off_f], dd[cnt_f])]
+        return out
+
+    def ctr(v, lg):
+        return _through(v, lg, r.ctr_off, r.ctr_map, 0xFFFFFFFF)
+
+    def id_actor(c, a, lg):      # counter 0 names no actor
+        return np.where(np.asarray(c) != 0, _through(a, lg, r.actor_off, r.actor_map, 0xFFFF), np.asarray(a, np.int64))
+
+    def map_insdel(o, lg):
+        c, rc = o["ctr"].copy(), o["ref_ctr"].copy()
+        o["actor"] = id_actor(c, o["actor"], lg); o["ref_actor"] = id_actor(rc, o["ref_actor"], lg)
+        o["ctr"] = ctr(c, lg); o["ref_ctr"] = ctr(rc, lg)
+
+    def map_marks(o, lg):
+        c, sc, ec = o["ctr"].copy(), o["start_ctr"].copy(), o["end_ctr"].copy()
+        o["actor"] = id_actor(c, o["actor"], lg)
+        o["start_actor"] = id_actor(sc, o["start_actor"], lg); o["end_actor"] = id_actor(ec, o["end_actor"], lg)
+        o["ctr"] = ctr(c, lg); o["start_ctr"] = ctr(sc, lg); o["end_ctr"] = ctr(ec, lg)
+        if r.comment_map is not None:
+            com = (((o["kind"] >> 1) & 3) == 2) & (o["attr"] != ATTR_NONE)
+            cm = np.asarray(r.comment_map, np.int64)
+            if (o["attr"][com] >= len(cm)).any():
+                raise ValueError("apply_append: a resident comment rank is outside comment_map")
+            o["attr"][com] = cm[o["attr"][com].astype(np.int64)]
+
+    insdel = splice(prev.insdel, delta.insdel, "insdel_off", "n_insdel", INSDEL_DT, map_insdel)
+    marks = splice(prev.marks, delta.marks, "mark_off", "n_mark", MARK_DT, map_marks)
+    changes = None
+    if (prev.changes is None) != (delta.changes is None):
+        raise ValueError("apply_append: a change table on one side only")
+    if prev.changes is not None:
+        oc, dcg = prev.changes, delta.changes
+        ocd, dcd = oc.desc, dcg.desc
+        cdesc = np.zeros(n, CDESC_DT)
+        cdesc["n_changes"] = ocd["n_changes"].astype(np.uint64) + dcd["n_changes"]
+        cdesc["n_deps"] = ocd["n_deps"].astype(np.uint64) + dcd["n_deps"]
+        cdesc["change_off"] = _excl_scan(cdesc["n_changes"]); cdesc["dep_off"] = _excl_scan(cdesc["n_deps"])
+
+        def cat(recs, drecs, off_f, cnt_f, dt, fix_old, fix_new):
+            out = np.zeros(int(cdesc[cnt_f].astype(np.int64).sum()), dt)
+            o = recs[_ranges(ocd[off_f], ocd[cnt_f])].copy()
+            fix_old(o, np.repeat(logs, ocd[cnt_f].astype(np.int64)))
+            d = drecs[_ranges(dcd[off_f], dcd[cnt_f])].copy()
+            fix_new(d, np.repeat(logs, dcd[cnt_f].astype(np.int64)))
+            out[_ranges(cdesc[off_f], ocd[cnt_f])] = o
+            out[_ranges(cdesc[off_f].astype(np.int64) + ocd[cnt_f], dcd[cnt_f])] = d
+            return out
+
+        def map_actor(o, lg):
+            o["actor"] = _through(o["actor"], lg, r.actor_off, r.actor_map, 0xFFFF)
+
+        def rebase(d, lg):
+            d["dep_off"] += ocd["n_deps"][lg]
+
+        changes = ChangeTable(cdesc, cat(oc.changes, dcg.changes, "change_off", "n_changes", CHANGE_DT, map_actor, rebase),
+                              cat(oc.deps, dcg.deps, "dep_off", "n_deps", DEP_DT, map_actor, lambda d, lg: None))
+    return PackedBatch(desc, insdel, marks, delta.values, delta.link_attrs, delta.comment_ids, delta.other_attrs, dict(prev.meta),
+                       delta.log_actors, delta.log_counters, changes, delta.log_lists)
 
 
 def elem_refs(batch: PackedBatch, logs: Sequence[int], elem_ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
