@@ -417,6 +417,27 @@ int pt_batch_download(pt_batch*, pt_spans_view* out);
 int pt_batch_download_patches(pt_batch*, pt_patch_view* out);
 int pt_batch_set_patch_pool(pt_batch*, uint64_t items);
 
+/* PT_FLAG_EMIT_PATCHES: restrict the Patch stream of the following merges to a suffix of every log's list ops — what an editor
+ * that has seen the first changes needs from Micromerge.applyChange for the rest (src/micromerge.ts:499-514).
+ * first_op[i] is the position of log i's first op inside the window, in the list-op order of pt_batch_render_patches_json:
+ * ins/del record j is at j + #{k : min(arrival_k, n) <= j}, mark record k at min(arrival_k, n) + k.  0 is the whole log,
+ * n_insdel + n_mark an empty window; first_op == NULL sets every log to 0.  After a pt_batch_append, first_op[i] = the log's
+ * old n_insdel + old n_mark gives exactly the new changes' ops.  With a change table whose n_ops counts the log's list ops,
+ * change c starts at the sum of n_ops over the log's earlier changes.
+ * A merge under a window computes what the whole-log merge computes for the ops inside it: their pt_patch_rec records are
+ * identical, the records before the window are {0, 0, PT_ATTR_NONE, 0}, and the item pool holds only the items of ops inside
+ * the window (n_items_needed is the window's demand, and a pool of that size is enough).  The patch status and its limits
+ * are those of the whole log.  pt_batch_render_patches_json renders each log as "[" + the inner arrays of the ops at positions
+ * >= first_op[i] + "]": the whole-log bytes with the first first_op[i] inner arrays removed.
+ * Cost: the per-op loops of the patch kernel are O(window x log) per log instead of O(log^2); the tables still cover the
+ * whole log (linear), and the merge itself is unchanged.
+ * The window persists across merges; every upload form and pt_batch_append reset it to whole logs.  Setting it after a merge
+ * makes the patch outputs of that merge stale: pt_batch_download_patches and pt_batch_render_patches_json return PT_ERR_STATE
+ * until the next merge.  Refused with nothing changed: n_logs other than the batch's, or a first_op[i] > n_insdel + n_mark
+ * (PT_ERR_INVALID, pt_last_error names the first such log); no batch, or a handle without PT_FLAG_EMIT_PATCHES (PT_ERR_STATE).
+ * n_logs == 0: PT_OK.  Synchronises; first_op may be freed on return. */
+int pt_batch_set_patch_window(pt_batch*, const uint32_t* first_op /* [n_logs] or NULL = whole logs */, uint32_t n_logs);
+
 /* Batched index -> element resolution on the materialised documents (PT_FLAG_EMIT_SEQUENCE, after a merge): what
  * op generation and cursors need (getListElementId, src/micromerge.ts:762-805; getCursor :465).  Query k asks log
  * `log` for its `index`-th visible element; with PT_QUERY_LOOK_AFTER_TOMBSTONES the answer moves to the LAST following
@@ -499,8 +520,9 @@ int pt_batch_render_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
  * different attrs objects, F and C are the first-seen attrs of the id (the span render's corner).
  * Pools and missing-entry errors as pt_batch_render_json.  Null arguments: PT_ERR_INVALID.  No completed merge, a handle
  * created without PT_FLAG_EMIT_PATCHES, or an item demand of the last merge above the patch pool's capacity (pt_last_error
- * gives the needed count: pt_batch_set_patch_pool and merge again), or a pt_batch_set_patch_pool since the last merge:
- * PT_ERR_STATE.  n_logs == 0: PT_OK with off[0] = 0.
+ * gives the needed count: pt_batch_set_patch_pool and merge again), or a pt_batch_set_patch_pool or pt_batch_set_patch_window
+ * since the last merge: PT_ERR_STATE.  n_logs == 0: PT_OK with off[0] = 0.  Under a patch window (pt_batch_set_patch_window)
+ * each log renders only the inner arrays of the window's ops.
  * Synchronises.  The view is engine-owned pinned memory of its own, valid until the next pt_batch_render_patches_json,
  * upload or destroy; a pt_batch_render_json view, the pt_spans_view and the pt_patch_view stay valid and unchanged.  The bytes
  * do not depend on the order of the item pool.

@@ -421,6 +421,7 @@ struct pt_batch {
     // batch
     bool have_batch = false, merged = false;
     bool patch_pool_changed = false;   // pt_batch_set_patch_pool replaced the item pool after the last merge
+    bool patch_window_changed = false; // pt_batch_set_patch_window changed the window after the last merge
     uint32_t n_logs = 0;
     uint64_t n_insdel = 0, n_mark = 0;
     std::vector<pt_log_desc> h_desc;
@@ -433,7 +434,8 @@ struct pt_batch {
     std::vector<pt_change_desc> h_cdesc;                 // its descriptors, and its totals
     uint64_t n_changes = 0, n_deps = 0;
     DevBuf d_patch_recs, d_patch_items, d_patch_status;   // PT_FLAG_EMIT_PATCHES
-    HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc;
+    DevBuf d_patch_first;                                 // [n_logs] the patch window's first list op per log (0: whole log)
+    HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc, h_patch_first;
     DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // both JSON renders: the caller's pools
     JsonBufs spans_json, patches_json;                                  // each render's own scratch and view
     DevBuf d_picnt, d_piseg, d_pibsum, d_pitmp, d_pisorted;             // pt_batch_render_patches_json: the ordered patch items
@@ -486,6 +488,9 @@ int alloc_and_upload_plan(pt_batch* b) {
         if ((rc = b->d_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
         if ((rc = b->d_patch_items.reserve(std::max<uint64_t>(1, b->patch_cap) * sizeof(pt_patch_item)))) return rc;
         if ((rc = b->d_patch_status.reserve(std::max<size_t>(1, n) * 4))) return rc;
+        if ((rc = b->d_patch_first.reserve(std::max<size_t>(1, n) * 4))) return rc;
+        PT_CUDA(cudaMemsetAsync(b->d_patch_first.p, 0, std::max<size_t>(1, n) * 4, b->stream));   // every upload / append: whole logs
+        b->patch_window_changed = false;
     }
     if ((rc = b->d_slab.reserve(std::max<size_t>((size_t)pl.slab_slots * pl.slab_bytes, 16)))) return rc;
     // stage the small host-derived arrays through pinned memory
@@ -1219,6 +1224,7 @@ static int enqueue_merge(pt_batch* b) {
     if ((b->limits.flags & PT_FLAG_EMIT_PATCHES) && b->n_logs) {
         ptk::PatchParams Q{};
         Q.desc = P.desc; Q.insdel = P.insdel; Q.marks = P.marks; Q.results = P.results; Q.text_off = P.text_off; Q.seq = P.seq;
+        Q.first_op = (const uint32_t*)b->d_patch_first.p;
         Q.n_logs = b->n_logs; Q.smem_bytes = b->plan.patch_smem;
         Q.recs = (pt_patch_rec*)b->d_patch_recs.p; Q.items = (pt_patch_item*)b->d_patch_items.p;
         Q.item_cursor = &c->patch_items; Q.item_cap = b->patch_cap;
@@ -1265,7 +1271,7 @@ int pt_batch_merge(pt_batch* b) {
         if (rc) return rc;
     }
     PT_CUDA(cudaEventRecord(b->ev1, b->stream));
-    b->merged = true; b->merges_since_upload++; b->dl_begun = false; b->patch_pool_changed = false;
+    b->merged = true; b->merges_since_upload++; b->dl_begun = false; b->patch_pool_changed = false; b->patch_window_changed = false;
     return PT_OK;
 }
 
@@ -1379,6 +1385,7 @@ int pt_batch_download_patches(pt_batch* b, pt_patch_view* out) {
     if (!b || !out) return PT_ERR_INVALID;
     if (!b->merged) { g_last_error = "download before merge"; return PT_ERR_STATE; }
     if (!(b->limits.flags & PT_FLAG_EMIT_PATCHES)) { g_last_error = "the handle was created without PT_FLAG_EMIT_PATCHES"; return PT_ERR_STATE; }
+    if (b->patch_window_changed) { g_last_error = "pt_batch_download_patches: the patch window was set after the last merge; merge again"; return PT_ERR_STATE; }
     int rc;
     if ((rc = b->h_patch_misc.reserve(16))) return rc;
     if ((rc = b->h_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
@@ -1407,6 +1414,41 @@ int pt_batch_set_patch_pool(pt_batch* b, uint64_t items) {
         if ((rc = b->d_patch_items.reserve(b->patch_cap * sizeof(pt_patch_item)))) return rc;
         drop_graph(b);                                   // the item pool pointer / capacity are baked in
     }
+    return PT_OK;
+}
+
+// The window lives in d_patch_first, allocated with the batch, so the captured merge graph reads whichever window is set.
+int pt_batch_set_patch_window(pt_batch* b, const uint32_t* first_op, uint32_t n_logs) {
+    static const char* fn = "pt_batch_set_patch_window";
+    if (!b) return PT_ERR_INVALID;
+    if (!(b->limits.flags & PT_FLAG_EMIT_PATCHES)) { g_last_error = std::string(fn) + ": the handle was created without PT_FLAG_EMIT_PATCHES"; return PT_ERR_STATE; }
+    if (!b->have_batch) { g_last_error = std::string(fn) + " before pt_batch_upload"; return PT_ERR_STATE; }
+    if (n_logs != b->n_logs) {
+        g_last_error = std::string(fn) + ": n_logs is " + std::to_string(n_logs) + ", the batch has " + std::to_string(b->n_logs);
+        return PT_ERR_INVALID;
+    }
+    if (first_op) {
+        for (uint32_t i = 0; i < n_logs; i++) {
+            const uint64_t ops = (uint64_t)b->h_desc[i].n_insdel + b->h_desc[i].n_mark;
+            if (first_op[i] > ops) {
+                g_last_error = std::string(fn) + ": log " + std::to_string(i) + ": first_op " + std::to_string(first_op[i]) + " > its " +
+                               std::to_string(ops) + " list ops";
+                return PT_ERR_INVALID;
+            }
+        }
+    }
+    if (!n_logs) return PT_OK;
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));           // the staging buffer of an earlier call may still be in flight
+    if (first_op) {
+        int rc;
+        if ((rc = b->h_patch_first.reserve((size_t)n_logs * 4))) return rc;
+        memcpy(b->h_patch_first.p, first_op, (size_t)n_logs * 4);
+        PT_CUDA(cudaMemcpyAsync(b->d_patch_first.p, b->h_patch_first.p, (size_t)n_logs * 4, cudaMemcpyHostToDevice, b->stream));
+    } else {
+        PT_CUDA(cudaMemsetAsync(b->d_patch_first.p, 0, (size_t)n_logs * 4, b->stream));
+    }
+    b->patch_window_changed = b->merged;
     return PT_OK;
 }
 
@@ -1454,6 +1496,7 @@ int pt_batch_render_patches_json(pt_batch* b, const pt_json_pools* pools, pt_jso
     if (!b->merged) { g_last_error = "render before merge"; return PT_ERR_STATE; }
     if (!(b->limits.flags & PT_FLAG_EMIT_PATCHES)) { g_last_error = "the handle was created without PT_FLAG_EMIT_PATCHES"; return PT_ERR_STATE; }
     if (b->patch_pool_changed) { g_last_error = std::string(fn) + ": the patch pool was replaced after the last merge; merge again"; return PT_ERR_STATE; }
+    if (b->patch_window_changed) { g_last_error = std::string(fn) + ": the patch window was set after the last merge; merge again"; return PT_ERR_STATE; }
     ptr::JsonPools P{};
     int rc;
     if ((rc = load_json_pools(b, pools, fn, &P))) return rc;
@@ -1498,7 +1541,7 @@ int pt_batch_render_patches_json(pt_batch* b, const pt_json_pools* pools, pt_jso
         }
         I.desc = desc; I.insdel = b->dp_insdel; I.marks = b->dp_marks; I.res = (const pt_log_result*)b->d_results.p;
         I.recs = (const pt_patch_rec*)b->d_patch_recs.p; I.pstatus = (const uint32_t*)b->d_patch_status.p;
-        I.seg = seg; I.items = sorted; I.n_insdel = b->n_insdel;
+        I.seg = seg; I.items = sorted; I.n_insdel = b->n_insdel; I.first_op = (const uint32_t*)b->d_patch_first.p;
     }
     return render_passes(b, fn, b->patches_json,
         [&](uint32_t grid, uint32_t threads, unsigned long long* sizes, unsigned long long* miss) {

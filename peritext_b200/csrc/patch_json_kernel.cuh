@@ -22,6 +22,7 @@
 // op_out<true> at its position.  Patches are small and independent, and a c4 log has about a thousand of them.
 #pragma once
 #include "render_kernel.cuh"
+#include "patch_window.cuh"
 
 namespace ptr {
 
@@ -34,6 +35,7 @@ struct PatchJsonIn {
     const uint32_t* __restrict__ pstatus;           // per log: 0 computed on the device
     const unsigned long long* __restrict__ seg;     // [n_owners + 1] the owners' segments of the ordered items
     const uint2* __restrict__ items;                // ordered items: (a, b)
+    const uint32_t* __restrict__ first_op;          // per log: list-op position of the patch window's first op (0: whole log)
     uint64_t n_insdel;                              // the batch's ins/del records: the mark owners start here
 };
 
@@ -178,15 +180,16 @@ __device__ uint32_t op_out(const PatchJsonIn& I, const JsonPools& P, const pt_lo
 
 // Log `log`'s patch JSON at d (W) or its byte count (!W).  Warp-collective; every lane returns the same count.
 // Op order: mark record k sits at position arrival_k + k, so it comes before ins/del record arrival_k; a trip's lanes learn
-// which of their positions hold mark ops from one OR-reduction of the 32 next marks' positions.
+// which of their positions hold mark ops from one OR-reduction of the 32 next marks' positions.  The trips start at the patch
+// window's first position, with the records before it counted by the patch kernel's own rule (patch_window.cuh).
 template <bool W>
 __device__ uint64_t render_patch_log(const PatchJsonIn& I, const JsonPools& P, uint32_t log, uint8_t* d, unsigned long long* miss, uint32_t lane) {
     const pt_log_desc L = I.desc[log];
-    const uint32_t n = L.n_insdel, m = L.n_mark, total = n + m;
+    const uint32_t n = L.n_insdel, m = L.n_mark, total = n + m, w0 = I.first_op[log];
     uint64_t pos = 0;
     PTR_LIT(W, d, pos, "[", lane);
-    uint32_t ri = 0, mi = 0;                                     // ins/del and mark records before this trip
-    for (uint32_t base = 0; base < total; base += 32) {
+    uint32_t mi = ptw::marks_before(I.marks + L.mark_off, n, m, w0, lane), ri = w0 - mi;   // ins/del and mark records before this trip
+    for (uint32_t base = w0; base < total; base += 32) {
         uint32_t bit = 0;
         if (mi + lane < m) {
             const uint32_t p = min(I.marks[L.mark_off + mi + lane].arrival, n) + mi + lane;
@@ -196,11 +199,11 @@ __device__ uint64_t render_patch_log(const PatchJsonIn& I, const JsonPools& P, u
         const bool is_mark = (mk >> lane) & 1u;
         const uint32_t j = is_mark ? mi + below : ri + lane - below, p = base + lane;
         const bool live = p < total && j < (is_mark ? m : n);
-        const uint32_t c = live ? (p ? 1u : 0u) + op_out<false>(I, P, L, log, is_mark, j, nullptr, miss) : 0u;
+        const uint32_t c = live ? (p != w0 ? 1u : 0u) + op_out<false>(I, P, L, log, is_mark, j, nullptr, miss) : 0u;
         const uint32_t incl = warp_incl_scan(c, lane);
         if (W && live) {
             uint8_t* o = d + pos + incl - c;
-            if (p) *o++ = ',';
+            if (p != w0) *o++ = ',';
             op_out<true>(I, P, L, log, is_mark, j, o, nullptr);
         }
         pos += __shfl_sync(kFull, incl, 31);

@@ -13,8 +13,16 @@
 // One warp per log; every count is a uniform loop over shared-memory tables (lane = one op, broadcast reads).  The loops
 // are quadratic in the log's size, which is what a document under interactive editing needs (the facade's use); logs
 // beyond PT_PATCH_MAX_* are reported as "not computed" and the host closed forms take over.
+//
+// Patch window (pt_batch_set_patch_window).  Every op's patch is a function of the two inputs above alone, so the ops of a
+// suffix of the log can be computed without the others.  The tables (T, PosOf, TIns, TDel, the mark slots) still cover the
+// whole log, because the window's ops count and cover elements of every age; only the per-op loops start at the window:
+// ins/del records [j0, n) and mark ops [k0, m), where k0 mark records and j0 ins/del records lie before list-op position
+// first_op (patch_window.cuh).  The records before the window are written as {0, 0, PT_ATTR_NONE, 0} and emit no items.  The
+// quadratic part becomes O(window x log) per log; the linear table phase is unchanged.
 #pragma once
 #include "warp_kernel.cuh"
+#include "patch_window.cuh"
 
 namespace ptk {
 
@@ -27,6 +35,7 @@ struct PatchParams {
     const pt_log_result* __restrict__ results;
     const uint64_t* __restrict__ text_off;      // capacity layout: where the log's element sequence starts
     const uint32_t* __restrict__ seq;           // element sequence (record index | deleted << 31)
+    const uint32_t* __restrict__ first_op;      // per log: list-op position of the window's first op (0: the whole log)
     uint32_t n_logs;
     uint32_t smem_bytes;                        // dynamic shared memory of the CTA (one warp)
     pt_patch_rec* recs;                         // one per ins/del record (same offsets as the records)
@@ -115,9 +124,11 @@ __global__ void __launch_bounds__(32) patch_logs_kernel(const PatchParams P) {
             mc += __popc(bal);
         }
         __syncwarp();
+        const uint32_t w0 = P.first_op[li], k0 = ptw::marks_before(mk, n, m, w0, lane), j0 = w0 - k0;
+        for (uint32_t i = lane; i < j0; i += 32) { pt_patch_rec z; z.index = 0; z.flags = 0; z.link_attr = PT_ATTR_NONE; z.reserved = 0; out[i] = z; }
 
         // ---- insert / delete patches: one lane per record, uniform loops over the elements / the mark ops -------------------
-        for (uint32_t ib = 0; ib < n; ib += 32) {
+        for (uint32_t ib = j0; ib < n; ib += 32) {
             const uint32_t i = ib + lane;
             const bool live = i < n;
             uint32_t p = 0; bool isIns = false;
@@ -170,7 +181,7 @@ __global__ void __launch_bounds__(32) patch_logs_kernel(const PatchParams P) {
         }
 
         // ---- mark patches: one lane per mark op X; intervals between consecutive slots defined at its arrival time ---------
-        for (uint32_t xb = 0; xb < m; xb += 32) {
+        for (uint32_t xb = k0; xb < m; xb += 32) {
             const uint32_t X = xb + lane;
             if (X >= m) continue;
             const uint32_t ps = Ps[X], pe = Pe[X];

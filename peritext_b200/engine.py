@@ -21,7 +21,7 @@ _lib = None
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
            "pt_batch_append", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
-           "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_query_elements", "pt_batch_find_elements",
+           "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
            "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
 
 
@@ -181,6 +181,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_set_comment_pool.argtypes = [vp, u64]
     L.pt_batch_download_patches.argtypes = [vp, vp]
     L.pt_batch_set_patch_pool.argtypes = [vp, u64]
+    L.pt_batch_set_patch_window.argtypes = [vp, vp, u32]
     L.pt_batch_query_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_find_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_render_json.argtypes = [vp, vp, vp]
@@ -217,6 +218,7 @@ class BatchEngine:
     def _uploaded(self, desc, n_insdel_total):
         """Record the shape of the batch just uploaded, in whichever form: what the downloads size their views by."""
         self.n_logs = len(desc)
+        self.patch_window = None                                             # every upload resets the window to whole logs
         self._n_insdel = int(n_insdel_total)                                 # patch records: one per ins/del record
         self._n_seq = int(desc["n_insdel"].astype(np.uint64).sum())          # element sequences: the capacity layout
 
@@ -255,6 +257,7 @@ class BatchEngine:
         _check(self._L.pt_batch_append(self._h, ctypes.byref(ops), ctypes.byref(st), ctypes.byref(ct[0]) if ct else None), "pt_batch_append")
         self._n_insdel += len(insdel)
         self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
+        self.patch_window = None                                             # so does an append
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion
@@ -356,16 +359,39 @@ class BatchEngine:
             return np.frombuffer(buf, dtype=dt, count=count).copy()
         return arr(v.recs, self._n_insdel, PATCH_REC_DT), arr(v.items, int(v.n_items), PATCH_ITEM_DT), arr(v.status, self.n_logs, np.uint32), int(v.n_items_needed)
 
-    def run_with_patches(self, batch: PackedBatch):
-        """upload -> merge (+ device Patch stream) -> download; returns (MergedBatch, DevicePatches)."""
-        out = self.run(batch)
+    def set_patch_window(self, first_ops=None):
+        """Restrict the Patch stream of the following merges to a suffix of every log's list ops (pt_batch_set_patch_window):
+        `first_ops[i]` is the position of log i's first op inside the window, in arrival order of the log's list ops (the
+        order of ``packing.list_ops`` / the patch JSON); None = whole logs.  After ``append``, the old n_insdel + n_mark of
+        each log gives exactly the new changes' ops.  Uploads and appends reset it; setting it after a merge makes that merge's
+        patches unavailable until the next merge."""
+        if first_ops is None:
+            _check(self._L.pt_batch_set_patch_window(self._h, None, self.n_logs), "pt_batch_set_patch_window")
+            self.patch_window = None
+            return
+        w = np.ascontiguousarray(first_ops, dtype=np.uint32)
+        _check(self._L.pt_batch_set_patch_window(self._h, w.ctypes.data if len(w) else None, len(w)), "pt_batch_set_patch_window")
+        self.patch_window = w.copy()
+
+    def run_with_patches(self, batch: PackedBatch, first_ops=None):
+        """upload -> merge (+ device Patch stream) -> download; returns (MergedBatch, DevicePatches).  `first_ops`: the
+        patch window of the merge (see ``set_patch_window``), carried into the DevicePatches."""
+        if first_ops is None:
+            out = self.run(batch)
+        else:
+            self.upload(batch)
+            if getattr(batch, "changes", None) is not None:
+                self.upload_changes(batch.changes)
+            self.set_patch_window(first_ops)
+            self.merge()
+            out = self._download_with_pool_retry()
         recs, items, status, needed = self.download_patches()
         if needed > len(items):
             _check(self._L.pt_batch_set_patch_pool(self._h, needed + 16), "pt_batch_set_patch_pool")
             self.merge(); out = self.download()
             recs, items, status, needed = self.download_patches()
         from .packing import DevicePatches
-        return out, DevicePatches(recs, items, status)
+        return out, DevicePatches(recs, items, status, self.patch_window)
 
     def query_elements(self, logs, indices, look_after_tombstones=False) -> np.ndarray:
         """Batched getListElementId on the device (reference src/micromerge.ts:762-805): for query k the index of the insert

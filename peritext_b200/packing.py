@@ -844,6 +844,8 @@ class DevicePatches:
     recs: np.ndarray      # PATCH_REC_DT per ins/del record (batch offsets)
     items: np.ndarray     # PATCH_ITEM_DT pool entries, any order
     status: np.ndarray    # per log: 0 computed on the device, 1 not computed (derive on the host)
+    first_op: np.ndarray | None = None   # per log: the patch window's first list op (None: whole logs); recs and items
+                                         # cover only the ops from there on
 
     def _index(self):
         if not hasattr(self, "_by_log"):
@@ -858,7 +860,7 @@ def patch_stream(batch: PackedBatch, dp: DevicePatches, i: int, ops: Sequence[di
     """Patches of log i as the reference's Patch objects (reference src/micromerge.ts:25-58), one list per list op of `ops`
     (= the log's list ops in arrival order, the same ops `pack_logs` packed).  insert: {path, action, index, values, marks};
     delete: {path, action, index, count: 1} (only the element's first delete emits); marks: {action, markType, path,
-    startIndex, [attrs], endIndex}."""
+    startIndex, [attrs], endIndex}.  Under a patch window (``dp.first_op``) the lists are those of ``ops[first_op[i]:]``."""
     if int(dp.status[i]) != 0:
         raise RangeError("patches of this log were not computed on the device")
     d = batch.desc[i]
@@ -872,8 +874,10 @@ def patch_stream(batch: PackedBatch, dp: DevicePatches, i: int, ops: Sequence[di
         else:
             comments.setdefault(tag, []).append(a)
     out = []
-    ri = mi = 0
-    for op in ops:
+    w0 = 0 if dp.first_op is None else int(dp.first_op[i])
+    mi = sum(1 for op in ops[:w0] if op["action"] in ("addMark", "removeMark"))
+    ri = w0 - mi
+    for op in ops[w0:]:
         act = op["action"]
         if act in ("addMark", "removeMark"):
             ps = []
