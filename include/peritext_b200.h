@@ -264,6 +264,15 @@ typedef struct pt_limits {
 } pt_limits;
 #define PT_FLAG_EMIT_SEQUENCE 1u   /* also emit the element sequence (needed by op generation / cursors on the host) */
 #define PT_FLAG_EMIT_PATCHES 2u    /* also derive the Patch stream of every op on the device (implies EMIT_SEQUENCE) */
+/* Also derive on the device the Patch stream of the logs the warp patch kernel declines (max_ctr x n_actors >= 0xFFFF, or
+ * tables above its 200 KB of shared memory), with a CTA-per-log arrival sweep (implies EMIT_PATCHES).  Then a log's patch
+ * status is 1 only if its merge failed (admission-rejected logs included); its records, items and item demand are what
+ * the warp kernel's contract below defines, window and pool rules included.  Cost: one more launch per merge when the
+ * batch has such logs, and a global scratch slab of min(such logs, SMs) slots, each sized by the largest such log
+ * (4 B per key of max_ctr x n_actors + ~13 B per ins/del record + 64 x next_pow2(2 n_mark + 1) B of mark trees + ~56 B
+ * per mark op, i.e. 180-320 B per mark op; the exact formula is ptp::large_layout in csrc/plan.h); pt_batch_upload /
+ * pt_batch_append fail with PT_ERR_NOMEM if it cannot be allocated. */
+#define PT_FLAG_EMIT_LARGE_PATCHES 4u
 
 /* ------------------------------------------------------------------------------------------------
  * Patch stream (PT_FLAG_EMIT_PATCHES): what Micromerge.applyChange returns for every op of a log, given the
@@ -289,7 +298,7 @@ typedef struct pt_patch_view {
     uint64_t n_items;
     uint64_t n_items_needed;       /* > the pool's capacity: call pt_batch_set_patch_pool(needed) and merge again */
     const uint32_t* status;        /* [n_logs] 0: computed; 1: not computed (log too large for the device patch kernel or
-                                      merge failed) — derive on the host                                          */
+                                      merge failed; with PT_FLAG_EMIT_LARGE_PATCHES merge failed only) — derive on the host */
 } pt_patch_view;
 
 typedef enum pt_status {

@@ -16,6 +16,7 @@
 #include "merge_kernel.cuh"
 #include "warp_kernel.cuh"
 #include "patch_kernel.cuh"
+#include "patch_large_kernel.cuh"
 #include "team_kernel.cuh"
 #include "render_kernel.cuh"
 #include "patch_json_kernel.cuh"
@@ -435,6 +436,7 @@ struct pt_batch {
     uint64_t n_changes = 0, n_deps = 0;
     DevBuf d_patch_recs, d_patch_items, d_patch_status;   // PT_FLAG_EMIT_PATCHES
     DevBuf d_patch_first;                                 // [n_logs] the patch window's first list op per log (0: whole log)
+    DevBuf d_large_cand, d_large_scratch;                 // PT_FLAG_EMIT_LARGE_PATCHES: candidate logs, scratch slots
     HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc, h_patch_first;
     DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // both JSON renders: the caller's pools
     JsonBufs spans_json, patches_json;                                  // each render's own scratch and view
@@ -491,10 +493,14 @@ int alloc_and_upload_plan(pt_batch* b) {
         if ((rc = b->d_patch_first.reserve(std::max<size_t>(1, n) * 4))) return rc;
         PT_CUDA(cudaMemsetAsync(b->d_patch_first.p, 0, std::max<size_t>(1, n) * 4, b->stream));   // every upload / append: whole logs
         b->patch_window_changed = false;
+        if (!pl.large_cand.empty()) {
+            if ((rc = b->d_large_cand.reserve(pl.large_cand.size() * 4))) return rc;
+            if ((rc = b->d_large_scratch.reserve((size_t)pl.large_slots * pl.large_bytes))) return rc;
+        }
     }
     if ((rc = b->d_slab.reserve(std::max<size_t>((size_t)pl.slab_slots * pl.slab_bytes, 16)))) return rc;
     // stage the small host-derived arrays through pinned memory
-    size_t stage = n * (sizeof(pt_log_desc) + 4 + 8 + 8) + 64;
+    size_t stage = n * (sizeof(pt_log_desc) + 4 + 8 + 8) + pl.large_cand.size() * 4 + 64;
     if ((rc = b->h_stage.reserve(stage))) return rc;
     char* s = (char*)b->h_stage.p;
     if (n) {
@@ -506,6 +512,10 @@ int alloc_and_upload_plan(pt_batch* b) {
         PT_CUDA(cudaMemcpyAsync(b->d_text_off.p, s, n * 8, cudaMemcpyHostToDevice, b->stream)); s += n * 8;
         memcpy(s, pl.span_off.data(), n * 8);
         PT_CUDA(cudaMemcpyAsync(b->d_span_off.p, s, n * 8, cudaMemcpyHostToDevice, b->stream)); s += n * 8;
+    }
+    if ((b->limits.flags & PT_FLAG_EMIT_PATCHES) && !pl.large_cand.empty()) {
+        memcpy(s, pl.large_cand.data(), pl.large_cand.size() * 4);
+        PT_CUDA(cudaMemcpyAsync(b->d_large_cand.p, s, pl.large_cand.size() * 4, cudaMemcpyHostToDevice, b->stream));
     }
     return PT_OK;
 }
@@ -770,6 +780,7 @@ int pt_batch_create(int device, const pt_limits* limits, void* cuda_stream, pt_b
     pt_batch* b = new pt_batch();
     b->device = device; b->stream = (cudaStream_t)cuda_stream; b->num_sms = prop.multiProcessorCount;
     if (limits) b->limits = *limits;
+    if (b->limits.flags & PT_FLAG_EMIT_LARGE_PATCHES) b->limits.flags |= PT_FLAG_EMIT_PATCHES;
     if (b->limits.flags & PT_FLAG_EMIT_PATCHES) b->limits.flags |= PT_FLAG_EMIT_SEQUENCE;
     if (cudaEventCreate(&b->ev0) != cudaSuccess || cudaEventCreate(&b->ev1) != cudaSuccess) { delete b; g_last_error = "cudaEventCreate failed"; return PT_ERR_CUDA; }
     if (b->stream != nullptr) {          // fork / join needs a real stream (not the legacy default stream)
@@ -1229,12 +1240,27 @@ static int enqueue_merge(pt_batch* b) {
         Q.recs = (pt_patch_rec*)b->d_patch_recs.p; Q.items = (pt_patch_item*)b->d_patch_items.p;
         Q.item_cursor = &c->patch_items; Q.item_cap = b->patch_cap;
         Q.status = (uint32_t*)b->d_patch_status.p;
-        PT_CUDA(cudaFuncSetAttribute(ptk::patch_logs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->plan.patch_smem));
-        const uint32_t per_sm = std::max<uint32_t>(1, std::min<uint32_t>(32, (227u * 1024u) / (b->plan.patch_smem + 1024u)));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(b->n_logs, (uint64_t)b->num_sms * per_sm);
-        ptk::patch_logs_kernel<<<grid, 32, b->plan.patch_smem, b->stream>>>(Q);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        const bool large = (b->limits.flags & PT_FLAG_EMIT_LARGE_PATCHES) && !b->plan.large_cand.empty();
+        const bool warp = !(b->limits.flags & PT_FLAG_EMIT_LARGE_PATCHES) || b->plan.cfg.patch_warp_on;
+        if (warp) {
+            PT_CUDA(cudaFuncSetAttribute(ptk::patch_logs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->plan.patch_smem));
+            const uint32_t per_sm = std::max<uint32_t>(1, std::min<uint32_t>(32, (227u * 1024u) / (b->plan.patch_smem + 1024u)));
+            const uint32_t grid = (uint32_t)std::min<uint64_t>(b->n_logs, (uint64_t)b->num_sms * per_sm);
+            ptk::patch_logs_kernel<<<grid, 32, b->plan.patch_smem, b->stream>>>(Q);
+            PT_CUDA(cudaGetLastError());
+            b->launches++;
+        }
+        if (large) {   // the logs the warp kernel declined (or, with PT_PATCH_WARP=0, every log)
+            ptk::LargePatchParams G{};
+            G.desc = Q.desc; G.insdel = Q.insdel; G.marks = Q.marks; G.results = Q.results; G.text_off = Q.text_off; G.seq = Q.seq;
+            G.first_op = Q.first_op;
+            G.cand = (const uint32_t*)b->d_large_cand.p; G.n_cand = (uint32_t)b->plan.large_cand.size(); G.after_warp = warp;
+            G.scratch = (char*)b->d_large_scratch.p; G.slot_bytes = b->plan.large_bytes;
+            G.recs = Q.recs; G.items = Q.items; G.item_cursor = Q.item_cursor; G.item_cap = Q.item_cap; G.status = Q.status;
+            ptk::patch_large_kernel<<<b->plan.large_slots, ptk::kLargeThreads, 0, b->stream>>>(G);
+            PT_CUDA(cudaGetLastError());
+            b->launches++;
+        }
     }
     return PT_OK;
 }

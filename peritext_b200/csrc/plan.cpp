@@ -12,6 +12,7 @@ RouteConfig RouteConfig::from_env() {
     RouteConfig c;
     if (const char* f = getenv("PT_WARP_FORCE")) c.force = atoi(f) != 0;
     if (const char* t = getenv("PT_TEAM")) c.team_on = atoi(t) != 0;
+    if (const char* pw = getenv("PT_PATCH_WARP")) c.patch_warp_on = atoi(pw) != 0;
     if (const char* w = getenv("PT_WARP")) {
         unsigned long a, wp, sl, ct;
         if (sscanf(w, "%lu:%lu:%lu:%lu", &a, &wp, &sl, &ct) == 4) {
@@ -86,6 +87,7 @@ const char* make_plan(const pt_packed_ops& ops, const pt_limits& limits, int num
     p.cfg = RouteConfig::from_env();
     const uint32_t nl = ops.n_logs;
     const bool emit_sequence = limits.flags & PT_FLAG_EMIT_SEQUENCE, emit_patches = limits.flags & PT_FLAG_EMIT_PATCHES;
+    const bool large = emit_patches && (limits.flags & PT_FLAG_EMIT_LARGE_PATCHES);
     std::vector<uint8_t> route(nl);
     p.text_off.resize(nl); p.span_off.resize(nl);
     uint64_t ncomment_bound = 0, patch_need = 4096;
@@ -107,9 +109,14 @@ const char* make_plan(const pt_packed_ops& ops, const pt_limits& limits, int num
             const uint64_t need = ((KS * 2 + 15) & ~15ull) + 3 * (((uint64_t)L.n_insdel * 2 + 15) & ~15ull) + (((uint64_t)L.n_insdel * 4 + 15) & ~15ull) +
                                   6 * (((uint64_t)L.n_mark * 4 + 15) & ~15ull) + (((uint64_t)L.n_mark * 2 + 15) & ~15ull) + 256;
             if (need <= 200 * 1024) patch_need = std::max(patch_need, need);
+            if (large && (!p.cfg.patch_warp_on || KS >= 0xFFFFull || need > 200 * 1024)) {
+                p.large_cand.push_back(i);
+                p.large_bytes = std::max<uint64_t>(p.large_bytes, large_patch_bytes(L.n_insdel, L.n_mark, KS, L.n_insdel));
+            }
         }
     }
     if (emit_patches) p.patch_smem = (uint32_t)((patch_need + 1023) & ~1023ull);   // one warp per CTA: the largest footprint
+    p.large_slots = (uint32_t)std::min<size_t>(p.large_cand.size(), (size_t)num_sms * kLargeCtasPerSm);
     // default pool: 4 entries per mark op (+slack) fits the generated workloads (c3, the densest, needs < 2); a batch that needs
     // more reports its exact demand and merges again (BatchEngine.run), so the pool need not be sized for the worst case
     p.pool_cap = limits.comment_pool_entries ? limits.comment_pool_entries : 4ull * ncomment_bound + 1024;

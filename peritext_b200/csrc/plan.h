@@ -33,11 +33,44 @@ constexpr uint32_t kTeamSmem = 55u * 1024u;
 //                              leaves the default bin
 //   PT_WARP_FORCE=1            send a log to the warp kernel without the host's footprint estimate (device-side deferral)
 //   PT_TEAM=0                  no team kernel
+//   PT_PATCH_WARP=0            with PT_FLAG_EMIT_LARGE_PATCHES: no patch_logs_kernel; every log is a candidate of
+//                              patch_large_kernel (tests reach the large kernel with small logs; the probe times it on them)
 struct RouteConfig {
     BinCfg warp = kWarpBin;
-    bool warp_on = true, team_on = true, force = false;
+    bool warp_on = true, team_on = true, force = false, patch_warp_on = true;
     static RouteConfig from_env();
 };
+
+#ifdef __CUDACC__
+#define PTP_HD __host__ __device__
+#else
+#define PTP_HD
+#endif
+// The global scratch slot of one patch_large_kernel log (patch_large_kernel.cuh): byte offsets of its tables, 16-aligned.
+// The host sizes a slot with N = n (N, the log's element count, is at most n); the kernel lays it out with the real N.
+struct LargeLayout {
+    uint64_t T, PosOf, TIns, TDel, Ps, Pe, PeRaw, MKey, MInf, MAttr, MArr, CIdx, Pres, Vis, PresPre, VisPre, SBits, SPre, Bnd, FirstDef, Tree, CSort, bytes;
+    uint32_t NW, SW, P2, P2c;   // bitmap words over positions / over slots; leaves per mark-type tree; comment sort length
+};
+PTP_HD inline uint64_t large_take(uint64_t& at, uint64_t bytes) { const uint64_t o = at; at += (bytes + 15) & ~15ull; return o; }
+PTP_HD inline LargeLayout large_layout(uint64_t n, uint64_t m, uint64_t KS, uint64_t N) {
+    LargeLayout g{};
+    uint64_t at = 0;
+    g.NW = (uint32_t)(N >> 5) + 1; g.SW = (uint32_t)((2 * N) >> 5) + 1;
+    g.P2 = 1; while (g.P2 < 2 * m + 1) g.P2 <<= 1;
+    g.P2c = 1; while (g.P2c < m) g.P2c <<= 1;
+    g.T = large_take(at, 4 * KS); g.PosOf = large_take(at, 4 * n); g.TIns = large_take(at, 4 * N); g.TDel = large_take(at, 4 * N);
+    g.Ps = large_take(at, 4 * m); g.Pe = large_take(at, 4 * m); g.PeRaw = large_take(at, 4 * m); g.MKey = large_take(at, 4 * m);
+    g.MInf = large_take(at, 4 * m); g.MAttr = large_take(at, 4 * m); g.MArr = large_take(at, 4 * m); g.CIdx = large_take(at, 4 * m);
+    g.Pres = large_take(at, 4ull * g.NW); g.Vis = large_take(at, 4ull * g.NW); g.PresPre = large_take(at, 4ull * (g.NW + 1)); g.VisPre = large_take(at, 4ull * (g.NW + 1));
+    g.SBits = large_take(at, 4ull * g.SW); g.SPre = large_take(at, 4ull * (g.SW + 1));
+    g.Bnd = large_take(at, 4 * (2 * m + 2)); g.FirstDef = large_take(at, 4 * (2 * m + 2));
+    g.Tree = large_take(at, 8ull * 4 * 2 * g.P2); g.CSort = large_take(at, 8ull * g.P2c);
+    g.bytes = at;
+    return g;
+}
+PTP_HD inline uint64_t large_patch_bytes(uint64_t n, uint64_t m, uint64_t KS, uint64_t N) { return large_layout(n, m, KS, N).bytes; }
+constexpr uint32_t kLargeCtasPerSm = 1;       // patch_large_kernel: 512 threads, one resident CTA per SM
 
 // Where a log is merged.  Bin 0's list holds, in this order, the warp kernel's three id-table launches and the team kernel.
 enum Route : uint8_t { kPacked3, kCompact, kDirect, kTeam, kCta1, kCta2, kCta3, kCta4, kNumRoutes };
@@ -58,6 +91,12 @@ struct Plan {
     uint32_t n_spill = 0, slab_slots = 0;     // logs that can spill to the global slab / slab slots to allocate
     size_t slab_bytes = 0;                    // per slot
     uint32_t patch_smem = 0;                  // patch kernel's shared memory (PT_FLAG_EMIT_PATCHES)
+    // PT_FLAG_EMIT_LARGE_PATCHES: the logs patch_logs_kernel can decline besides failed merges (key space >= 0xFFFF, or a
+    // host footprint estimate above its 200 KB cap; every log with PT_PATCH_WARP=0), the scratch bytes of one slot (the
+    // largest candidate) and the slots (one per resident CTA of patch_large_kernel, at most one per candidate)
+    std::vector<uint32_t> large_cand;
+    uint64_t large_bytes = 0;
+    uint32_t large_slots = 0;
 };
 
 // Plans the batch into `plan`; returns nullptr, or what is wrong with the descriptors (then `plan` is unchanged).

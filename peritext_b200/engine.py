@@ -143,6 +143,7 @@ PATCH_REC_DT = np.dtype([("index", "<u4"), ("flags", "<u4"), ("link_attr", "<u4"
 PATCH_ITEM_DT = np.dtype([("log", "<u4"), ("tag", "<u4"), ("a", "<u4"), ("b", "<u4")])
 FLAG_EMIT_SEQUENCE = 1
 FLAG_EMIT_PATCHES = 2
+FLAG_EMIT_LARGE_PATCHES = 4
 
 
 def load_library() -> ctypes.CDLL:
@@ -204,12 +205,17 @@ class BatchEngine:
     """One handle per (GPU, batch).  ``upload`` -> ``merge`` -> ``download``."""
 
     def __init__(self, device: int = 0, stream: int | None = None, comment_pool_entries: int = 0, emit_sequence: bool = False,
-                 emit_patches: bool = False):
+                 emit_patches: bool = False, large_patches: bool = False):
+        """``large_patches`` (PT_FLAG_EMIT_LARGE_PATCHES, implies ``emit_patches``): the device also derives the Patch stream of
+        the logs too large for the warp patch kernel, so a log's patch status is 1 only if its merge failed."""
         L = load_library()
         self._L = L
         self._h = ctypes.c_void_p()
+        emit_patches = emit_patches or large_patches
         self.emit_patches = emit_patches
-        flags = (FLAG_EMIT_SEQUENCE if (emit_sequence or emit_patches) else 0) | (FLAG_EMIT_PATCHES if emit_patches else 0)
+        self.large_patches = large_patches
+        flags = (FLAG_EMIT_SEQUENCE if (emit_sequence or emit_patches) else 0) | (FLAG_EMIT_PATCHES if emit_patches else 0) | \
+            (FLAG_EMIT_LARGE_PATCHES if large_patches else 0)
         lim = _Limits(comment_pool_entries, flags, 0, (ctypes.c_uint32 * 4)())
         _check(L.pt_batch_create(device, ctypes.byref(lim), ctypes.c_void_p(stream or 0), ctypes.byref(self._h)), "pt_batch_create")
         self._keep = None
