@@ -407,6 +407,90 @@ typedef struct pt_append_remap {      /* NULL pointer = identity everywhere */
  * batch. */
 int pt_batch_append(pt_batch*, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* delta_changes);
 
+/* ------------------------------------------------------------------------------------------------
+ * Local changes: Micromerge.change (src/micromerge.ts:308-441, changeMark src/peritext.ts:458-501) for many documents at
+ * once.  Each log's InputOperations are resolved on the device against the document of the last merge, in order, each
+ * generated op applied before the next (so an index refers to the document after the earlier InputOperations of the same
+ * change), and the generated records are appended to the resident batch without leaving the device.
+ * ---------------------------------------------------------------------------------------------- */
+#define PT_INPUT_INSERT 0u
+#define PT_INPUT_DELETE 1u
+#define PT_INPUT_ADD_MARK 2u
+#define PT_INPUT_REMOVE_MARK 3u
+typedef struct pt_input_op {   /* one InputOperation on the log's text list. 32 B */
+    uint8_t  action;     /* PT_INPUT_*                                                                                */
+    uint8_t  mark_type;  /* marks: PT_MARK_*; 0 otherwise                                                             */
+    uint16_t reserved0;  /* 0                                                                                         */
+    int32_t  index;      /* insert / delete: index; marks: startIndex (negative: out of bounds, as in the reference)  */
+    int32_t  arg;        /* insert: number of values (>= 0); delete: count (<= 0 generates nothing); marks: endIndex    */
+    uint32_t attr;       /* marks: as pt_mark_rec.attr (link url id < n_links, comment rank < n_comments; PT_ATTR_NONE
+                            for strong / em); PT_ATTR_NONE otherwise                                                  */
+    uint32_t first_ctr;  /* packed counter of the first op the record generates; op j gets first_ctr + j (makeNewOp,
+                            src/micromerge.ts:483-493).  A record that generates no op still needs a value > the log's
+                            max_ctr and >= the previous record's next counter                                         */
+    uint32_t reserved1;  /* 0                                                                                         */
+    uint64_t tok_off;    /* insert: its `arg` value tokens are tokens[tok_off ..] (PT_PAYLOAD_TOKEN values: a code point
+                            <= 0x10FFFF, or PT_TOKEN_POOLED | value-pool index < n_values)                             */
+} pt_input_op;
+#define PT_CHANGE_NO_ACTOR 0xFFFFFFFFu
+typedef struct pt_change_input {
+    uint32_t n_logs;             /* must equal the batch's n_logs                                                       */
+    const uint32_t* actor;       /* [n_logs] the acting actor's rank in the log, or PT_CHANGE_NO_ACTOR: no change        */
+    const uint64_t* input_off;   /* [n_logs + 1] log i's InputOperations are ops[input_off[i] .. input_off[i+1]), in the
+                                    change's order (a log without an actor must have none)                              */
+    const pt_input_op* ops;
+    const uint32_t* tokens;      /* [n_tokens] */
+    uint64_t n_tokens;
+    uint32_t n_values, n_links, n_comments;   /* the pools the tokens and attrs index (bounds of the checks above)     */
+    uint32_t reserved;
+} pt_change_input;
+#define PT_CHANGE_OK 0u
+#define PT_CHANGE_OUT_OF_BOUNDS 1u   /* "List index out of bounds" (src/micromerge.ts:804): the log appends nothing */
+typedef struct pt_change_status { uint32_t status; uint32_t input; } pt_change_status;   /* 8 B; input: the failing
+                                                    InputOperation relative to the log's first, 0xFFFFFFFF when OK */
+typedef struct pt_change_view {
+    uint32_t n_logs;
+    const pt_change_status* status;   /* [n_logs]                                                                     */
+    pt_packed_ops delta;              /* the generated records: descriptor i = log i's new records (n_insdel = n_mark = 0
+                                         for a failed log or one without a change), with the log's n_actors and new max_ctr */
+} pt_change_view;
+
+/* Generate every log's local change from its InputOperations on the device and append the generated records to the resident
+ * batch.  Per InputOperation, against the document of the last merge with the earlier generated ops applied (exactly the list
+ * ops of Micromerge.change):
+ *   insert      reference = HEAD if index == 0, else the (index - 1)-th visible element with lookAfterTombstones (the last
+ *               following tombstone whose markOpsAfter slot is defined, src/micromerge.ts:775-797), evaluated before the values,
+ *               so a zero-value insert out of bounds still fails; value j references value j - 1 and lands right after it
+ *   delete      `arg` times: the index-th visible element, which is deleted before the next
+ *   add/remove  start = before(elem[startIndex]); end = endOfText for strong / em when endIndex >= the visible length, else
+ *   Mark        before(elem[endIndex]); for comment / link after(elem[endIndex - 1]), which defines that element's after slot
+ *               for the InputOperations that follow; arrival = the log's ins/del records before the mark
+ * Generated records: ins/del op j of a record has ctr first_ctr + j and the actor's rank; insert references, delete targets and
+ * mark boundaries are the resolved elements' packed opIds.  A log whose change hits "List index out of bounds" appends
+ * nothing (status PT_CHANGE_OUT_OF_BOUNDS, `input` names the failing InputOperation) and the other logs proceed; the
+ * reference instead bumps seq and keeps the ops it generated before the throw.
+ * `changes` is the change table of the new changes (one pt_change_rec per log that has a change, as for pt_batch_append;
+ * NULL iff the handle has no change table); the records of failed logs are dropped.  A new actor or comment id shifts packed
+ * ranks: introduce it first with a pt_batch_append of an empty delta and its remap, then call this with the new ranks.
+ * Refused before anything changes:
+ *   PT_ERR_STATE    no completed merge since the last upload, append or change; a handle without PT_FLAG_EMIT_SEQUENCE
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) n_logs differs; input_off not increasing from 0 or past the ops; a log
+ *                   with inputs and no actor; an actor rank >= the log's n_actors; a log with a change whose merge status is not
+ *                   PT_LOG_OK; an unknown action or mark type; first_ctr not above the log's max_ctr, or below the previous
+ *                   record's next counter, or a counter past 2^32 - 1; an attr or a token out of range; a log that would hold
+ *                   2^22 elements or more, or whose max_ctr x n_actors would reach 2^31; a change table on one side only
+ * On success the handle holds exactly the batch pt_batch_append of the view's delta with identity maps would give (the same
+ * re-plan; no merge, so views of the last merge are invalid; the patch window is reset; pools persist).  A following merge
+ * under pt_batch_set_patch_window(first_op = old n_insdel + n_mark) gives the Patch stream change() returns.
+ * The view is engine-owned pinned memory, valid until the next upload, append, change or destroy.  Synchronises; the caller's
+ * arrays may be freed on return.
+ * Device: one warp per log with InputOperations copies the log's element sequence into a scratch slot (n_elems + its insert
+ * values words) and resolves the InputOperations in order: ballot / popcount selection of the k-th visible element (O(N) per
+ * InputOperation, the reference's own cost), one warp-cooperative splice per insert, the deleted bit per delete, the
+ * after-slot bit per `after` end; it writes the records into the delta as it goes.  The delta goes through pt_batch_append's
+ * splice on the device. */
+int pt_batch_change(pt_batch*, const pt_change_input* in, const pt_change_table* changes, pt_change_view* out);
+
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */
 int pt_batch_merge(pt_batch*);

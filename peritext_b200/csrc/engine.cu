@@ -21,6 +21,7 @@
 #include "render_kernel.cuh"
 #include "patch_json_kernel.cuh"
 #include "append_kernel.cuh"
+#include "change_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -448,6 +449,7 @@ struct pt_batch {
     const pt_mark_rec* dp_marks = nullptr;
     // pinned host
     HostBuf h_stage, h_results, h_text, h_spans, h_pool, h_misc, h_seq, h_ctoff, h_csoff;
+    HostBuf h_chg_status, h_chg_desc, h_chg_insdel, h_chg_marks;   // the view of the last pt_batch_change
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -1000,7 +1002,7 @@ int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
 
 // Host checks of a delta and its remap against the resident batch (include/peritext_b200.h, pt_batch_append); on success
 // nd / ncd hold the descriptors of the concatenated batch and its change table.  Returns the problem, or an empty string.
-static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, const pt_append_remap& R, const pt_change_table* dch,
+static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, bool delta_on_device, const pt_append_remap& R, const pt_change_table* dch,
                                 std::vector<pt_log_desc>& nd, std::vector<pt_change_desc>& ncd, uint32_t& maxR) {
     const uint32_t n = b->n_logs;
     auto at = [](uint32_t i) { return "log " + std::to_string(i) + ": "; };
@@ -1045,7 +1047,7 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, c
         } else if (O.max_ctr > D.max_ctr) {
             return at(i) + "the new max_ctr is below the old (identity counter map)";
         }
-        for (uint32_t k = 0; k < D.n_mark; k++) {
+        for (uint32_t k = 0; !delta_on_device && k < D.n_mark; k++) {     // device records (pt_batch_change) carry their arrival by construction
             const uint32_t a = delta.marks[D.mark_off + k].arrival;
             if (a < O.n_insdel || a > (uint64_t)O.n_insdel + D.n_insdel) return at(i) + "delta mark " + std::to_string(k) + " has arrival " + std::to_string(a) +
                                                                                  " outside [" + std::to_string(O.n_insdel) + ", " + std::to_string((uint64_t)O.n_insdel + D.n_insdel) + "]";
@@ -1071,21 +1073,21 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, c
     return std::string();
 }
 
-int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* dch) {
-    if (!b || !delta || (delta->n_logs && !delta->logs)) return PT_ERR_INVALID;
-    if (!b->have_batch) { g_last_error = "pt_batch_append before pt_batch_upload"; return PT_ERR_STATE; }
-    const pt_append_remap R = remap ? *remap : pt_append_remap{};
+// pt_batch_append after its host checks, and the append of pt_batch_change: `delta`'s records are host memory, or device memory
+// the caller keeps alive (delta_on_device).  The delta's descriptors, the remap and the change table are host memory.
+static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R, const pt_change_table* dch) {
+    static const char* fn_name[2] = {"pt_batch_append: ", "pt_batch_change: "};
     std::vector<pt_log_desc> nd;
     std::vector<pt_change_desc> ncd;
     uint32_t maxR = 1;
-    std::string err = check_append(b, *delta, R, dch, nd, ncd, maxR);
+    std::string err = check_append(b, *delta, delta_on_device, R, dch, nd, ncd, maxR);
     const uint32_t n = b->n_logs;
     const bool sized = err.empty() && n;                      // nd is filled only when the checks passed
     const uint64_t n_ins = sized ? nd[n - 1].insdel_off + nd[n - 1].n_insdel : 0, n_mk = sized ? nd[n - 1].mark_off + nd[n - 1].n_mark : 0;
     const pt_packed_ops ops{n, nd.data(), nullptr, n_ins, nullptr, n_mk};
     ptp::Plan plan;
     if (err.empty()) if (const char* e = ptp::make_plan(ops, b->limits, b->num_sms, plan)) err = e;
-    if (!err.empty()) { g_last_error = "pt_batch_append: " + err; return PT_ERR_INVALID; }
+    if (!err.empty()) { g_last_error = fn_name[delta_on_device] + err; return PT_ERR_INVALID; }
     PT_CUDA(cudaSetDevice(b->device));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge and downloads of the resident batch are done
     // The delta and the remap go to the device; the splice writes NEW buffers, so the resident batch stays intact until the
@@ -1095,14 +1097,19 @@ int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_rem
     DevBuf ndesc, nins, nmarks, ncdesc, nch, ndp;              // the new batch's descriptors, records and change table
     DevBuf ddesc, dins, dmarks, dcdesc, dchg, ddep, amap[5], abad;   // the delta, its remap and the refusal flag: freed on return
     if ((rc = ddesc.reserve(dsz)) || (rc = ndesc.reserve(dsz)) || (rc = abad.reserve(4)) ||
-        (rc = dins.reserve(std::max<uint64_t>(1, delta->n_insdel_total) * sizeof(pt_insdel_rec))) ||
-        (rc = dmarks.reserve(std::max<uint64_t>(1, delta->n_mark_total) * sizeof(pt_mark_rec))) ||
         (rc = nins.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = nmarks.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec)))) return rc;
     auto h2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
     PT_CUDA(h2d(ddesc.p, delta->logs, (size_t)n * sizeof(pt_log_desc)));
     PT_CUDA(h2d(ndesc.p, nd.data(), (size_t)n * sizeof(pt_log_desc)));
-    PT_CUDA(h2d(dins.p, delta->insdel, delta->n_insdel_total * sizeof(pt_insdel_rec)));
-    PT_CUDA(h2d(dmarks.p, delta->marks, delta->n_mark_total * sizeof(pt_mark_rec)));
+    const pt_insdel_rec* d_dins = delta->insdel;
+    const pt_mark_rec* d_dmarks = delta->marks;
+    if (!delta_on_device) {
+        if ((rc = dins.reserve(std::max<uint64_t>(1, delta->n_insdel_total) * sizeof(pt_insdel_rec))) ||
+            (rc = dmarks.reserve(std::max<uint64_t>(1, delta->n_mark_total) * sizeof(pt_mark_rec)))) return rc;
+        PT_CUDA(h2d(dins.p, delta->insdel, delta->n_insdel_total * sizeof(pt_insdel_rec)));
+        PT_CUDA(h2d(dmarks.p, delta->marks, delta->n_mark_total * sizeof(pt_mark_rec)));
+        d_dins = (const pt_insdel_rec*)dins.p; d_dmarks = (const pt_mark_rec*)dmarks.p;
+    }
     pta::Remap DR{};
     const void* hsrc[5] = {R.actor_off, R.actor_map, R.ctr_off, R.ctr_map, R.comment_map};
     const size_t hbytes[5] = {R.actor_off ? ((size_t)n + 1) * 8 : 0, R.actor_off ? (size_t)R.actor_off[n] * 2 : 0,
@@ -1127,7 +1134,7 @@ int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_rem
         const uint32_t slices = (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, most / 8192));
         const dim3 rgrid(std::max<uint32_t>(1, std::min<uint32_t>(grid, (uint32_t)b->num_sms * 16 / slices)), slices);
         pta::splice_records_kernel<<<rgrid, threads, 0, b->stream>>>((const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, n, DR,
-                                                                    b->dp_insdel, b->dp_marks, (const pt_insdel_rec*)dins.p, (const pt_mark_rec*)dmarks.p,
+                                                                    b->dp_insdel, b->dp_marks, d_dins, d_dmarks,
                                                                     (pt_insdel_rec*)nins.p, (pt_mark_rec*)nmarks.p, (uint32_t*)abad.p);
         PT_CUDA(cudaGetLastError());
         b->launches++;
@@ -1156,7 +1163,7 @@ int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_rem
     uint32_t bad = 0;
     PT_CUDA(cudaMemcpyAsync(&bad, abad.p, 4, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // also: the caller's arrays may be freed on return
-    if (bad) { g_last_error = "pt_batch_append: a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
+    if (bad) { g_last_error = std::string(fn_name[delta_on_device]) + "a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
     // Accepted: the new records and change table replace the old ones (freed with the locals), and the batch is re-planned.
     b->have_batch = false; b->merged = false; b->dl_begun = false;
     drop_graph(b);
@@ -1169,6 +1176,172 @@ int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_rem
     PT_CUDA(cudaStreamSynchronize(b->stream));
     b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p;
     b->have_batch = true;
+    return PT_OK;
+}
+
+int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* dch) {
+    if (!b || !delta || (delta->n_logs && !delta->logs)) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_append before pt_batch_upload"; return PT_ERR_STATE; }
+    return splice_append(b, delta, false, remap ? *remap : pt_append_remap{}, dch);
+}
+
+// pt_batch_change's host checks of the InputOperations (include/peritext_b200.h).  On success dd holds the delta layout for
+// every log succeeding (records in log order, the new max_ctr), new_elems each log's insert values and work the logs with a
+// change.  Returns the problem, or an empty string.
+static std::string check_change(const pt_batch* b, const pt_change_input& in, std::vector<pt_log_desc>& dd, std::vector<uint32_t>& new_elems,
+                                std::vector<uint32_t>& work) {
+    const uint32_t n = b->n_logs;
+    auto at = [](uint32_t i) { return "log " + std::to_string(i) + ": "; };
+    if (in.n_logs != n) return "the input has " + std::to_string(in.n_logs) + " logs and the batch " + std::to_string(n);
+    if (!n) return std::string();
+    if (!in.actor || !in.input_off) return "null actor or input_off";
+    if (in.input_off[0] != 0) return "input_off[0] is not 0";
+    if ((in.input_off[n] && !in.ops) || (in.n_tokens && !in.tokens)) return "null ops or tokens with a nonzero count";
+    dd.resize(n); new_elems.assign(n, 0);
+    uint64_t io = 0, mo = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const pt_log_desc& L = b->h_desc[i];
+        const uint64_t lo = in.input_off[i], hi = in.input_off[i + 1];
+        if (hi < lo) return "input_off decreases at log " + std::to_string(i);
+        dd[i] = pt_log_desc{io, mo, 0, 0, L.n_actors, L.max_ctr};
+        const uint32_t A = in.actor[i];
+        if (A == PT_CHANGE_NO_ACTOR) {
+            if (hi > lo) return at(i) + "InputOperations without an actor";
+            continue;
+        }
+        if (A >= L.n_actors) return at(i) + "actor rank " + std::to_string(A) + " >= the log's " + std::to_string(L.n_actors) + " actors";
+        uint64_t next = (uint64_t)L.max_ctr + 1, last = L.max_ctr, nid = 0, nmk = 0, nel = 0;
+        for (uint64_t k = lo; k < hi; k++) {
+            const pt_input_op& op = in.ops[k];
+            const std::string here = at(i) + "InputOperation " + std::to_string(k - lo) + ": ";
+            uint64_t gen = 0;
+            if (op.action == PT_INPUT_INSERT) {
+                if (op.arg < 0) return here + "a negative number of values";
+                gen = (uint64_t)op.arg;
+                if (op.tok_off > in.n_tokens || gen > in.n_tokens - op.tok_off) return here + "tokens out of range";
+                for (uint64_t j = 0; j < gen; j++) {
+                    const uint32_t t = in.tokens[op.tok_off + j];
+                    const bool ok = (t & PT_TOKEN_POOLED) ? (t >> 30) == 0 && (t & (PT_TOKEN_POOLED - 1)) < in.n_values : t <= 0x10FFFFu;
+                    if (!ok) return here + "token " + std::to_string(j) + " (" + std::to_string(t) + ") out of range";
+                }
+                nid += gen; nel += gen;
+            } else if (op.action == PT_INPUT_DELETE) {
+                gen = op.arg > 0 ? (uint64_t)op.arg : 0;
+                nid += gen;
+            } else if (op.action == PT_INPUT_ADD_MARK || op.action == PT_INPUT_REMOVE_MARK) {
+                if (op.mark_type > PT_MARK_LINK) return here + "unknown mark type " + std::to_string(op.mark_type);
+                const bool ok = op.mark_type == PT_MARK_LINK ? op.attr < in.n_links : op.mark_type == PT_MARK_COMMENT ? op.attr < in.n_comments : op.attr == PT_ATTR_NONE;
+                if (!ok) return here + "attr " + std::to_string(op.attr) + " out of range";
+                gen = 1; nmk++;
+            } else {
+                return here + "unknown action " + std::to_string(op.action);
+            }
+            if (op.first_ctr < next)
+                return here + "first_ctr " + std::to_string(op.first_ctr) + " is below " + std::to_string(next) + " (the log's max_ctr + 1, or the previous InputOperation's next counter)";
+            if (op.first_ctr + gen - (gen ? 1 : 0) > 0xFFFFFFFFull) return here + "counters past 2^32 - 1";
+            next = op.first_ctr + gen;
+            if (gen) last = op.first_ctr + gen - 1;
+        }
+        if (last * std::max<uint32_t>(1, L.n_actors) > 0x7FFFFFFFull) return at(i) + "max_ctr x n_actors would reach 2^31";
+        if (L.n_insdel + nid > 0xFFFFFFFFull || L.n_mark + nmk > 0xFFFFFFFFull) return at(i) + "more than 2^32 - 1 records";
+        dd[i].n_insdel = (uint32_t)nid; dd[i].n_mark = (uint32_t)nmk; dd[i].max_ctr = (uint32_t)last;
+        new_elems[i] = (uint32_t)std::min<uint64_t>(nel, 0xFFFFFFFFu);
+        work.push_back(i);
+        io += nid; mo += nmk;
+    }
+    return std::string();
+}
+
+int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_table* changes, pt_change_view* out) {
+    if (!b || !in || !out) return PT_ERR_INVALID;
+    if (!b->have_batch || !b->merged) { g_last_error = "pt_batch_change: no completed merge since the last upload, append or change"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = "pt_batch_change: the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs;
+    std::string err;
+    if ((changes != nullptr) != b->have_changes)
+        err = b->have_changes ? "the batch has a change table and the change none" : "the change has a change table and the batch none";
+    else if (changes && (changes->n_logs != n || (n && !changes->logs)))
+        err = "the change table does not match the batch";
+    std::vector<pt_log_desc> dd;
+    std::vector<uint32_t> new_elems, work;
+    if (err.empty()) err = check_change(b, *in, dd, new_elems, work);
+    if (!err.empty()) { g_last_error = "pt_batch_change: " + err; return PT_ERR_INVALID; }
+    const uint64_t n_ins = n ? dd[n - 1].insdel_off + dd[n - 1].n_insdel : 0, n_mk = n ? dd[n - 1].mark_off + dd[n - 1].n_mark : 0;
+    std::vector<unsigned long long> soff(std::max<uint32_t>(1, n), 0);
+    uint64_t n_scratch = 0;
+    for (uint32_t i : work) {                          // a slot holds the log's elements and its new ones, 16-byte aligned
+        soff[i] = n_scratch;
+        n_scratch += ((uint64_t)b->h_desc[i].n_insdel + new_elems[i] + 3) & ~3ull;
+    }
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge is complete
+    int rc;
+    DevBuf dwork, dactor, dioff, dops, dtok, ddelta, dnel, dsoff, dscr, dst, dgi, dgm;   // freed on return
+    const uint64_t n_ops = n ? in->input_off[n] : 0;
+    const size_t nn = std::max<uint32_t>(1, n);
+    if ((rc = dwork.reserve(std::max<size_t>(1, work.size()) * 4)) || (rc = dactor.reserve(nn * 4)) || (rc = dioff.reserve((nn + 1) * 8)) ||
+        (rc = dops.reserve(std::max<uint64_t>(1, n_ops) * sizeof(pt_input_op))) || (rc = dtok.reserve(std::max<uint64_t>(1, in->n_tokens) * 4)) ||
+        (rc = ddelta.reserve(nn * sizeof(pt_log_desc))) || (rc = dnel.reserve(nn * 4)) || (rc = dsoff.reserve(nn * 8)) ||
+        (rc = dscr.reserve(std::max<uint64_t>(4, n_scratch) * 4)) || (rc = dst.reserve(nn * sizeof(pt_change_status))) ||
+        (rc = dgi.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = dgm.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))))
+        return rc;
+    auto h2d = [&](void* dst_, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst_, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
+    PT_CUDA(h2d(dwork.p, work.data(), work.size() * 4));
+    if (n) {
+        PT_CUDA(h2d(dactor.p, in->actor, (size_t)n * 4));
+        PT_CUDA(h2d(dioff.p, in->input_off, ((size_t)n + 1) * 8));
+        PT_CUDA(h2d(ddelta.p, dd.data(), (size_t)n * sizeof(pt_log_desc)));
+        PT_CUDA(h2d(dnel.p, new_elems.data(), (size_t)n * 4));
+        PT_CUDA(h2d(dsoff.p, soff.data(), (size_t)n * 8));
+    }
+    if (n) PT_CUDA(cudaMemsetAsync(dst.p, 0, (size_t)n * sizeof(pt_change_status), b->stream));   // logs without a change: OK
+    PT_CUDA(h2d(dops.p, in->ops, n_ops * sizeof(pt_input_op)));
+    PT_CUDA(h2d(dtok.p, in->tokens, in->n_tokens * 4));
+    if (!work.empty()) {
+        ptc::ChangeParams P{};
+        P.work = (const uint32_t*)dwork.p; P.n_work = (uint32_t)work.size();
+        P.desc = (const pt_log_desc*)b->d_desc.p; P.insdel = b->dp_insdel; P.results = (const pt_log_result*)b->d_results.p;
+        P.seq_off = (const uint64_t*)b->d_text_off.p; P.seq = (const uint32_t*)b->d_seq.p;
+        P.actor = (const uint32_t*)dactor.p; P.input_off = (const unsigned long long*)dioff.p; P.ops = (const pt_input_op*)dops.p;
+        P.tokens = (const uint32_t*)dtok.p; P.delta = (const pt_log_desc*)ddelta.p; P.new_elems = (const uint32_t*)dnel.p;
+        P.scratch_off = (const unsigned long long*)dsoff.p; P.scratch = (uint32_t*)dscr.p;
+        P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.status = (pt_change_status*)dst.p;
+        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)work.size() * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+        ptc::change_resolve_kernel<<<grid, threads, 0, b->stream>>>(P);
+        PT_CUDA(cudaGetLastError());
+        b->launches++;
+    }
+    // the status of every log (the logs without a change are OK) and the generated records, into the view's pinned buffers
+    if ((rc = b->h_chg_status.reserve(nn * sizeof(pt_change_status))) || (rc = b->h_chg_desc.reserve(nn * sizeof(pt_log_desc))) ||
+        (rc = b->h_chg_insdel.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = b->h_chg_marks.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))))
+        return rc;
+    pt_change_status* st = (pt_change_status*)b->h_chg_status.p;
+    if (n) PT_CUDA(cudaMemcpyAsync(st, dst.p, (size_t)n * sizeof(pt_change_status), cudaMemcpyDeviceToHost, b->stream));
+    if (n_ins) PT_CUDA(cudaMemcpyAsync(b->h_chg_insdel.p, dgi.p, n_ins * sizeof(pt_insdel_rec), cudaMemcpyDeviceToHost, b->stream));
+    if (n_mk) PT_CUDA(cudaMemcpyAsync(b->h_chg_marks.p, dgm.p, n_mk * sizeof(pt_mark_rec), cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    for (uint32_t i = 0; i < n; i++) if (st[i].status == PT_CHANGE_OK) st[i].input = 0xFFFFFFFFu;
+    for (uint32_t i : work)
+        if (st[i].status == ptc::kRefuseMergeStatus || st[i].status == ptc::kRefuseElements) {
+            g_last_error = "pt_batch_change: log " + std::to_string(i) + (st[i].status == ptc::kRefuseMergeStatus ? ": its merge status is not PT_LOG_OK"
+                                                                                                                  : ": the change would bring it to 2^22 elements or more");
+            return PT_ERR_INVALID;
+        }
+    // a log whose change failed appends nothing: no records, its old max_ctr, no change record
+    std::vector<pt_change_desc> cdesc;
+    pt_change_table ct{};
+    if (changes) { cdesc.assign(changes->logs, changes->logs + n); ct = *changes; ct.logs = cdesc.data(); }
+    for (uint32_t i : work)
+        if (st[i].status != PT_CHANGE_OK) {
+            dd[i].n_insdel = 0; dd[i].n_mark = 0; dd[i].max_ctr = b->h_desc[i].max_ctr;
+            if (changes) { cdesc[i].n_changes = 0; cdesc[i].n_deps = 0; }
+        }
+    memcpy(b->h_chg_desc.p, dd.data(), (size_t)n * sizeof(pt_log_desc));
+    const pt_packed_ops delta{n, dd.data(), (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
+    if ((rc = splice_append(b, &delta, true, pt_append_remap{}, changes ? &ct : nullptr))) return rc;
+    out->n_logs = n;
+    out->status = st;
+    out->delta = pt_packed_ops{n, (const pt_log_desc*)b->h_chg_desc.p, (const pt_insdel_rec*)b->h_chg_insdel.p, n_ins, (const pt_mark_rec*)b->h_chg_marks.p, n_mk};
     return PT_OK;
 }
 

@@ -11,15 +11,15 @@ import os
 
 import numpy as np
 
-from .packing import (CDESC_DT, CHANGE_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT,
-                      AppendRemap, ChangeTable, MergedBatch, PackedBatch, elem_refs)
+from .packing import (CDESC_DT, CHANGE_DT, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
+                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
 _lib = None
 
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
-           "pt_batch_append", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
+           "pt_batch_append", "pt_batch_change", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
            "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
@@ -111,6 +111,16 @@ def _change_struct(table: ChangeTable):
     return _ChangeTable(len(d), d.ctypes.data, c.ctypes.data if len(c) else 0, len(c), p.ctypes.data if len(p) else 0, len(p)), (d, c, p)
 
 
+class _ChangeInput(ctypes.Structure):
+    _fields_ = [("n_logs", ctypes.c_uint32), ("actor", ctypes.c_void_p), ("input_off", ctypes.c_void_p), ("ops", ctypes.c_void_p),
+                ("tokens", ctypes.c_void_p), ("n_tokens", ctypes.c_uint64), ("n_values", ctypes.c_uint32), ("n_links", ctypes.c_uint32),
+                ("n_comments", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class _ChangeView(ctypes.Structure):
+    _fields_ = [("n_logs", ctypes.c_uint32), ("status", ctypes.c_void_p), ("delta", _PackedOps)]
+
+
 class _SpansView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("results", ctypes.c_void_p), ("text_off", ctypes.c_void_p),
                 ("span_off", ctypes.c_void_p), ("text", ctypes.c_void_p), ("spans", ctypes.c_void_p),
@@ -162,6 +172,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_compress_runs.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(u64), ctypes.POINTER(u64)]
     L.pt_batch_upload_changes.argtypes = [vp, vp]
     L.pt_batch_append.argtypes = [vp, vp, vp, vp]
+    L.pt_batch_change.argtypes = [vp, vp, vp, vp]
     L.pt_compact_ops.argtypes = [vp, vp, vp, ctypes.c_int]
     L.pt_batch_upload_compact.argtypes = [vp, vp]
     L.pt_ingest_create.argtypes = [ctypes.POINTER(vp)]
@@ -264,6 +275,44 @@ class BatchEngine:
         self._n_insdel += len(insdel)
         self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
         self.patch_window = None                                             # so does an append
+
+    def change(self, batch: PackedBatch, inputs, actor_ranks, changes: ChangeTable | None = None):
+        """Micromerge.change for many documents on the device (pt_batch_change): ``inputs[i]`` is None (no change) or
+        {"seq", "deps", "startOp", "ops": [InputOperation...]} of the change that actor ``batch.log_actors[i][actor_ranks[i]]``
+        makes on log i, resolved against the last merge (``batch`` = the batch that merge merged, with its pools and tables).
+        ``changes`` is the change table of the new changes, required exactly when the resident batch has one.  Returns
+        (the batch the handle now holds = ``apply_append`` of the generated records, the Change objects (None where there is no
+        change or it failed), the per-log CHANGE_STATUS_DT rows); a failed log ("List index out of bounds") appends nothing
+        and its row names the failing InputOperation.  Needs emit_sequence; the handle needs a merge afterwards."""
+        n = batch.n_logs
+        actor, off, ops, tokens, values, links, counters = change_inputs(batch, inputs, actor_ranks)
+        ptr = lambda a: a.ctypes.data if len(a) else None
+        inp = _ChangeInput(n, ptr(actor), ptr(off), ptr(ops), ptr(tokens), len(tokens), len(values), len(links), len(batch.comment_ids), 0)
+        ct = _change_struct(changes) if changes is not None else None
+        v = _ChangeView()
+        _check(self._L.pt_batch_change(self._h, ctypes.byref(inp), ctypes.byref(ct[0]) if ct else None, ctypes.byref(v)), "pt_batch_change")
+
+        def arr(p, count, dt):
+            if not count or not p:
+                return np.zeros(0, dt)
+            return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
+        status = arr(v.status, n, CHANGE_STATUS_DT)
+        desc = arr(v.delta.logs, n, DESC_DT)
+        failed = [i for i in range(n) if int(status[i]["status"]) != CHANGE_OK]
+        for i in failed:                                 # no records: the counter table stays as it was
+            counters[i] = batch.log_counters[i] if batch.log_counters else None
+        dch = None
+        if changes is not None:
+            cd = changes.desc.copy()
+            cd["n_changes"][failed] = 0; cd["n_deps"][failed] = 0
+            dch = ChangeTable(cd, changes.changes, changes.deps)
+        delta = PackedBatch(desc, arr(v.delta.insdel, int(v.delta.n_insdel_total), INSDEL_DT), arr(v.delta.marks, int(v.delta.n_mark_total), MARK_DT),
+                            values, links, batch.comment_ids, batch.other_attrs, dict(batch.meta), list(batch.log_actors), counters, dch,
+                            list(batch.log_lists))
+        self._n_insdel += int(desc["n_insdel"].astype(np.uint64).sum())
+        self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
+        self.patch_window = None                                             # the append resets the window
+        return apply_append(batch, delta), change_dicts(batch, inputs, actor_ranks, status, delta), status
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion

@@ -907,3 +907,227 @@ def patch_stream(batch: PackedBatch, dp: DevicePatches, i: int, ops: Sequence[di
             out.append([{"path": ["text"], "action": "delete", "index": idx, "count": 1}] if emits else [])
         ri += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Local changes (include/peritext_b200.h pt_batch_change)
+# ------------------------------------------------------------------------------------------------------------------
+INPUT_OP_DT = np.dtype([("action", "u1"), ("mark_type", "u1"), ("reserved0", "<u2"), ("index", "<i4"), ("arg", "<i4"), ("attr", "<u4"),
+                        ("first_ctr", "<u4"), ("reserved1", "<u4"), ("tok_off", "<u8")])
+CHANGE_STATUS_DT = np.dtype([("status", "<u4"), ("input", "<u4")])
+assert INPUT_OP_DT.itemsize == 32 and CHANGE_STATUS_DT.itemsize == 8
+INPUT_ACTIONS = {"insert": 0, "delete": 1, "addMark": 2, "removeMark": 3}
+CHANGE_OK, CHANGE_OUT_OF_BOUNDS = 0, 1
+CHANGE_NO_ACTOR = 0xFFFFFFFF
+INCLUSIVE_MARKS = ("strong", "em")          # markSpec.inclusive, reference src/schema.ts:45-96
+
+
+class ChangeOutOfBounds(RangeError):
+    """``List index out of bounds`` thrown while generating a change; ``input`` is the failing InputOperation's index."""
+
+    def __init__(self, msg: str, input: int):
+        super().__init__(msg)
+        self.input = input
+
+
+def _list_element_id(meta, index: int, look_after_tombstones: bool = False) -> int:
+    """getListElementId (reference src/micromerge.ts:762-805) on a mirror `meta` = [[elemId, deleted, after_defined], ...]:
+    the position of the element, or ChangeOutOfBounds (input -1, set by the caller)."""
+    visible = -1
+    for pos, e in enumerate(meta):
+        if not e[1]:
+            visible += 1
+            if visible == index:
+                if look_after_tombstones:
+                    peek, latest = pos + 1, 0
+                    while peek < len(meta) and meta[peek][1]:
+                        if meta[peek][2]:
+                            latest = peek
+                        peek += 1
+                    if latest:
+                        return latest
+                return pos
+    raise ChangeOutOfBounds(f"List index out of bounds: {index}", -1)
+
+
+def generate_change(meta, change: dict, list_id: str) -> dict:
+    """The host specification of ``pt_batch_change`` for one document: the Change object that the reference's
+    ``Micromerge.change`` (src/micromerge.ts:308-441; changeMark src/peritext.ts:458-501) returns, on a mirror of the text
+    list's metadata as the facade keeps it (``meta`` = [[elemId, deleted, after_defined, ...], ...] in list order, e.g. the
+    engine's element sequence or the oracle's ``elements()``; not modified).  ``change`` = {"actor", "seq", "deps",
+    "startOp", "ops": [InputOperation...]}: the header is the replica's (seq / clock / maxOp + 1) and passes through.
+    ROOT-map InputOperations (path []) take a counter each and touch no list.  Raises ``ChangeOutOfBounds`` naming the failing
+    InputOperation (the whole change is dropped, the deviation of pt_batch_change)."""
+    meta = [list(e[:3]) for e in meta]
+    actor, ctr = change["actor"], int(change["startOp"])
+    ops = []
+
+    def make(body):
+        nonlocal ctr
+        op = {"opId": f"{ctr}@{actor}", **body}
+        ctr += 1
+        ops.append(op)
+        return op
+
+    def elem(k, index, look=False):
+        try:
+            return _list_element_id(meta, index, look)
+        except ChangeOutOfBounds as e:
+            raise ChangeOutOfBounds(str(e), k) from None
+
+    for k, inp in enumerate(change["ops"]):
+        path = list(inp.get("path") or [])
+        action = inp["action"]
+        if path == []:
+            if action not in ("makeList", "makeMap", "del", "set") or inp.get("key") == "text":
+                raise ValueError(f"InputOperation {k}: unsupported ROOT-map operation")
+            body = {"action": action, "obj": "_root", "key": inp["key"]}
+            if action == "set":
+                body["value"] = inp.get("value")
+            make(body)
+            continue
+        if path != ["text"]:
+            raise ValueError(f"InputOperation {k}: no object at path {path!r}")
+        visible_len = sum(1 for e in meta if not e[1])
+        if action == "insert":
+            pos = -1 if inp["index"] == 0 else elem(k, inp["index"] - 1, True)       # :347-350, before the values
+            ref = "_head" if pos < 0 else meta[pos][0]
+            for value in inp["values"]:
+                if not isinstance(value, str):
+                    raise TypeError("Expected value inserted into text to be a string")
+                op = make({"action": "set", "obj": list_id, "elemId": ref, "insert": True, "value": value})
+                pos += 1                                    # its opId exceeds every other: it lands right after its reference
+                meta.insert(pos, [op["opId"], False, False])
+                ref = op["opId"]
+        elif action == "delete":
+            for _ in range(inp["count"]):
+                pos = elem(k, inp["index"])
+                make({"action": "del", "obj": list_id, "elemId": meta[pos][0]})
+                meta[pos][1] = True
+        elif action in ("addMark", "removeMark"):
+            mt = inp["markType"]
+            start = {"type": "before", "elemId": meta[elem(k, inp["startIndex"])][0]}        # peritext.ts:488
+            after = None
+            if mt in INCLUSIVE_MARKS and inp["endIndex"] >= visible_len:
+                end = {"type": "endOfText"}                                                 # :491-492
+            elif mt in INCLUSIVE_MARKS:
+                end = {"type": "before", "elemId": meta[elem(k, inp["endIndex"])][0]}      # :494
+            else:
+                after = elem(k, inp["endIndex"] - 1)
+                end = {"type": "after", "elemId": meta[after][0]}                          # :496
+            body = {"action": action, "obj": list_id, "start": start, "end": end, "markType": mt}
+            if isinstance(inp.get("attrs"), dict):
+                body["attrs"] = inp["attrs"]
+            make(body)
+            if after is not None:
+                meta[after][2] = True
+        else:
+            raise ValueError(f"InputOperation {k}: unimplemented action {action!r}")
+    return {"actor": actor, "seq": change["seq"], "deps": dict(change["deps"]), "startOp": change["startOp"], "ops": ops}
+
+
+def change_inputs(batch: PackedBatch, changes: Sequence[dict | None], actor_ranks: Sequence[int | None]):
+    """The device input of ``pt_batch_change`` for ``changes[i]`` (None: no change; else {"startOp", "ops", ...} as for
+    ``generate_change``) made by actor ``batch.log_actors[i][actor_ranks[i]]``.  Returns (actor u32 [n], input_off u64
+    [n + 1], INPUT_OP_DT ops, u32 tokens, values, link_attrs, counters): the value and link pools with the change's new strings
+    appended (neither carries an order), and per log the counter table extended by the new counters of a dense log.  A comment
+    id the batch does not know shifts ranks: ValueError (append it first)."""
+    n = batch.n_logs
+    actor = np.full(n, CHANGE_NO_ACTOR, np.uint32)
+    off = np.zeros(n + 1, np.uint64)
+    rows, tokens = [], []
+    pools = _Pools(batch.values, batch.link_attrs)
+    comment_rank = {c["id"]: r for r, c in enumerate(batch.comment_ids)}
+    counters = list(batch.log_counters) if batch.log_counters else [None] * n
+    for i in range(n):
+        ch = changes[i]
+        if ch is not None:
+            actor[i] = actor_ranks[i]
+            cmap = counters[i]
+            ctr = int(ch["startOp"])                     # the original counter of the next op
+            new = []                                     # original counters of a dense log's new list ops
+            if cmap is not None and ctr <= int(cmap[-1]):
+                raise ValueError(f"log {i}: startOp {ctr} does not exceed the log's counters")
+            for inp in ch["ops"]:
+                if list(inp.get("path") or []) == []:
+                    ctr += 1
+                    continue
+                a = INPUT_ACTIONS[inp["action"]]
+                first = ctr if cmap is None else len(cmap) + len(new)
+                row = [a, 0, 0, 0, 0, ATTR_NONE, first, 0, len(tokens)]
+                if a == 0:
+                    row[3], row[4] = inp["index"], len(inp["values"])
+                    tokens += [pools.token_of(v) for v in inp["values"]]
+                    gen = len(inp["values"])
+                elif a == 1:
+                    row[3], row[4] = inp["index"], inp["count"]
+                    gen = max(0, inp["count"])
+                else:
+                    mt = inp["markType"]
+                    row[1], row[3], row[4] = MARK_TYPES.index(mt), inp["startIndex"], inp["endIndex"]
+                    attrs = inp.get("attrs")
+                    if mt == "link":
+                        k = canon(attrs)
+                        if k not in pools.link_index:
+                            pools.link_index[k] = len(pools.link_attrs)
+                            pools.link_attrs.append(attrs)
+                        row[5] = pools.link_index[k]
+                    elif mt == "comment":
+                        if attrs["id"] not in comment_rank:
+                            raise ValueError(f"log {i}: comment id {attrs['id']!r} is new to the batch: introduce it with an append first")
+                        row[5] = comment_rank[attrs["id"]]
+                    gen = 1
+                rows.append(tuple(row))
+                if cmap is not None:
+                    new += range(ctr, ctr + gen)
+                ctr += gen
+            if cmap is not None:
+                counters[i] = np.concatenate([cmap, np.array(new, np.uint64)])
+        off[i + 1] = len(rows)
+    ops = np.array(rows, INPUT_OP_DT) if rows else np.zeros(0, INPUT_OP_DT)
+    return actor, off, ops, np.array(tokens, np.uint32), pools.values, pools.link_attrs, counters
+
+
+def change_dicts(batch: PackedBatch, changes: Sequence[dict | None], actor_ranks, status: np.ndarray, delta: PackedBatch) -> list:
+    """The Change objects of ``pt_batch_change``'s view: per log, None for no change or a failed one, else {"actor", "seq",
+    "deps", "startOp", "ops"} with the generated records' packed ids turned back into strings through ``delta``'s actor and
+    counter tables (the batch after the change) and the ROOT-map InputOperations in their places."""
+    out = []
+    for i, ch in enumerate(changes):
+        if ch is None or int(status[i]["status"]) != CHANGE_OK:
+            out.append(None)
+            continue
+        actors = delta.log_actors[i]
+        cmap = delta.log_counters[i] if delta.log_counters else None
+        oc = (lambda c: int(c)) if cmap is None else (lambda c: int(cmap[int(c)]))
+        eid = lambda c, a: "_head" if int(c) == 0 else f"{oc(c)}@{actors[int(a)]}"
+        ins, mk = delta.log_slice(i)
+        lid = batch.log_lists[i]
+        me, ri, mi, ops = actors[int(actor_ranks[i])], 0, 0, []
+        for inp in ch["ops"]:
+            if list(inp.get("path") or []) == []:        # the ops of a change have consecutive counters from startOp
+                body = {"opId": f"{int(ch['startOp']) + len(ops)}@{me}", "action": inp["action"], "obj": "_root", "key": inp["key"]}
+                if inp["action"] == "set":
+                    body["value"] = inp.get("value")
+                ops.append(body)
+                continue
+            a = inp["action"]
+            if a == "insert":
+                for v in inp["values"]:
+                    r = ins[ri]; ri += 1
+                    ops.append({"opId": eid(r["ctr"], r["actor"]), "action": "set", "obj": lid, "elemId": eid(r["ref_ctr"], r["ref_actor"]), "insert": True, "value": v})
+            elif a == "delete":
+                for _ in range(max(0, inp["count"])):
+                    r = ins[ri]; ri += 1
+                    ops.append({"opId": eid(r["ctr"], r["actor"]), "action": "del", "obj": lid, "elemId": eid(r["ref_ctr"], r["ref_actor"])})
+            else:
+                m = mk[mi]; mi += 1
+                eb = BOUND_TYPES[(int(m["bounds"]) >> 2) & 3]
+                end = {"type": eb} if eb == "endOfText" else {"type": eb, "elemId": eid(m["end_ctr"], m["end_actor"])}
+                body = {"opId": eid(m["ctr"], m["actor"]), "action": a, "obj": lid, "start": {"type": "before", "elemId": eid(m["start_ctr"], m["start_actor"])},
+                        "end": end, "markType": inp["markType"]}
+                if isinstance(inp.get("attrs"), dict):
+                    body["attrs"] = inp["attrs"]
+                ops.append(body)
+        out.append({"actor": me, "seq": ch["seq"], "deps": dict(ch["deps"]), "startOp": ch["startOp"], "ops": ops})
+    return out
