@@ -491,6 +491,87 @@ typedef struct pt_change_view {
  * splice on the device. */
 int pt_batch_change(pt_batch*, const pt_change_input* in, const pt_change_table* changes, pt_change_view* out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Sync between logs of the batch: getMissingChanges(source, target) followed by applyChanges(target, missing) (reference
+ * test/merge.ts:4-38, called both ways per step at test/fuzz.ts:198-199), for many (source, target) pairs of resident logs at
+ * once.  A document's replicas are logs of one batch; the changes one of them generated (pt_batch_change) or received
+ * (pt_batch_append) reach another without leaving the device.  Needs a change table whose n_ops counts each change's list ops.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_exchange_pair { uint32_t src, dst; } pt_exchange_pair;
+typedef struct pt_exchange_input {
+    uint32_t n_pairs;
+    const pt_exchange_pair* pairs;   /* deliver to log dst what it is missing from log src                                   */
+    const uint64_t* actor_off;       /* [n_pairs + 1]; pair p's map is actor_map[actor_off[p] .. actor_off[p+1])              */
+    const uint16_t* actor_map;       /* src actor rank -> dst actor rank, exactly src's n_actors entries; 0xFFFF = the actor has
+                                        no rank in dst                                                                        */
+    const uint64_t* ctr_off;         /* [n_pairs + 1] or NULL = identity for every pair                                       */
+    const uint32_t* ctr_map;         /* src packed counter -> dst packed counter (needed only where the packer re-ranked sparse
+                                        counters in either log); empty range = identity; entry 0 = 0; 0xFFFFFFFF = no image in
+                                        dst; a counter past the map has no image                                              */
+} pt_exchange_input;
+
+#define PT_EXCHANGE_OK 0u
+#define PT_EXCHANGE_BAD_TABLE 1u  /* src's or dst's change table is not seq-contiguous per actor, names an actor >= n_actors or
+                                     deps outside the log's, or src's n_ops do not sum to its n_insdel + n_mark (or its mark
+                                     arrivals do not fit those positions)                                                      */
+#define PT_EXCHANGE_STUCK 2u      /* a pass over the queue admitted nothing: a missing change depends on a change neither log
+                                     holds                                                                                     */
+#define PT_EXCHANGE_UNMAPPED 3u   /* a missing change, one of its deps or one of its records names an actor or counter without
+                                     an image in dst                                                                           */
+typedef struct pt_exchange_view {
+    uint32_t n_pairs;
+    const uint32_t* status;        /* [n_pairs] PT_EXCHANGE_*; a pair that is not OK delivers nothing                          */
+    const uint64_t* delivered_off; /* [n_pairs + 1]                                                                            */
+    const uint32_t* delivered;     /* pair p: delivered[delivered_off[p] .. delivered_off[p+1]) = indices into src's change
+                                      table, in delivery order                                                                 */
+    const pt_log_desc* delta;      /* [n_logs] per log the records it received (n_insdel, n_mark; offsets into the engine's
+                                      delta, not meaningful to the caller), its n_actors and its new max_ctr                   */
+} pt_exchange_view;
+
+/* For every pair, deliver to log dst the changes it is missing from log src, in the order the reference's sync applies them.
+ * All pairs read the batch as it is BEFORE the call, so {A->B, B->A} in one call is the reference's two-way sync (what A lacks
+ * from B cannot include what B just received from A: those are A's own), and {A->B, B->C} does not forward A's changes to C.
+ * Per pair:
+ *   1. clocks   clock[a] = the number of changes by actor a in the log's change table, for src and for dst.  While counting,
+ *               every change of both logs must have seq == count + 1 (PT_EXCHANGE_BAD_TABLE otherwise).  No merge is needed:
+ *               in a sync loop the call follows pt_batch_change, which leaves the batch unmerged.
+ *   2. missing  getMissingChanges order (test/merge.ts:25-38): src's actors in the order src first saw them (the insertion
+ *               order of source.clock), and for each the changes with seq > clock_dst[map(actor)], ascending; an actor without
+ *               a rank in dst has clock 0.
+ *   3. order    the order applyChanges admits them (test/merge.ts:4-23): the queue front is delivered if seq == clock + 1 and
+ *               every dep <= clock (src/micromerge.ts:501-509; a zero clock entry fails), else it moves to the back.  That is
+ *               repeated in-order passes over the remaining queue.  The reference gives up after 10 001 iterations; the engine
+ *               has no such cap: it ends a pair with PT_EXCHANGE_STUCK after a full pass that delivers nothing, and otherwise
+ *               delivers however many passes it takes.
+ *   4. records  change c of src holds the list ops at positions [P_c, P_c + n_ops_c), P_c = the sum of the earlier n_ops (the
+ *               positions of pt_batch_set_patch_window).  The delivered changes' ins/del records are concatenated in delivery
+ *               order, and so are their mark records.  Actor fields go through the actor map and counters (ctr, ref_ctr,
+ *               start_ctr, end_ctr) through the counter map; an id whose counter is 0 keeps its actor field, as in
+ *               pt_batch_append.  Value tokens, link ids and comment ranks are per batch and are copied.  A mark's arrival
+ *               becomes dst's old n_insdel + the delivered ins/del records before it.  Change records keep seq and n_ops; their
+ *               actor and their deps' actors go through the actor map.
+ *   5. splice   the delta is appended with identity maps: the handle then holds exactly what pt_batch_append of that delta would
+ *               give (re-planned; no merge, so views of the last merge are invalid; the patch window is reset; pools persist).
+ *               pt_batch_set_patch_window(first_op = old n_insdel + n_mark) then gives the Patches applyChanges returned.
+ * A pair whose status is not PT_EXCHANGE_OK delivers nothing and does not fail the call; the other pairs proceed.  A new actor,
+ * or a counter that moves dst's packed ranks, is introduced first by a pt_batch_append of an empty delta with its remap, as for
+ * pt_batch_change; without that the pair reports PT_EXCHANGE_UNMAPPED.
+ * Refused with nothing changed:
+ *   PT_ERR_STATE    no batch, or a handle without a change table
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) null arguments; src or dst >= n_logs; src == dst; a dst named
+ *                   twice; an actor map whose length is not src's n_actors, whose mapped entries are not strictly increasing or
+ *                   name a rank >= dst's n_actors; a counter map whose entry 0 is not 0 or whose mapped entries are not strictly
+ *                   increasing; a log that would exceed 2^32 - 1 records, and whatever pt_batch_append refuses for the resulting
+ *                   batch (the same messages)
+ * n_pairs == 0: PT_OK, nothing launched, nothing changed.  Synchronises; the caller's arrays may be freed on return.  The view
+ * is engine-owned pinned memory, valid until the next upload, append, change, exchange or destroy.
+ * Device: a select kernel, one warp per pair (clocks in shared memory; the queue, 32 candidates per trip, in a scratch slot),
+ * the per-pair totals back to the host (32 B per pair), a gather kernel, one warp per delivered change (up to 64 for a long
+ * one) with 16-byte coalesced copies, then pt_batch_append's splice with the delta records and the delta change table both
+ * on the device: no record and no change record crosses PCIe; besides the totals only the view's delivered indices come back.
+ * Peak device memory: old + delta + new records and change tables, plus 40 B of scratch per change of every pair's src. */
+int pt_batch_exchange(pt_batch*, const pt_exchange_input* in, pt_exchange_view* out);
+
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */
 int pt_batch_merge(pt_batch*);

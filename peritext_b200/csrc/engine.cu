@@ -22,6 +22,7 @@
 #include "patch_json_kernel.cuh"
 #include "append_kernel.cuh"
 #include "change_kernel.cuh"
+#include "exchange_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -450,6 +451,7 @@ struct pt_batch {
     // pinned host
     HostBuf h_stage, h_results, h_text, h_spans, h_pool, h_misc, h_seq, h_ctoff, h_csoff;
     HostBuf h_chg_status, h_chg_desc, h_chg_insdel, h_chg_marks;   // the view of the last pt_batch_change
+    HostBuf h_xch_totals, h_xch_status, h_xch_off, h_xch_delivered, h_xch_desc;   // the view of the last pt_batch_exchange
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -1073,10 +1075,11 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, b
     return std::string();
 }
 
-// pt_batch_append after its host checks, and the append of pt_batch_change: `delta`'s records are host memory, or device memory
-// the caller keeps alive (delta_on_device).  The delta's descriptors, the remap and the change table are host memory.
-static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R, const pt_change_table* dch) {
-    static const char* fn_name[2] = {"pt_batch_append: ", "pt_batch_change: "};
+// pt_batch_append after its host checks, and the append of pt_batch_change and pt_batch_exchange (`fn` prefixes the error text):
+// `delta`'s records are host memory, or device memory the caller keeps alive (delta_on_device); so are the change and dep
+// records of `dch` (table_on_device).  The delta's descriptors, the remap and the change table's descriptors are host memory.
+static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R,
+                         const pt_change_table* dch, bool table_on_device) {
     std::vector<pt_log_desc> nd;
     std::vector<pt_change_desc> ncd;
     uint32_t maxR = 1;
@@ -1087,7 +1090,7 @@ static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_
     const pt_packed_ops ops{n, nd.data(), nullptr, n_ins, nullptr, n_mk};
     ptp::Plan plan;
     if (err.empty()) if (const char* e = ptp::make_plan(ops, b->limits, b->num_sms, plan)) err = e;
-    if (!err.empty()) { g_last_error = fn_name[delta_on_device] + err; return PT_ERR_INVALID; }
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
     PT_CUDA(cudaSetDevice(b->device));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge and downloads of the resident batch are done
     // The delta and the remap go to the device; the splice writes NEW buffers, so the resident batch stays intact until the
@@ -1144,17 +1147,22 @@ static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_
         n_ch = n ? ncd[n - 1].change_off + ncd[n - 1].n_changes : 0; n_dp = n ? ncd[n - 1].dep_off + ncd[n - 1].n_deps : 0;
         const size_t csz = std::max<size_t>(1, n) * sizeof(pt_change_desc);
         if ((rc = dcdesc.reserve(csz)) || (rc = ncdesc.reserve(csz)) ||
-            (rc = dchg.reserve(std::max<uint64_t>(1, dch->n_changes_total) * sizeof(pt_change_rec))) ||
-            (rc = ddep.reserve(std::max<uint64_t>(1, dch->n_deps_total) * sizeof(pt_dep_rec))) ||
             (rc = nch.reserve(std::max<uint64_t>(1, n_ch) * sizeof(pt_change_rec))) || (rc = ndp.reserve(std::max<uint64_t>(1, n_dp) * sizeof(pt_dep_rec)))) return rc;
         PT_CUDA(h2d(dcdesc.p, dch->logs, (size_t)n * sizeof(pt_change_desc)));
         PT_CUDA(h2d(ncdesc.p, ncd.data(), (size_t)n * sizeof(pt_change_desc)));
-        PT_CUDA(h2d(dchg.p, dch->changes, dch->n_changes_total * sizeof(pt_change_rec)));
-        PT_CUDA(h2d(ddep.p, dch->deps, dch->n_deps_total * sizeof(pt_dep_rec)));
+        const pt_change_rec* d_dchg = dch->changes;
+        const pt_dep_rec* d_ddep = dch->deps;
+        if (!table_on_device) {
+            if ((rc = dchg.reserve(std::max<uint64_t>(1, dch->n_changes_total) * sizeof(pt_change_rec))) ||
+                (rc = ddep.reserve(std::max<uint64_t>(1, dch->n_deps_total) * sizeof(pt_dep_rec)))) return rc;
+            PT_CUDA(h2d(dchg.p, dch->changes, dch->n_changes_total * sizeof(pt_change_rec)));
+            PT_CUDA(h2d(ddep.p, dch->deps, dch->n_deps_total * sizeof(pt_dep_rec)));
+            d_dchg = (const pt_change_rec*)dchg.p; d_ddep = (const pt_dep_rec*)ddep.p;
+        }
         if (n) {
             pta::splice_changes_kernel<<<grid, threads, 0, b->stream>>>((const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p,
                                                                         n, DR, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p,
-                                                                        (const pt_change_rec*)dchg.p, (const pt_dep_rec*)ddep.p,
+                                                                        d_dchg, d_ddep,
                                                                         (pt_change_rec*)nch.p, (pt_dep_rec*)ndp.p);
             PT_CUDA(cudaGetLastError());
             b->launches++;
@@ -1163,7 +1171,7 @@ static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_
     uint32_t bad = 0;
     PT_CUDA(cudaMemcpyAsync(&bad, abad.p, 4, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // also: the caller's arrays may be freed on return
-    if (bad) { g_last_error = std::string(fn_name[delta_on_device]) + "a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
+    if (bad) { g_last_error = std::string(fn) + "a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
     // Accepted: the new records and change table replace the old ones (freed with the locals), and the batch is re-planned.
     b->have_batch = false; b->merged = false; b->dl_begun = false;
     drop_graph(b);
@@ -1182,7 +1190,7 @@ static int splice_append(pt_batch* b, const pt_packed_ops* delta, bool delta_on_
 int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* dch) {
     if (!b || !delta || (delta->n_logs && !delta->logs)) return PT_ERR_INVALID;
     if (!b->have_batch) { g_last_error = "pt_batch_append before pt_batch_upload"; return PT_ERR_STATE; }
-    return splice_append(b, delta, false, remap ? *remap : pt_append_remap{}, dch);
+    return splice_append(b, "pt_batch_append: ", delta, false, remap ? *remap : pt_append_remap{}, dch, false);
 }
 
 // pt_batch_change's host checks of the InputOperations (include/peritext_b200.h).  On success dd holds the delta layout for
@@ -1338,10 +1346,173 @@ int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_tabl
         }
     memcpy(b->h_chg_desc.p, dd.data(), (size_t)n * sizeof(pt_log_desc));
     const pt_packed_ops delta{n, dd.data(), (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
-    if ((rc = splice_append(b, &delta, true, pt_append_remap{}, changes ? &ct : nullptr))) return rc;
+    if ((rc = splice_append(b, "pt_batch_change: ", &delta, true, pt_append_remap{}, changes ? &ct : nullptr, false))) return rc;
     out->n_logs = n;
     out->status = st;
     out->delta = pt_packed_ops{n, (const pt_log_desc*)b->h_chg_desc.p, (const pt_insdel_rec*)b->h_chg_insdel.p, n_ins, (const pt_mark_rec*)b->h_chg_marks.p, n_mk};
+    return PT_OK;
+}
+
+// pt_batch_exchange's host checks of the pairs and their maps (include/peritext_b200.h).  On success slot_off holds each
+// pair's scratch slot (exclusive scan of its src's n_changes).  Returns the problem, or an empty string.
+static std::string check_exchange(const pt_batch* b, const pt_exchange_input& in, std::vector<unsigned long long>& slot_off) {
+    const uint32_t n = b->n_logs, np = in.n_pairs;
+    auto at = [](uint32_t p) { return "pair " + std::to_string(p) + ": "; };
+    if (!in.pairs || !in.actor_off) return "null pairs or actor_off";
+    if (in.actor_off[np] > in.actor_off[0] && !in.actor_map) return "null actor_map with a nonzero length";
+    if (in.ctr_off && in.ctr_off[np] > in.ctr_off[0] && !in.ctr_map) return "null ctr_map with a nonzero length";
+    std::vector<char> is_dst(n, 0);
+    slot_off.assign((size_t)np + 1, 0);
+    for (uint32_t p = 0; p < np; p++) {
+        const uint32_t src = in.pairs[p].src, dst = in.pairs[p].dst;
+        if (src >= n || dst >= n) return at(p) + "log " + std::to_string(src >= n ? src : dst) + " is outside the batch's " + std::to_string(n) + " logs";
+        if (src == dst) return at(p) + "src and dst are both log " + std::to_string(src);
+        if (is_dst[dst]) return at(p) + "log " + std::to_string(dst) + " is the dst of an earlier pair";
+        is_dst[dst] = 1;
+        if (in.actor_off[p + 1] < in.actor_off[p]) return "actor_off decreases";
+        const uint64_t na = in.actor_off[p + 1] - in.actor_off[p];
+        if (na != b->h_desc[src].n_actors)
+            return at(p) + "the actor map has " + std::to_string(na) + " entries and log " + std::to_string(src) + " has " + std::to_string(b->h_desc[src].n_actors) + " actors";
+        const uint16_t* a = in.actor_map + in.actor_off[p];
+        int64_t last = -1;
+        for (uint64_t k = 0; k < na; k++) {
+            if (a[k] == 0xFFFFu) continue;
+            if ((int64_t)a[k] <= last) return at(p) + "the actor map is not strictly increasing";
+            if (a[k] >= b->h_desc[dst].n_actors) return at(p) + "the actor map names a rank >= log " + std::to_string(dst) + "'s n_actors";
+            last = a[k];
+        }
+        if (in.ctr_off) {
+            if (in.ctr_off[p + 1] < in.ctr_off[p]) return "ctr_off decreases";
+            const uint64_t nc = in.ctr_off[p + 1] - in.ctr_off[p];
+            const uint32_t* c = in.ctr_map + in.ctr_off[p];
+            if (nc > 0xFFFFFFFFull) return at(p) + "the counter map has more than 2^32 - 1 entries";
+            if (nc && c[0] != 0) return at(p) + "ctr_map[0] is not 0";
+            uint32_t prev = 0;
+            for (uint64_t k = 1; k < nc; k++) {
+                if (c[k] == 0xFFFFFFFFu) continue;
+                if (c[k] <= prev) return at(p) + "the counter map is not strictly increasing";
+                prev = c[k];
+            }
+        }
+        slot_off[p + 1] = slot_off[p] + b->h_cdesc[src].n_changes;
+    }
+    return std::string();
+}
+
+int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view* out) {
+    if (!b || !in || !out) { g_last_error = "pt_batch_exchange: null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_exchange before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = "pt_batch_exchange: the handle has no change table"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs, np = in->n_pairs;
+    int rc;
+    const size_t nn = std::max<uint32_t>(1, n), npp = std::max<uint32_t>(1, np);
+    if ((rc = b->h_xch_totals.reserve(npp * sizeof(ptx::PairTotals))) || (rc = b->h_xch_status.reserve(npp * 4)) ||
+        (rc = b->h_xch_off.reserve((npp + 1) * 8)) || (rc = b->h_xch_desc.reserve(nn * sizeof(pt_log_desc)))) return rc;
+    ptx::PairTotals* tot = (ptx::PairTotals*)b->h_xch_totals.p;
+    uint32_t* status = (uint32_t*)b->h_xch_status.p;
+    uint64_t* doff = (uint64_t*)b->h_xch_off.p;
+    pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
+    if (!np) {
+        PT_CUDA(cudaSetDevice(b->device));
+        PT_CUDA(cudaStreamSynchronize(b->stream));          // the pinned view buffers may still be the target of an earlier copy
+        if ((rc = b->h_xch_delivered.reserve(4))) return rc;
+        for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
+        doff[0] = 0;
+        *out = pt_exchange_view{0, status, doff, (const uint32_t*)b->h_xch_delivered.p, dd};
+        return PT_OK;
+    }
+    std::vector<unsigned long long> slot_off;
+    std::string err = check_exchange(b, *in, slot_off);
+    if (!err.empty()) { g_last_error = "pt_batch_exchange: " + err; return PT_ERR_INVALID; }
+    const uint64_t n_slot = slot_off[np];
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    // the pairs, their maps and the select kernel's scratch: freed on return
+    DevBuf dpairs, daoff, damap, dcoff, dcmap, dslot, dqueue, dpos, ddlv, dtot, ddoff, dbase, dgi, dgm, dgc, dgd, dgx;
+    const uint64_t n_amap = in->actor_off[np], n_cmap = in->ctr_off ? in->ctr_off[np] : 0;
+    if ((rc = dpairs.reserve((size_t)np * sizeof(pt_exchange_pair))) || (rc = daoff.reserve(((size_t)np + 1) * 8)) || (rc = damap.reserve(std::max<uint64_t>(1, n_amap) * 2)) ||
+        (rc = dslot.reserve(((size_t)np + 1) * 8)) || (rc = dqueue.reserve(std::max<uint64_t>(1, n_slot) * 4)) || (rc = dpos.reserve(std::max<uint64_t>(1, n_slot) * 4)) ||
+        (rc = ddlv.reserve(std::max<uint64_t>(1, n_slot) * sizeof(ptx::Delivered))) || (rc = dtot.reserve((size_t)np * sizeof(ptx::PairTotals))) ||
+        (rc = ddoff.reserve(((size_t)np + 1) * 8)) || (rc = dbase.reserve((size_t)np * sizeof(ptx::PairBase)))) return rc;
+    if (in->ctr_off && ((rc = dcoff.reserve(((size_t)np + 1) * 8)) || (rc = dcmap.reserve(std::max<uint64_t>(1, n_cmap) * 4)))) return rc;
+    auto h2d = [&](void* dst_, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst_, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
+    PT_CUDA(h2d(dpairs.p, in->pairs, (size_t)np * sizeof(pt_exchange_pair)));
+    PT_CUDA(h2d(daoff.p, in->actor_off, ((size_t)np + 1) * 8));
+    PT_CUDA(h2d(damap.p, in->actor_map, n_amap * 2));
+    PT_CUDA(h2d(dslot.p, slot_off.data(), ((size_t)np + 1) * 8));
+    if (in->ctr_off) {
+        PT_CUDA(h2d(dcoff.p, in->ctr_off, ((size_t)np + 1) * 8));
+        PT_CUDA(h2d(dcmap.p, in->ctr_map, n_cmap * 4));
+    }
+    ptx::ExchangeParams P{};
+    P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = np; P.maxR = b->adm_maxR;
+    P.actor_off = (const unsigned long long*)daoff.p; P.actor_map = (const uint16_t*)damap.p;
+    P.ctr_off = in->ctr_off ? (const unsigned long long*)dcoff.p : nullptr; P.ctr_map = (const uint32_t*)dcmap.p;
+    P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
+    P.insdel = b->dp_insdel; P.marks = b->dp_marks;
+    P.slot_off = (const unsigned long long*)dslot.p; P.queue = (uint32_t*)dqueue.p; P.pos = (uint32_t*)dpos.p; P.dlv = (ptx::Delivered*)ddlv.p;
+    P.totals = (ptx::PairTotals*)dtot.p;
+    {   // like the admission pre-pass: 4 warps per CTA while the per-actor tables fit, else one warp with up to 200 KB
+        const size_t per_warp = (size_t)2 * b->adm_maxR * 4;
+        const uint32_t wpb = per_warp * 4 <= 48 * 1024 ? 4u : 1u;
+        const size_t smem = per_warp * wpb;
+        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptx::exchange_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)np + wpb - 1) / wpb, (uint64_t)b->num_sms * 16);
+        ptx::exchange_select_kernel<<<grid, wpb * 32, smem, b->stream>>>(P);
+        PT_CUDA(cudaGetLastError());
+        b->launches++;
+    }
+    PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    // the delta's layout: the pairs' records, change and dep records back to back in pair order
+    std::vector<ptx::PairBase> base(np);
+    std::vector<unsigned long long> dlv_off((size_t)np + 1, 0);
+    uint64_t n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0, most = 0;
+    for (uint32_t p = 0; p < np; p++) {
+        base[p] = ptx::PairBase{n_ins, n_mk, n_ch, n_dp};
+        n_ins += tot[p].n_insdel; n_mk += tot[p].n_mark; n_ch += tot[p].n_changes; n_dp += tot[p].n_deps;
+        dlv_off[p + 1] = n_ch;
+        most = std::max<uint64_t>(most, (uint64_t)tot[p].n_insdel + 2ull * tot[p].n_mark);
+    }
+    if ((rc = dgi.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = dgm.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))) ||
+        (rc = dgc.reserve(std::max<uint64_t>(1, n_ch) * sizeof(pt_change_rec))) || (rc = dgd.reserve(std::max<uint64_t>(1, n_dp) * sizeof(pt_dep_rec))) ||
+        (rc = dgx.reserve(std::max<uint64_t>(1, n_ch) * 4)) || (rc = b->h_xch_delivered.reserve(std::max<uint64_t>(1, n_ch) * 4))) return rc;
+    uint32_t* delivered = (uint32_t*)b->h_xch_delivered.p;
+    if (n_ch) {
+        PT_CUDA(h2d(ddoff.p, dlv_off.data(), ((size_t)np + 1) * 8));
+        PT_CUDA(h2d(dbase.p, base.data(), (size_t)np * sizeof(ptx::PairBase)));
+        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p;
+        P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
+        P.out_delivered = (uint32_t*)dgx.p;
+        // a pair's records are an upper bound of its longest change: up to 64 warps per change, 8 K records per slice
+        const uint32_t threads = 128, slices = (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, most / 8192));
+        const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_ch * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16 / slices));
+        ptx::exchange_gather_kernel<<<dim3(gx, slices), threads, 0, b->stream>>>(P);
+        PT_CUDA(cudaGetLastError());
+        b->launches++;
+        PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));   // status and max_ctr
+        PT_CUDA(cudaMemcpyAsync(delivered, dgx.p, n_ch * 4, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    // the delta per log; a pair that found an id without an image delivers nothing: its records are never spliced
+    std::vector<pt_change_desc> cdesc(n, pt_change_desc{0, 0, 0, 0});
+    for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
+    doff[0] = 0;
+    for (uint32_t p = 0; p < np; p++) {
+        status[p] = tot[p].status;
+        const uint32_t dst = in->pairs[p].dst, cnt = status[p] == PT_EXCHANGE_OK ? tot[p].n_changes : 0u;
+        if (cnt) {
+            dd[dst] = pt_log_desc{base[p].insdel, base[p].mark, tot[p].n_insdel, tot[p].n_mark, b->h_desc[dst].n_actors, std::max(b->h_desc[dst].max_ctr, tot[p].max_ctr)};
+            cdesc[dst] = pt_change_desc{base[p].change, base[p].dep, tot[p].n_changes, tot[p].n_deps};
+            if (doff[p] != dlv_off[p]) memmove(delivered + doff[p], delivered + dlv_off[p], (size_t)cnt * 4);
+        }
+        doff[p + 1] = doff[p] + cnt;
+    }
+    const pt_packed_ops delta{n, dd, (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
+    const pt_change_table ct{n, cdesc.data(), (const pt_change_rec*)dgc.p, n_ch, (const pt_dep_rec*)dgd.p, n_dp};
+    if ((rc = splice_append(b, "pt_batch_exchange: ", &delta, true, pt_append_remap{}, &ct, true))) return rc;
+    *out = pt_exchange_view{np, status, doff, delivered, dd};
     return PT_OK;
 }
 

@@ -1,0 +1,327 @@
+// exchange_kernel.cuh — the device side of pt_batch_exchange (include/peritext_b200.h): which changes of log src log dst is
+// missing, in the order applyChanges admits them, and the gather of their records into a delta in dst's id space.
+//
+// exchange_select_kernel: one warp per pair, grid-stride.  Per-warp shared memory holds dst's clock (by dst actor rank) and a
+// per-src-actor word (first the actor's change count, then the queue slot of its first missing change).
+//   1. clocks: both change tables 32 changes per trip; match_any groups give each change its rank among the trip's changes of
+//      the same actor, so seq == count + 1 is checked per lane (admit_kernel's scheme).  The src pass also writes each change's
+//      list-op position (running sum of n_ops) into the pair's scratch slot.
+//   2. queue, getMissingChanges order (reference test/merge.ts:25-38): actors in the order src first saw them, ascending seq.
+//      In a seq-contiguous table an actor's first change is its seq 1, so one pass in table order gives every actor the
+//      slot of its first missing change (a warp scan over the trip's seq-1 lanes), and the change (actor, seq) goes to
+//      slot[actor] + seq - clock_dst - 1.
+//   3. delivery, applyChanges order (test/merge.ts:4-23): repeated in-order passes over the queue, 32 candidates per trip.
+//      All lanes test seq and deps against the clock of the trip's start.  A pass is final (clocks only grow, and a
+//      seq-contiguous table has no second change with the same actor and seq); a lane that failed is tested again in lane
+//      order, after the clock bumps of the delivered lanes before it, so it sees exactly what the reference's queue front
+//      would.  Lanes that fail stay in the queue (compacted in place) for the next pass; a pass that delivers nothing ends
+//      the pair with PT_EXCHANGE_STUCK.
+//    A delivered change's record ranges come from its list-op positions: marks before position X = the first k with
+//    min(arrival_k, n) + k >= X (ptw::marks_before_lane, the per-lane form of the patch window's cut), ins/del records before
+//    it = X - k.  Running sums over the delivered changes give each its place in the delta.
+// exchange_gather_kernel: one warp per delivered change (blockIdx.y slices a long change, as splice_records_kernel slices a
+// long log): 16-byte coalesced copies with the pair's actor and counter maps applied (a mark is a lane pair, as in the
+// splice), mark arrivals rebased onto dst's records; slice 0 also writes the change record, its deps and the delivered index.
+// An id without an image sets the pair's status, and the host drops that pair's delta.
+#pragma once
+#include <cstdint>
+
+#include "../../include/peritext_b200.h"
+#include "patch_window.cuh"
+
+namespace ptx {
+
+struct PairTotals { uint32_t n_insdel, n_mark, n_changes, n_deps, max_ctr, status, reserved0, reserved1; };   // 32 B per pair
+struct Delivered {          // one per delivered change, in delivery order.  32 B
+    uint32_t change;                    // index in src's change table
+    uint32_t ins_lo, mk_lo;             // its first ins/del and mark record in src's log
+    uint32_t n_insdel, n_mark;
+    uint32_t ins_off, mk_off, dep_off;  // its place among the pair's delivered records
+};
+struct PairBase { unsigned long long insdel, mark, change, dep; };   // where a pair's records start in the delta arrays
+
+// One pair's maps, src id space -> dst id space.  The actor map has exactly src's n_actors entries; nc == 0 is the identity
+// counter map.  No image: 0xFFFF / 0xFFFFFFFF.
+struct PairMaps {
+    const uint16_t* a; uint32_t na;
+    const uint32_t* c; uint32_t nc;
+    __device__ __forceinline__ uint32_t actor(uint32_t x) const { return x < na ? (uint32_t)__ldg(a + x) : 0xFFFFu; }
+    __device__ __forceinline__ uint32_t ctr(uint32_t x) const { return nc ? (x < nc ? __ldg(c + x) : 0xFFFFFFFFu) : x; }
+    // the actor of an id whose counter is ctr_old: counter 0 is HEAD / a text boundary and names no actor
+    __device__ __forceinline__ uint32_t id_actor(uint32_t ctr_old, uint32_t x) const { return ctr_old ? actor(x) : x; }
+};
+
+struct ExchangeParams {
+    const pt_exchange_pair* pairs; uint32_t n_pairs; uint32_t maxR;
+    const unsigned long long* actor_off; const uint16_t* actor_map;
+    const unsigned long long* ctr_off;  const uint32_t* ctr_map;       // ctr_off null: identity for every pair
+    const pt_log_desc* desc; const pt_change_desc* cdesc; const pt_change_rec* changes; const pt_dep_rec* deps;
+    const pt_insdel_rec* insdel; const pt_mark_rec* marks;
+    const unsigned long long* slot_off;   // [n_pairs + 1] a pair's scratch slot: src's n_changes entries of queue, pos and dlv
+    uint32_t* queue; uint32_t* pos; Delivered* dlv;
+    PairTotals* totals;
+    // gather only
+    const unsigned long long* dlv_off;    // [n_pairs + 1] exclusive scan of the pairs' delivered changes
+    unsigned long long n_dlv;
+    const PairBase* base;
+    pt_insdel_rec* out_insdel; pt_mark_rec* out_marks; pt_change_rec* out_changes; pt_dep_rec* out_deps; uint32_t* out_delivered;
+};
+
+__device__ __forceinline__ PairMaps pair_maps(const ExchangeParams& P, uint32_t p) {
+    PairMaps m{nullptr, 0u, nullptr, 0u};
+    const unsigned long long ao = P.actor_off[p];
+    m.a = P.actor_map + ao; m.na = (uint32_t)(P.actor_off[p + 1] - ao);
+    if (P.ctr_off) { const unsigned long long o = P.ctr_off[p]; m.c = P.ctr_map + o; m.nc = (uint32_t)(P.ctr_off[p + 1] - o); }
+    return m;
+}
+
+__device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, uint32_t& total) {
+    uint32_t s = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, d); if (lane >= (uint32_t)d) s += y; }
+    total = __shfl_sync(0xffffffffu, s, 31);
+    return s - v;
+}
+
+// Step 1 for one change table: cnt[actor] = the actor's changes (cnt zeroed by the caller); false if a change names an actor
+// >= R, breaks seq == count + 1, or its deps leave the log's dep records.  With pos: pos[k] = sum of n_ops before change k,
+// *ops = the sum over the table.
+__device__ __forceinline__ bool count_clock(const pt_change_rec* __restrict__ c0, uint32_t n, uint32_t n_deps, uint32_t R, uint32_t* cnt,
+                                            uint32_t* __restrict__ pos, unsigned long long* ops, uint32_t lane) {
+    const uint32_t lt = (1u << lane) - 1u;
+    unsigned long long run = 0;
+    bool ok = true;
+    for (uint32_t base = 0; base < n && ok; base += 32) {
+        const uint32_t k = base + lane;
+        const bool valid = k < n;
+        uint4 r = make_uint4(0, 0, 0, 0);
+        if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
+        const uint32_t actor = r.y & 0xFFFFu;
+        const bool aok = valid && actor < R;
+        const uint32_t mask = __match_any_sync(0xffffffffu, aok ? actor : (0x10000u + lane));
+        const bool bad = valid && (!aok || r.x != cnt[aok ? actor : 0] + __popc(mask & lt) + 1u || (unsigned long long)r.z + (r.y >> 16) > n_deps);
+        ok = !__any_sync(0xffffffffu, bad);
+        if (pos) {
+            uint32_t tot;
+            const uint32_t ex = warp_excl_scan(valid ? r.w : 0u, lane, tot);   // a trip's n_ops can wrap only in a table the total check refuses
+            unsigned long long wide = valid ? r.w : 0u;
+            for (int o = 16; o > 0; o >>= 1) wide += __shfl_xor_sync(0xffffffffu, wide, o);
+            if (valid) pos[k] = (uint32_t)run + ex;
+            run += wide;
+        }
+        __syncwarp();
+        if (aok && (mask & lt) == 0) cnt[actor] += __popc(mask);
+        __syncwarp();
+    }
+    if (ops) *ops = run;
+    return ok;
+}
+
+// applyChange's admission test (reference src/micromerge.ts:501-509) of a src change against dst's clock; the change's and
+// its deps' actors are known to have images (step 2 checked them).
+__device__ __forceinline__ bool admits(const PairMaps& m, const uint32_t* clk, const pt_dep_rec* __restrict__ d0, uint4 r) {
+    if (r.x != clk[m.actor(r.y & 0xFFFFu)] + 1u) return false;
+    for (uint32_t d = 0; d < (r.y >> 16); d++) {
+        const pt_dep_rec q = d0[r.z + d];
+        const uint32_t have = clk[m.actor(q.actor)];
+        if (have == 0 || have < q.seq) return false;
+    }
+    return true;
+}
+
+__global__ void exchange_select_kernel(ExchangeParams P) {
+    extern __shared__ uint32_t xch_smem[];
+    const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    const uint32_t lt = (1u << lane) - 1u;
+    uint32_t* clk = xch_smem + (size_t)wib * 2 * P.maxR;     // dst's clock, by dst actor rank
+    uint32_t* cs = clk + P.maxR;                             // by src actor rank: change count, then first queue slot
+    for (uint32_t p = blockIdx.x * wpb + wib; p < P.n_pairs; p += gridDim.x * wpb) {
+        const pt_exchange_pair pr = P.pairs[p];
+        const pt_log_desc S = P.desc[pr.src], D = P.desc[pr.dst];
+        const pt_change_desc CS = P.cdesc[pr.src], CD = P.cdesc[pr.dst];
+        const PairMaps m = pair_maps(P, p);
+        const uint32_t Rs = S.n_actors, Rd = D.n_actors;
+        for (uint32_t a = lane; a < Rd; a += 32) clk[a] = 0;
+        for (uint32_t a = lane; a < Rs; a += 32) cs[a] = 0;
+        __syncwarp();
+        const pt_change_rec* c0 = P.changes + CS.change_off;
+        const pt_dep_rec* d0 = P.deps + CS.dep_off;
+        uint32_t* queue = P.queue + P.slot_off[p];
+        uint32_t* pos = P.pos + P.slot_off[p];
+        Delivered* dlv = P.dlv + P.slot_off[p];
+        uint32_t status = PT_EXCHANGE_OK;
+        unsigned long long ops = 0;
+        if (!count_clock(P.changes + CD.change_off, CD.n_changes, CD.n_deps, Rd, clk, nullptr, nullptr, lane) ||
+            !count_clock(c0, CS.n_changes, CS.n_deps, Rs, cs, pos, &ops, lane) ||
+            ops != (unsigned long long)S.n_insdel + S.n_mark || ops > 0xFFFFFFFFull)
+            status = PT_EXCHANGE_BAD_TABLE;
+        // ---- step 2: the queue ----
+        uint32_t nq = 0;
+        if (status == PT_EXCHANGE_OK) {
+            bool bad = false, unmapped = false;
+            for (uint32_t base = 0; base < CS.n_changes; base += 32) {
+                const uint32_t k = base + lane;
+                const bool valid = k < CS.n_changes;
+                uint4 r = make_uint4(0, 0, 0, 0);
+                if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
+                const uint32_t actor = r.y & 0xFFFFu, ma = valid ? m.actor(actor) : 0xFFFFu;
+                const uint32_t have = ma < Rd ? clk[ma] : 0u;            // an actor dst has no rank for: clock 0
+                const bool first = valid && r.x == 1u;
+                uint32_t tot;
+                const uint32_t ex = warp_excl_scan(first && cs[actor] > have ? cs[actor] - have : 0u, lane, tot);
+                __syncwarp();
+                if (first) cs[actor] = nq + ex;
+                __syncwarp();
+                nq += tot;
+                if (valid && r.x > have) {
+                    queue[cs[actor] + r.x - have - 1u] = k;
+                    if (ma >= Rd) unmapped = true;
+                    for (uint32_t d = 0; d < (r.y >> 16); d++) {
+                        const uint32_t da = d0[r.z + d].actor;
+                        if (da >= Rs) bad = true;
+                        else if (m.actor(da) >= Rd) unmapped = true;
+                    }
+                }
+            }
+            if (__any_sync(0xffffffffu, bad)) status = PT_EXCHANGE_BAD_TABLE;
+            else if (__any_sync(0xffffffffu, unmapped)) status = PT_EXCHANGE_UNMAPPED;
+        }
+        // ---- step 3: delivery ----
+        uint32_t t_ins = 0, t_mk = 0, t_ch = 0, t_dep = 0;
+        const pt_mark_rec* mk = P.marks + S.mark_off;
+        uint32_t remaining = nq;
+        __syncwarp();
+        while (status == PT_EXCHANGE_OK && remaining) {
+            uint32_t kept = 0;
+            const uint32_t before = t_ch;
+            for (uint32_t base = 0; base < remaining && status == PT_EXCHANGE_OK; base += 32) {
+                const bool valid = base + lane < remaining;
+                const uint32_t c = valid ? queue[base + lane] : 0u;
+                uint4 r = make_uint4(0, 0, 0, 0);
+                if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + c));
+                const uint32_t ma = m.actor(r.y & 0xFFFFu);
+                bool ok = valid && admits(m, clk, d0, r);
+                const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+                uint32_t pass = __ballot_sync(0xffffffffu, ok), applied = 0;
+                // failing lanes in lane order: first the bumps of the delivered lanes before them, then their test again
+                for (uint32_t fail = vmask & ~pass; fail; fail &= fail - 1) {
+                    const uint32_t f = __ffs(fail) - 1, due = pass & ((1u << f) - 1u) & ~applied;
+                    if ((due >> lane) & 1u) atomicMax(&clk[ma], r.x);
+                    applied |= due;
+                    __syncwarp();
+                    if (lane == f) ok = admits(m, clk, d0, r);
+                    pass |= __ballot_sync(0xffffffffu, lane == f && ok);
+                }
+                if (((pass & ~applied) >> lane) & 1u) atomicMax(&clk[ma], r.x);
+                __syncwarp();
+                // the delivered lanes' record ranges and their places in the delta
+                uint32_t ins_lo = 0, ins_n = 0, mk_lo = 0, mk_n = 0;
+                bool broken = false;
+                if (ok) {
+                    const uint32_t x0 = pos[c], x1 = x0 + r.w;
+                    const uint32_t k0 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x0), k1 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x1);
+                    broken = k0 > x0 || k1 > x1 || k1 < k0 || x1 - k1 > S.n_insdel || x1 - k1 < x0 - k0;   // arrivals that do not fit the table
+                    if (!broken) { ins_lo = x0 - k0; ins_n = (x1 - k1) - ins_lo; mk_lo = k0; mk_n = k1 - k0; }
+                }
+                if (__any_sync(0xffffffffu, broken)) { status = PT_EXCHANGE_BAD_TABLE; break; }
+                uint32_t n_i, n_m, n_d;
+                const uint32_t e_i = warp_excl_scan(ins_n, lane, n_i), e_m = warp_excl_scan(mk_n, lane, n_m),
+                               e_d = warp_excl_scan(ok ? (r.y >> 16) : 0u, lane, n_d);
+                if (ok) dlv[t_ch + __popc(pass & lt)] = Delivered{c, ins_lo, mk_lo, ins_n, mk_n, t_ins + e_i, t_mk + e_m, t_dep + e_d};
+                t_ins += n_i; t_mk += n_m; t_dep += n_d; t_ch += __popc(pass);
+                // the others go back to the queue; slot kept + rank <= base + lane, which this trip has already read
+                if (valid && !ok) queue[kept + __popc(vmask & ~pass & lt)] = c;
+                kept += __popc(vmask & ~pass);
+                __syncwarp();
+            }
+            if (status == PT_EXCHANGE_OK && t_ch == before) status = PT_EXCHANGE_STUCK;
+            remaining = kept;
+        }
+        if (lane == 0)
+            P.totals[p] = status == PT_EXCHANGE_OK ? PairTotals{t_ins, t_mk, t_ch, t_dep, 0u, PT_EXCHANGE_OK, 0u, 0u}
+                                                   : PairTotals{0u, 0u, 0u, 0u, 0u, status, 0u, 0u};
+        __syncwarp();
+    }
+}
+
+__global__ void exchange_gather_kernel(ExchangeParams P) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+    const uint32_t first = blockIdx.y * 32u + lane, step = gridDim.y * 32u;       // this warp's slice of each change
+    for (unsigned long long j = warp; j < P.n_dlv; j += nwarps) {
+        uint32_t lo = 0, hi = P.n_pairs;                   // the pair: the last p with dlv_off[p] <= j
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (P.dlv_off[mid] <= j) lo = mid; else hi = mid; }
+        const uint32_t p = lo, k = (uint32_t)(j - P.dlv_off[p]);
+        const pt_exchange_pair pr = P.pairs[p];
+        const pt_log_desc S = P.desc[pr.src], D = P.desc[pr.dst];
+        const PairMaps m = pair_maps(P, p);
+        const PairBase B = P.base[p];
+        const Delivered d = P.dlv[P.slot_off[p] + k];
+        uint32_t top = 0;                                  // the largest mapped opId counter this lane wrote
+        bool unmapped = false;
+        auto ctr = [&](uint32_t c) { const uint32_t x = m.ctr(c); unmapped |= x == 0xFFFFFFFFu; return x; };
+        auto id_actor = [&](uint32_t c, uint32_t a) { const uint32_t x = m.id_actor(c, a); unmapped |= c && x == 0xFFFFu; return x; };
+        // ins/del records: {ctr, ref_ctr, actor | ref_actor << 16, payload}
+        const uint4* is = reinterpret_cast<const uint4*>(P.insdel + S.insdel_off + d.ins_lo);
+        uint4* id = reinterpret_cast<uint4*>(P.out_insdel + B.insdel + d.ins_off);
+        for (uint32_t i = first; i < d.n_insdel; i += step) {
+            uint4 r = __ldg(is + i);
+            const uint32_t a = id_actor(r.x, r.z & 0xFFFFu), ra = id_actor(r.y, r.z >> 16);
+            r.x = ctr(r.x); r.y = ctr(r.y); r.z = (a & 0xFFFFu) | (ra << 16);
+            top = max(top, r.x);
+            id[i] = r;
+        }
+        // mark records, two words each: A = {ctr, actor | kind << 16 | bounds << 24, start_ctr, end_ctr},
+        // B = {start_actor | end_actor << 16, attr, arrival, reserved}
+        const uint4* ms = reinterpret_cast<const uint4*>(P.marks + S.mark_off + d.mk_lo);
+        uint4* md = reinterpret_cast<uint4*>(P.out_marks + B.mark + d.mk_off);
+        const uint32_t nq = 2u * d.n_mark;
+        for (uint32_t base = first - lane; base < nq; base += step) {             // 32-aligned: a mark's two words share a trip
+            const uint32_t i = base + lane;
+            const bool valid = i < nq;
+            uint4 q = valid ? __ldg(ms + i) : make_uint4(0, 0, 0, 0);
+            const uint32_t pz = __shfl_xor_sync(0xffffffffu, q.z, 1), pw = __shfl_xor_sync(0xffffffffu, q.w, 1);
+            if (!valid) continue;
+            if (!(lane & 1u)) {
+                const uint32_t a = id_actor(q.x, q.y & 0xFFFFu);
+                q.x = ctr(q.x); q.y = (q.y & 0xFFFF0000u) | (a & 0xFFFFu); q.z = ctr(q.z); q.w = ctr(q.w);
+                top = max(top, q.x);
+            } else {
+                const uint32_t sa = id_actor(pz, q.x & 0xFFFFu), ea = id_actor(pw, q.x >> 16);
+                q.x = (sa & 0xFFFFu) | (ea << 16);
+                // arrival: dst's old records, then the delivered ins/del records before the mark
+                const uint32_t within = q.z < d.ins_lo ? 0u : min(q.z - d.ins_lo, d.n_insdel);
+                q.z = D.n_insdel + d.ins_off + within;
+            }
+            md[i] = q;
+        }
+        if (blockIdx.y == 0) {
+            // change record {seq, actor | n_deps << 16, dep_off, n_ops} and its deps {seq, actor | reserved << 16}
+            const pt_change_desc CS = P.cdesc[pr.src];
+            uint4 r = __ldg(reinterpret_cast<const uint4*>(P.changes + CS.change_off + d.change));
+            const uint2* ps = reinterpret_cast<const uint2*>(P.deps + CS.dep_off + r.z);
+            uint2* pd = reinterpret_cast<uint2*>(P.out_deps + B.dep + d.dep_off);
+            for (uint32_t t = lane; t < (r.y >> 16); t += 32) {
+                uint2 q = __ldg(ps + t);
+                const uint32_t a = m.actor(q.y & 0xFFFFu);
+                unmapped |= a == 0xFFFFu;
+                q.y = (q.y & 0xFFFF0000u) | a;
+                pd[t] = q;
+            }
+            if (lane == 0) {
+                const uint32_t a = m.actor(r.y & 0xFFFFu);
+                unmapped |= a == 0xFFFFu;
+                r.y = (r.y & 0xFFFF0000u) | a; r.z = d.dep_off;
+                reinterpret_cast<uint4*>(P.out_changes + B.change)[k] = r;
+                P.out_delivered[j] = d.change;
+            }
+        }
+        for (int o = 16; o > 0; o >>= 1) top = max(top, __shfl_xor_sync(0xffffffffu, top, o));
+        const bool any_unmapped = __any_sync(0xffffffffu, unmapped);
+        if (lane == 0) {
+            if (top) atomicMax(&P.totals[p].max_ctr, top);
+            if (any_unmapped) atomicMax(&P.totals[p].status, (uint32_t)PT_EXCHANGE_UNMAPPED);
+        }
+    }
+}
+
+}  // namespace ptx

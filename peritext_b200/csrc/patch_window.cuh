@@ -25,4 +25,15 @@ __device__ __forceinline__ uint32_t marks_before(const pt_mark_rec* __restrict__
     return k0;
 }
 
+// The same count by one thread: the mark positions strictly increase, so k0 is the first k with min(arrival_k, n) + k >=
+// first_op, found by bisection.  For callers whose lanes cut different logs or positions (pt_batch_exchange's select kernel).
+__device__ __forceinline__ uint32_t marks_before_lane(const pt_mark_rec* __restrict__ mk, uint32_t n, uint32_t m, uint32_t first_op) {
+    uint32_t lo = 0, hi = m;
+    while (lo < hi) {
+        const uint32_t k = lo + ((hi - lo) >> 1);
+        if ((unsigned long long)min(__ldg(&mk[k].arrival), n) + k < first_op) lo = k + 1; else hi = k;
+    }
+    return lo;
+}
+
 }  // namespace ptw

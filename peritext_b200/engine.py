@@ -12,14 +12,14 @@ import os
 import numpy as np
 
 from .packing import (CDESC_DT, CHANGE_DT, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
-                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs)
+                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
 _lib = None
 
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
-           "pt_batch_append", "pt_batch_change", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
+           "pt_batch_append", "pt_batch_change", "pt_batch_exchange", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
            "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
@@ -121,6 +121,19 @@ class _ChangeView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("status", ctypes.c_void_p), ("delta", _PackedOps)]
 
 
+class _ExchangeInput(ctypes.Structure):
+    _fields_ = [("n_pairs", ctypes.c_uint32), ("pairs", ctypes.c_void_p), ("actor_off", ctypes.c_void_p), ("actor_map", ctypes.c_void_p),
+                ("ctr_off", ctypes.c_void_p), ("ctr_map", ctypes.c_void_p)]
+
+
+class _ExchangeView(ctypes.Structure):
+    _fields_ = [("n_pairs", ctypes.c_uint32), ("status", ctypes.c_void_p), ("delivered_off", ctypes.c_void_p), ("delivered", ctypes.c_void_p),
+                ("delta", ctypes.c_void_p)]
+
+
+PAIR_DT = np.dtype([("src", "<u4"), ("dst", "<u4")])
+
+
 class _SpansView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("results", ctypes.c_void_p), ("text_off", ctypes.c_void_p),
                 ("span_off", ctypes.c_void_p), ("text", ctypes.c_void_p), ("spans", ctypes.c_void_p),
@@ -173,6 +186,7 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_upload_changes.argtypes = [vp, vp]
     L.pt_batch_append.argtypes = [vp, vp, vp, vp]
     L.pt_batch_change.argtypes = [vp, vp, vp, vp]
+    L.pt_batch_exchange.argtypes = [vp, vp, vp]
     L.pt_compact_ops.argtypes = [vp, vp, vp, ctypes.c_int]
     L.pt_batch_upload_compact.argtypes = [vp, vp]
     L.pt_ingest_create.argtypes = [ctypes.POINTER(vp)]
@@ -313,6 +327,39 @@ class BatchEngine:
         self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
         self.patch_window = None                                             # the append resets the window
         return apply_append(batch, delta), change_dicts(batch, inputs, actor_ranks, status, delta), status
+
+    def exchange(self, pairs, maps: ExchangeMaps):
+        """Sync between logs of the resident batch on the device (pt_batch_exchange): for every (src, dst) of `pairs` (a list of
+        tuples or an (n, 2) array), log dst receives the changes it is missing from log src, in the reference's
+        getMissingChanges / applyChanges order, all pairs reading the batch as it is before the call.  `maps` comes from
+        ``packing.exchange_maps``, after its pre-append if it returned one.  Returns (per-pair status EXCHANGE_*, the delivered
+        indices into each src's change table in delivery order as (u64 offsets [n_pairs + 1], u32 indices), the DESC_DT delta:
+        per log the records it received, its n_actors and new max_ctr).  The handle then holds ``packing.apply_exchange`` of
+        the batch and needs a merge; a log's old n_insdel + n_mark as its patch window gives the Patches applyChanges
+        returned.  Needs a change table."""
+        a = np.asarray(pairs, np.int64).reshape(-1, 2)
+        pr = np.zeros(len(a), PAIR_DT)
+        pr["src"], pr["dst"] = a[:, 0], a[:, 1]
+        arrs = [None if a is None else np.ascontiguousarray(a, dtype=dt)
+                for a, dt in ((maps.actor_off, np.uint64), (maps.actor_map, np.uint16), (maps.ctr_off, np.uint64), (maps.ctr_map, np.uint32))]
+        ptr = lambda a: None if a is None or not len(a) else a.ctypes.data
+        inp = _ExchangeInput(len(pr), ptr(pr), *[ptr(a) for a in arrs])
+        v = _ExchangeView()
+        _check(self._L.pt_batch_exchange(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_exchange")
+
+        def arr(p, count, dt):
+            if not count or not p:
+                return np.zeros(0, dt)
+            return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
+        status = arr(v.status, v.n_pairs, np.uint32)
+        off = arr(v.delivered_off, v.n_pairs + 1, np.uint64)
+        flat = arr(v.delivered, int(off[-1]) if len(off) else 0, np.uint32)
+        desc = arr(v.delta, self.n_logs, DESC_DT)
+        got = int(desc["n_insdel"].astype(np.uint64).sum())
+        self._n_insdel += got
+        self._n_seq += got
+        self.patch_window = None                                             # the splice resets the window
+        return status, (off, flat), desc
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion

@@ -433,6 +433,52 @@ def _flat_maps(maps: Sequence[Sequence[int] | None], dtype) -> tuple[np.ndarray 
     return off, np.array(flat, dtype)
 
 
+def _grown_ids(prev: PackedBatch, i: int, new_actors, new_max_ctr: int, n_new_ops: int, new_used):
+    """Log i's packed id space after it gains `n_new_ops` ops that name the actors `new_actors`, have opId counters up to
+    `new_max_ctr` and name the counters `new_used()` (original counters; called only where the grown log is dense): ``pack_logs``'s
+    rules on the full log.  Returns (actors in rank order, actor -> rank, old rank -> new rank or None for the identity, the
+    dense counter table or None, original -> packed counter, the packed max_ctr, old packed -> new packed counter or None)."""
+    d = prev.desc[i]
+    old_actors = list(prev.log_actors[i])
+    ranked = sorted(set(old_actors) | set(new_actors), key=js_key)
+    if len(ranked) > 0xFFFF:
+        raise ValueError("more than 65535 actors in one log")
+    rank = {a: r for r, a in enumerate(ranked)}
+    amap = [rank[a] for a in old_actors]
+    old_dense = prev.log_counters[i] if i < len(prev.log_counters) else None
+    old_max_ctr = int(d["max_ctr"])
+    full_max = max(int(old_dense[old_max_ctr]) if old_dense is not None else old_max_ctr, new_max_ctr)
+    full_ops = int(d["n_insdel"]) + int(d["n_mark"]) + n_new_ops
+    if _wants_dense(full_max, full_ops):
+        if old_dense is not None:
+            old_used = set(int(c) for c in old_dense[1:])
+        else:
+            ins, mk = prev.log_slice(i)
+            old_used = set(np.concatenate([ins["ctr"], ins["ref_ctr"], mk["ctr"], mk["start_ctr"], mk["end_ctr"]]).astype(np.int64).tolist())
+            old_used.discard(0)
+        order = sorted(old_used | new_used())
+        dense = {c: k + 1 for k, c in enumerate(order)}
+        dense[0] = 0
+        table = np.array([0] + order, dtype=np.uint64)
+        dc = dense.__getitem__
+        new_max = dense[full_max]
+        if old_dense is not None:
+            cm = [dense[int(c)] for c in old_dense]
+        else:
+            # the domain: every counter the old records name (a mark boundary may name an element inserted later), up
+            # to a bound that keeps a reference far past the log's opIds from sizing the map
+            cap = 2 * (old_max_ctr + int(d["n_insdel"]) + int(d["n_mark"])) + 16
+            hi = max([old_max_ctr] + [c for c in old_used if c <= cap])
+            cm = [dense.get(c, CTR_UNUSED) for c in range(hi + 1)]
+    else:
+        table = None
+        dc = (lambda c: c)
+        new_max = full_max
+        cm = [int(c) for c in old_dense] if old_dense is not None else None
+    return (ranked, rank, amap if amap != list(range(len(amap))) else None, table, dc, new_max,
+            cm if cm is not None and cm != list(range(len(cm))) else None)
+
+
 def pack_append(prev: PackedBatch, new_logs: Sequence[Sequence[dict]], *, with_changes: bool = False,
                 list_ids: Sequence[str | None] | None = None) -> tuple[PackedBatch, AppendRemap]:
     """The delta and remap of ``pt_batch_append`` that extend every log of ``prev`` (a ``pack_logs`` batch) with the Change
@@ -484,45 +530,9 @@ def pack_append(prev: PackedBatch, new_logs: Sequence[Sequence[dict]], *, with_c
     actor_maps, ctr_maps, log_actors, counters, ranks = [], [], [], [], []
     for i, b in enumerate(builders):
         d = prev.desc[i]
-        old_actors = list(prev.log_actors[i])
-        ranked = sorted(set(old_actors) | b.actors, key=js_key)
-        if len(ranked) > 0xFFFF:
-            raise ValueError("more than 65535 actors in one log")
-        rank = {a: r for r, a in enumerate(ranked)}
+        ranked, rank, amap, table, dc, new_max, cm = _grown_ids(prev, i, b.actors, b.max_ctr, len(b.insdel) + len(b.marks), lambda b=b: _used_counters(b))
         ranks.append(rank); log_actors.append(ranked)
-        amap = [rank[a] for a in old_actors]
-        actor_maps.append(amap if amap != list(range(len(amap))) else None)
-        old_dense = prev.log_counters[i] if i < len(prev.log_counters) else None
-        old_max_ctr = int(d["max_ctr"])
-        full_max = max(int(old_dense[old_max_ctr]) if old_dense is not None else old_max_ctr, b.max_ctr)
-        full_ops = int(d["n_insdel"]) + int(d["n_mark"]) + len(b.insdel) + len(b.marks)
-        if _wants_dense(full_max, full_ops):
-            if old_dense is not None:
-                old_used = set(int(c) for c in old_dense[1:])
-            else:
-                ins, mk = prev.log_slice(i)
-                old_used = set(np.concatenate([ins["ctr"], ins["ref_ctr"], mk["ctr"], mk["start_ctr"], mk["end_ctr"]]).astype(np.int64).tolist())
-                old_used.discard(0)
-            order = sorted(old_used | _used_counters(b))
-            dense = {c: k + 1 for k, c in enumerate(order)}
-            dense[0] = 0
-            counters.append(np.array([0] + order, dtype=np.uint64))
-            dc = dense.__getitem__
-            new_max = dense[full_max]
-            if old_dense is not None:
-                cm = [dense[int(c)] for c in old_dense]
-            else:
-                # the domain: every counter the old records name (a mark boundary may name an element inserted later), up
-                # to a bound that keeps a reference far past the log's opIds from sizing the map
-                cap = 2 * (old_max_ctr + int(d["n_insdel"]) + int(d["n_mark"])) + 16
-                hi = max([old_max_ctr] + [c for c in old_used if c <= cap])
-                cm = [dense.get(c, CTR_UNUSED) for c in range(hi + 1)]
-        else:
-            counters.append(None)
-            dc = (lambda c: c)
-            new_max = full_max
-            cm = [int(c) for c in old_dense] if old_dense is not None else None
-        ctr_maps.append(cm if cm is not None and cm != list(range(len(cm))) else None)
+        actor_maps.append(amap); counters.append(table); ctr_maps.append(cm)
         desc[i] = (io, mo, len(b.insdel), len(b.marks), max(1, len(ranked)), new_max)
         _emit_log(b, rank, dc, comment_rank, insdel, io, marks, mo, arrival_base=int(d["n_insdel"]))
         io += len(b.insdel); mo += len(b.marks)
@@ -676,6 +686,276 @@ def apply_append(prev: PackedBatch, delta: PackedBatch, remap: AppendRemap | Non
                               cat(oc.deps, dcg.deps, "dep_off", "n_deps", DEP_DT, map_actor, lambda d, lg: None))
     return PackedBatch(desc, insdel, marks, delta.values, delta.link_attrs, delta.comment_ids, delta.other_attrs, dict(prev.meta),
                        delta.log_actors, delta.log_counters, changes, delta.log_lists)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Exchange (include/peritext_b200.h pt_batch_exchange)
+# ------------------------------------------------------------------------------------------------------------------
+EXCHANGE_OK, EXCHANGE_BAD_TABLE, EXCHANGE_STUCK, EXCHANGE_UNMAPPED = 0, 1, 2, 3
+ACTOR_UNMAPPED = 0xFFFF      # an actor-map entry for a src actor without a rank in dst
+
+
+@dataclass
+class ExchangeMaps:
+    """The maps of ``pt_batch_exchange`` (pt_exchange_input), flat like ``AppendRemap``: pair p's actor map is
+    actor_map[actor_off[p]:actor_off[p+1]] (src actor rank -> dst actor rank, ACTOR_UNMAPPED = none; exactly src's n_actors
+    entries), its counter map ctr_map[ctr_off[p]:ctr_off[p+1]] (src packed counter -> dst packed counter, entry 0 = 0,
+    CTR_UNUSED = none; an empty range, or ctr_off None, is the identity)."""
+    actor_off: np.ndarray                    # u64 [n_pairs + 1]
+    actor_map: np.ndarray                    # u16
+    ctr_off: np.ndarray | None = None        # u64 [n_pairs + 1]
+    ctr_map: np.ndarray | None = None        # u32
+
+    @staticmethod
+    def of(actor_maps: Sequence, ctr_maps: Sequence | None = None) -> "ExchangeMaps":
+        """From one array per pair (a counter map may be None: identity)."""
+        def flat(maps, dt):
+            off = np.zeros(len(maps) + 1, np.uint64)
+            off[1:] = np.cumsum([0 if m is None else len(m) for m in maps])
+            return off, np.concatenate([np.asarray(m, dt) for m in maps if m is not None] + [np.zeros(0, dt)])
+        aoff, amap = flat(actor_maps, np.uint16)
+        if ctr_maps is None or all(m is None for m in ctr_maps):
+            return ExchangeMaps(aoff, amap)
+        return ExchangeMaps(aoff, amap, *flat(ctr_maps, np.uint32))
+
+    def actor(self, p: int) -> np.ndarray:
+        return self.actor_map[int(self.actor_off[p]): int(self.actor_off[p + 1])]
+
+    def ctr(self, p: int) -> np.ndarray | None:
+        if self.ctr_off is None or self.ctr_off[p + 1] == self.ctr_off[p]:
+            return None
+        return self.ctr_map[int(self.ctr_off[p]): int(self.ctr_off[p + 1])]
+
+
+def change_record_ranges(batch: PackedBatch, i: int) -> np.ndarray | None:
+    """Per change of log i (rows) the record ranges [ins_lo, ins_hi, mk_lo, mk_hi) of its list ops: change c holds the
+    list-op positions [P_c, P_c + n_ops_c), P_c = the sum of the earlier n_ops; mark record k sits at position
+    min(arrival_k, n_insdel) + k.  None if n_ops does not sum to the log's records or the arrivals do not fit."""
+    cd = batch.changes.desc[i]
+    ch = batch.changes.changes[int(cd["change_off"]): int(cd["change_off"]) + int(cd["n_changes"])]
+    ins, mk = batch.log_slice(i)
+    n, m = len(ins), len(mk)
+    ends = np.cumsum(ch["n_ops"].astype(np.int64))
+    if (int(ends[-1]) if len(ends) else 0) != n + m:
+        return None
+    x = np.stack([ends - ch["n_ops"], ends], 1)
+    mpos = np.minimum(mk["arrival"].astype(np.int64), n) + np.arange(m)
+
+    def before(pos):             # the first k with mpos[k] >= pos, by the bisection the device uses
+        lo, hi = 0, m
+        while lo < hi:
+            k = (lo + hi) // 2
+            if mpos[k] < pos:
+                lo = k + 1
+            else:
+                hi = k
+        return lo
+    k = np.array([[before(int(a)), before(int(b))] for a, b in x], np.int64).reshape(len(ch), 2)
+    r = np.stack([x[:, 0] - k[:, 0], x[:, 1] - k[:, 1], k[:, 0], k[:, 1]], 1)
+    if len(r) and ((r < 0).any() or (r[:, 1] > n).any() or (r[:, 1] < r[:, 0]).any() or (r[:, 3] < r[:, 2]).any()):
+        return None
+    return r
+
+
+def _log_changes(batch: PackedBatch, i: int):
+    cd = batch.changes.desc[i]
+    ch = batch.changes.changes[int(cd["change_off"]): int(cd["change_off"]) + int(cd["n_changes"])]
+    dp = batch.changes.deps[int(cd["dep_off"]): int(cd["dep_off"]) + int(cd["n_deps"])]
+    return ch, dp
+
+
+def exchange_maps(batch: PackedBatch, pairs) -> tuple[ExchangeMaps, tuple[PackedBatch, AppendRemap] | None]:
+    """The maps of ``pt_batch_exchange`` for `pairs` = [(src, dst), ...] on `batch` (a ``pack_logs(..., with_changes=True)``
+    batch or one grown from it), and the empty pre-append that introduces what the deliveries bring to each dst: new actors
+    (``log_actors``) and, where ``pack_logs`` would rank the grown log's counters densely (``log_counters``), its new counter
+    ranks.  Returns (maps, (delta, remap)) or (maps, None) if no log's id space moves; the maps are in the id spaces AFTER
+    ``apply_append(batch, delta, remap)`` / ``BatchEngine.append(delta, remap)``, so {A->B, B->A} sees both logs grown.
+    What a dst will receive is read from the change tables alone: src's changes by an actor past dst's count of that actor."""
+    n = batch.n_logs
+    names = [list(a) for a in batch.log_actors]
+    tables = list(batch.log_counters) if batch.log_counters else [None] * n
+    n_actors = batch.desc["n_actors"].astype(np.int64)
+    max_ctr = batch.desc["max_ctr"].astype(np.int64)
+    actor_maps_pre, ctr_maps_pre = [None] * n, [None] * n
+    moved = False
+    for src, dst in pairs:
+        sch, sdp = _log_changes(batch, src)
+        dch, _ = _log_changes(batch, dst)
+        have: dict[str, int] = {}
+        for c in dch:
+            a = batch.log_actors[dst][int(c["actor"])]
+            have[a] = have.get(a, 0) + 1
+        sn = batch.log_actors[src]
+        miss = [k for k, c in enumerate(sch) if int(c["seq"]) > have.get(sn[int(c["actor"])], 0)]
+        rng = change_record_ranges(batch, src)
+        if not miss or rng is None:
+            continue
+        ins, mk = batch.log_slice(src)
+        ins = np.concatenate([ins[rng[k, 0]: rng[k, 1]] for k in miss]); mk = np.concatenate([mk[rng[k, 2]: rng[k, 3]] for k in miss])
+        st = batch.log_counters[src] if batch.log_counters else None      # src's records are in the batch's id space
+        orig = (lambda c: int(c)) if st is None else (lambda c, st=st: int(st[int(c)]) if int(c) < len(st) else int(c))
+        actors = {sn[int(sch[k]["actor"])] for k in miss}
+        actors |= {sn[int(q["actor"])] for k in miss for q in sdp[int(sch[k]["dep_off"]): int(sch[k]["dep_off"]) + int(sch[k]["n_deps"])]}
+        for recs, ids in ((ins, (("ctr", "actor"), ("ref_ctr", "ref_actor"))), (mk, (("ctr", "actor"), ("start_ctr", "start_actor"), ("end_ctr", "end_actor")))):
+            for cf, af in ids:
+                actors |= {sn[int(a)] for c, a in zip(recs[cf], recs[af]) if int(c)}
+        used = lambda: {orig(c) for recs, fs in ((ins, ("ctr", "ref_ctr")), (mk, ("ctr", "start_ctr", "end_ctr"))) for f in fs for c in recs[f] if int(c)}
+        top = max([0] + [orig(c) for c in ins["ctr"]] + [orig(c) for c in mk["ctr"]])
+        ranked, _, amap, table, _, _, cm = _grown_ids(batch, dst, actors, top, len(ins) + len(mk), used)
+        old_max = int(batch.desc[dst]["max_ctr"])
+        moved = moved or ranked != names[dst] or amap is not None or cm is not None or (table is None) != (tables[dst] is None) or \
+            (table is not None and len(table) != len(tables[dst]))
+        names[dst], tables[dst] = ranked, table
+        actor_maps_pre[dst], ctr_maps_pre[dst] = amap, cm
+        n_actors[dst] = max(1, len(ranked))
+        max_ctr[dst] = old_max if cm is None else cm[old_max]       # the image of the old max_ctr: nothing is delivered yet
+    amaps, cmaps = [], []
+    for src, dst in pairs:
+        rank = {a: r for r, a in enumerate(names[dst])}
+        amaps.append(np.array([rank.get(a, ACTOR_UNMAPPED) for a in names[src]] + [ACTOR_UNMAPPED] * (int(n_actors[src]) - len(names[src])), np.uint16))
+        st, dt = tables[src], tables[dst]
+        if st is None and dt is None:
+            cmaps.append(None)
+            continue
+        orig = np.arange(int(max_ctr[src]) + 1, dtype=np.uint64) if st is None else np.asarray(st[: int(max_ctr[src]) + 1], np.uint64)
+        if dt is None:
+            cm = np.where(orig < CTR_UNUSED, orig, CTR_UNUSED).astype(np.uint32)
+        else:
+            at = np.minimum(np.searchsorted(dt, orig), len(dt) - 1)
+            cm = np.where(dt[at] == orig, at, CTR_UNUSED).astype(np.uint32)
+        cmaps.append(cm)
+    maps = ExchangeMaps.of(amaps, cmaps)
+    if not moved:
+        return maps, None
+    desc = np.zeros(n, DESC_DT)
+    desc["n_actors"], desc["max_ctr"] = n_actors, max_ctr
+    aoff, aflat = _flat_maps(actor_maps_pre, np.uint16)
+    coff, cflat = _flat_maps(ctr_maps_pre, np.uint32)
+    delta = PackedBatch(desc, np.zeros(0, INSDEL_DT), np.zeros(0, MARK_DT), batch.values, batch.link_attrs, batch.comment_ids, batch.other_attrs,
+                        dict(batch.meta), names, tables, ChangeTable(np.zeros(n, CDESC_DT), np.zeros(0, CHANGE_DT), np.zeros(0, DEP_DT)), list(batch.log_lists))
+    return maps, (delta, AppendRemap(aoff, aflat, coff, cflat))
+
+
+def _exchange_order(batch: PackedBatch, src: int, dst: int, amap: np.ndarray) -> tuple[int, list[int]]:
+    """Steps 1-3 of ``pt_batch_exchange`` for one pair: (status, src change indices in delivery order)."""
+    sch, sdp = _log_changes(batch, src)
+    dch, ddp = _log_changes(batch, dst)
+
+    def clock(ch, n_deps, n_actors):
+        cnt: dict[int, int] = {}
+        for c in ch:
+            a = int(c["actor"])
+            if a >= n_actors or int(c["seq"]) != cnt.get(a, 0) + 1 or int(c["dep_off"]) + int(c["n_deps"]) > n_deps:
+                return None
+            cnt[a] = cnt.get(a, 0) + 1
+        return cnt
+    rs, rd = int(batch.desc[src]["n_actors"]), int(batch.desc[dst]["n_actors"])
+    clk = clock(dch, len(ddp), rd)
+    cs = clock(sch, len(sdp), rs)
+    if clk is None or cs is None or change_record_ranges(batch, src) is None:
+        return EXCHANGE_BAD_TABLE, []
+    image = lambda a: int(amap[a]) if a < len(amap) else ACTOR_UNMAPPED
+    have = lambda a: clk.get(image(a), 0) if image(a) != ACTOR_UNMAPPED else 0
+    deps = lambda c: sdp[int(c["dep_off"]): int(c["dep_off"]) + int(c["n_deps"])]
+    # getMissingChanges (reference test/merge.ts:25-38): actors in the order src first saw them, ascending seq
+    queue = [k for a in dict.fromkeys(int(c["actor"]) for c in sch) for k, c in enumerate(sch) if int(c["actor"]) == a and int(c["seq"]) > have(a)]
+    if any(int(q["actor"]) >= rs for k in queue for q in deps(sch[k])):
+        return EXCHANGE_BAD_TABLE, []
+    if any(image(int(sch[k]["actor"])) == ACTOR_UNMAPPED or any(image(int(q["actor"])) == ACTOR_UNMAPPED for q in deps(sch[k])) for k in queue):
+        return EXCHANGE_UNMAPPED, []
+    # applyChanges (test/merge.ts:4-23): the front is applied or goes to the back
+    order = []
+    since = 0                        # requeues since the last delivery: a whole queue of them is a pass that admitted nothing
+    while queue:
+        k = queue.pop(0)
+        c = sch[k]
+        a = image(int(c["actor"]))
+        if int(c["seq"]) == clk.get(a, 0) + 1 and all(0 < clk.get(image(int(q["actor"])), 0) >= int(q["seq"]) for q in deps(c)):
+            clk[a] = int(c["seq"]); order.append(k); since = 0
+        else:
+            queue.append(k); since += 1
+            if since >= len(queue):
+                return EXCHANGE_STUCK, []
+    return EXCHANGE_OK, order
+
+
+def apply_exchange(batch: PackedBatch, pairs, maps: ExchangeMaps) -> tuple[PackedBatch, np.ndarray, list[list[int]], np.ndarray]:
+    """The readable host specification of ``pt_batch_exchange``: every pair (src, dst) delivers to log dst the changes it is
+    missing from log src, all pairs reading `batch` as it is.  Returns (the batch the handle holds afterwards, the per-pair
+    status EXCHANGE_*, per pair the delivered indices into src's change table in delivery order, the DESC_DT delta: per log
+    the records it received, its n_actors and new max_ctr).  Order: ``getMissingChanges`` then ``applyChanges`` (reference
+    test/merge.ts:4-38).  Records: the delivered changes' ins/del records in delivery order, then likewise their marks, ids
+    through the pair's maps (an id with counter 0 keeps its actor field), a mark's arrival = dst's old n_insdel + the delivered
+    ins/del records before it; change and dep actors through the actor map, dep_off relative to the delivered deps.  A pair
+    that is not EXCHANGE_OK delivers nothing.  Pools and per-log tables are `batch`'s."""
+    n = batch.n_logs
+    if batch.changes is None:
+        raise ValueError("apply_exchange: the batch has no change table")
+    seen = set()
+    for src, dst in pairs:
+        if not (0 <= src < n and 0 <= dst < n) or src == dst or dst in seen:
+            raise ValueError(f"apply_exchange: bad pair ({src}, {dst})")
+        seen.add(dst)
+    status = np.zeros(len(pairs), np.uint32)
+    delivered: list[list[int]] = []
+    ddesc = np.zeros(n, DESC_DT)
+    ddesc["n_actors"], ddesc["max_ctr"] = batch.desc["n_actors"], batch.desc["max_ctr"]
+    cdesc = np.zeros(n, CDESC_DT)
+    parts = {}
+    for p, (src, dst) in enumerate(pairs):
+        amap = maps.actor(p).astype(np.int64)
+        cmap = maps.ctr(p)
+        st, order = _exchange_order(batch, src, dst, amap)
+        if st == EXCHANGE_OK and order:
+            rng = change_record_ranges(batch, src)
+            sins, smk = batch.log_slice(src)
+            sch, sdp = _log_changes(batch, src)
+            ins = np.concatenate([sins[rng[k, 0]: rng[k, 1]] for k in order]).copy()
+            mk = np.concatenate([smk[rng[k, 2]: rng[k, 3]] for k in order]).copy()
+            # arrivals: dst's old records, the delivered ins/del records of the earlier changes, the mark's place in its own
+            before = np.cumsum([0] + [rng[k, 1] - rng[k, 0] for k in order])
+            mk["arrival"] = np.concatenate([int(batch.desc[dst]["n_insdel"]) + before[j] + np.clip(smk["arrival"][rng[k, 2]: rng[k, 3]].astype(np.int64) - rng[k, 0], 0, rng[k, 1] - rng[k, 0])
+                                            for j, k in enumerate(order)] + [np.zeros(0, np.int64)])
+            ch = sch[order].copy()
+            dp = np.concatenate([sdp[int(c["dep_off"]): int(c["dep_off"]) + int(c["n_deps"])] for c in ch] + [sdp[:0]]).copy()
+            ch["dep_off"] = np.cumsum([0] + [int(c["n_deps"]) for c in ch])[:-1]
+            ok = True
+
+            def actor(c, a):             # counter 0 names no actor
+                nonlocal ok
+                img = np.where(a < len(amap), amap[np.minimum(a, len(amap) - 1)] if len(amap) else ACTOR_UNMAPPED, ACTOR_UNMAPPED)
+                ok = ok and not ((c != 0) & (img == ACTOR_UNMAPPED)).any()
+                return np.where(c != 0, img, a)
+
+            def ctr(c):
+                nonlocal ok
+                if cmap is None or len(cmap) == 0:
+                    return c
+                img = np.where(c < len(cmap), np.asarray(cmap, np.int64)[np.minimum(c, len(cmap) - 1)], CTR_UNUSED)
+                ok = ok and not (img == CTR_UNUSED).any()
+                return img
+            for recs, ids in ((ins, (("ctr", "actor"), ("ref_ctr", "ref_actor"))), (mk, (("ctr", "actor"), ("start_ctr", "start_actor"), ("end_ctr", "end_actor")))):
+                for cf, af in ids:
+                    c = recs[cf].astype(np.int64)
+                    recs[af] = actor(c, recs[af].astype(np.int64)); recs[cf] = ctr(c)
+            one = np.ones(1, np.int64)
+            ch["actor"] = actor(np.repeat(one, len(ch)), ch["actor"].astype(np.int64)); dp["actor"] = actor(np.repeat(one, len(dp)), dp["actor"].astype(np.int64))
+            if not ok:
+                st, order = EXCHANGE_UNMAPPED, []
+            else:
+                parts[dst] = (ins, mk, ch, dp)
+                ddesc[dst]["n_insdel"], ddesc[dst]["n_mark"] = len(ins), len(mk)
+                ddesc[dst]["max_ctr"] = max([int(batch.desc[dst]["max_ctr"])] + [int(x) for x in ins["ctr"]] + [int(x) for x in mk["ctr"]])
+                cdesc[dst]["n_changes"], cdesc[dst]["n_deps"] = len(ch), len(dp)
+        status[p] = st
+        delivered.append([int(k) for k in order] if st == EXCHANGE_OK else [])
+    ddesc["insdel_off"], ddesc["mark_off"] = _excl_scan(ddesc["n_insdel"]), _excl_scan(ddesc["n_mark"])
+    cdesc["change_off"], cdesc["dep_off"] = _excl_scan(cdesc["n_changes"]), _excl_scan(cdesc["n_deps"])
+    got = [parts[i] for i in sorted(parts)]
+    cat = lambda j, dt: np.concatenate([g[j] for g in got] + [np.zeros(0, dt)])
+    delta = PackedBatch(ddesc, cat(0, INSDEL_DT), cat(1, MARK_DT), batch.values, batch.link_attrs, batch.comment_ids, batch.other_attrs, dict(batch.meta),
+                        batch.log_actors, batch.log_counters, ChangeTable(cdesc, cat(2, CHANGE_DT), cat(3, DEP_DT)), batch.log_lists)
+    return apply_append(batch, delta), status, delivered, ddesc
 
 
 def elem_refs(batch: PackedBatch, logs: Sequence[int], elem_ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:

@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-from .packing import DESC_DT, INSDEL_DT, MARK_DT, PackedBatch
+from .packing import CDESC_DT, CHANGE_DT, CHANGE_NO_ACTOR, DEP_DT, DESC_DT, INPUT_OP_DT, INSDEL_DT, MARK_DT, ChangeTable, ExchangeMaps, PackedBatch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpt_workload.so")
@@ -89,6 +89,56 @@ def generate(config: str, *, n_docs: int | None = None, ops_per_doc: int | None 
                                   ops_per_doc=cfg["ops_per_doc"], unique_ops=int(b.unique_ops), seed=seed, doc_first=doc_first))
     L.ptw_free(out)
     return batch
+
+
+def history_table(batch: PackedBatch) -> ChangeTable:
+    """A change table for a generated batch: every log's records as ONE change (seq 1 by actor rank 0, no deps, n_ops = all the
+    log's list ops), so all replicas of a document start with equal clocks.  Enough for the calls that need a table
+    (admission, pt_batch_change, pt_batch_exchange); the generated records carry no change boundaries of their own."""
+    n = batch.n_logs
+    cd = np.zeros(n, CDESC_DT)
+    cd["change_off"] = np.arange(n); cd["n_changes"] = 1
+    ch = np.zeros(n, CHANGE_DT)
+    ch["seq"] = 1
+    ch["n_ops"] = batch.desc["n_insdel"].astype(np.uint64) + batch.desc["n_mark"]
+    return ChangeTable(cd, ch, np.zeros(0, DEP_DT))
+
+
+def sync_round(batch: PackedBatch, seed: int = 1):
+    """One fuzz step (reference test/fuzz.ts:167-199) per document of a generated batch that carries ``history_table``: replica
+    r (random) of every document inserts one character at index 0 as actor rank r, then syncs both ways with another random
+    replica.  Returns (actor, input_off, ops, tokens: the arrays of pt_change_input; the change table of the new changes;
+    the pairs as an (n, 2) array, document by document {changer -> other, other -> changer}; their ExchangeMaps, all identity).
+    Vectorised: no per-document Python."""
+    R = int(batch.meta["replicas"])
+    n = batch.n_logs
+    docs = n // R
+    rng = np.random.default_rng(seed)
+    r = rng.integers(0, R, docs)
+    other = (r + 1 + rng.integers(0, R - 1, docs)) % R
+    log = np.arange(docs) * R + r
+    actor = np.full(n, CHANGE_NO_ACTOR, np.uint32)
+    actor[log] = r
+    off = np.zeros(n + 1, np.uint64)
+    off[1:] = np.cumsum(actor != CHANGE_NO_ACTOR)
+    ops = np.zeros(docs, INPUT_OP_DT)
+    ops["arg"] = 1; ops["attr"] = 0xFFFFFFFF
+    ops["first_ctr"] = batch.desc["max_ctr"][log].astype(np.uint64) + 1
+    ops["tok_off"] = np.arange(docs)
+    tokens = np.full(docs, ord("x"), np.uint32)
+    cd = np.zeros(n, CDESC_DT)
+    cd["n_changes"][log] = 1; cd["n_deps"][log] = r != 0
+    cd["change_off"] = np.cumsum(cd["n_changes"]) - cd["n_changes"]; cd["dep_off"] = np.cumsum(cd["n_deps"]) - cd["n_deps"]
+    ch = np.zeros(docs, CHANGE_DT)                    # actor 0 made the history's change: its next is seq 2; the others depend on it
+    ch["seq"] = np.where(r == 0, 2, 1); ch["actor"] = r; ch["n_deps"] = r != 0; ch["n_ops"] = 1
+    dp = np.zeros(int((r != 0).sum()), DEP_DT)
+    dp["seq"] = 1
+    pairs = np.stack([np.stack([log, np.arange(docs) * R + other], 1), np.stack([np.arange(docs) * R + other, log], 1)], 1).reshape(-1, 2)
+    na = batch.desc["n_actors"][pairs[:, 0]].astype(np.int64)
+    aoff = np.zeros(len(pairs) + 1, np.uint64)
+    aoff[1:] = np.cumsum(na)
+    amap = (np.arange(int(aoff[-1])) - np.repeat(aoff[:-1].astype(np.int64), na)).astype(np.uint16)
+    return actor, off, ops, tokens, ChangeTable(cd, ch, dp), pairs, ExchangeMaps(aoff, amap)
 
 
 def to_change_json(batch: PackedBatch, i: int) -> str:
