@@ -23,6 +23,10 @@
 #include "append_kernel.cuh"
 #include "change_kernel.cuh"
 #include "exchange_kernel.cuh"
+#include "upload_kernel.cuh"
+#include "scan_kernel.cuh"
+#include "admit_kernel.cuh"
+#include "query_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -63,6 +67,10 @@ using HostBuf = Buf<true>;
 using ptp::kNumBins;
 using ptp::kCtaBins;
 
+// Room for n elements of T, at least one: a batch without logs or records still gets valid pointers.
+template <class T, bool kPinned>
+int reserve_n(Buf<kPinned>& buf, uint64_t n) { return buf.reserve(std::max<uint64_t>(1, n) * sizeof(T)); }
+
 // One JSON render's buffers: per-log sizes, scan, offsets, missing-entry key and output on the device; the view's offsets
 // and bytes and the read-back of the total in pinned memory.
 struct JsonBufs {
@@ -81,338 +89,6 @@ struct DevCounters {
     uint32_t retry_head[kNumBins];        // work-queue heads of the CTA bins' retry launches ([0] unused)
     uint32_t deferred[kNumBins];          // logs deferred into bin k, appended to list k of d_retry ([0] unused)
 };
-
-// Expands run-compressed ins/del streams into pt_insdel_rec records (one warp per log, lanes over the runs; a run's
-// records are written by its lane — runs are short, and the expanded array is consumed from L2/HBM by the merge kernel).
-__global__ void expand_runs_kernel(const pt_log_desc* __restrict__ desc, const unsigned long long* __restrict__ run_off,
-                                   const unsigned long long* __restrict__ tok_off, const pt_run_rec* __restrict__ runs,
-                                   const uint32_t* __restrict__ tokens, pt_insdel_rec* __restrict__ out, uint32_t n_logs) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t li = warp; li < n_logs; li += nwarps) {
-        const unsigned long long r0 = run_off[li], r1 = run_off[li + 1];
-        pt_insdel_rec* o = out + desc[li].insdel_off;
-        const uint32_t* tk = tokens + tok_off[li];
-        uint32_t rec_base = 0, tok_base = 0;
-        for (unsigned long long rb = r0; rb < r1; rb += 32) {
-            const unsigned long long ri = rb + lane;
-            uint4 r = make_uint4(0, 0, 0, 0);
-            uint32_t cnt = 0, kind = 0;
-            if (ri < r1) { r = __ldg(reinterpret_cast<const uint4*>(runs + ri)); cnt = r.w & 0x3FFFFFFFu; kind = r.w >> 30; }
-            uint32_t tcnt = kind == PT_KIND_INSERT ? cnt : 0u;
-            // exclusive prefix sums of the record and token counts inside the warp
-            uint32_t pr = cnt, pt = tcnt;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint32_t a = __shfl_up_sync(0xffffffffu, pr, d), b2 = __shfl_up_sync(0xffffffffu, pt, d); if (lane >= (uint32_t)d) { pr += a; pt += b2; } }
-            const uint32_t tot_r = __shfl_sync(0xffffffffu, pr, 31), tot_t = __shfl_sync(0xffffffffu, pt, 31);
-            uint32_t ro = rec_base + pr - cnt, to = tok_base + pt - tcnt;
-            const uint32_t actor = r.z & 0xFFFFu;
-            for (uint32_t k = 0; k < cnt; k++) {
-                uint4 w;
-                w.x = r.x + k;
-                if (kind == PT_KIND_INSERT) {
-                    w.y = k == 0 ? r.y : r.x + k - 1;
-                    w.z = actor | ((k == 0 ? (r.z >> 16) : actor) << 16);
-                    w.w = (PT_KIND_INSERT << 30) | tk[to + k];
-                } else {
-                    w.y = r.y + k; w.z = r.z; w.w = kind << 30;
-                }
-                reinterpret_cast<uint4*>(o)[ro + k] = w;
-            }
-            rec_base += tot_r; tok_base += tot_t;
-        }
-    }
-}
-
-
-// ---- compact wire format: elementwise expansion to the 16 / 32 byte records the merge kernels read -------------------------
-__global__ void expand_insdel_c8_kernel(const pt_insdel_c8* __restrict__ in, pt_insdel_rec* __restrict__ out, unsigned long long n) {
-    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
-        const uint2 q = __ldg(reinterpret_cast<const uint2*>(in + i));
-        const uint32_t tok22 = q.y >> 10;
-        uint4 o;
-        o.x = q.x & 0xFFFFu; o.y = q.x >> 16;
-        o.z = (q.y & 0xFu) | (((q.y >> 4) & 0xFu) << 16);
-        o.w = (((q.y >> 8) & 3u) << 30) | ((tok22 & 0x200000u) ? PT_TOKEN_POOLED : 0u) | (tok22 & 0x1FFFFFu);
-        reinterpret_cast<uint4*>(out)[i] = o;
-    }
-}
-__global__ void expand_mark_c16_kernel(const pt_mark_c16* __restrict__ in, pt_mark_rec* __restrict__ out, unsigned long long n) {
-    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
-        const uint4 q = __ldg(reinterpret_cast<const uint4*>(in + i));
-        // pt_mark_rec: {ctr, actor | kind << 16 | bounds << 24, start_ctr, end_ctr} {start_actor | end_actor << 16, attr, arrival, 0}
-        uint4 a, b;
-        a.x = q.x & 0xFFFFu;
-        a.y = (q.w & 0xFu) | (((q.w >> 12) & 7u) << 16) | (((q.w >> 15) & 0xFu) << 24);
-        a.z = q.x >> 16; a.w = q.y & 0xFFFFu;
-        b.x = ((q.w >> 4) & 0xFu) | (((q.w >> 8) & 0xFu) << 16);
-        b.y = q.z; b.z = q.y >> 16; b.w = 0;
-        reinterpret_cast<uint4*>(out)[2 * i] = a; reinterpret_cast<uint4*>(out)[2 * i + 1] = b;
-    }
-}
-
-// ---- output compaction (download path) ---------------------------------------------------------------------------------
-// The merge kernels write each log's tokens / spans at offsets derived from the descriptors alone (capacity = n_insdel
-// tokens, min(n_insdel, 2 n_mark + 1) spans), typically a few percent full (c4: 5 visible characters per 500-record log).
-// Before the device -> host copy the used prefixes are packed back to back: exclusive scan of (n_visible, n_spans) over
-// the logs (block sums -> one-block scan -> offsets), then one warp per log copies its tokens and spans.
-// The scan kernels take the per-log counts from a source functor: two channels (a, c) per log.  The JSON render
-// (render_kernel.cuh) scans its per-log byte counts through the same kernels, on channel a only.
-constexpr uint32_t kScanBlock = 1024;
-struct MergedCounts {      // (n_visible, n_spans) of the logs that merged, 0 for the others
-    const pt_log_result* __restrict__ res;
-    __device__ void operator()(uint32_t i, unsigned long long& a, unsigned long long& c) const {
-        if (res[i].status == 0) { a = res[i].n_visible; c = res[i].n_spans; }
-    }
-};
-struct PlainCounts {       // a u64 count per log on channel a
-    const unsigned long long* __restrict__ cnt;
-    __device__ void operator()(uint32_t i, unsigned long long& a, unsigned long long&) const { a = cnt[i]; }
-};
-template <class Src>
-__global__ void out_block_sums_kernel(Src src, uint32_t n, unsigned long long* __restrict__ bsum) {
-    __shared__ unsigned long long sa[32], sb[32];
-    const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned long long a = 0, c = 0;
-    if (i < n) src(i, a, c);
-    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
-    if (lane == 0) { sa[warp] = a; sb[warp] = c; }
-    __syncthreads();
-    if (warp == 0) {
-        a = sa[lane]; c = sb[lane];
-        for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
-        if (lane == 0) { bsum[2 * blockIdx.x] = a; bsum[2 * blockIdx.x + 1] = c; }
-    }
-}
-__global__ void out_scan_blocks_kernel(unsigned long long* bsum, uint32_t nb) {   // one block; exclusive scan in place, totals at [2 nb]
-    __shared__ unsigned long long ca, cb;
-    __shared__ unsigned long long wa[32], wb[32];
-    if (threadIdx.x == 0) { ca = 0; cb = 0; }
-    __syncthreads();
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (uint32_t base = 0; base < nb; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const unsigned long long va = i < nb ? bsum[2 * i] : 0ull, vb = i < nb ? bsum[2 * i + 1] : 0ull;
-        unsigned long long a = va, c = vb;
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long ya = __shfl_up_sync(0xffffffffu, a, o), yb = __shfl_up_sync(0xffffffffu, c, o);
-            if (lane >= (uint32_t)o) { a += ya; c += yb; }
-        }
-        if (lane == 31) { wa[warp] = a; wb[warp] = c; }
-        __syncthreads();
-        if (warp == 0) {
-            unsigned long long x = wa[lane], y = wb[lane];
-            const unsigned long long x0 = x, y0 = y;
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned long long yx = __shfl_up_sync(0xffffffffu, x, o), yy = __shfl_up_sync(0xffffffffu, y, o);
-                if (lane >= (uint32_t)o) { x += yx; y += yy; }
-            }
-            wa[lane] = x - x0; wb[lane] = y - y0;
-        }
-        __syncthreads();
-        const unsigned long long ea = ca + wa[warp] + a - va, eb = cb + wb[warp] + c - vb;
-        if (i < nb) { bsum[2 * i] = ea; bsum[2 * i + 1] = eb; }
-        __syncthreads();
-        if (threadIdx.x == 1023) { ca = ea + va; cb = eb + vb; }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { bsum[2 * nb] = ca; bsum[2 * nb + 1] = cb; }
-}
-template <class Src>   // soff may be null (one-channel sources)
-__global__ void out_offsets_kernel(Src src, uint32_t n, const unsigned long long* __restrict__ bsum, uint32_t nb,
-                                   unsigned long long* __restrict__ toff, unsigned long long* __restrict__ soff) {
-    __shared__ unsigned long long wa[32], wb[32];
-    const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned long long va = 0, vb = 0;
-    if (i < n) src(i, va, vb);
-    unsigned long long a = va, c = vb;
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long ya = __shfl_up_sync(0xffffffffu, a, o), yb = __shfl_up_sync(0xffffffffu, c, o);
-        if (lane >= (uint32_t)o) { a += ya; c += yb; }
-    }
-    if (lane == 31) { wa[warp] = a; wb[warp] = c; }
-    __syncthreads();
-    if (warp == 0) {
-        unsigned long long x = wa[lane], y = wb[lane];
-        const unsigned long long x0 = x, y0 = y;
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long yx = __shfl_up_sync(0xffffffffu, x, o), yy = __shfl_up_sync(0xffffffffu, y, o);
-            if (lane >= (uint32_t)o) { x += yx; y += yy; }
-        }
-        wa[lane] = x - x0; wb[lane] = y - y0;
-    }
-    __syncthreads();
-    if (i < n) { toff[i] = bsum[2 * blockIdx.x] + wa[warp] + a - va; if (soff) soff[i] = bsum[2 * blockIdx.x + 1] + wb[warp] + c - vb; }
-    if (i == 0) { toff[n] = bsum[2 * nb]; if (soff) soff[n] = bsum[2 * nb + 1]; }
-}
-__global__ void out_gather_kernel(const pt_log_result* __restrict__ res, uint32_t n, const uint64_t* __restrict__ cap_toff, const uint64_t* __restrict__ cap_soff,
-                                  const unsigned long long* __restrict__ toff, const unsigned long long* __restrict__ soff,
-                                  const uint32_t* __restrict__ text, const pt_span* __restrict__ spans, uint32_t* __restrict__ ctext, pt_span* __restrict__ cspans) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t li = warp; li < n; li += nwarps) {
-        if (res[li].status != 0) continue;
-        const uint32_t nv = res[li].n_visible, ns = res[li].n_spans;
-        const uint32_t* ts = text + cap_toff[li]; uint32_t* td = ctext + toff[li];
-        for (uint32_t k = lane; k < nv; k += 32) td[k] = ts[k];
-        const uint4* ss = reinterpret_cast<const uint4*>(spans + cap_soff[li]); uint4* sd = reinterpret_cast<uint4*>(cspans + soff[li]);
-        for (uint32_t k = lane; k < ns; k += 32) sd[k] = ss[k];
-    }
-}
-
-
-// ---- admission pre-pass: Micromerge.applyChange's causal checks (reference src/micromerge.ts:499-511) for every log -------
-// One warp per log, one lane per change, 32 changes per trip.  The reference keeps clock[actor] = seq of the last applied
-// change; as long as every earlier change of the log was admitted that is the NUMBER of earlier changes by that actor, so
-// each change can be checked independently against per-actor prefix counts (match_any groups inside the trip + running
-// counts in shared memory), and the FIRST failing change — what the reference would throw at — is a min over lanes.
-__global__ void admit_kernel(const pt_change_desc* __restrict__ cd, const pt_change_rec* __restrict__ ch, const pt_dep_rec* __restrict__ dp,
-                             const pt_log_desc* __restrict__ desc, uint32_t n_logs, uint32_t maxR, uint32_t* __restrict__ admit, pt_log_result* __restrict__ results) {
-    extern __shared__ uint32_t adm_smem[];
-    const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-    uint32_t* cnt = adm_smem + (size_t)wib * 2 * maxR;      // changes admitted so far, per actor
-    uint32_t* cmask = cnt + maxR;                           // lanes of the current trip, per actor
-    const uint32_t lt = (1u << lane) - 1u;
-    for (uint32_t li = blockIdx.x * wpb + wib; li < n_logs; li += gridDim.x * wpb) {
-        const pt_change_desc D = cd[li];
-        const uint32_t R = desc[li].n_actors ? desc[li].n_actors : 1u;
-        for (uint32_t a = lane; a < R; a += 32) { cnt[a] = 0; cmask[a] = 0; }
-        __syncwarp();
-        const pt_change_rec* c0 = ch + D.change_off; const pt_dep_rec* d0 = dp + D.dep_off;
-        uint32_t fail_idx = 0xFFFFFFFFu, fail_code = 0;
-        for (uint32_t base = 0; base < D.n_changes; base += 32) {
-            const uint32_t k = base + lane;
-            const bool valid = k < D.n_changes;
-            uint4 r = make_uint4(0, 0, 0, 0);
-            if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
-            const uint32_t seq = r.x, actor = r.y & 0xFFFFu, n_deps = r.y >> 16, dep_off = r.z;
-            const bool aok = valid && actor < R;
-            const uint32_t a = aok ? actor : (0x10000u + lane);
-            const uint32_t mask = __match_any_sync(0xffffffffu, a);
-            const bool leader = (mask & lt) == 0;
-            if (aok && leader) cmask[actor] = mask;
-            __syncwarp();
-            uint32_t code = 0;
-            if (valid) {
-                if (!aok) code = PT_LOG_BAD_OPID;
-                else if (seq != cnt[actor] + __popc(mask & lt) + 1u) code = PT_LOG_SEQ_GAP;            // src/micromerge.ts:501-504
-                else if (dep_off + n_deps > D.n_deps) code = PT_LOG_BAD_OPID;
-                else for (uint32_t d = 0; d < n_deps; d++) {                                            // src/micromerge.ts:505-509
-                    const pt_dep_rec q = d0[dep_off + d];
-                    const uint32_t have = q.actor < R ? cnt[q.actor] + __popc(cmask[q.actor] & lt) : 0u;
-                    if (have == 0 || have < q.seq) { code = PT_LOG_MISSING_DEP; break; }
-                }
-            }
-            const uint32_t bal = __ballot_sync(0xffffffffu, code != 0);
-            if (bal) { const uint32_t f = __ffs(bal) - 1; fail_idx = base + f; fail_code = __shfl_sync(0xffffffffu, code, f); break; }
-            __syncwarp();
-            if (aok && leader) { cnt[actor] += __popc(mask); cmask[actor] = 0; }
-            __syncwarp();
-        }
-        if (lane == 0) {
-            admit[li] = fail_code;
-            if (fail_code) { pt_log_result r{}; r.status = fail_code; r.n_elems = fail_idx; results[li] = r; }
-        }
-        __syncwarp();
-    }
-}
-
-
-// ---- batched getListElementId (reference src/micromerge.ts:762-805) over the materialised element sequences ----------------
-// One warp per query: ballot / popcount over the sequence words finds the k-th visible element; lookAfterTombstones then
-// scans the run of tombstones that follows for the last one whose markOpsAfter slot is defined (bit 30).
-__global__ void query_elements_kernel(const pt_elem_query* __restrict__ q, uint32_t n, const pt_log_result* __restrict__ res,
-                                      const uint64_t* __restrict__ seq_off, const uint32_t* __restrict__ seq, uint32_t n_logs, uint32_t* __restrict__ out) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t k = warp; k < n; k += nwarps) {
-        const pt_elem_query Q = q[k];
-        uint32_t ans = PT_ELEM_NOT_FOUND;
-        if (Q.log < n_logs && res[Q.log].status == 0) {
-            const uint32_t N = res[Q.log].n_elems;
-            const uint32_t* s = seq + seq_off[Q.log];
-            uint32_t seen = 0, pos = 0xFFFFFFFFu;
-            for (uint32_t b = 0; b < N && pos == 0xFFFFFFFFu; b += 32) {
-                const uint32_t e = b + lane < N ? s[b + lane] : 0x80000000u;
-                const uint32_t vis = __ballot_sync(0xffffffffu, !(e >> 31));
-                const uint32_t c = __popc(vis);
-                if (seen + c > Q.index) {
-                    uint32_t m = vis;                                        // (index - seen)-th set bit
-                    for (uint32_t r = Q.index - seen; r; r--) m &= m - 1;
-                    pos = b + (__ffs(m) - 1);
-                }
-                seen += c;
-            }
-            if (pos != 0xFFFFFFFFu) {
-                uint32_t best = pos;
-                if (Q.flags & PT_QUERY_LOOK_AFTER_TOMBSTONES) {
-                    bool open = true;
-                    for (uint32_t b = pos + 1; b < N && open; b += 32) {
-                        const uint32_t e = b + lane < N ? s[b + lane] : 0u;      // past the end counts as "not a tombstone"
-                        const uint32_t live = __ballot_sync(0xffffffffu, !(e >> 31));
-                        const uint32_t upto = live ? ((1u << (__ffs(live) - 1)) - 1u) : 0xFFFFFFFFu;    // tombstones before the next visible element
-                        const uint32_t marked = __ballot_sync(0xffffffffu, (e >> 30) & 1u) & upto;
-                        if (marked) best = b + (31 - __clz(marked));
-                        open = live == 0;
-                    }
-                }
-                ans = s[best] & 0x3FFFFFFFu;
-            }
-        }
-        if (lane == 0) out[k] = ans;
-    }
-}
-
-// ---- batched findListElement (reference src/micromerge.ts:731-755; resolveCursor :475 = .visible) -------------------------
-// One warp per query, the inverse of query_elements_kernel.  Stage 1 finds the element's insert record: the log's ins/del
-// records 32 per trip (coalesced 16-byte loads), first ballot hit (a log that merged OK has no duplicate insert opIds).
-// Stage 2 finds the sequence word that names that record, 32 words per trip, and counts the visible elements before it:
-// the running popcount of the live ballot plus the live lanes below the matching one.  O(n_insdel + n_elems) reads per
-// query, like the reference's linear scan.
-__global__ void find_elements_kernel(const pt_elem_ref* __restrict__ q, uint32_t n, const pt_log_desc* __restrict__ desc,
-                                     const pt_insdel_rec* __restrict__ insdel, const pt_log_result* __restrict__ res,
-                                     const uint64_t* __restrict__ seq_off, const uint32_t* __restrict__ seq, uint32_t n_logs,
-                                     pt_elem_pos* __restrict__ out) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t k = warp; k < n; k += nwarps) {
-        const uint4 Q = __ldg(reinterpret_cast<const uint4*>(q + k));
-        const uint32_t log = Q.x, ctr = Q.y, actor = Q.z & 0xFFFFu;
-        uint4 ans = make_uint4(PT_ELEM_NOT_FOUND, 0u, PT_ELEM_NOT_FOUND, 0u);      // index, visible, record, flags
-        if (log >= n_logs || res[log].status != PT_LOG_OK) {
-            ans.w = PT_ELEM_LOG_FAILED;
-        } else if (ctr != 0) {
-            const pt_log_desc D = desc[log];
-            const uint4* r = reinterpret_cast<const uint4*>(insdel + D.insdel_off);
-            uint32_t rec = PT_ELEM_NOT_FOUND;
-            for (uint32_t b = 0; b < D.n_insdel; b += 32) {
-                bool hit = false;
-                if (b + lane < D.n_insdel) {
-                    const uint4 w = __ldg(r + b + lane);
-                    hit = w.x == ctr && (w.z & 0xFFFFu) == actor && PT_PAYLOAD_KIND(w.w) == PT_KIND_INSERT;
-                }
-                const uint32_t bal = __ballot_sync(0xffffffffu, hit);
-                if (bal) { rec = b + __ffs(bal) - 1; break; }
-            }
-            if (rec != PT_ELEM_NOT_FOUND) {
-                const uint32_t N = res[log].n_elems;
-                const uint32_t* s = seq + seq_off[log];
-                uint32_t seen = 0;
-                for (uint32_t b = 0; b < N; b += 32) {
-                    const bool valid = b + lane < N;
-                    const uint32_t e = valid ? s[b + lane] : 0u;
-                    const uint32_t live = __ballot_sync(0xffffffffu, valid && !(e >> 31));
-                    const uint32_t match = __ballot_sync(0xffffffffu, valid && (e & 0x3FFFFFFFu) == rec);
-                    if (match) {
-                        const uint32_t m = __ffs(match) - 1;
-                        const uint32_t em = __shfl_sync(0xffffffffu, e, m);
-                        ans = make_uint4(b + m, seen + __popc(live & ((1u << m) - 1u)), rec,
-                                         ((em >> 31) ? PT_ELEM_DELETED : 0u) | (((em >> 30) & 1u) ? PT_ELEM_AFTER_DEFINED : 0u));
-                        break;
-                    }
-                    seen += __popc(live);
-                }
-            }
-        }
-        if (lane == 0) reinterpret_cast<uint4*>(out)[k] = ans;
-    }
-}
 
 }  // namespace
 
@@ -474,28 +150,84 @@ void drop_graph(pt_batch* b) {
     b->graph_exec = nullptr; b->graph_ok = false; b->graph_tried = false; b->merges_since_upload = 0;
 }
 
+// Every kernel launch is followed by PT_CUDA(launched(b)): the launch's error, else one more in pt_batch_launch_count.
+cudaError_t launched(pt_batch* b) {
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) b->launches++;
+    return e;
+}
+
+// reserve_n, then (n > 0) the copy of n elements from the host on the batch's stream.
+template <class T>
+int upload_n(pt_batch* b, DevBuf& buf, const T* src, uint64_t n) {
+    int rc;
+    if ((rc = reserve_n<T>(buf, n))) return rc;
+    if (n) PT_CUDA(cudaMemcpyAsync(buf.p, src, n * sizeof(T), cudaMemcpyHostToDevice, b->stream));
+    return PT_OK;
+}
+
+// CTAs of `threads` threads for a grid-stride loop over n_items items of `lanes` threads (a warp): at most 16 per SM.
+uint32_t warp_grid(const pt_batch* b, uint64_t n_items, uint32_t threads, uint32_t lanes = 32) {
+    return (uint32_t)std::min<uint64_t>((n_items * lanes + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+}
+
+// One warp per item (n_items > 0), and an item with many records shared by up to 64 warps, one per slice of 8 K records
+// (gridDim.y): a few huge items (c5) must not leave the copy to a handful of warps.  most: the largest item's records.
+dim3 slice_grid(const pt_batch* b, uint64_t n_items, uint64_t most, uint32_t threads) {
+    const uint32_t slices = (uint32_t)std::clamp<uint64_t>(most / 8192, 1, 64);
+    return dim3(std::min<uint32_t>(warp_grid(b, n_items, threads), (uint32_t)b->num_sms * 16 / slices), slices);
+}
+
+// admit_kernel and exchange_select_kernel keep two words per actor for each warp in shared memory, at most kAdmitMaxBytes.
+constexpr size_t kAdmitMaxBytes = 200 * 1024;
+size_t actor_table_bytes(uint32_t maxR) { return (size_t)2 * maxR * 4; }
+
+// Their launch shape (warps per CTA, shared bytes): 4 warps while the tables fit the default 48 KB, else one warp.
+std::pair<uint32_t, size_t> actor_shape(uint32_t maxR) {
+    const size_t per_warp = actor_table_bytes(maxR);
+    const uint32_t wpb = per_warp * 4 <= 48 * 1024 ? 4u : 1u;
+    return {wpb, per_warp * wpb};
+}
+
+// The scan triple over n per-log counts of src (scan_kernel.cuh): block sums into bsum, their scan, then each log's
+// exclusive offset in off0 (channel a) and off1 (channel c; may be null), the totals at [n].
+template <class Src>
+int scan_offsets(pt_batch* b, Src src, uint32_t n, DevBuf& bsum_buf, unsigned long long* off0, unsigned long long* off1) {
+    const uint32_t nb = (n + pts::kScanBlock - 1) / pts::kScanBlock;
+    int rc;
+    if ((rc = reserve_n<unsigned long long>(bsum_buf, 2 * nb + 2))) return rc;
+    unsigned long long* bsum = (unsigned long long*)bsum_buf.p;
+    pts::out_block_sums_kernel<<<nb, pts::kScanBlock, 0, b->stream>>>(src, n, bsum);
+    PT_CUDA(launched(b));
+    pts::out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
+    PT_CUDA(launched(b));
+    pts::out_offsets_kernel<<<nb, pts::kScanBlock, 0, b->stream>>>(src, n, bsum, nb, off0, off1);
+    PT_CUDA(launched(b));
+    return PT_OK;
+}
+
 int alloc_and_upload_plan(pt_batch* b) {
     int rc;
     const size_t n = b->n_logs;
     const ptp::Plan& pl = b->plan;
-    if ((rc = b->d_desc.reserve(std::max<size_t>(1, n) * sizeof(pt_log_desc)))) return rc;
-    if ((rc = b->d_order.reserve(std::max<size_t>(1, n) * 4))) return rc;
+    if ((rc = reserve_n<pt_log_desc>(b->d_desc, n))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->d_order, n))) return rc;
     if ((rc = b->d_counters.reserve(sizeof(DevCounters)))) return rc;
-    if ((rc = b->d_results.reserve(std::max<size_t>(1, n) * sizeof(pt_log_result)))) return rc;
-    if ((rc = b->d_text_off.reserve(std::max<size_t>(1, n) * 8))) return rc;
-    if ((rc = b->d_span_off.reserve(std::max<size_t>(1, n) * 8))) return rc;
-    if ((rc = b->d_text.reserve(std::max<uint64_t>(1, pl.n_text) * 4))) return rc;
-    if ((b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && (rc = b->d_seq.reserve(std::max<uint64_t>(1, pl.n_text) * 4))) return rc;
-    if ((rc = b->d_spans.reserve(std::max<uint64_t>(1, pl.n_span) * sizeof(pt_span)))) return rc;
-    if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, pl.pool_cap) * 4))) return rc;
-    if ((rc = b->d_retry.reserve(std::max<size_t>(1, n) * 4 * kNumBins + 16))) return rc;
+    if ((rc = reserve_n<pt_log_result>(b->d_results, n))) return rc;
+    if ((rc = reserve_n<uint64_t>(b->d_text_off, n))) return rc;
+    if ((rc = reserve_n<uint64_t>(b->d_span_off, n))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->d_text, pl.n_text))) return rc;
+    if ((b->limits.flags & PT_FLAG_EMIT_SEQUENCE) && (rc = reserve_n<uint32_t>(b->d_seq, pl.n_text))) return rc;
+    if ((rc = reserve_n<pt_span>(b->d_spans, pl.n_span))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->d_pool, pl.pool_cap))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->d_retry, n * kNumBins + 4))) return rc;
     if (b->limits.flags & PT_FLAG_EMIT_PATCHES) {
         b->patch_cap = b->limits.patch_pool_items ? b->limits.patch_pool_items : 4ull * (b->n_insdel + b->n_mark) + 1024;
-        if ((rc = b->d_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
-        if ((rc = b->d_patch_items.reserve(std::max<uint64_t>(1, b->patch_cap) * sizeof(pt_patch_item)))) return rc;
-        if ((rc = b->d_patch_status.reserve(std::max<size_t>(1, n) * 4))) return rc;
-        if ((rc = b->d_patch_first.reserve(std::max<size_t>(1, n) * 4))) return rc;
-        PT_CUDA(cudaMemsetAsync(b->d_patch_first.p, 0, std::max<size_t>(1, n) * 4, b->stream));   // every upload / append: whole logs
+        if ((rc = reserve_n<pt_patch_rec>(b->d_patch_recs, b->n_insdel))) return rc;
+        if ((rc = reserve_n<pt_patch_item>(b->d_patch_items, b->patch_cap))) return rc;
+        if ((rc = reserve_n<uint32_t>(b->d_patch_status, n))) return rc;
+        if ((rc = reserve_n<uint32_t>(b->d_patch_first, n))) return rc;
+        PT_CUDA(cudaMemsetAsync(b->d_patch_first.p, 0, n * 4, b->stream));   // every upload / append: whole logs
         b->patch_window_changed = false;
         if (!pl.large_cand.empty()) {
             if ((rc = b->d_large_cand.reserve(pl.large_cand.size() * 4))) return rc;
@@ -547,8 +279,7 @@ int launch_bin_t(pt_batch* b, int k, ptk::BatchParams P, bool retry) {
     P.smem_arena_bytes = cfg.smem;
     PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_kernel<BLOCK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem));
     ptk::merge_logs_kernel<BLOCK><<<grid, BLOCK, cfg.smem, b->launch_stream>>>(P);
-    PT_CUDA(cudaGetLastError());
-    b->launches++;
+    PT_CUDA(launched(b));
     return PT_OK;
 }
 // cnt logs of bin 0's list from position first, on one id-table form of the warp kernel
@@ -567,8 +298,7 @@ int launch_warp_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t 
     const int smem = (int)(cfg.smem * WARPS);
     PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_warp_kernel<WARPS, IDM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     ptk::merge_logs_warp_kernel<WARPS, IDM><<<grid, WARPS * 32, smem, b->launch_stream>>>(P);
-    PT_CUDA(cudaGetLastError());
-    b->launches++;
+    PT_CUDA(launched(b));
     return PT_OK;
 }
 int launch_team_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t cnt) {
@@ -582,8 +312,7 @@ int launch_team_range(pt_batch* b, ptk::BatchParams P, uint32_t first, uint32_t 
     P.smem_arena_bytes = ptp::kTeamSmem;
     PT_CUDA(cudaFuncSetAttribute(ptk::merge_logs_team_kernel<ptp::kTeamWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ptp::kTeamSmem));
     ptk::merge_logs_team_kernel<ptp::kTeamWarps><<<grid, ptp::kTeamWarps * 32, ptp::kTeamSmem, b->launch_stream>>>(P);
-    PT_CUDA(cudaGetLastError());
-    b->launches++;
+    PT_CUDA(launched(b));
     return PT_OK;
 }
 // bin 0's list, in route order: the warp kernel with the packed3, compact and direct id tables, then the team kernel
@@ -624,8 +353,8 @@ int install_plan(pt_batch* b, const pt_packed_ops& ops, ptp::Plan&& plan, bool o
     int rc;
     if ((rc = alloc_and_upload_plan(b))) return rc;
     if (own_records) {
-        if ((rc = b->d_insdel.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_rec)))) return rc;
-        if ((rc = b->d_marks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_rec)))) return rc;
+        if ((rc = reserve_n<pt_insdel_rec>(b->d_insdel, b->n_insdel))) return rc;
+        if ((rc = reserve_n<pt_mark_rec>(b->d_marks, b->n_mark))) return rc;
     }
     return PT_OK;
 }
@@ -671,20 +400,14 @@ int run_queries(pt_batch* b, const char* fn, const char* verb, const Q* queries,
     if ((rc = dq.reserve((size_t)n * sizeof(Q))) || (rc = da.reserve((size_t)n * sizeof(A)))) return rc;
     cudaError_t e = cudaMemcpyAsync(dq.p, queries, (size_t)n * sizeof(Q), cudaMemcpyHostToDevice, b->stream);
     if (e == cudaSuccess) {
-        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-        launch(grid, threads, (const Q*)dq.p, (A*)da.p);
-        e = cudaGetLastError();
-        b->launches++;
+        launch(warp_grid(b, n, 128), 128u, (const Q*)dq.p, (A*)da.p);
+        e = launched(b);
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, da.p, (size_t)n * sizeof(A), cudaMemcpyDeviceToHost, b->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
     if (e != cudaSuccess) { g_last_error = std::string(fn) + ": " + cudaGetErrorString(e); return PT_ERR_CUDA; }
     return PT_OK;
 }
-
-}  // namespace
-
-namespace {
 
 // The caller's pools of both JSON renders: checked on the host, then (for a batch with logs) copied into the handle's device
 // buffers and described for the kernels in *P.
@@ -707,9 +430,9 @@ int load_json_pools(pt_batch* b, const pt_json_pools* pools, const char* fn, ptr
     for (int k = 0; k < 3; k++) {
         const Pool& p = ps[k];
         const uint64_t lo = p.count ? p.off[0] : 0, hi = p.count ? p.off[p.count] : 0;     // entries address data[lo, hi)
-        if ((rc = p.dd->reserve(std::max<uint64_t>(1, hi))) || (rc = p.doff->reserve((p.count + 1) * 8))) return rc;
+        if ((rc = reserve_n<uint8_t>(*p.dd, hi))) return rc;
         if (hi > lo) PT_CUDA(cudaMemcpyAsync((uint8_t*)p.dd->p + lo, p.data + lo, hi - lo, cudaMemcpyHostToDevice, b->stream));
-        if (p.count) PT_CUDA(cudaMemcpyAsync(p.doff->p, p.off, (p.count + 1) * 8, cudaMemcpyHostToDevice, b->stream));
+        if ((rc = upload_n(b, *p.doff, p.off, p.count ? p.count + 1 : 0))) return rc;
         *pdata[k] = (const uint8_t*)p.dd->p; *poff[k] = (const uint64_t*)p.doff->p; *pcount[k] = p.count;
     }
     return PT_OK;
@@ -729,19 +452,13 @@ int render_passes(pt_batch* b, const char* fn, JsonBufs& J, Size size, Write wri
         *out = pt_json_view{0, hoff, (const char*)J.hbytes.p, 0};
         return PT_OK;
     }
-    const uint32_t nb = (n + kScanBlock - 1) / kScanBlock;
-    if ((rc = J.size.reserve((size_t)n * 8)) || (rc = J.bsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = J.off.reserve(((size_t)n + 1) * 8)) ||
-        (rc = J.miss.reserve(8))) return rc;
-    unsigned long long *sizes = (unsigned long long*)J.size.p, *bsum = (unsigned long long*)J.bsum.p, *doff = (unsigned long long*)J.off.p,
-                       *miss = (unsigned long long*)J.miss.p;
-    const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
+    if ((rc = J.size.reserve((size_t)n * 8)) || (rc = J.off.reserve(((size_t)n + 1) * 8)) || (rc = J.miss.reserve(8))) return rc;
+    unsigned long long *sizes = (unsigned long long*)J.size.p, *doff = (unsigned long long*)J.off.p, *miss = (unsigned long long*)J.miss.p;
+    const uint32_t threads = 128, grid = warp_grid(b, n, threads);
     PT_CUDA(cudaMemsetAsync(miss, 0xFF, 8, b->stream));
     size(grid, threads, sizes, miss);
-    out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum);
-    out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
-    out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{sizes}, n, bsum, nb, doff, (unsigned long long*)nullptr);
-    PT_CUDA(cudaGetLastError());
-    b->launches += 4;
+    PT_CUDA(launched(b));
+    if ((rc = scan_offsets(b, pts::PlainCounts{sizes}, n, J.bsum, doff, nullptr))) return rc;
     uint64_t* hm = (uint64_t*)J.hmisc.p;
     PT_CUDA(cudaMemcpyAsync(hm, doff + n, 8, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaMemcpyAsync(hm + 1, miss, 8, cudaMemcpyDeviceToHost, b->stream));
@@ -753,10 +470,9 @@ int render_passes(pt_batch* b, const char* fn, JsonBufs& J, Size size, Write wri
                        std::to_string(key & 0xFFFFFFFFull) + ", which the caller's pools do not hold";
         return PT_ERR_INVALID;
     }
-    if ((rc = J.bytes.reserve(std::max<uint64_t>(1, total))) || (rc = J.hbytes.reserve(std::max<uint64_t>(1, total)))) return rc;
+    if ((rc = reserve_n<uint8_t>(J.bytes, total)) || (rc = reserve_n<uint8_t>(J.hbytes, total))) return rc;
     write(grid, threads, (const unsigned long long*)doff, (uint8_t*)J.bytes.p);
-    PT_CUDA(cudaGetLastError());
-    b->launches++;
+    PT_CUDA(launched(b));
     PT_CUDA(cudaMemcpyAsync(hoff, doff, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
     if (total) PT_CUDA(cudaMemcpyAsync(J.hbytes.p, J.bytes.p, total, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
@@ -836,25 +552,15 @@ int pt_batch_upload_runs(pt_batch* b, const pt_packed_runs* rr) {
     if (rc) return rc;
     const size_t nl = rr->n_logs;
     const uint64_t n_runs = nl ? rr->run_off[nl] : 0, n_tok = nl ? rr->tok_off[nl] : 0;
-    if ((rc = b->d_runs.reserve(std::max<uint64_t>(1, n_runs) * sizeof(pt_run_rec)))) return rc;
-    if ((rc = b->d_tokens.reserve(std::max<uint64_t>(1, n_tok) * 4))) return rc;
-    if ((rc = b->d_run_off.reserve((nl + 1) * 8))) return rc;
-    if ((rc = b->d_tok_off.reserve((nl + 1) * 8))) return rc;
-    if (nl) {
-        PT_CUDA(cudaMemcpyAsync(b->d_run_off.p, rr->run_off, (nl + 1) * 8, cudaMemcpyHostToDevice, b->stream));
-        PT_CUDA(cudaMemcpyAsync(b->d_tok_off.p, rr->tok_off, (nl + 1) * 8, cudaMemcpyHostToDevice, b->stream));
-    }
-    if (n_runs) PT_CUDA(cudaMemcpyAsync(b->d_runs.p, rr->runs, n_runs * sizeof(pt_run_rec), cudaMemcpyHostToDevice, b->stream));
-    if (n_tok) PT_CUDA(cudaMemcpyAsync(b->d_tokens.p, rr->tokens, n_tok * 4, cudaMemcpyHostToDevice, b->stream));
+    if ((rc = upload_n(b, b->d_run_off, rr->run_off, nl ? nl + 1 : 0)) || (rc = upload_n(b, b->d_tok_off, rr->tok_off, nl ? nl + 1 : 0)) ||
+        (rc = upload_n(b, b->d_runs, rr->runs, n_runs)) || (rc = upload_n(b, b->d_tokens, rr->tokens, n_tok))) return rc;
     if (b->n_mark) PT_CUDA(cudaMemcpyAsync(b->d_marks.p, rr->marks, b->n_mark * sizeof(pt_mark_rec), cudaMemcpyHostToDevice, b->stream));
     if (nl) {
-        const uint32_t threads = 128, warps_needed = (uint32_t)nl;
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)warps_needed * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-        expand_runs_kernel<<<grid, threads, 0, b->stream>>>((const pt_log_desc*)b->d_desc.p, (const unsigned long long*)b->d_run_off.p,
-                                                          (const unsigned long long*)b->d_tok_off.p, (const pt_run_rec*)b->d_runs.p,
-                                                          (const uint32_t*)b->d_tokens.p, (pt_insdel_rec*)b->d_insdel.p, (uint32_t)nl);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        const uint32_t threads = 128;
+        ptu::expand_runs_kernel<<<warp_grid(b, nl, threads), threads, 0, b->stream>>>(
+            (const pt_log_desc*)b->d_desc.p, (const unsigned long long*)b->d_run_off.p, (const unsigned long long*)b->d_tok_off.p,
+            (const pt_run_rec*)b->d_runs.p, (const uint32_t*)b->d_tokens.p, (pt_insdel_rec*)b->d_insdel.p, (uint32_t)nl);
+        PT_CUDA(launched(b));
     }
     return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{rr->runs, n_runs}, {rr->tokens, n_tok}, {rr->marks, b->n_mark}, {rr->run_off, nl}, {rr->tok_off, nl}});
 }
@@ -954,22 +660,19 @@ int pt_batch_upload_compact(pt_batch* b, const pt_packed_compact* cc) {
     if (!b || !cc || (cc->n_logs && !cc->logs)) return PT_ERR_INVALID;
     int rc = begin_upload(b, pt_packed_ops{cc->n_logs, cc->logs, nullptr, cc->n_insdel_total, nullptr, cc->n_mark_total}, true);
     if (rc) return rc;
-    if ((rc = b->d_cins.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_insdel_c8)))) return rc;
-    if ((rc = b->d_cmarks.reserve(std::max<uint64_t>(1, b->n_mark) * sizeof(pt_mark_c16)))) return rc;
-    const uint32_t threads = 256, gmax = (uint32_t)b->num_sms * 16;
+    const uint32_t threads = 256;      // one thread per record
+    if ((rc = upload_n(b, b->d_cins, cc->insdel, b->n_insdel))) return rc;
     if (b->n_insdel) {
-        PT_CUDA(cudaMemcpyAsync(b->d_cins.p, cc->insdel, b->n_insdel * sizeof(pt_insdel_c8), cudaMemcpyHostToDevice, b->stream));
-        expand_insdel_c8_kernel<<<(uint32_t)std::min<uint64_t>((b->n_insdel + threads - 1) / threads, gmax), threads, 0, b->stream>>>(
+        ptu::expand_insdel_c8_kernel<<<warp_grid(b, b->n_insdel, threads, 1), threads, 0, b->stream>>>(
             (const pt_insdel_c8*)b->d_cins.p, (pt_insdel_rec*)b->d_insdel.p, b->n_insdel);
-        b->launches++;
+        PT_CUDA(launched(b));
     }
+    if ((rc = upload_n(b, b->d_cmarks, cc->marks, b->n_mark))) return rc;
     if (b->n_mark) {
-        PT_CUDA(cudaMemcpyAsync(b->d_cmarks.p, cc->marks, b->n_mark * sizeof(pt_mark_c16), cudaMemcpyHostToDevice, b->stream));
-        expand_mark_c16_kernel<<<(uint32_t)std::min<uint64_t>((b->n_mark + threads - 1) / threads, gmax), threads, 0, b->stream>>>(
+        ptu::expand_mark_c16_kernel<<<warp_grid(b, b->n_mark, threads, 1), threads, 0, b->stream>>>(
             (const pt_mark_c16*)b->d_cmarks.p, (pt_mark_rec*)b->d_marks.p, b->n_mark);
-        b->launches++;
+        PT_CUDA(launched(b));
     }
-    PT_CUDA(cudaGetLastError());
     return finish_upload(b, b->d_insdel.p, b->d_marks.p, {{cc->insdel, b->n_insdel}, {cc->marks, b->n_mark}});
 }
 
@@ -985,16 +688,11 @@ int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
         if (D.change_off + D.n_changes > t->n_changes_total || D.dep_off + D.n_deps > t->n_deps_total) { g_last_error = "change descriptor out of range"; return PT_ERR_INVALID; }
         maxR = std::max<uint32_t>(maxR, b->h_desc[i].n_actors);
     }
-    if ((size_t)2 * maxR * 4 > 200 * 1024) { g_last_error = "more than 25600 actors in one log: not supported by the admission pre-pass"; return PT_ERR_INVALID; }
+    if (actor_table_bytes(maxR) > kAdmitMaxBytes) { g_last_error = "more than 25600 actors in one log: not supported by the admission pre-pass"; return PT_ERR_INVALID; }
     int rc;
     const size_t n = b->n_logs;
-    if ((rc = b->d_cdesc.reserve(std::max<size_t>(1, n) * sizeof(pt_change_desc)))) return rc;
-    if ((rc = b->d_changes.reserve(std::max<uint64_t>(1, t->n_changes_total) * sizeof(pt_change_rec)))) return rc;
-    if ((rc = b->d_deps.reserve(std::max<uint64_t>(1, t->n_deps_total) * sizeof(pt_dep_rec)))) return rc;
-    if ((rc = b->d_admit.reserve(std::max<size_t>(1, n) * 4))) return rc;
-    if (n) PT_CUDA(cudaMemcpyAsync(b->d_cdesc.p, t->logs, n * sizeof(pt_change_desc), cudaMemcpyHostToDevice, b->stream));
-    if (t->n_changes_total) PT_CUDA(cudaMemcpyAsync(b->d_changes.p, t->changes, t->n_changes_total * sizeof(pt_change_rec), cudaMemcpyHostToDevice, b->stream));
-    if (t->n_deps_total) PT_CUDA(cudaMemcpyAsync(b->d_deps.p, t->deps, t->n_deps_total * sizeof(pt_dep_rec), cudaMemcpyHostToDevice, b->stream));
+    if ((rc = upload_n(b, b->d_cdesc, t->logs, n)) || (rc = upload_n(b, b->d_changes, t->changes, t->n_changes_total)) ||
+        (rc = upload_n(b, b->d_deps, t->deps, t->n_deps_total)) || (rc = reserve_n<uint32_t>(b->d_admit, n))) return rc;
     PT_CUDA(cudaStreamSynchronize(b->stream));            // the caller's arrays may be freed on return
     b->h_cdesc.assign(t->logs, t->logs + n); b->n_changes = t->n_changes_total; b->n_deps = t->n_deps_total;
     b->adm_maxR = maxR; b->have_changes = true;
@@ -1002,12 +700,28 @@ int pt_batch_upload_changes(pt_batch* b, const pt_change_table* t) {
     return PT_OK;
 }
 
+static std::string at(uint32_t log) { return "log " + std::to_string(log) + ": "; }   // an error's prefix
+
+// A counter map c[0, nc): entry 0 (HEAD) maps to 0 and the mapped entries (all but 0xFFFFFFFF) strictly increase.  Returns
+// the problem, or null; bound gets the image of the last mapped entry at or below `upto`.
+static const char* check_ctr_map(const uint32_t* c, uint64_t nc, uint64_t upto, uint32_t& bound) {
+    if (nc && c[0] != 0) return "ctr_map[0] is not 0";
+    uint32_t last = 0;
+    bound = 0;
+    for (uint64_t k = 1; k < nc; k++) {
+        if (c[k] == 0xFFFFFFFFu) continue;
+        if (c[k] <= last) return "the counter map is not strictly increasing";
+        last = c[k];
+        if (k <= upto) bound = c[k];
+    }
+    return nullptr;
+}
+
 // Host checks of a delta and its remap against the resident batch (include/peritext_b200.h, pt_batch_append); on success
 // nd / ncd hold the descriptors of the concatenated batch and its change table.  Returns the problem, or an empty string.
 static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, bool delta_on_device, const pt_append_remap& R, const pt_change_table* dch,
                                 std::vector<pt_log_desc>& nd, std::vector<pt_change_desc>& ncd, uint32_t& maxR) {
     const uint32_t n = b->n_logs;
-    auto at = [](uint32_t i) { return "log " + std::to_string(i) + ": "; };
     if (delta.n_logs != n) return "the delta has " + std::to_string(delta.n_logs) + " logs and the batch " + std::to_string(n);
     if ((dch != nullptr) != b->have_changes)
         return b->have_changes ? "the batch has a change table and the delta none" : "the delta has a change table and the batch none";
@@ -1035,16 +749,9 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, b
             return at(i) + "the new n_actors is below the old (identity actor map)";
         }
         if (nc) {
-            const uint32_t* c = R.ctr_map + R.ctr_off[i];
             if (nc <= (uint64_t)O.max_ctr) return at(i) + "the counter map has " + std::to_string(nc) + " entries and the log's old max_ctr is " + std::to_string(O.max_ctr);
-            if (c[0] != 0) return at(i) + "ctr_map[0] is not 0";
-            uint32_t last = 0, bound = 0;         // bound: the image of the old max_ctr (the last mapped entry up to it)
-            for (uint64_t k = 1; k < nc; k++) {
-                if (c[k] == 0xFFFFFFFFu) continue;
-                if (c[k] <= last) return at(i) + "the counter map is not strictly increasing";
-                last = c[k];
-                if (k <= O.max_ctr) bound = c[k];
-            }
+            uint32_t bound;                       // the image of the old max_ctr
+            if (const char* e = check_ctr_map(R.ctr_map + R.ctr_off[i], nc, O.max_ctr, bound)) return at(i) + e;
             if (bound > D.max_ctr) return at(i) + "the counter map sends the old max_ctr past the new max_ctr";
         } else if (O.max_ctr > D.max_ctr) {
             return at(i) + "the new max_ctr is below the old (identity counter map)";
@@ -1061,7 +768,7 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, b
     if (dch) {
         if (dch->n_logs != n || (n && !dch->logs)) return "the delta's change table does not match the batch";
         if ((dch->n_changes_total && !dch->changes) || (dch->n_deps_total && !dch->deps)) return "null delta change records with a nonzero count";
-        if ((size_t)2 * maxR * 4 > 200 * 1024) return "more than 25600 actors in one log: not supported by the admission pre-pass";
+        if (actor_table_bytes(maxR) > kAdmitMaxBytes) return "more than 25600 actors in one log: not supported by the admission pre-pass";
         ncd.resize(n);
         uint64_t co = 0, po = 0;
         for (uint32_t i = 0; i < n; i++) {
@@ -1096,21 +803,14 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
     // The delta and the remap go to the device; the splice writes NEW buffers, so the resident batch stays intact until the
     // device has accepted every record.
     int rc;
-    const size_t dsz = std::max<size_t>(1, n) * sizeof(pt_log_desc);
     DevBuf ndesc, nins, nmarks, ncdesc, nch, ndp;              // the new batch's descriptors, records and change table
     DevBuf ddesc, dins, dmarks, dcdesc, dchg, ddep, amap[5], abad;   // the delta, its remap and the refusal flag: freed on return
-    if ((rc = ddesc.reserve(dsz)) || (rc = ndesc.reserve(dsz)) || (rc = abad.reserve(4)) ||
-        (rc = nins.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = nmarks.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec)))) return rc;
-    auto h2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
-    PT_CUDA(h2d(ddesc.p, delta->logs, (size_t)n * sizeof(pt_log_desc)));
-    PT_CUDA(h2d(ndesc.p, nd.data(), (size_t)n * sizeof(pt_log_desc)));
+    if ((rc = upload_n(b, ddesc, delta->logs, n)) || (rc = upload_n(b, ndesc, nd.data(), n)) || (rc = abad.reserve(4)) ||
+        (rc = reserve_n<pt_insdel_rec>(nins, n_ins)) || (rc = reserve_n<pt_mark_rec>(nmarks, n_mk))) return rc;
     const pt_insdel_rec* d_dins = delta->insdel;
     const pt_mark_rec* d_dmarks = delta->marks;
     if (!delta_on_device) {
-        if ((rc = dins.reserve(std::max<uint64_t>(1, delta->n_insdel_total) * sizeof(pt_insdel_rec))) ||
-            (rc = dmarks.reserve(std::max<uint64_t>(1, delta->n_mark_total) * sizeof(pt_mark_rec)))) return rc;
-        PT_CUDA(h2d(dins.p, delta->insdel, delta->n_insdel_total * sizeof(pt_insdel_rec)));
-        PT_CUDA(h2d(dmarks.p, delta->marks, delta->n_mark_total * sizeof(pt_mark_rec)));
+        if ((rc = upload_n(b, dins, delta->insdel, delta->n_insdel_total)) || (rc = upload_n(b, dmarks, delta->marks, delta->n_mark_total))) return rc;
         d_dins = (const pt_insdel_rec*)dins.p; d_dmarks = (const pt_mark_rec*)dmarks.p;
     }
     pta::Remap DR{};
@@ -1121,51 +821,38 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
     for (int k = 0; k < 5; k++) {
         if (!hsrc[k]) continue;
         if ((rc = amap[k].reserve(std::max<size_t>(16, hbytes[k])))) return rc;
-        PT_CUDA(h2d(amap[k].p, hsrc[k], hbytes[k]));
+        if (hbytes[k]) PT_CUDA(cudaMemcpyAsync(amap[k].p, hsrc[k], hbytes[k], cudaMemcpyHostToDevice, b->stream));
         dptr[k] = amap[k].p;
     }
     DR.actor_off = (const unsigned long long*)dptr[0]; DR.actor_map = (const uint16_t*)dptr[1];
     DR.ctr_off = (const unsigned long long*)dptr[2]; DR.ctr_map = (const uint32_t*)dptr[3];
     DR.comment_map = (const uint32_t*)dptr[4]; DR.n_comment = R.comment_map ? R.n_comment_map : 0;
     PT_CUDA(cudaMemsetAsync(abad.p, 0, 4, b->stream));
-    const uint32_t threads = 128, grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16));
+    const uint32_t threads = 128;
     if (n) {
-        // a log with many records gets up to 64 warps, one per slice (8 K records per slice): few huge logs (c5) must not
-        // leave the copy to a handful of warps
         uint64_t most = 0;
         for (uint32_t i = 0; i < n; i++) most = std::max<uint64_t>(most, (uint64_t)nd[i].n_insdel + 2ull * nd[i].n_mark);
-        const uint32_t slices = (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, most / 8192));
-        const dim3 rgrid(std::max<uint32_t>(1, std::min<uint32_t>(grid, (uint32_t)b->num_sms * 16 / slices)), slices);
-        pta::splice_records_kernel<<<rgrid, threads, 0, b->stream>>>((const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, n, DR,
-                                                                    b->dp_insdel, b->dp_marks, d_dins, d_dmarks,
-                                                                    (pt_insdel_rec*)nins.p, (pt_mark_rec*)nmarks.p, (uint32_t*)abad.p);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        pta::splice_records_kernel<<<slice_grid(b, n, most, threads), threads, 0, b->stream>>>(
+            (const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, n, DR, b->dp_insdel, b->dp_marks,
+            d_dins, d_dmarks, (pt_insdel_rec*)nins.p, (pt_mark_rec*)nmarks.p, (uint32_t*)abad.p);
+        PT_CUDA(launched(b));
     }
     uint64_t n_ch = 0, n_dp = 0;
     if (dch) {
         n_ch = n ? ncd[n - 1].change_off + ncd[n - 1].n_changes : 0; n_dp = n ? ncd[n - 1].dep_off + ncd[n - 1].n_deps : 0;
-        const size_t csz = std::max<size_t>(1, n) * sizeof(pt_change_desc);
-        if ((rc = dcdesc.reserve(csz)) || (rc = ncdesc.reserve(csz)) ||
-            (rc = nch.reserve(std::max<uint64_t>(1, n_ch) * sizeof(pt_change_rec))) || (rc = ndp.reserve(std::max<uint64_t>(1, n_dp) * sizeof(pt_dep_rec)))) return rc;
-        PT_CUDA(h2d(dcdesc.p, dch->logs, (size_t)n * sizeof(pt_change_desc)));
-        PT_CUDA(h2d(ncdesc.p, ncd.data(), (size_t)n * sizeof(pt_change_desc)));
+        if ((rc = upload_n(b, dcdesc, dch->logs, n)) || (rc = upload_n(b, ncdesc, ncd.data(), n)) ||
+            (rc = reserve_n<pt_change_rec>(nch, n_ch)) || (rc = reserve_n<pt_dep_rec>(ndp, n_dp))) return rc;
         const pt_change_rec* d_dchg = dch->changes;
         const pt_dep_rec* d_ddep = dch->deps;
         if (!table_on_device) {
-            if ((rc = dchg.reserve(std::max<uint64_t>(1, dch->n_changes_total) * sizeof(pt_change_rec))) ||
-                (rc = ddep.reserve(std::max<uint64_t>(1, dch->n_deps_total) * sizeof(pt_dep_rec)))) return rc;
-            PT_CUDA(h2d(dchg.p, dch->changes, dch->n_changes_total * sizeof(pt_change_rec)));
-            PT_CUDA(h2d(ddep.p, dch->deps, dch->n_deps_total * sizeof(pt_dep_rec)));
+            if ((rc = upload_n(b, dchg, dch->changes, dch->n_changes_total)) || (rc = upload_n(b, ddep, dch->deps, dch->n_deps_total))) return rc;
             d_dchg = (const pt_change_rec*)dchg.p; d_ddep = (const pt_dep_rec*)ddep.p;
         }
         if (n) {
-            pta::splice_changes_kernel<<<grid, threads, 0, b->stream>>>((const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p,
-                                                                        n, DR, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p,
-                                                                        d_dchg, d_ddep,
-                                                                        (pt_change_rec*)nch.p, (pt_dep_rec*)ndp.p);
-            PT_CUDA(cudaGetLastError());
-            b->launches++;
+            pta::splice_changes_kernel<<<warp_grid(b, n, threads), threads, 0, b->stream>>>(
+                (const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p, n, DR,
+                (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p, d_dchg, d_ddep, (pt_change_rec*)nch.p, (pt_dep_rec*)ndp.p);
+            PT_CUDA(launched(b));
         }
     }
     uint32_t bad = 0;
@@ -1199,7 +886,6 @@ int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_rem
 static std::string check_change(const pt_batch* b, const pt_change_input& in, std::vector<pt_log_desc>& dd, std::vector<uint32_t>& new_elems,
                                 std::vector<uint32_t>& work) {
     const uint32_t n = b->n_logs;
-    auto at = [](uint32_t i) { return "log " + std::to_string(i) + ": "; };
     if (in.n_logs != n) return "the input has " + std::to_string(in.n_logs) + " logs and the batch " + std::to_string(n);
     if (!n) return std::string();
     if (!in.actor || !in.input_off) return "null actor or input_off";
@@ -1275,7 +961,7 @@ int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_tabl
     if (err.empty()) err = check_change(b, *in, dd, new_elems, work);
     if (!err.empty()) { g_last_error = "pt_batch_change: " + err; return PT_ERR_INVALID; }
     const uint64_t n_ins = n ? dd[n - 1].insdel_off + dd[n - 1].n_insdel : 0, n_mk = n ? dd[n - 1].mark_off + dd[n - 1].n_mark : 0;
-    std::vector<unsigned long long> soff(std::max<uint32_t>(1, n), 0);
+    std::vector<unsigned long long> soff(n, 0);
     uint64_t n_scratch = 0;
     for (uint32_t i : work) {                          // a slot holds the log's elements and its new ones, 16-byte aligned
         soff[i] = n_scratch;
@@ -1286,25 +972,14 @@ int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_tabl
     int rc;
     DevBuf dwork, dactor, dioff, dops, dtok, ddelta, dnel, dsoff, dscr, dst, dgi, dgm;   // freed on return
     const uint64_t n_ops = n ? in->input_off[n] : 0;
-    const size_t nn = std::max<uint32_t>(1, n);
-    if ((rc = dwork.reserve(std::max<size_t>(1, work.size()) * 4)) || (rc = dactor.reserve(nn * 4)) || (rc = dioff.reserve((nn + 1) * 8)) ||
-        (rc = dops.reserve(std::max<uint64_t>(1, n_ops) * sizeof(pt_input_op))) || (rc = dtok.reserve(std::max<uint64_t>(1, in->n_tokens) * 4)) ||
-        (rc = ddelta.reserve(nn * sizeof(pt_log_desc))) || (rc = dnel.reserve(nn * 4)) || (rc = dsoff.reserve(nn * 8)) ||
-        (rc = dscr.reserve(std::max<uint64_t>(4, n_scratch) * 4)) || (rc = dst.reserve(nn * sizeof(pt_change_status))) ||
-        (rc = dgi.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = dgm.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))))
+    if ((rc = upload_n(b, dwork, work.data(), work.size())) || (rc = upload_n(b, dactor, in->actor, n)) ||
+        (rc = upload_n(b, dioff, in->input_off, n ? n + 1 : 0)) || (rc = upload_n(b, ddelta, dd.data(), n)) ||
+        (rc = upload_n(b, dnel, new_elems.data(), n)) || (rc = upload_n(b, dsoff, soff.data(), n)) || (rc = reserve_n<pt_change_status>(dst, n)))
         return rc;
-    auto h2d = [&](void* dst_, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst_, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
-    PT_CUDA(h2d(dwork.p, work.data(), work.size() * 4));
-    if (n) {
-        PT_CUDA(h2d(dactor.p, in->actor, (size_t)n * 4));
-        PT_CUDA(h2d(dioff.p, in->input_off, ((size_t)n + 1) * 8));
-        PT_CUDA(h2d(ddelta.p, dd.data(), (size_t)n * sizeof(pt_log_desc)));
-        PT_CUDA(h2d(dnel.p, new_elems.data(), (size_t)n * 4));
-        PT_CUDA(h2d(dsoff.p, soff.data(), (size_t)n * 8));
-    }
     if (n) PT_CUDA(cudaMemsetAsync(dst.p, 0, (size_t)n * sizeof(pt_change_status), b->stream));   // logs without a change: OK
-    PT_CUDA(h2d(dops.p, in->ops, n_ops * sizeof(pt_input_op)));
-    PT_CUDA(h2d(dtok.p, in->tokens, in->n_tokens * 4));
+    if ((rc = upload_n(b, dops, in->ops, n_ops)) || (rc = upload_n(b, dtok, in->tokens, in->n_tokens)) ||
+        (rc = dscr.reserve(std::max<uint64_t>(4, n_scratch) * 4)) || (rc = reserve_n<pt_insdel_rec>(dgi, n_ins)) || (rc = reserve_n<pt_mark_rec>(dgm, n_mk)))
+        return rc;
     if (!work.empty()) {
         ptc::ChangeParams P{};
         P.work = (const uint32_t*)dwork.p; P.n_work = (uint32_t)work.size();
@@ -1314,14 +989,12 @@ int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_tabl
         P.tokens = (const uint32_t*)dtok.p; P.delta = (const pt_log_desc*)ddelta.p; P.new_elems = (const uint32_t*)dnel.p;
         P.scratch_off = (const unsigned long long*)dsoff.p; P.scratch = (uint32_t*)dscr.p;
         P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.status = (pt_change_status*)dst.p;
-        const uint32_t threads = 128, grid = (uint32_t)std::min<uint64_t>(((uint64_t)work.size() * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16);
-        ptc::change_resolve_kernel<<<grid, threads, 0, b->stream>>>(P);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        ptc::change_resolve_kernel<<<warp_grid(b, work.size(), 128), 128, 0, b->stream>>>(P);
+        PT_CUDA(launched(b));
     }
     // the status of every log (the logs without a change are OK) and the generated records, into the view's pinned buffers
-    if ((rc = b->h_chg_status.reserve(nn * sizeof(pt_change_status))) || (rc = b->h_chg_desc.reserve(nn * sizeof(pt_log_desc))) ||
-        (rc = b->h_chg_insdel.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = b->h_chg_marks.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))))
+    if ((rc = reserve_n<pt_change_status>(b->h_chg_status, n)) || (rc = reserve_n<pt_log_desc>(b->h_chg_desc, n)) ||
+        (rc = reserve_n<pt_insdel_rec>(b->h_chg_insdel, n_ins)) || (rc = reserve_n<pt_mark_rec>(b->h_chg_marks, n_mk)))
         return rc;
     pt_change_status* st = (pt_change_status*)b->h_chg_status.p;
     if (n) PT_CUDA(cudaMemcpyAsync(st, dst.p, (size_t)n * sizeof(pt_change_status), cudaMemcpyDeviceToHost, b->stream));
@@ -1384,15 +1057,9 @@ static std::string check_exchange(const pt_batch* b, const pt_exchange_input& in
         if (in.ctr_off) {
             if (in.ctr_off[p + 1] < in.ctr_off[p]) return "ctr_off decreases";
             const uint64_t nc = in.ctr_off[p + 1] - in.ctr_off[p];
-            const uint32_t* c = in.ctr_map + in.ctr_off[p];
             if (nc > 0xFFFFFFFFull) return at(p) + "the counter map has more than 2^32 - 1 entries";
-            if (nc && c[0] != 0) return at(p) + "ctr_map[0] is not 0";
-            uint32_t prev = 0;
-            for (uint64_t k = 1; k < nc; k++) {
-                if (c[k] == 0xFFFFFFFFu) continue;
-                if (c[k] <= prev) return at(p) + "the counter map is not strictly increasing";
-                prev = c[k];
-            }
+            uint32_t bound;
+            if (const char* e = check_ctr_map(in.ctr_map + in.ctr_off[p], nc, 0, bound)) return at(p) + e;
         }
         slot_off[p + 1] = slot_off[p] + b->h_cdesc[src].n_changes;
     }
@@ -1405,9 +1072,8 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     if (!b->have_changes) { g_last_error = "pt_batch_exchange: the handle has no change table"; return PT_ERR_STATE; }
     const uint32_t n = b->n_logs, np = in->n_pairs;
     int rc;
-    const size_t nn = std::max<uint32_t>(1, n), npp = std::max<uint32_t>(1, np);
-    if ((rc = b->h_xch_totals.reserve(npp * sizeof(ptx::PairTotals))) || (rc = b->h_xch_status.reserve(npp * 4)) ||
-        (rc = b->h_xch_off.reserve((npp + 1) * 8)) || (rc = b->h_xch_desc.reserve(nn * sizeof(pt_log_desc)))) return rc;
+    if ((rc = reserve_n<ptx::PairTotals>(b->h_xch_totals, np)) || (rc = reserve_n<uint32_t>(b->h_xch_status, np)) ||
+        (rc = reserve_n<uint64_t>(b->h_xch_off, (uint64_t)np + 1)) || (rc = reserve_n<pt_log_desc>(b->h_xch_desc, n))) return rc;
     ptx::PairTotals* tot = (ptx::PairTotals*)b->h_xch_totals.p;
     uint32_t* status = (uint32_t*)b->h_xch_status.p;
     uint64_t* doff = (uint64_t*)b->h_xch_off.p;
@@ -1430,20 +1096,11 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     // the pairs, their maps and the select kernel's scratch: freed on return
     DevBuf dpairs, daoff, damap, dcoff, dcmap, dslot, dqueue, dpos, ddlv, dtot, ddoff, dbase, dgi, dgm, dgc, dgd, dgx;
     const uint64_t n_amap = in->actor_off[np], n_cmap = in->ctr_off ? in->ctr_off[np] : 0;
-    if ((rc = dpairs.reserve((size_t)np * sizeof(pt_exchange_pair))) || (rc = daoff.reserve(((size_t)np + 1) * 8)) || (rc = damap.reserve(std::max<uint64_t>(1, n_amap) * 2)) ||
-        (rc = dslot.reserve(((size_t)np + 1) * 8)) || (rc = dqueue.reserve(std::max<uint64_t>(1, n_slot) * 4)) || (rc = dpos.reserve(std::max<uint64_t>(1, n_slot) * 4)) ||
-        (rc = ddlv.reserve(std::max<uint64_t>(1, n_slot) * sizeof(ptx::Delivered))) || (rc = dtot.reserve((size_t)np * sizeof(ptx::PairTotals))) ||
-        (rc = ddoff.reserve(((size_t)np + 1) * 8)) || (rc = dbase.reserve((size_t)np * sizeof(ptx::PairBase)))) return rc;
-    if (in->ctr_off && ((rc = dcoff.reserve(((size_t)np + 1) * 8)) || (rc = dcmap.reserve(std::max<uint64_t>(1, n_cmap) * 4)))) return rc;
-    auto h2d = [&](void* dst_, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst_, src, bytes, cudaMemcpyHostToDevice, b->stream) : cudaSuccess; };
-    PT_CUDA(h2d(dpairs.p, in->pairs, (size_t)np * sizeof(pt_exchange_pair)));
-    PT_CUDA(h2d(daoff.p, in->actor_off, ((size_t)np + 1) * 8));
-    PT_CUDA(h2d(damap.p, in->actor_map, n_amap * 2));
-    PT_CUDA(h2d(dslot.p, slot_off.data(), ((size_t)np + 1) * 8));
-    if (in->ctr_off) {
-        PT_CUDA(h2d(dcoff.p, in->ctr_off, ((size_t)np + 1) * 8));
-        PT_CUDA(h2d(dcmap.p, in->ctr_map, n_cmap * 4));
-    }
+    if ((rc = upload_n(b, dpairs, in->pairs, np)) || (rc = upload_n(b, daoff, in->actor_off, (uint64_t)np + 1)) ||
+        (rc = upload_n(b, damap, in->actor_map, n_amap)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)np + 1)) ||
+        (rc = reserve_n<uint32_t>(dqueue, n_slot)) || (rc = reserve_n<uint32_t>(dpos, n_slot)) ||
+        (rc = reserve_n<ptx::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptx::PairTotals>(dtot, np))) return rc;
+    if (in->ctr_off && ((rc = upload_n(b, dcoff, in->ctr_off, (uint64_t)np + 1)) || (rc = upload_n(b, dcmap, in->ctr_map, n_cmap)))) return rc;
     ptx::ExchangeParams P{};
     P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = np; P.maxR = b->adm_maxR;
     P.actor_off = (const unsigned long long*)daoff.p; P.actor_map = (const uint16_t*)damap.p;
@@ -1453,16 +1110,10 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     P.insdel = b->dp_insdel; P.marks = b->dp_marks;
     P.slot_off = (const unsigned long long*)dslot.p; P.queue = (uint32_t*)dqueue.p; P.pos = (uint32_t*)dpos.p; P.dlv = (ptx::Delivered*)ddlv.p;
     P.totals = (ptx::PairTotals*)dtot.p;
-    {   // like the admission pre-pass: 4 warps per CTA while the per-actor tables fit, else one warp with up to 200 KB
-        const size_t per_warp = (size_t)2 * b->adm_maxR * 4;
-        const uint32_t wpb = per_warp * 4 <= 48 * 1024 ? 4u : 1u;
-        const size_t smem = per_warp * wpb;
-        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptx::exchange_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)np + wpb - 1) / wpb, (uint64_t)b->num_sms * 16);
-        ptx::exchange_select_kernel<<<grid, wpb * 32, smem, b->stream>>>(P);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
-    }
+    const auto [wpb, smem] = actor_shape(b->adm_maxR);
+    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptx::exchange_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ptx::exchange_select_kernel<<<warp_grid(b, np, wpb * 32), wpb * 32, smem, b->stream>>>(P);
+    PT_CUDA(launched(b));
     PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
     // the delta's layout: the pairs' records, change and dep records back to back in pair order
@@ -1475,22 +1126,18 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
         dlv_off[p + 1] = n_ch;
         most = std::max<uint64_t>(most, (uint64_t)tot[p].n_insdel + 2ull * tot[p].n_mark);
     }
-    if ((rc = dgi.reserve(std::max<uint64_t>(1, n_ins) * sizeof(pt_insdel_rec))) || (rc = dgm.reserve(std::max<uint64_t>(1, n_mk) * sizeof(pt_mark_rec))) ||
-        (rc = dgc.reserve(std::max<uint64_t>(1, n_ch) * sizeof(pt_change_rec))) || (rc = dgd.reserve(std::max<uint64_t>(1, n_dp) * sizeof(pt_dep_rec))) ||
-        (rc = dgx.reserve(std::max<uint64_t>(1, n_ch) * 4)) || (rc = b->h_xch_delivered.reserve(std::max<uint64_t>(1, n_ch) * 4))) return rc;
+    if ((rc = reserve_n<pt_insdel_rec>(dgi, n_ins)) || (rc = reserve_n<pt_mark_rec>(dgm, n_mk)) ||
+        (rc = reserve_n<pt_change_rec>(dgc, n_ch)) || (rc = reserve_n<pt_dep_rec>(dgd, n_dp)) ||
+        (rc = reserve_n<uint32_t>(dgx, n_ch)) || (rc = reserve_n<uint32_t>(b->h_xch_delivered, n_ch))) return rc;
     uint32_t* delivered = (uint32_t*)b->h_xch_delivered.p;
     if (n_ch) {
-        PT_CUDA(h2d(ddoff.p, dlv_off.data(), ((size_t)np + 1) * 8));
-        PT_CUDA(h2d(dbase.p, base.data(), (size_t)np * sizeof(ptx::PairBase)));
+        if ((rc = upload_n(b, ddoff, dlv_off.data(), (uint64_t)np + 1)) || (rc = upload_n(b, dbase, base.data(), np))) return rc;
         P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p;
         P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
         P.out_delivered = (uint32_t*)dgx.p;
-        // a pair's records are an upper bound of its longest change: up to 64 warps per change, 8 K records per slice
-        const uint32_t threads = 128, slices = (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, most / 8192));
-        const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_ch * 32 + threads - 1) / threads, (uint64_t)b->num_sms * 16 / slices));
-        ptx::exchange_gather_kernel<<<dim3(gx, slices), threads, 0, b->stream>>>(P);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        // one warp per delivered change; a pair's records are an upper bound of its longest change
+        ptx::exchange_gather_kernel<<<slice_grid(b, n_ch, most, 128), 128, 0, b->stream>>>(P);
+        PT_CUDA(launched(b));
         PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));   // status and max_ctr
         PT_CUDA(cudaMemcpyAsync(delivered, dgx.p, n_ch * 4, cudaMemcpyDeviceToHost, b->stream));
         PT_CUDA(cudaStreamSynchronize(b->stream));
@@ -1532,16 +1179,12 @@ static int enqueue_merge(pt_batch* b) {
     P.stats = c->stats;
     P.admit = nullptr;
     if (b->have_changes && b->n_logs) {
-        // admission pre-pass: 4 warps per CTA while the per-actor tables fit, else one warp with up to 200 KB
-        const size_t per_warp = (size_t)2 * b->adm_maxR * 4;
-        const uint32_t wpb = per_warp * 4 <= 48 * 1024 ? 4u : 1u;
-        const size_t smem = per_warp * wpb;
-        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(admit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)b->n_logs + wpb - 1) / wpb, (uint64_t)b->num_sms * 16);
-        admit_kernel<<<grid, wpb * 32, smem, b->stream>>>((const pt_change_desc*)b->d_cdesc.p, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p,
-                                                       (const pt_log_desc*)b->d_desc.p, b->n_logs, b->adm_maxR, (uint32_t*)b->d_admit.p, (pt_log_result*)b->d_results.p);
-        PT_CUDA(cudaGetLastError());
-        b->launches++;
+        const auto [wpb, smem] = actor_shape(b->adm_maxR);     // admission pre-pass
+        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptadm::admit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ptadm::admit_kernel<<<warp_grid(b, b->n_logs, wpb * 32), wpb * 32, smem, b->stream>>>(
+            (const pt_change_desc*)b->d_cdesc.p, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p, (const pt_log_desc*)b->d_desc.p,
+            b->n_logs, b->adm_maxR, (uint32_t*)b->d_admit.p, (pt_log_result*)b->d_results.p);
+        PT_CUDA(launched(b));
         P.admit = (const uint32_t*)b->d_admit.p;
     }
     { const char* e = getenv("PT_PREFETCH"); P.prefetch_next = e ? (uint32_t)atoi(e) : 0u; }
@@ -1560,8 +1203,6 @@ static int enqueue_merge(pt_batch* b) {
         PT_CUDA(cudaEventRecord(b->ev_fork, b->stream));
         PT_CUDA(cudaStreamWaitEvent(b->side, b->ev_fork, 0));
         b->launch_stream = b->side;
-    }
-    if (fork) {
         for (int k = 1; k < kNumBins; k++) if ((rc = launch_bin(b, k, P, false))) { b->launch_stream = b->stream; return rc; }
         PT_CUDA(cudaEventRecord(b->ev_join, b->side));
         b->launch_stream = b->stream;
@@ -1588,11 +1229,10 @@ static int enqueue_merge(pt_batch* b) {
         const bool warp = !(b->limits.flags & PT_FLAG_EMIT_LARGE_PATCHES) || b->plan.cfg.patch_warp_on;
         if (warp) {
             PT_CUDA(cudaFuncSetAttribute(ptk::patch_logs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->plan.patch_smem));
-            const uint32_t per_sm = std::max<uint32_t>(1, std::min<uint32_t>(32, (227u * 1024u) / (b->plan.patch_smem + 1024u)));
+            const uint32_t per_sm = std::clamp<uint32_t>((227u * 1024u) / (b->plan.patch_smem + 1024u), 1, 32);
             const uint32_t grid = (uint32_t)std::min<uint64_t>(b->n_logs, (uint64_t)b->num_sms * per_sm);
             ptk::patch_logs_kernel<<<grid, 32, b->plan.patch_smem, b->stream>>>(Q);
-            PT_CUDA(cudaGetLastError());
-            b->launches++;
+            PT_CUDA(launched(b));
         }
         if (large) {   // the logs the warp kernel declined (or, with PT_PATCH_WARP=0, every log)
             ptk::LargePatchParams G{};
@@ -1602,8 +1242,7 @@ static int enqueue_merge(pt_batch* b) {
             G.scratch = (char*)b->d_large_scratch.p; G.slot_bytes = b->plan.large_bytes;
             G.recs = Q.recs; G.items = Q.items; G.item_cursor = Q.item_cursor; G.item_cap = Q.item_cap; G.status = Q.status;
             ptk::patch_large_kernel<<<b->plan.large_slots, ptk::kLargeThreads, 0, b->stream>>>(G);
-            PT_CUDA(cudaGetLastError());
-            b->launches++;
+            PT_CUDA(launched(b));
         }
     }
     return PT_OK;
@@ -1664,7 +1303,7 @@ int pt_batch_download_results(pt_batch* b, pt_log_result* out, uint32_t n_logs) 
     if (!b->merged) { g_last_error = "download before merge"; return PT_ERR_STATE; }
     if (n_logs > b->n_logs) return PT_ERR_INVALID;
     int rc;
-    if ((rc = b->h_results.reserve(std::max<size_t>(1, b->n_logs) * sizeof(pt_log_result)))) return rc;
+    if ((rc = reserve_n<pt_log_result>(b->h_results, b->n_logs))) return rc;
     if (n_logs) PT_CUDA(cudaMemcpyAsync(b->h_results.p, b->d_results.p, (size_t)n_logs * sizeof(pt_log_result), cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
     if (n_logs) memcpy(out, b->h_results.p, (size_t)n_logs * sizeof(pt_log_result));
@@ -1680,30 +1319,24 @@ int pt_batch_download_begin(pt_batch* b) {
     if (!b->merged) { g_last_error = "download before merge"; return PT_ERR_STATE; }
     int rc;
     const size_t n = b->n_logs;
-    const uint32_t nb = (uint32_t)((n + kScanBlock - 1) / kScanBlock);
-    if ((rc = b->h_results.reserve(std::max<size_t>(1, n) * sizeof(pt_log_result)))) return rc;
+    if ((rc = reserve_n<pt_log_result>(b->h_results, n))) return rc;
     if ((rc = b->h_ctoff.reserve((n + 1) * 8))) return rc;
     if ((rc = b->h_csoff.reserve((n + 1) * 8))) return rc;
     if ((rc = b->h_misc.reserve(16))) return rc;
-    if ((rc = b->d_bsum.reserve((size_t)(2 * nb + 2) * 8))) return rc;
     if ((rc = b->d_ctoff.reserve((n + 1) * 8))) return rc;
     if ((rc = b->d_csoff.reserve((n + 1) * 8))) return rc;
     // packed outputs can never exceed the capacities; sized once per batch
-    if ((rc = b->d_ctext.reserve(std::max<uint64_t>(1, b->plan.n_text) * 4))) return rc;
-    if ((rc = b->d_cspans.reserve(std::max<uint64_t>(1, b->plan.n_span) * sizeof(pt_span)))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->d_ctext, b->plan.n_text))) return rc;
+    if ((rc = reserve_n<pt_span>(b->d_cspans, b->plan.n_span))) return rc;
     PT_CUDA(cudaMemcpyAsync(b->h_misc.p, &counters(b)->comment_used, 8, cudaMemcpyDeviceToHost, b->stream));   // pool cursor = the batch's demand
     if (n) {
         const pt_log_result* res = (const pt_log_result*)b->d_results.p;
-        unsigned long long* bsum = (unsigned long long*)b->d_bsum.p;
         unsigned long long *toff = (unsigned long long*)b->d_ctoff.p, *soff = (unsigned long long*)b->d_csoff.p;
-        out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(MergedCounts{res}, (uint32_t)n, bsum);
-        out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
-        out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(MergedCounts{res}, (uint32_t)n, bsum, nb, toff, soff);
-        const uint32_t gthreads = 256, ggrid = (uint32_t)std::min<uint64_t>((n * 32 + gthreads - 1) / gthreads, (uint64_t)b->num_sms * 16);
-        out_gather_kernel<<<ggrid, gthreads, 0, b->stream>>>(res, (uint32_t)n, (const uint64_t*)b->d_text_off.p, (const uint64_t*)b->d_span_off.p, toff, soff,
-                                                           (const uint32_t*)b->d_text.p, (const pt_span*)b->d_spans.p, (uint32_t*)b->d_ctext.p, (pt_span*)b->d_cspans.p);
-        PT_CUDA(cudaGetLastError());
-        b->launches += 4;
+        if ((rc = scan_offsets(b, pts::MergedCounts{res}, (uint32_t)n, b->d_bsum, toff, soff))) return rc;
+        pts::out_gather_kernel<<<warp_grid(b, n, 256), 256, 0, b->stream>>>(res, (uint32_t)n, (const uint64_t*)b->d_text_off.p, (const uint64_t*)b->d_span_off.p,
+                                                                       toff, soff, (const uint32_t*)b->d_text.p, (const pt_span*)b->d_spans.p,
+                                                                       (uint32_t*)b->d_ctext.p, (pt_span*)b->d_cspans.p);
+        PT_CUDA(launched(b));
         PT_CUDA(cudaMemcpyAsync(b->h_results.p, b->d_results.p, n * sizeof(pt_log_result), cudaMemcpyDeviceToHost, b->stream));
         PT_CUDA(cudaMemcpyAsync(b->h_ctoff.p, b->d_ctoff.p, (n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
         PT_CUDA(cudaMemcpyAsync(b->h_csoff.p, b->d_csoff.p, (n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
@@ -1711,7 +1344,7 @@ int pt_batch_download_begin(pt_batch* b) {
         ((uint64_t*)b->h_ctoff.p)[0] = 0; ((uint64_t*)b->h_csoff.p)[0] = 0;
     }
     if (b->limits.flags & PT_FLAG_EMIT_SEQUENCE) {
-        if ((rc = b->h_seq.reserve(std::max<uint64_t>(1, b->plan.n_text) * 4))) return rc;
+        if ((rc = reserve_n<uint32_t>(b->h_seq, b->plan.n_text))) return rc;
         if (b->plan.n_text) PT_CUDA(cudaMemcpyAsync(b->h_seq.p, b->d_seq.p, b->plan.n_text * 4, cudaMemcpyDeviceToHost, b->stream));
     }
     b->dl_begun = true;
@@ -1730,9 +1363,9 @@ int pt_batch_download(pt_batch* b, pt_spans_view* out) {
     const uint64_t used = std::min<uint64_t>(demand, b->plan.pool_cap);
     const uint64_t n_ctext = ((const uint64_t*)b->h_ctoff.p)[n], n_cspan = ((const uint64_t*)b->h_csoff.p)[n];
     b->pool_used_host = used;
-    if ((rc = b->h_pool.reserve(std::max<uint64_t>(1, used) * 4))) return rc;
-    if ((rc = b->h_text.reserve(std::max<uint64_t>(1, n_ctext) * 4))) return rc;
-    if ((rc = b->h_spans.reserve(std::max<uint64_t>(1, n_cspan) * sizeof(pt_span)))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->h_pool, used))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->h_text, n_ctext))) return rc;
+    if ((rc = reserve_n<pt_span>(b->h_spans, n_cspan))) return rc;
     if (n_ctext) PT_CUDA(cudaMemcpyAsync(b->h_text.p, b->d_ctext.p, n_ctext * 4, cudaMemcpyDeviceToHost, b->stream));
     if (n_cspan) PT_CUDA(cudaMemcpyAsync(b->h_spans.p, b->d_cspans.p, n_cspan * sizeof(pt_span), cudaMemcpyDeviceToHost, b->stream));
     if (used) PT_CUDA(cudaMemcpyAsync(b->h_pool.p, b->d_pool.p, used * 4, cudaMemcpyDeviceToHost, b->stream));
@@ -1758,14 +1391,14 @@ int pt_batch_download_patches(pt_batch* b, pt_patch_view* out) {
     if (b->patch_window_changed) { g_last_error = "pt_batch_download_patches: the patch window was set after the last merge; merge again"; return PT_ERR_STATE; }
     int rc;
     if ((rc = b->h_patch_misc.reserve(16))) return rc;
-    if ((rc = b->h_patch_recs.reserve(std::max<uint64_t>(1, b->n_insdel) * sizeof(pt_patch_rec)))) return rc;
-    if ((rc = b->h_patch_status.reserve(std::max<size_t>(1, b->n_logs) * 4))) return rc;
+    if ((rc = reserve_n<pt_patch_rec>(b->h_patch_recs, b->n_insdel))) return rc;
+    if ((rc = reserve_n<uint32_t>(b->h_patch_status, b->n_logs))) return rc;
     PT_CUDA(cudaMemcpyAsync(b->h_patch_misc.p, &counters(b)->patch_items, 8, cudaMemcpyDeviceToHost, b->stream));
     if (b->n_insdel) PT_CUDA(cudaMemcpyAsync(b->h_patch_recs.p, b->d_patch_recs.p, b->n_insdel * sizeof(pt_patch_rec), cudaMemcpyDeviceToHost, b->stream));
     if (b->n_logs) PT_CUDA(cudaMemcpyAsync(b->h_patch_status.p, b->d_patch_status.p, (size_t)b->n_logs * 4, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
     const uint64_t demand = *(unsigned long long*)b->h_patch_misc.p, used = std::min<uint64_t>(demand, b->patch_cap);
-    if ((rc = b->h_patch_items.reserve(std::max<uint64_t>(1, used) * sizeof(pt_patch_item)))) return rc;
+    if ((rc = reserve_n<pt_patch_item>(b->h_patch_items, used))) return rc;
     if (used) { PT_CUDA(cudaMemcpyAsync(b->h_patch_items.p, b->d_patch_items.p, used * sizeof(pt_patch_item), cudaMemcpyDeviceToHost, b->stream)); PT_CUDA(cudaStreamSynchronize(b->stream)); }
     out->recs = (const pt_patch_rec*)b->h_patch_recs.p; out->items = (const pt_patch_item*)b->h_patch_items.p;
     out->n_items = used; out->n_items_needed = demand; out->status = (const uint32_t*)b->h_patch_status.p;
@@ -1824,15 +1457,15 @@ int pt_batch_set_patch_window(pt_batch* b, const uint32_t* first_op, uint32_t n_
 
 int pt_batch_query_elements(pt_batch* b, const pt_elem_query* queries, uint32_t n, uint32_t* out) {
     return run_queries(b, "pt_batch_query_elements", "query", queries, n, out, [&](uint32_t grid, uint32_t threads, const pt_elem_query* dq, uint32_t* da) {
-        query_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_result*)b->d_results.p, (const uint64_t*)b->d_text_off.p,
-                                                              (const uint32_t*)b->d_seq.p, b->n_logs, da);
+        ptq::query_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_result*)b->d_results.p, (const uint64_t*)b->d_text_off.p,
+                                                                   (const uint32_t*)b->d_seq.p, b->n_logs, da);
     });
 }
 
 int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out) {
     return run_queries(b, "pt_batch_find_elements", "find", refs, n, out, [&](uint32_t grid, uint32_t threads, const pt_elem_ref* dq, pt_elem_pos* da) {
-        find_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel, (const pt_log_result*)b->d_results.p,
-                                                             (const uint64_t*)b->d_text_off.p, (const uint32_t*)b->d_seq.p, b->n_logs, da);
+        ptq::find_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel, (const pt_log_result*)b->d_results.p,
+                                                                  (const uint64_t*)b->d_text_off.p, (const uint32_t*)b->d_seq.p, b->n_logs, da);
     });
 }
 
@@ -1883,29 +1516,28 @@ int pt_batch_render_patches_json(pt_batch* b, const pt_json_pools* pools, pt_jso
             return PT_ERR_STATE;
         }
         if (owners >= 0xFFFFFFFFull) { g_last_error = std::string(fn) + ": more than 2^32 - 2 op records"; return PT_ERR_INVALID; }
-        const uint32_t no = (uint32_t)owners, nb = (no + kScanBlock - 1) / kScanBlock;
-        if ((rc = b->d_picnt.reserve(std::max<uint64_t>(1, owners) * 8)) || (rc = b->d_piseg.reserve((owners + 1) * 8)) ||
-            (rc = b->d_pibsum.reserve((size_t)(2 * nb + 2) * 8)) || (rc = b->d_pitmp.reserve(std::max<uint64_t>(1, items) * sizeof(pt_patch_item))) ||
-            (rc = b->d_pisorted.reserve(std::max<uint64_t>(1, items) * sizeof(uint2)))) return rc;
-        unsigned long long *cnt = (unsigned long long*)b->d_picnt.p, *seg = (unsigned long long*)b->d_piseg.p, *bsum = (unsigned long long*)b->d_pibsum.p;
+        const uint32_t no = (uint32_t)owners;
+        if ((rc = reserve_n<uint64_t>(b->d_picnt, owners)) || (rc = b->d_piseg.reserve((owners + 1) * 8)) ||
+            (rc = reserve_n<pt_patch_item>(b->d_pitmp, items)) || (rc = reserve_n<uint2>(b->d_pisorted, items))) return rc;
+        unsigned long long *cnt = (unsigned long long*)b->d_picnt.p, *seg = (unsigned long long*)b->d_piseg.p;
         const pt_log_desc* desc = (const pt_log_desc*)b->d_desc.p;
         const pt_patch_item* pool = (const pt_patch_item*)b->d_patch_items.p;
         pt_patch_item* tmp = (pt_patch_item*)b->d_pitmp.p;
         uint2* sorted = (uint2*)b->d_pisorted.p;
         if (no) {
-            const uint32_t threads = 256, grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + threads - 1) / threads, (uint64_t)b->num_sms * 16));
+            const uint32_t threads = 256, grid = warp_grid(b, items, threads, 1);     // one thread per item
             PT_CUDA(cudaMemsetAsync(cnt, 0, owners * 8, b->stream));
-            if (items) ptr::pitem_count_kernel<<<grid, threads, 0, b->stream>>>(pool, items, desc, b->n_insdel, cnt);
-            out_block_sums_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{cnt}, no, bsum);
-            out_scan_blocks_kernel<<<1, 1024, 0, b->stream>>>(bsum, nb);
-            out_offsets_kernel<<<nb, kScanBlock, 0, b->stream>>>(PlainCounts{cnt}, no, bsum, nb, seg, (unsigned long long*)nullptr);
-            b->launches += 3;
+            if (items) {
+                ptr::pitem_count_kernel<<<grid, threads, 0, b->stream>>>(pool, items, desc, b->n_insdel, cnt);
+                PT_CUDA(launched(b));
+            }
+            if ((rc = scan_offsets(b, pts::PlainCounts{cnt}, no, b->d_pibsum, seg, nullptr))) return rc;
             if (items) {
                 ptr::pitem_scatter_kernel<<<grid, threads, 0, b->stream>>>(pool, items, desc, b->n_insdel, cnt, seg, tmp);
+                PT_CUDA(launched(b));
                 ptr::pitem_rank_kernel<<<grid, threads, 0, b->stream>>>(tmp, items, desc, b->n_insdel, seg, sorted);
-                b->launches += 3;
+                PT_CUDA(launched(b));
             }
-            PT_CUDA(cudaGetLastError());
         } else {
             PT_CUDA(cudaMemsetAsync(seg, 0, 8, b->stream));
         }
@@ -1966,7 +1598,7 @@ int pt_batch_set_comment_pool(pt_batch* b, uint64_t entries) {
     if (b->have_batch && entries) {
         b->plan.pool_cap = entries;
         int rc;
-        if ((rc = b->d_pool.reserve(std::max<uint64_t>(1, b->plan.pool_cap) * 4))) return rc;
+        if ((rc = reserve_n<uint32_t>(b->d_pool, b->plan.pool_cap))) return rc;
         drop_graph(b);                                   // the pool pointer / capacity are baked in
     }
     return PT_OK;
