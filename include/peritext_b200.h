@@ -704,6 +704,94 @@ int pt_batch_render_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
  * per log and one lane per op. */
 int pt_batch_render_patches_json(pt_batch*, const pt_json_pools*, pt_json_view* out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Changes as JSON: the reference's Change objects (src/micromerge.ts:60-71; "can be JSON-encoded to send to another node",
+ * :304-307) of resident logs, rendered on the device from the change table and the records, so a batch can serve a peer
+ * what it is missing (getMissingChanges, reference test/merge.ts:25-38) or save a document's history.
+ *
+ * The records hold only the ops that target the log's text list.  The other ops of a change (the ROOT makeList, ops on other
+ * objects) and each change's startOp come from an optional side table, the EXTRAS, built where those ops are still visible
+ * (pt_ingest_change_extras, packing.change_extras / input_extras).  Without extras the call renders the list-op projection
+ * of every change: its list ops only, and startOp = the original counter of its first list op.
+ * ---------------------------------------------------------------------------------------------- */
+#define PT_EXTRA_NONE 0xFFFFFFFFFFFFFFFFull
+typedef struct pt_change_extra {   /* 32 B; sorted by (log, change, pos) */
+    uint32_t log;
+    uint32_t change;    /* index in the log's change table                                                               */
+    uint32_t pos;       /* index in change.ops                                                                           */
+    uint32_t reserved;  /* 0                                                                                             */
+    uint64_t start_op;  /* change.startOp; every entry of one change has the same value                                  */
+    uint64_t op;        /* the op's canonical JSON: entry `op` of the extra-ops pool; PT_EXTRA_NONE: no op, the entry only
+                           supplies startOp (then it is the change's only entry and pos is 0)                            */
+} pt_change_extra;
+
+#define PT_CHANGES_RANGE 0u     /* changes [first, first + count) of the log's table, clipped at its end                  */
+#define PT_CHANGES_MISSING 1u   /* the changes not covered by the request's clock, in getMissingChanges order            */
+typedef struct pt_changes_request {   /* 32 B */
+    uint32_t log, mode, first, count;
+    uint64_t clock_off;                /* MISSING: the peer's clock is clock[clock_off .. clock_off + n_clock)             */
+    uint32_t n_clock, reserved;
+} pt_changes_request;
+typedef struct pt_clock_entry { uint32_t actor; uint32_t seq; } pt_clock_entry;   /* actor rank in the request's log */
+typedef struct pt_changes_json_input {
+    uint32_t n_requests, reserved;
+    const pt_changes_request* requests;
+    const pt_clock_entry* clock; uint64_t n_clock;
+    pt_json_pools pools;                                       /* as pt_batch_render_json takes them                  */
+    const uint8_t* actors; const uint64_t* actors_off;         /* PT_POOL_ACTORS: UTF-16LE ids, byte offsets [count + 1] */
+    const uint64_t* actors_first;                              /* [n_logs + 1] log i's actor rank r is entry first[i] + r */
+    const uint64_t* counters; const uint64_t* counters_first;  /* PT_POOL_COUNTERS as u64 entries, [n_logs + 1] ranges;
+                                                                  an empty range: the log's counters are the original ones */
+    const uint8_t* list_ids; const uint64_t* list_ids_off;     /* PT_POOL_LIST_IDS: one UTF-16LE id per log, [n_logs + 1] */
+    const pt_change_extra* extras; uint64_t n_extras;          /* NULL / 0: the list-op projection                     */
+    const uint8_t* extra_ops; const uint64_t* extra_ops_off; uint64_t n_extra_ops;   /* PT_POOL_EXTRA_OPS               */
+} pt_changes_json_input;
+#define PT_CHANGES_OK 0u
+#define PT_CHANGES_BAD_TABLE 1u  /* MISSING on a table that is not seq-contiguous per actor, or any mode where the table's n_ops
+                                    do not sum to the log's n_insdel + n_mark or a change's deps (dep_off + n_deps) leave the
+                                    log's dep records                                                                        */
+typedef struct pt_changes_json_view {
+    uint32_t n_requests;
+    const uint64_t* off;        /* [n_requests + 1] request r's text is bytes[off[r] .. off[r+1])                                */
+    const char* bytes; uint64_t n_bytes;
+    const uint32_t* status;     /* [n_requests] PT_CHANGES_*; a request that is not OK renders zero bytes                        */
+} pt_changes_json_view;
+
+/* Render each request's changes of a resident log as the UTF-8 JSON text of a Change[]: "[" + changes joined by "," + "]".
+ *   change    {"actor":A,"deps":{...},"ops":[...],"seq":S,"startOp":N}  top-level keys sorted; deps in the table's stored order
+ *   insert    {"action":"set","elemId":E,"insert":true,"obj":L,"opId":O,"value":V}
+ *   delete    {"action":"del","elemId":E,"obj":L,"opId":O}
+ *   mark      {"action":"addMark|removeMark",["attrs":F,]"end":B,"markType":T,"obj":L,"opId":O,"start":B}
+ *   boundary  {"elemId":E,"type":"before|after"} or {"type":"startOfText|endOfText"}
+ * opIds and elemIds are "ctr@actor" with the original counter (through the counter pool) in decimal; HEAD is "_head" (the form
+ * of the oracle and of packing.change_dicts, not the reference's Symbol-dropping JSON.stringify).  Actor ids, L (the log's list
+ * id) and V (the element's value alone) follow the span render's JSON.stringify string rules.  "attrs" is present exactly when
+ * the mark record's attr is not PT_ATTR_NONE: the links pool fragment, or the comments pool fragment of the rank, which is the
+ * first-seen attrs object of the comment id (the renders' corner); strong / em {"active":true} attrs are dropped by the packers
+ * and do not come back.  Ops: extra entry e sits at index e.pos of change.ops, the list ops fill the other indices in arrival
+ * order (mark record k before ins/del record arrival_k); startOp is the extras' start_op, else the original counter of the
+ * change's first list op.  pt_ingest_parse of a rendered log rebuilds the batch's records, change table and pools exactly.
+ * Requests:
+ *   RANGE    changes [first, first + count) of the log's table, clipped at its end (count 0 or first past the end: "[]")
+ *   MISSING  the changes whose seq exceeds the clock's entry for their actor (an absent actor counts as 0), actors in the order
+ *            the log's table first shows them, then ascending seq: getMissingChanges with that clock (pt_batch_exchange step 2)
+ * Per request status: PT_CHANGES_BAD_TABLE (see above) renders zero bytes; the other requests proceed.  A table that admission
+ * rejected still renders when it is seq-gapped or misses a dependency, since RANGE does not need causal order.
+ * Refused, no view (pt_last_error names the first offender):
+ *   PT_ERR_STATE    no batch, or a handle without a change table
+ *   PT_ERR_INVALID  null arguments; a request's log >= n_logs, unknown mode, or clock range outside the clock array; a clock
+ *                   actor >= the log's n_actors; extras out of order, naming a log or change outside the batch, with different
+ *                   start_op in one change, a NONE entry beside another entry, an op outside the extra-ops pool, or a pos past
+ *                   the change's ops; a pool entry the output needs and the pools do not hold (actor, counter, value, link,
+ *                   comment); a selected change with neither list ops nor extras (it has no startOp)
+ * n_requests == 0: PT_OK, nothing launched.  Needs no merge and works on logs whose merge failed.  Every other view of the handle
+ * stays valid and unchanged.  Synchronises.  The view is engine-owned pinned memory of its own, valid until the next
+ * pt_batch_render_changes_json, upload or destroy.
+ * Device: a select kernel, one warp per request (the list-op positions, for MISSING the peer's clock in shared memory and the
+ * queue as pt_batch_exchange builds it); the selected changes cut into work items of at most 1024 list ops; a size pass, a scan
+ * and a write pass, one warp per item and one lane per op.  Two read-backs: the item count and the byte total. */
+int pt_batch_render_changes_json(pt_batch*, const pt_changes_json_input* in, pt_changes_json_view* out);
+
 /* Copy only the per-log result headers (status, counts, digest). Synchronises the stream. */
 int pt_batch_download_results(pt_batch*, pt_log_result* out, uint32_t n_logs);
 
@@ -744,12 +832,19 @@ typedef struct pt_ingest pt_ingest;
 #define PT_POOL_ACTORS 4        /* actor ids UTF-16LE, rank order per log; per_log_first[i] .. per_log_first[i+1]       */
 #define PT_POOL_COUNTERS 5      /* dense counter rank -> original counter (u64 each) of logs whose counters were
                                    re-ranked; empty range otherwise; per_log_first as above                            */
+#define PT_POOL_LIST_IDS 6      /* each log's text-list object id, UTF-16LE, one entry per log (empty: no list)        */
+#define PT_POOL_EXTRA_OPS 7     /* the canonical JSON (UTF-8) of every op that does not target its log's text list, in
+                                   the order of the extras (pt_change_extra.op indexes it)                             */
 int pt_ingest_create(pt_ingest** out);
 int pt_ingest_parse(pt_ingest*, const char* const* logs_json, const uint64_t* lens, uint32_t n_logs, int threads /* 0 = all cores */);
 /* Views into the parsed batch (valid until the next pt_ingest_parse / pt_ingest_destroy). */
 int pt_ingest_packed(pt_ingest*, pt_packed_ops* ops, pt_change_table* changes);
 int pt_ingest_pool(pt_ingest*, int kind, const uint8_t** data, const uint64_t** offsets /* [count + 1] */, uint64_t* count,
                    const uint64_t** per_log_first /* may be NULL */);
+/* The extras of the parsed batch (pt_batch_render_changes_json): per change, in order, one entry per op that does not target
+ * the log's text list, and a PT_EXTRA_NONE entry for a change that has no such op but has no list op either, or whose startOp
+ * is not the counter of its first list op.  Sorted by (log, change, pos). */
+int pt_ingest_change_extras(pt_ingest*, const pt_change_extra** out, uint64_t* n);
 const char* pt_ingest_error(pt_ingest*);
 void pt_ingest_destroy(pt_ingest*);
 

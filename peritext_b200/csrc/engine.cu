@@ -23,6 +23,7 @@
 #include "append_kernel.cuh"
 #include "change_kernel.cuh"
 #include "exchange_kernel.cuh"
+#include "changes_json_kernel.cuh"
 #include "upload_kernel.cuh"
 #include "scan_kernel.cuh"
 #include "admit_kernel.cuh"
@@ -118,6 +119,8 @@ struct pt_batch {
     HostBuf h_patch_recs, h_patch_items, h_patch_status, h_patch_misc, h_patch_first;
     DevBuf d_jval, d_jvoff, d_jlink, d_jloff, d_jcom, d_jcoff;          // both JSON renders: the caller's pools
     JsonBufs spans_json, patches_json;                                  // each render's own scratch and view
+    JsonBufs changes_json;                                              // pt_batch_render_changes_json: its own scratch and view
+    HostBuf h_cj_status;                                                //   and its per-request status
     DevBuf d_picnt, d_piseg, d_pibsum, d_pitmp, d_pisorted;             // pt_batch_render_patches_json: the ordered patch items
     uint64_t patch_cap = 0;
     bool have_changes = false;
@@ -1552,6 +1555,177 @@ int pt_batch_render_patches_json(pt_batch* b, const pt_json_pools* pools, pt_jso
         [&](uint32_t grid, uint32_t threads, const unsigned long long* off, uint8_t* bytes) {
             ptr::patches_json_write_kernel<<<grid, threads, 0, b->stream>>>(I, n, P, off, bytes);
         }, out);
+}
+
+// pt_batch_render_changes_json's host checks of the requests, the string pools and the extras (include/peritext_b200.h).  On
+// success slot_off holds each request's scratch slot (exclusive scan of its log's n_changes).  Returns the problem, or "".
+static std::string check_changes_json(const pt_batch* b, const pt_changes_json_input& in, std::vector<unsigned long long>& slot_off) {
+    const uint32_t n = b->n_logs, nr = in.n_requests;
+    auto req = [](uint32_t r) { return "request " + std::to_string(r) + ": "; };
+    if (!in.requests) return "null requests";
+    if (in.n_clock && !in.clock) return "null clock with a nonzero n_clock";
+    if (!in.actors_first || !in.actors_off || !in.counters_first || !in.list_ids_off) return "null actor, counter or list-id pool";
+    if (in.n_extras && !in.extras) return "null extras with a nonzero n_extras";
+    if (in.n_extra_ops && (!in.extra_ops || !in.extra_ops_off)) return "null extra-ops pool with a nonzero count";
+    for (uint32_t i = 0; i < n; i++) {
+        if (in.actors_first[i + 1] < in.actors_first[i] || in.counters_first[i + 1] < in.counters_first[i] || in.list_ids_off[i + 1] < in.list_ids_off[i])
+            return at(i) + "a pool's per-log offsets decrease";
+        if ((in.list_ids_off[i + 1] - in.list_ids_off[i]) & 1) return at(i) + "the list id is not UTF-16LE (odd byte count)";
+    }
+    if (in.actors_first[0] != 0 || in.counters_first[0] != 0) return "the actor and counter ranges must start at entry 0";
+    if (in.counters_first[n] && !in.counters) return "null counter pool with a nonzero count";
+    if (in.actors_first[n] && !in.actors) return "null actor pool with a nonzero count";
+    for (uint64_t k = 0; k < in.actors_first[n]; k++)
+        if (in.actors_off[k + 1] < in.actors_off[k] || ((in.actors_off[k + 1] - in.actors_off[k]) & 1)) return "actor pool entry " + std::to_string(k) + " is not UTF-16LE";
+    for (uint64_t k = 0; k < in.n_extra_ops; k++)
+        if (in.extra_ops_off[k + 1] < in.extra_ops_off[k]) return "extra-ops offsets decrease";
+    slot_off.assign((size_t)nr + 1, 0);
+    for (uint32_t r = 0; r < nr; r++) {
+        const pt_changes_request& q = in.requests[r];
+        if (q.log >= n) return req(r) + "log " + std::to_string(q.log) + " is outside the batch's " + std::to_string(n) + " logs";
+        if (q.mode != PT_CHANGES_RANGE && q.mode != PT_CHANGES_MISSING) return req(r) + "unknown mode " + std::to_string(q.mode);
+        if (q.mode == PT_CHANGES_MISSING) {
+            if (q.clock_off > in.n_clock || q.n_clock > in.n_clock - q.clock_off) return req(r) + "the clock range is outside the clock array";
+            for (uint32_t k = 0; k < q.n_clock; k++)
+                if (in.clock[q.clock_off + k].actor >= b->h_desc[q.log].n_actors)
+                    return req(r) + "clock entry " + std::to_string(k) + " names actor " + std::to_string(in.clock[q.clock_off + k].actor) + " and log " +
+                           std::to_string(q.log) + " has " + std::to_string(b->h_desc[q.log].n_actors) + " actors";
+        }
+        slot_off[r + 1] = slot_off[r] + b->h_cdesc[q.log].n_changes;
+    }
+    for (uint64_t e = 0; e < in.n_extras; e++) {
+        const pt_change_extra& x = in.extras[e];
+        const std::string ex = "extra " + std::to_string(e) + ": ";
+        if (x.log >= n || x.change >= b->h_cdesc[x.log].n_changes) return ex + "log " + std::to_string(x.log) + " has no change " + std::to_string(x.change);
+        if (x.op != PT_EXTRA_NONE && x.op >= in.n_extra_ops) return ex + "op " + std::to_string(x.op) + " is outside the extra-ops pool";
+        if (e == 0) continue;
+        const pt_change_extra& p = in.extras[e - 1];
+        if (p.log > x.log || (p.log == x.log && p.change > x.change)) return ex + "the extras are not sorted by (log, change, pos)";
+        if (p.log == x.log && p.change == x.change) {
+            if (p.pos >= x.pos) return ex + "the extras are not sorted by (log, change, pos)";
+            if (p.start_op != x.start_op) return ex + "a different start_op than the change's other extras";
+            if (p.op == PT_EXTRA_NONE || x.op == PT_EXTRA_NONE) return ex + "a PT_EXTRA_NONE entry beside another entry of the change";
+        }
+    }
+    return std::string();
+}
+
+// JSON render of Change objects (changes_json_kernel.cuh): select, then the item passes.
+int pt_batch_render_changes_json(pt_batch* b, const pt_changes_json_input* in, pt_changes_json_view* out) {
+    static const char* fn = "pt_batch_render_changes_json";
+    if (!b || !in || !out) { g_last_error = std::string(fn) + ": null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = std::string(fn) + " before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = std::string(fn) + ": the handle has no change table"; return PT_ERR_STATE; }
+    const uint32_t nr = in->n_requests, n = b->n_logs;
+    JsonBufs& J = b->changes_json;
+    int rc;
+    if ((rc = J.hoff.reserve(((size_t)nr + 1) * 8)) || (rc = J.hbytes.reserve(1)) || (rc = J.hmisc.reserve(32)) ||
+        (rc = reserve_n<uint32_t>(b->h_cj_status, nr))) return rc;
+    uint64_t* hoff = (uint64_t*)J.hoff.p;
+    uint32_t* hstatus = (uint32_t*)b->h_cj_status.p;
+    if (!nr) {
+        PT_CUDA(cudaSetDevice(b->device));
+        PT_CUDA(cudaStreamSynchronize(b->stream));          // the pinned view buffers may still be the target of an earlier copy
+        hoff[0] = 0;
+        *out = pt_changes_json_view{0, hoff, (const char*)J.hbytes.p, 0, hstatus};
+        return PT_OK;
+    }
+    std::vector<unsigned long long> slot_off;
+    std::string err = check_changes_json(b, *in, slot_off);
+    if (!err.empty()) { g_last_error = std::string(fn) + ": " + err; return PT_ERR_INVALID; }
+    ptr::JsonPools P{};
+    if ((rc = load_json_pools(b, &in->pools, fn, &P))) return rc;
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    // the requests, the string pools, the extras and the select kernel's scratch: freed on return
+    DevBuf dreq, dclock, dact, dactoff, dactfirst, dctr, dctrfirst, dlid, dlidoff, dx, dxops, dxoff, dslot, dpos, dsel, dnsel, dstat, ditems, dbad,
+           ditemoff, dbsum, dsizes, dboff, doff, dmiss, dbytes;
+    const uint64_t n_slot = slot_off[nr], n_act = in->actors_first[n], n_ctr = in->counters_first[n];
+    const uint64_t act_bytes = n_act ? in->actors_off[n_act] : 0, lid_bytes = in->list_ids_off[n], xop_bytes = in->n_extra_ops ? in->extra_ops_off[in->n_extra_ops] : 0;
+    if ((rc = upload_n(b, dreq, in->requests, nr)) || (rc = upload_n(b, dclock, in->clock, in->n_clock)) ||
+        (rc = upload_n(b, dact, in->actors, act_bytes)) || (rc = upload_n(b, dactoff, in->actors_off, n_act + 1)) ||
+        (rc = upload_n(b, dactfirst, in->actors_first, (uint64_t)n + 1)) || (rc = upload_n(b, dctr, in->counters, n_ctr)) ||
+        (rc = upload_n(b, dctrfirst, in->counters_first, (uint64_t)n + 1)) || (rc = upload_n(b, dlid, in->list_ids, lid_bytes)) ||
+        (rc = upload_n(b, dlidoff, in->list_ids_off, (uint64_t)n + 1)) || (rc = upload_n(b, dx, in->extras, in->n_extras)) ||
+        (rc = upload_n(b, dxops, in->extra_ops, xop_bytes)) || (rc = upload_n(b, dxoff, in->extra_ops_off, in->n_extra_ops ? in->n_extra_ops + 1 : 0)) ||
+        (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)nr + 1)) || (rc = reserve_n<uint32_t>(dpos, n_slot)) ||
+        (rc = reserve_n<ptcj::Sel>(dsel, n_slot)) || (rc = reserve_n<uint32_t>(dnsel, nr)) || (rc = reserve_n<uint32_t>(dstat, nr)) ||
+        (rc = reserve_n<unsigned long long>(ditems, nr)) || (rc = reserve_n<unsigned long long>(dbad, 2)) ||
+        (rc = reserve_n<unsigned long long>(ditemoff, (uint64_t)nr + 1)) || (rc = reserve_n<unsigned long long>(dmiss, 2)) ||
+        (rc = reserve_n<unsigned long long>(doff, (uint64_t)nr + 1))) return rc;
+    ptcj::ChangesParams C{};
+    C.req = (const pt_changes_request*)dreq.p; C.n_req = nr; C.maxR = b->adm_maxR; C.clock = (const pt_clock_entry*)dclock.p;
+    C.desc = (const pt_log_desc*)b->d_desc.p; C.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    C.changes = (const pt_change_rec*)b->d_changes.p; C.deps = (const pt_dep_rec*)b->d_deps.p;
+    C.insdel = b->dp_insdel; C.marks = b->dp_marks;
+    C.slot_off = (const unsigned long long*)dslot.p; C.pos = (uint32_t*)dpos.p; C.sel = (ptcj::Sel*)dsel.p;
+    C.n_sel = (uint32_t*)dnsel.p; C.status = (uint32_t*)dstat.p; C.items = (unsigned long long*)ditems.p;
+    C.extras = (const pt_change_extra*)dx.p; C.n_extras = in->n_extras; C.bad = (unsigned long long*)dbad.p;
+    C.item_off = (const unsigned long long*)ditemoff.p;
+    C.actors = (const uint8_t*)dact.p; C.actors_off = (const unsigned long long*)dactoff.p; C.actors_first = (const unsigned long long*)dactfirst.p;
+    C.counters = (const unsigned long long*)dctr.p; C.counters_first = (const unsigned long long*)dctrfirst.p;
+    C.list_ids = (const uint8_t*)dlid.p; C.list_ids_off = (const unsigned long long*)dlidoff.p;
+    C.xops = (const uint8_t*)dxops.p; C.xops_off = (const unsigned long long*)dxoff.p;
+    unsigned long long* bad = (unsigned long long*)dbad.p;
+    unsigned long long* miss = (unsigned long long*)dmiss.p;
+    PT_CUDA(cudaMemsetAsync(bad, 0xFF, 16, b->stream));
+    const auto [wpb, smem] = actor_shape(b->adm_maxR);
+    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptcj::changes_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ptcj::changes_select_kernel<<<warp_grid(b, nr, wpb * 32), wpb * 32, smem, b->stream>>>(C);
+    PT_CUDA(launched(b));
+    if ((rc = scan_offsets(b, pts::PlainCounts{C.items}, nr, dbsum, (unsigned long long*)ditemoff.p, nullptr))) return rc;
+    // read-back 1: the item count and the select kernel's findings
+    uint64_t* hm = (uint64_t*)J.hmisc.p;
+    PT_CUDA(cudaMemcpyAsync(hm, (unsigned long long*)ditemoff.p + nr, 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(hm + 1, bad, 16, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    const uint64_t n_items = hm[0];
+    for (int k = 0; k < 2; k++)
+        if (hm[1 + k] != ~0ull) {
+            g_last_error = std::string(fn) + ": log " + std::to_string(hm[1 + k] >> 32) + " change " + std::to_string(hm[1 + k] & 0xFFFFFFFFull) +
+                           (k == 0 ? " has neither list ops nor extras, so nothing gives its startOp" : ": its extras' positions lie past the change's ops");
+            return PT_ERR_INVALID;
+        }
+    if (n_items >= 0xFFFFFFFFull) { g_last_error = std::string(fn) + ": more than 2^32 - 2 work items"; return PT_ERR_INVALID; }
+    C.n_items = n_items;
+    uint64_t total = 0;
+    if (n_items) {
+        if ((rc = reserve_n<unsigned long long>(dsizes, n_items)) || (rc = reserve_n<unsigned long long>(dboff, n_items + 1))) return rc;
+        unsigned long long *sizes = (unsigned long long*)dsizes.p, *boff = (unsigned long long*)dboff.p;
+        const uint32_t threads = 128, grid = warp_grid(b, n_items, threads);
+        PT_CUDA(cudaMemsetAsync(miss, 0xFF, 16, b->stream));
+        ptcj::changes_json_size_kernel<<<grid, threads, 0, b->stream>>>(C, P, sizes, miss, miss + 1);
+        PT_CUDA(launched(b));
+        if ((rc = scan_offsets(b, pts::PlainCounts{sizes}, (uint32_t)n_items, dbsum, boff, nullptr))) return rc;
+        ptcj::changes_offsets_kernel<<<warp_grid(b, (uint64_t)nr + 1, 256, 1), 256, 0, b->stream>>>(C.item_off, boff, nr, (unsigned long long*)doff.p);
+        PT_CUDA(launched(b));
+        // read-back 2: the byte total and the missing pool entries
+        PT_CUDA(cudaMemcpyAsync(hm, boff + n_items, 8, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaMemcpyAsync(hm + 1, miss, 16, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+        total = hm[0];
+        if (hm[1] != ~0ull) {
+            static const char* kinds[3] = {"value", "link", "comment"};
+            g_last_error = std::string(fn) + ": log " + std::to_string(hm[1] >> 34) + " names " + kinds[(hm[1] >> 32) & 3] + " pool entry " +
+                           std::to_string(hm[1] & 0xFFFFFFFFull) + ", which the caller's pools do not hold";
+            return PT_ERR_INVALID;
+        }
+        if (hm[2] != ~0ull) {
+            g_last_error = std::string(fn) + ": log " + std::to_string(hm[2] >> 34) + " names " + ((hm[2] >> 32) & 3 ? "counter" : "actor") + " " +
+                           std::to_string(hm[2] & 0xFFFFFFFFull) + ", which the caller's " + ((hm[2] >> 32) & 3 ? "counter" : "actor") + " pool does not hold";
+            return PT_ERR_INVALID;
+        }
+        if ((rc = reserve_n<uint8_t>(J.bytes, total)) || (rc = reserve_n<uint8_t>(J.hbytes, total))) return rc;
+        ptcj::changes_json_write_kernel<<<grid, threads, 0, b->stream>>>(C, P, boff, (uint8_t*)J.bytes.p);
+        PT_CUDA(launched(b));
+        PT_CUDA(cudaMemcpyAsync(hoff, doff.p, ((size_t)nr + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
+        if (total) PT_CUDA(cudaMemcpyAsync(J.hbytes.p, J.bytes.p, total, cudaMemcpyDeviceToHost, b->stream));
+    } else {
+        memset(hoff, 0, ((size_t)nr + 1) * 8);              // every request failed: zero bytes each
+    }
+    PT_CUDA(cudaMemcpyAsync(hstatus, dstat.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    *out = pt_changes_json_view{nr, hoff, (const char*)J.hbytes.p, total, hstatus};
+    return PT_OK;
 }
 
 int pt_batch_device_results(pt_batch* b, void** dev_ptr, uint32_t* n_logs) {

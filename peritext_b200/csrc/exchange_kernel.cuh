@@ -6,10 +6,10 @@
 //   1. clocks: both change tables 32 changes per trip; match_any groups give each change its rank among the trip's changes of
 //      the same actor, so seq == count + 1 is checked per lane (admit_kernel's scheme).  The src pass also writes each change's
 //      list-op position (running sum of n_ops) into the pair's scratch slot.
-//   2. queue, getMissingChanges order (reference test/merge.ts:25-38): actors in the order src first saw them, ascending seq.
-//      In a seq-contiguous table an actor's first change is its seq 1, so one pass in table order gives every actor the
-//      slot of its first missing change (a warp scan over the trip's seq-1 lanes), and the change (actor, seq) goes to
-//      slot[actor] + seq - clock_dst - 1.
+//   2. queue, getMissingChanges order (reference test/merge.ts:25-38): actors in the order src first saw them, ascending seq
+//      (missing_queue, shared with pt_batch_render_changes_json's select kernel).  In a seq-contiguous table an actor's first
+//      change is its seq 1, so one pass in table order gives every actor the slot of its first missing change (a warp scan over
+//      the trip's seq-1 lanes), and the change (actor, seq) goes to slot[actor] + seq - clock_dst - 1.
 //   3. delivery, applyChanges order (test/merge.ts:4-23): repeated in-order passes over the queue, 32 candidates per trip.
 //      All lanes test seq and deps against the clock of the trip's start.  A pass is final (clocks only grow, and a
 //      seq-contiguous table has no second change with the same actor and seq); a lane that failed is tested again in lane
@@ -117,6 +117,32 @@ __device__ __forceinline__ bool count_clock(const pt_change_rec* __restrict__ c0
     return ok;
 }
 
+// getMissingChanges order (reference test/merge.ts:25-38) of a seq-contiguous table c0[0 .. n) whose clock count_clock left in
+// cs[actor]: actors in the order the table first shows them, then ascending seq.  have(actor) is the peer's clock entry for the
+// table's actor rank.  An actor's first change is its seq 1, so one pass in table order gives every actor the slot of its first
+// missing change (a warp scan over the trip's seq-1 lanes, overwriting cs), and change k = (actor, seq) with seq > have goes to
+// slot cs[actor] + seq - have - 1: queued(k, its record, slot).  Returns the queue length.  Warp-collective.
+template <class Have, class Queued>
+__device__ __forceinline__ uint32_t missing_queue(const pt_change_rec* __restrict__ c0, uint32_t n, uint32_t* cs, Have have_of, Queued queued, uint32_t lane) {
+    uint32_t nq = 0;
+    for (uint32_t base = 0; base < n; base += 32) {
+        const uint32_t k = base + lane;
+        const bool valid = k < n;
+        uint4 r = make_uint4(0, 0, 0, 0);
+        if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
+        const uint32_t actor = r.y & 0xFFFFu, have = valid ? have_of(actor) : 0u;
+        const bool first = valid && r.x == 1u;
+        uint32_t tot;
+        const uint32_t ex = warp_excl_scan(first && cs[actor] > have ? cs[actor] - have : 0u, lane, tot);
+        __syncwarp();
+        if (first) cs[actor] = nq + ex;
+        __syncwarp();
+        nq += tot;
+        if (valid && r.x > have) queued(k, r, cs[actor] + r.x - have - 1u);
+    }
+    return nq;
+}
+
 // applyChange's admission test (reference src/micromerge.ts:501-509) of a src change against dst's clock; the change's and
 // its deps' actors are known to have images (step 2 checked them).
 __device__ __forceinline__ bool admits(const PairMaps& m, const uint32_t* clk, const pt_dep_rec* __restrict__ d0, uint4 r) {
@@ -159,30 +185,17 @@ __global__ void exchange_select_kernel(ExchangeParams P) {
         uint32_t nq = 0;
         if (status == PT_EXCHANGE_OK) {
             bool bad = false, unmapped = false;
-            for (uint32_t base = 0; base < CS.n_changes; base += 32) {
-                const uint32_t k = base + lane;
-                const bool valid = k < CS.n_changes;
-                uint4 r = make_uint4(0, 0, 0, 0);
-                if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
-                const uint32_t actor = r.y & 0xFFFFu, ma = valid ? m.actor(actor) : 0xFFFFu;
-                const uint32_t have = ma < Rd ? clk[ma] : 0u;            // an actor dst has no rank for: clock 0
-                const bool first = valid && r.x == 1u;
-                uint32_t tot;
-                const uint32_t ex = warp_excl_scan(first && cs[actor] > have ? cs[actor] - have : 0u, lane, tot);
-                __syncwarp();
-                if (first) cs[actor] = nq + ex;
-                __syncwarp();
-                nq += tot;
-                if (valid && r.x > have) {
-                    queue[cs[actor] + r.x - have - 1u] = k;
-                    if (ma >= Rd) unmapped = true;
-                    for (uint32_t d = 0; d < (r.y >> 16); d++) {
-                        const uint32_t da = d0[r.z + d].actor;
-                        if (da >= Rs) bad = true;
-                        else if (m.actor(da) >= Rd) unmapped = true;
-                    }
-                }
-            }
+            nq = missing_queue(c0, CS.n_changes, cs,
+                               [&](uint32_t actor) { const uint32_t ma = m.actor(actor); return ma < Rd ? clk[ma] : 0u; },   // no rank in dst: 0
+                               [&](uint32_t k, uint4 r, uint32_t slot) {
+                                   queue[slot] = k;
+                                   if (m.actor(r.y & 0xFFFFu) >= Rd) unmapped = true;
+                                   for (uint32_t d = 0; d < (r.y >> 16); d++) {
+                                       const uint32_t da = d0[r.z + d].actor;
+                                       if (da >= Rs) bad = true;
+                                       else if (m.actor(da) >= Rd) unmapped = true;
+                                   }
+                               }, lane);
             if (__any_sync(0xffffffffu, bad)) status = PT_EXCHANGE_BAD_TABLE;
             else if (__any_sync(0xffffffffu, unmapped)) status = PT_EXCHANGE_UNMAPPED;
         }

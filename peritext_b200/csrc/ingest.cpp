@@ -9,6 +9,8 @@
 //   * link attrs / multi-character values are interned per batch in first-appearance order, comment ids are ranked by JS
 //     string order (sortBy, src/peritext.ts:318); counters far beyond the op count are re-ranked densely
 //   * every Change also yields one pt_change_rec (actor, seq, deps) for the admission pre-pass (src/micromerge.ts:501-509)
+//   * the ops that are not packed (ROOT-map ops, other objects) and each change's startOp are kept as extras (pt_change_extra,
+//     packing.change_extras) with each log's list id, so pt_batch_render_changes_json can give the changes back exactly
 #include <algorithm>
 #include <atomic>
 #include <cstdint>
@@ -176,10 +178,12 @@ struct Bound { uint32_t type = 0; uint64_t ctr = 0; int actor = -1; };
 struct InsDel { uint64_t ctr, rctr; int actor, ractor; uint32_t kind, tok; };
 struct Mark { uint64_t ctr; int actor; bool add; uint32_t mt; Bound sb, eb; int attr_kind; uint32_t attr_local; uint32_t arrival; };   // attr_kind 0 none, 1 link, 2 comment
 struct Change { int actor; uint32_t seq; std::vector<std::pair<int, uint32_t>> deps; uint32_t n_ops; };
+struct Extra { uint32_t change, pos; uint64_t start_op; bool none; std::string op; };   // an op off the text list, or startOp alone
 struct LogB {
     std::vector<u16s> actors;                       // local actor ids, first-appearance order
     std::unordered_map<std::string, int> actor_ix;  // key: raw bytes of the u16 string
     std::vector<InsDel> insdel; std::vector<Mark> marks; std::vector<Change> changes;
+    std::vector<Extra> extras; u16s list_id;
     std::vector<u16s> values; std::unordered_map<std::string, uint32_t> value_ix;          // local pools (merged in log order)
     std::vector<std::string> links; std::unordered_map<std::string, uint32_t> link_ix;
     std::vector<u16s> comments; std::vector<std::string> comment_attrs; std::unordered_map<std::string, uint32_t> comment_ix;
@@ -215,8 +219,15 @@ bool build_log(const JV& root, LogB& b) {
     }
     auto lt = children.find(u"text");
     const bool have_list = lt != children.end();
+    if (have_list) b.list_id = lt->second;
     for (auto& ch : root.a) {
         Change C; C.n_ops = 0;
+        const JV* so = ch.get(u"startOp");
+        const bool have_start = so && so->t == JV::Num;
+        const uint64_t start_op = have_start ? strtoull(so->num.c_str(), nullptr, 10) : 0;
+        const size_t ex0 = b.extras.size();
+        uint64_t first_ctr = 0;
+        uint32_t op_pos = 0;
         const JV* ca = ch.get(u"actor"); const JV* cs = ch.get(u"seq");
         if (!ca || ca->t != JV::Str || !cs || cs->t != JV::Num) { b.err = "change without actor/seq"; return false; }
         C.actor = b.actor_of(ca->s); C.seq = (uint32_t)strtoull(cs->num.c_str(), nullptr, 10);
@@ -224,15 +235,21 @@ bool build_log(const JV& root, LogB& b) {
             for (auto& kv : deps->o) { if (kv.second.t != JV::Num) { b.err = "bad deps"; return false; } C.deps.emplace_back(b.actor_of(kv.first), (uint32_t)strtoull(kv.second.num.c_str(), nullptr, 10)); }
         const JV* ops = ch.get(u"ops");
         for (auto& op : ops->a) {
+            const uint32_t pos = op_pos++;
             const JV* obj = op.get(u"obj");
-            if (!have_list || !obj || obj->t != JV::Str || obj->s != lt->second) continue;
+            if (!have_list || !obj || obj->t != JV::Str || obj->s != lt->second) {
+                Extra x{(uint32_t)b.changes.size(), pos, start_op, false, std::string()};
+                canon(op, x.op);
+                b.extras.push_back(std::move(x));
+                continue;
+            }
             const JV* id = op.get(u"opId"); const JV* act = op.get(u"action");
             uint64_t ctr; u16s actor;
             if (!id || id->t != JV::Str || !parse_opid(id->s, ctr, actor)) { b.err = "Invalid operation ID"; return false; }
             if (!act || act->t != JV::Str) { b.err = "op without action"; return false; }
             const int ai = b.actor_of(actor);
             b.max_ctr = std::max(b.max_ctr, ctr);
-            C.n_ops++;
+            if (C.n_ops++ == 0) first_ctr = ctr;
             auto elem = [&](const JV* e, uint64_t& c, int& a) -> bool {       // elemId -> (ctr, actor); false: HEAD / absent
                 if (!e || e->t != JV::Str || e->s == u"_head") return false;
                 u16s ea; if (!parse_opid(e->s, c, ea)) { b.err = "Invalid operation ID"; return false; }
@@ -290,6 +307,9 @@ bool build_log(const JV& root, LogB& b) {
                 b.insdel.push_back(r);
             } else { b.err = "unsupported action on a list"; return false; }               // src/micromerge.ts:567
         }
+        // a change whose ops cannot say its startOp keeps it in an entry without an op
+        if (b.extras.size() == ex0 && have_start && (C.n_ops == 0 || first_ctr != start_op))
+            b.extras.push_back(Extra{(uint32_t)b.changes.size(), 0, start_op, true, std::string()});
         b.changes.push_back(std::move(C));
     }
     return true;
@@ -304,6 +324,8 @@ struct pt_ingest {
     // pools: concatenated bytes + offsets
     struct Pool { std::vector<uint8_t> data; std::vector<uint64_t> off{0}; void add(const void* p, size_t n) { data.insert(data.end(), (const uint8_t*)p, (const uint8_t*)p + n); off.push_back(data.size()); } void clear() { data.clear(); off.assign(1, 0); } };
     Pool values, links, comments, comment_attrs, actors, counters;   // actors / counters: per log ranges via *_first
+    Pool list_ids, extra_ops;                                        // one entry per log; one per extra with an op
+    std::vector<pt_change_extra> extras;
     std::vector<uint64_t> actors_first{0}, counters_first{0};
 };
 
@@ -341,6 +363,7 @@ int pt_ingest_parse(pt_ingest* g, const char* const* logs_json, const uint64_t* 
     for (uint32_t i = 0; i < n_logs; i++) if (!B[i].err.empty()) { g->err = "log " + std::to_string(i) + ": " + B[i].err; return PT_ERR_INVALID; }
     // merge the local pools in log order (first-appearance order over the whole batch, as the sequential packer does)
     g->values.clear(); g->links.clear(); g->comments.clear(); g->comment_attrs.clear(); g->actors.clear(); g->counters.clear();
+    g->list_ids.clear(); g->extra_ops.clear(); g->extras.clear();
     g->actors_first.assign(1, 0); g->counters_first.assign(1, 0);
     std::unordered_map<std::string, uint32_t> vix, lix; std::map<u16s, uint32_t> cset; std::vector<std::string> cattr_of;
     std::vector<std::vector<uint32_t>> vmap(n_logs), lmap(n_logs);
@@ -406,6 +429,12 @@ int pt_ingest_parse(pt_ingest* g, const char* const* logs_json, const uint64_t* 
             o.seq = c.seq; o.actor = (uint16_t)rank[c.actor]; o.n_deps = (uint16_t)c.deps.size(); o.dep_off = CD.n_deps; o.n_ops = c.n_ops;
             for (auto& d : c.deps) { pt_dep_rec& q = g->deps[dpo++]; q.seq = d.second; q.actor = (uint16_t)rank[d.first]; q.reserved = 0; CD.n_deps++; }
         }
+        g->list_ids.add(b.list_id.data(), b.list_id.size() * 2);
+        for (auto& x : b.extras) {
+            uint64_t op = PT_EXTRA_NONE;
+            if (!x.none) { op = g->extra_ops.off.size() - 1; g->extra_ops.add(x.op.data(), x.op.size()); }
+            g->extras.push_back(pt_change_extra{i, x.change, x.pos, 0, x.start_op, op});
+        }
     }
     return PT_OK;
 }
@@ -420,10 +449,17 @@ int pt_ingest_packed(pt_ingest* g, pt_packed_ops* ops, pt_change_table* ch) {
 int pt_ingest_pool(pt_ingest* g, int kind, const uint8_t** data, const uint64_t** offsets, uint64_t* count, const uint64_t** per_log_first) {
     if (!g || !data || !offsets || !count) return PT_ERR_INVALID;
     pt_ingest::Pool* p = kind == PT_POOL_VALUES ? &g->values : kind == PT_POOL_LINK_ATTRS ? &g->links : kind == PT_POOL_COMMENT_IDS ? &g->comments
-                       : kind == PT_POOL_COMMENT_ATTRS ? &g->comment_attrs : kind == PT_POOL_ACTORS ? &g->actors : kind == PT_POOL_COUNTERS ? &g->counters : nullptr;
+                       : kind == PT_POOL_COMMENT_ATTRS ? &g->comment_attrs : kind == PT_POOL_ACTORS ? &g->actors : kind == PT_POOL_COUNTERS ? &g->counters
+                       : kind == PT_POOL_LIST_IDS ? &g->list_ids : kind == PT_POOL_EXTRA_OPS ? &g->extra_ops : nullptr;
     if (!p) return PT_ERR_INVALID;
     *data = p->data.data(); *offsets = p->off.data(); *count = p->off.size() - 1;
     if (per_log_first) *per_log_first = kind == PT_POOL_ACTORS ? g->actors_first.data() : kind == PT_POOL_COUNTERS ? g->counters_first.data() : nullptr;
+    return PT_OK;
+}
+
+int pt_ingest_change_extras(pt_ingest* g, const pt_change_extra** out, uint64_t* n) {
+    if (!g || !out || !n) return PT_ERR_INVALID;
+    *out = g->extras.data(); *n = g->extras.size();
     return PT_OK;
 }
 

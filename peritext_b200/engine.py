@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-from .packing import (CDESC_DT, CHANGE_DT, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
+from .packing import (CDESC_DT, CHANGE_DT, CLOCK_DT, CHANGES_REQUEST_DT, EXTRA_DT, ChangeExtras, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
                       RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -22,7 +22,7 @@ EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_com
            "pt_batch_append", "pt_batch_change", "pt_batch_exchange", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
-           "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
+           "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_render_changes_json", "pt_ingest_change_extras", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
 
 
 class EngineError(RuntimeError):
@@ -161,6 +161,19 @@ class _JsonView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("off", ctypes.c_void_p), ("bytes", ctypes.c_void_p), ("n_bytes", ctypes.c_uint64)]
 
 
+class _ChangesJsonInput(ctypes.Structure):
+    _fields_ = [("n_requests", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("requests", ctypes.c_void_p), ("clock", ctypes.c_void_p),
+                ("n_clock", ctypes.c_uint64), ("pools", _JsonPools), ("actors", ctypes.c_void_p), ("actors_off", ctypes.c_void_p),
+                ("actors_first", ctypes.c_void_p), ("counters", ctypes.c_void_p), ("counters_first", ctypes.c_void_p),
+                ("list_ids", ctypes.c_void_p), ("list_ids_off", ctypes.c_void_p), ("extras", ctypes.c_void_p), ("n_extras", ctypes.c_uint64),
+                ("extra_ops", ctypes.c_void_p), ("extra_ops_off", ctypes.c_void_p), ("n_extra_ops", ctypes.c_uint64)]
+
+
+class _ChangesJsonView(ctypes.Structure):
+    _fields_ = [("n_requests", ctypes.c_uint32), ("off", ctypes.c_void_p), ("bytes", ctypes.c_void_p), ("n_bytes", ctypes.c_uint64),
+                ("status", ctypes.c_void_p)]
+
+
 QUERY_DT = np.dtype([("log", "<u4"), ("index", "<u4"), ("flags", "<u4"), ("reserved", "<u4")])
 PATCH_REC_DT = np.dtype([("index", "<u4"), ("flags", "<u4"), ("link_attr", "<u4"), ("reserved", "<u4")])
 PATCH_ITEM_DT = np.dtype([("log", "<u4"), ("tag", "<u4"), ("a", "<u4"), ("b", "<u4")])
@@ -212,6 +225,8 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_find_elements.argtypes = [vp, vp, u32, vp]
     L.pt_batch_render_json.argtypes = [vp, vp, vp]
     L.pt_batch_render_patches_json.argtypes = [vp, vp, vp]
+    L.pt_batch_render_changes_json.argtypes = [vp, vp, vp]
+    L.pt_ingest_change_extras.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u64)]
     L.pt_batch_destroy.argtypes = [vp]; L.pt_batch_destroy.restype = None
     L.pt_strerror.argtypes = [ctypes.c_int]; L.pt_strerror.restype = ctypes.c_char_p
     L.pt_last_error.restype = ctypes.c_char_p
@@ -570,6 +585,43 @@ class BatchEngine:
         """``render_patches_json`` as one bytes object per log."""
         return self._split(*self.render_patches_json(batch, pools))
 
+    def render_changes_json(self, batch: PackedBatch, requests, extras: ChangeExtras | None = None, pools=None):
+        """Change objects of resident logs as UTF-8 JSON text rendered on the device (pt_batch_render_changes_json; needs a change
+        table, no merge).  ``requests``: a CHANGES_REQUEST_DT array of RANGE requests (``packing.range_requests``), or the
+        (requests, CLOCK_DT clock) pair of ``packing.clock_requests``.  ``batch`` = the batch the handle holds (its actor, counter
+        and list-id tables); ``extras`` = the ``ChangeExtras`` of its changes (None: the list-op projection); ``pools`` as for
+        ``render_json``.  Returns (uint8 bytes, uint64 offsets [n_requests + 1], uint32 status per request): request r is
+        bytes[off[r]:off[r+1]], a Change[] array, empty for a request whose status is not CHANGES_OK."""
+        from .packing import json_pools, string_pools
+        req, clock = requests if isinstance(requests, tuple) else (requests, np.zeros(0, CLOCK_DT))
+        req = np.ascontiguousarray(req, CHANGES_REQUEST_DT); clock = np.ascontiguousarray(clock, CLOCK_DT)
+        p = json_pools(batch) if pools is None else pools
+        jp = [np.ascontiguousarray(a, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, a in enumerate(p)]
+        sp = string_pools(batch)
+        ex = extras if extras is not None else ChangeExtras(np.zeros(0, EXTRA_DT), [])
+        rows = np.ascontiguousarray(ex.rows, EXTRA_DT)
+        xdata, xoff = ex.pools()
+        keep = [req, clock, jp, sp, rows, xdata, xoff]
+        ptr = lambda a: a.ctypes.data if a.size else None
+        st = _JsonPools(ptr(jp[0]), ptr(jp[1]), max(0, len(jp[1]) - 1), ptr(jp[2]), ptr(jp[3]), max(0, len(jp[3]) - 1),
+                        ptr(jp[4]), ptr(jp[5]), max(0, len(jp[5]) - 1))
+        inp = _ChangesJsonInput(len(req), 0, ptr(req), ptr(clock), len(clock), st, ptr(sp["actors"]), ptr(sp["actors_off"]), ptr(sp["actors_first"]),
+                                ptr(sp["counters"]), ptr(sp["counters_first"]), ptr(sp["list_ids"]), ptr(sp["list_ids_off"]),
+                                ptr(rows), len(rows), ptr(xdata), ptr(xoff), len(ex.ops))
+        v = _ChangesJsonView()
+        _check(self._L.pt_batch_render_changes_json(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_render_changes_json")
+        del keep
+        nr = len(req)
+        off = np.frombuffer((ctypes.c_char * ((nr + 1) * 8)).from_address(v.off), np.uint64).copy()
+        data = np.frombuffer((ctypes.c_char * v.n_bytes).from_address(v.bytes), np.uint8).copy() if v.n_bytes else np.zeros(0, np.uint8)
+        status = np.frombuffer((ctypes.c_char * (nr * 4)).from_address(v.status), np.uint32).copy() if nr else np.zeros(0, np.uint32)
+        return data, off, status
+
+    def render_changes_json_list(self, batch: PackedBatch, requests, extras: ChangeExtras | None = None, pools=None) -> list[bytes]:
+        """``render_changes_json`` as one bytes object per request."""
+        data, off, _ = self.render_changes_json(batch, requests, extras, pools)
+        return self._split(data, off)
+
     def set_comment_pool(self, entries: int):
         _check(self._L.pt_batch_set_comment_pool(self._h, int(entries)), "pt_batch_set_comment_pool")
 
@@ -661,6 +713,17 @@ def pack_logs_native(logs_json, threads: int = 0) -> PackedBatch:
     """Native (C++, multithreaded) wire-format ingest: ``logs_json[i]`` = JSON text (str or bytes) of the Change objects
     replica i applied, in arrival order -> PackedBatch with its change table (csrc/ingest.cpp, pt_ingest_*).  Packs exactly
     like ``packing.pack_logs(..., with_changes=True)``."""
+    return _ingest(logs_json, threads)[0]
+
+
+def ingest_native(logs_json, threads: int = 0):
+    """``pack_logs_native`` plus what ``render_changes_json`` needs to give the logs back exactly: returns (PackedBatch with
+    ``log_lists`` set from the list-id pool, its ``ChangeExtras`` (pt_ingest_change_extras and the extra-ops pool), the raw
+    pools {kind: (bytes, u64 offsets, u64 per-log first or None)} of every PT_POOL_* kind 0-7)."""
+    return _ingest(logs_json, threads, with_extras=True)
+
+
+def _ingest(logs_json, threads: int = 0, with_extras: bool = False):
     import json
     L = load_library()
     blobs = [s.encode("utf-8", "surrogatepass") if isinstance(s, str) else bytes(s) for s in logs_json]
@@ -703,7 +766,20 @@ def pack_logs_native(logs_json, threads: int = 0) -> PackedBatch:
             c = counters[int(cfirst[i]): int(cfirst[i + 1])]
             log_counters.append(np.array([int.from_bytes(x, "little") for x in c], dtype=np.uint64) if c else None)
         table = ChangeTable(arr(tab.logs, tab.n_logs, CDESC_DT), arr(tab.changes, tab.n_changes_total, CHANGE_DT), arr(tab.deps, tab.n_deps_total, DEP_DT))
-        return PackedBatch(arr(ops.logs, ops.n_logs, DESC_DT), arr(ops.insdel, ops.n_insdel_total, INSDEL_DT), arr(ops.marks, ops.n_mark_total, MARK_DT),
-                           values, link_attrs, comment_attrs, [], log_actors=log_actors, log_counters=log_counters, changes=table)
+        batch = PackedBatch(arr(ops.logs, ops.n_logs, DESC_DT), arr(ops.insdel, ops.n_insdel_total, INSDEL_DT), arr(ops.marks, ops.n_mark_total, MARK_DT),
+                            values, link_attrs, comment_attrs, [], log_actors=log_actors, log_counters=log_counters, changes=table)
+        if not with_extras:
+            return batch, None, None
+        raw = {}
+        for kind in range(8):
+            data, off, cnt, first = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_void_p()
+            _check(L.pt_ingest_pool(h, kind, ctypes.byref(data), ctypes.byref(off), ctypes.byref(cnt), ctypes.byref(first)), "pt_ingest_pool")
+            o = arr(off.value, cnt.value + 1, np.uint64)
+            raw[kind] = (bytes(arr(data.value, int(o[-1]), np.uint8)) if cnt.value else b"", o, arr(first.value, n + 1, np.uint64) if first.value else None)
+        batch.log_lists = [u16(x) or None for x in pool(6)[0]]
+        xp, xn = ctypes.c_void_p(), ctypes.c_uint64()
+        _check(L.pt_ingest_change_extras(h, ctypes.byref(xp), ctypes.byref(xn)), "pt_ingest_change_extras")
+        extras = ChangeExtras(arr(xp.value, xn.value, EXTRA_DT), [b.decode("utf-8", "surrogatepass") for b in pool(7)[0]])
+        return batch, extras, raw
     finally:
         L.pt_ingest_destroy(h)

@@ -1411,3 +1411,130 @@ def change_dicts(batch: PackedBatch, changes: Sequence[dict | None], actor_ranks
                 ops.append(body)
         out.append({"actor": me, "seq": ch["seq"], "deps": dict(ch["deps"]), "startOp": ch["startOp"], "ops": ops})
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Changes as JSON (include/peritext_b200.h pt_batch_render_changes_json)
+# ------------------------------------------------------------------------------------------------------------------
+EXTRA_DT = np.dtype([("log", "<u4"), ("change", "<u4"), ("pos", "<u4"), ("reserved", "<u4"), ("start_op", "<u8"), ("op", "<u8")])
+CHANGES_REQUEST_DT = np.dtype([("log", "<u4"), ("mode", "<u4"), ("first", "<u4"), ("count", "<u4"), ("clock_off", "<u8"), ("n_clock", "<u4"),
+                               ("reserved", "<u4")])
+CLOCK_DT = np.dtype([("actor", "<u4"), ("seq", "<u4")])
+assert EXTRA_DT.itemsize == 32 and CHANGES_REQUEST_DT.itemsize == 32
+EXTRA_NONE = 0xFFFFFFFFFFFFFFFF
+CHANGES_RANGE, CHANGES_MISSING = 0, 1
+CHANGES_OK, CHANGES_BAD_TABLE = 0, 1
+
+
+@dataclass
+class ChangeExtras:
+    """What the packed records lose of each change (pt_change_extra): one row per op that does not target the log's text list,
+    at its index in ``change.ops``, with the change's startOp; a row with op == EXTRA_NONE carries only the startOp of a change
+    that has no such op and either no list op or a startOp other than its first list op's counter.  ``ops[k]`` is the canonical
+    JSON (``canon``) of the op of rows whose op is k."""
+    rows: np.ndarray                                   # EXTRA_DT, sorted by (log, change, pos)
+    ops: list[str] = field(default_factory=list)
+
+    def pools(self) -> tuple[np.ndarray, np.ndarray]:
+        """The extra-ops pool as pt_ingest_pool kind 7 holds it: UTF-8 bytes and u64 offsets [count + 1]."""
+        return _pool([o.encode("utf-8", "surrogatepass") for o in self.ops])
+
+
+def join_extras(*parts: ChangeExtras) -> ChangeExtras:
+    """Several ChangeExtras as one (op indices re-based, rows sorted by (log, change, pos))."""
+    rows, ops = [], []
+    for p in parts:
+        r = p.rows.copy()
+        has = r["op"] != np.uint64(EXTRA_NONE)
+        r["op"][has] += np.uint64(len(ops))
+        rows.append(r); ops += p.ops
+    r = np.concatenate(rows + [np.zeros(0, EXTRA_DT)])
+    return ChangeExtras(r[np.lexsort((r["pos"], r["change"], r["log"]))], ops)
+
+
+def _extra_rows(li: int, ci: int, ops: Sequence[dict], start, is_list, rows: list, out_ops: list) -> None:
+    n0, first = len(rows), None
+    for pos, op in enumerate(ops):
+        if not is_list(op):
+            rows.append((li, ci, pos, 0, int(start or 0), len(out_ops)))
+            out_ops.append(canon(op))
+        elif first is None:
+            first = parse_op_id(op["opId"])[0]
+    if len(rows) == n0 and start is not None and (first is None or first != int(start)):
+        rows.append((li, ci, 0, 0, int(start), EXTRA_NONE))
+
+
+def change_extras(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] | None = None) -> tuple[ChangeExtras, list[str]]:
+    """The host specification of the native ingest's extras (pt_ingest_change_extras, pool PT_POOL_EXTRA_OPS) and of its list-id
+    pool (PT_POOL_LIST_IDS): (ChangeExtras of ``logs`` packed as ``pack_logs`` packs them, each log's text-list id or "")."""
+    rows, ops, lids = [], [], []
+    for li, changes in enumerate(logs):
+        lid = list_ids[li] if list_ids is not None and list_ids[li] is not None else _root_text_list(changes)
+        lids.append(lid or "")
+        for ci, ch in enumerate(changes):
+            _extra_rows(li, ci, ch["ops"], ch.get("startOp"), lambda op: lid is not None and op.get("obj") == lid, rows, ops)
+    return ChangeExtras(np.array(rows, EXTRA_DT) if rows else np.zeros(0, EXTRA_DT), ops), lids
+
+
+def input_extras(batch: PackedBatch, changes: Sequence[dict | None], actor_ranks, status: np.ndarray) -> ChangeExtras:
+    """The extras of the changes ``pt_batch_change`` generated from ``changes`` (as for ``change_inputs``; ``batch`` = the batch
+    before the call, with its change table; ``status`` = the call's rows): the ROOT-map InputOperations (path []) at their places
+    in ``change.ops``, so that ``render_changes_json`` of a log's new change gives exactly the Change object ``change_dicts``
+    returns.  A failed log, or one without a change, has no new change and no rows."""
+    rows, ops = [], []
+    for i, ch in enumerate(changes):
+        if ch is None or int(status[i]["status"]) != CHANGE_OK:
+            continue
+        me, ctr, body = batch.log_actors[i][int(actor_ranks[i])], int(ch["startOp"]), []
+        for inp in ch["ops"]:
+            if list(inp.get("path") or []) == []:
+                op = {"opId": f"{ctr}@{me}", "action": inp["action"], "obj": "_root", "key": inp["key"]}
+                if inp["action"] == "set":
+                    op["value"] = inp.get("value")
+                body.append(op); ctr += 1
+                continue
+            a = inp["action"]
+            gen = len(inp["values"]) if a == "insert" else max(0, inp["count"]) if a == "delete" else 1
+            body += [{"opId": f"{ctr + k}@{me}", "obj": None} for k in range(gen)]
+            ctr += gen
+        ci = int(batch.changes.desc[i]["n_changes"])
+        _extra_rows(i, ci, body, ch["startOp"], lambda op: "key" not in op, rows, ops)
+    return ChangeExtras(np.array(rows, EXTRA_DT) if rows else np.zeros(0, EXTRA_DT), ops)
+
+
+def range_requests(logs: Sequence[int], first: int = 0, count: int = 0xFFFFFFFF) -> np.ndarray:
+    """RANGE requests: changes [first, first + count) of each log's table (default: the whole table)."""
+    req = np.zeros(len(logs), CHANGES_REQUEST_DT)
+    req["log"] = np.asarray(logs, np.uint32) if len(logs) else 0
+    req["mode"] = CHANGES_RANGE; req["first"] = first; req["count"] = count
+    return req
+
+
+def clock_requests(batch: PackedBatch, logs: Sequence[int], clocks: Sequence[dict]) -> tuple[np.ndarray, np.ndarray]:
+    """MISSING requests: what a peer whose clock is ``clocks[k]`` ({actorId: seq}) is missing from log ``logs[k]``.  Actor ids
+    become the log's ranks; an actor the log does not know is dropped (it has no change there to send).  Returns (requests,
+    CLOCK_DT entries)."""
+    req = np.zeros(len(logs), CHANGES_REQUEST_DT)
+    entries = []
+    for k, (log, clock) in enumerate(zip(logs, clocks)):
+        rank = {a: r for r, a in enumerate(batch.log_actors[int(log)])}
+        e = [(rank[a], int(s)) for a, s in clock.items() if a in rank]
+        req[k] = (int(log), CHANGES_MISSING, 0, 0, len(entries), len(e), 0)
+        entries += e
+    return req, np.array(entries, CLOCK_DT) if entries else np.zeros(0, CLOCK_DT)
+
+
+def string_pools(batch: PackedBatch) -> dict:
+    """The per-log string pools of ``pt_batch_render_changes_json`` from a PackedBatch (the layouts of pt_ingest_pool kinds 4, 5
+    and 6): actors (UTF-16LE, byte offsets, u64 first [n_logs + 1]), counters (u64 entries, first [n_logs + 1]) and list ids."""
+    n = batch.n_logs
+    actors = [a.encode("utf-16-le", "surrogatepass") for acts in (batch.log_actors or [[]] * n) for a in acts]
+    afirst = np.zeros(n + 1, np.uint64)
+    afirst[1:] = np.cumsum([len(acts) for acts in (batch.log_actors or [[]] * n)], dtype=np.uint64)
+    counters = [np.zeros(0, np.uint64) if c is None else np.asarray(c, np.uint64) for c in (batch.log_counters or [None] * n)]
+    cfirst = np.zeros(n + 1, np.uint64)
+    cfirst[1:] = np.cumsum([len(c) for c in counters], dtype=np.uint64)
+    lids = _pool([(l or "").encode("utf-16-le", "surrogatepass") for l in (batch.log_lists or [""] * n)])
+    a = _pool(actors)
+    return {"actors": a[0], "actors_off": a[1], "actors_first": afirst, "counters": np.concatenate(counters + [np.zeros(0, np.uint64)]),
+            "counters_first": cfirst, "list_ids": lids[0], "list_ids_off": lids[1]}
