@@ -572,6 +572,99 @@ typedef struct pt_exchange_view {
  * Peak device memory: old + delta + new records and change tables, plus 40 B of scratch per change of every pair's src. */
 int pt_batch_exchange(pt_batch*, const pt_exchange_input* in, pt_exchange_view* out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Actor tables: each log's actor ids on the device, so that a sync step derives pt_batch_exchange's maps and its pre-append
+ * there (pt_batch_sync_pairs) and the caller needs no host copy of the records.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_actor_tables {
+    uint32_t n_logs;
+    const uint8_t* data; const uint64_t* off; uint64_t count;   /* PT_POOL_ACTORS: UTF-16LE ids, byte offsets [count + 1]       */
+    const uint64_t* per_log_first;                              /* [n_logs + 1] log i's ids are per_log_first[i] .. [i + 1]     */
+    const uint64_t* counters_first;                             /* [n_logs + 1] PT_POOL_COUNTERS ranges, or NULL: a non-empty
+                                                                   range marks a log whose counters were re-ranked densely      */
+} pt_actor_tables;
+
+/* Attach the batch's per-log actor ids: pt_ingest_pool's PT_POOL_ACTORS (and PT_POOL_COUNTERS' per-log ranges) or
+ * packing.string_pools pass straight through.  Of counters_first the handle keeps one bit per log.
+ * Refused with PT_ERR_INVALID, pt_last_error naming the first bad log: n_logs differs; per_log_first does not run from 0 to
+ * count or decreases; a log's count is not its n_actors (0 is allowed only when n_actors == 1); an id of odd byte length; ids
+ * not strictly increasing in UTF-16 code-unit order (JS string order, compareOpIds).  No batch: PT_ERR_STATE.
+ * Lifetime: every upload form and pt_batch_adopt_device drop the tables (as they drop the change table); pt_batch_change and
+ * pt_batch_exchange keep them; pt_batch_append keeps them only when its remap has no actor map, no counter map and no log's
+ * n_actors changes (a comment-only remap keeps them).  Synchronises; the caller's arrays may be freed on return. */
+int pt_batch_upload_actors(pt_batch*, const pt_actor_tables* tables);
+
+/* The current tables in the PT_POOL_ACTORS layout (counters_first = NULL): the `actors` pool pt_batch_render_changes_json
+ * takes.  No tables: PT_ERR_STATE.  Synchronises.  The view is engine-owned pinned memory, valid until the next call of it,
+ * upload or destroy. */
+int pt_batch_download_actors(pt_batch*, pt_actor_tables* out);
+
+/* Introduce actor ids per log, in any order (duplicates and ids the log knows allowed): the acting actor before its first
+ * pt_batch_change on a replica, for example.  Each log's table becomes the sorted union and its n_actors max(1, count).
+ * Where a rank moves or an n_actors grows, the records, change records and dep records go through pt_batch_append's splice
+ * with the derived actor maps (an empty delta, counters untouched): the handle then holds exactly what pt_batch_append of
+ * packing.add_actors' delta and remap gives, with no merge (the patch window is reset, pools persist).  Otherwise the batch
+ * and its last merge are untouched.  View (engine-owned pinned memory, valid until the next call of it, upload or destroy):
+ * the rank of every given id after the call, and the per-log old -> new actor maps (empty range: unchanged), so the caller
+ * can move its own rank-indexed data.  Refused: no batch or no actor tables (PT_ERR_STATE); n_logs differs, per_log_first
+ * not from 0 to count or decreasing, an id of odd byte length, a log that would have more than 65535 actors, and what
+ * pt_batch_append refuses (PT_ERR_INVALID, nothing changed).  Synchronises; the caller's arrays may be freed on return.
+ * Device: one warp per log sorts and deduplicates its ids by counting (O(m^2) compares for a log given m ids), the merge
+ * kernel of pt_batch_sync_pairs writes the grown tables, then the splice and a rank kernel. */
+typedef struct pt_actor_input {
+    uint32_t n_logs;
+    const uint8_t* data; const uint64_t* off; uint64_t count;   /* UTF-16LE ids, byte offsets [count + 1]                         */
+    const uint64_t* per_log_first;                              /* [n_logs + 1] log i's ids are per_log_first[i] .. [i + 1]       */
+} pt_actor_input;
+typedef struct pt_actor_view {
+    uint32_t n_logs; uint64_t count;
+    const uint16_t* rank;          /* [count] each given id's rank in its log after the call                                  */
+    const uint64_t* actor_off;     /* [n_logs + 1] per-log old -> new actor rank maps; empty range: unchanged                 */
+    const uint16_t* actor_map;
+    uint32_t spliced;              /* 1: the splice ran (the batch needs a merge, the patch window was reset)                 */
+} pt_actor_view;
+int pt_batch_add_actors(pt_batch*, const pt_actor_input* in, pt_actor_view* out);
+
+#define PT_EXCHANGE_DENSE 4u      /* pt_batch_sync_pairs only: src or dst is densely ranked, or dst would be once grown; the
+                                     pair delivers nothing and dst does not grow (exchange it with caller maps instead)        */
+typedef struct pt_sync_view {
+    uint32_t n_pairs;
+    const uint32_t* status;        /* [n_pairs] PT_EXCHANGE_*, PT_EXCHANGE_DENSE included                                     */
+    const uint64_t* delivered_off; /* [n_pairs + 1]  as pt_exchange_view                                                       */
+    const uint32_t* delivered;
+    const pt_log_desc* delta;      /* [n_logs]                                                                                 */
+    const uint64_t* actor_off;     /* [n_logs + 1] the pre-append's per-log old -> new actor rank maps (empty range: unchanged) */
+    const uint16_t* actor_map;
+} pt_sync_view;
+
+/* pt_batch_exchange with its maps and its pre-append derived on the device from the actor tables (pt_batch_upload_actors).
+ * (Named pt_batch_sync_pairs because pt_batch_sync already names the stream synchronisation above.)  The caller sends only
+ * the pairs.  The pair rules, the refusals of the pairs and "every pair reads the batch as it is before
+ * the call" are pt_batch_exchange's.  Per pair:
+ *   1. missing  src's changes whose seq exceeds dst's count of the same actor ID (the two tables joined by name).
+ *   2. named    the src actors those changes name: the change actor, dep actors, and the actor of every ins/del and mark
+ *               record id whose counter is non-zero; and the top opId counter and the op count of their records.
+ *   3. growth   dst's table becomes the sorted union (packing._grown_ids).  If src or dst is densely ranked, or the grown dst
+ *               would be (packing._wants_dense of max(dst max_ctr, top) and dst's ops + the missing ops), the pair is
+ *               PT_EXCHANGE_DENSE: it delivers nothing and dst does not grow.
+ *   4. pre      if a dst's ranks move or its n_actors grows, one pt_batch_append splice of an empty delta applies every pair's
+ *               growth (derived before any is applied, so {A->B, B->A} sees both logs grown), identity counters.
+ *   5. maps     src rank -> dst rank of the same name in the grown tables (0xFFFF for a rank without a name or an image);
+ *               identity counter maps.
+ *   6. exchange pt_batch_exchange's select, gather and splice with those maps; STUCK / BAD_TABLE / UNMAPPED as there.
+ * Afterwards the handle and the tables equal packing.sync_maps' exchange_maps of the pairs that are not DENSE, then
+ * apply_append of its pre-append, then apply_exchange.  A refusal of the delivery's splice after a pre-append leaves the
+ * pre-append applied.
+ * Refused: PT_ERR_STATE without a batch, change table or actor tables; PT_ERR_INVALID for null arguments, the pair rules of
+ * pt_batch_exchange, a log that would have more than 65535 actors, and what pt_batch_append refuses.
+ * n_pairs == 0: PT_OK, nothing launched.  Synchronises.  The view is engine-owned pinned memory, valid until the next
+ * upload, append, change, exchange, sync or destroy.
+ * Device: a derive kernel (one warp per pair; clocks, the name join and a bitmap over src ranks in shared memory, the missing
+ * records read by the whole warp), a merge kernel (one warp per log) writing the grown tables and the rank maps, the splice,
+ * a map kernel (one warp per pair), then pt_batch_exchange's kernels.  Besides the pairs, 32 B per pair and the moved logs'
+ * rank maps cross PCIe. */
+int pt_batch_sync_pairs(pt_batch*, const pt_exchange_pair* pairs, uint32_t n_pairs, pt_sync_view* out);
+
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */
 int pt_batch_merge(pt_batch*);

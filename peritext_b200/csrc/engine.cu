@@ -28,6 +28,7 @@
 #include "scan_kernel.cuh"
 #include "admit_kernel.cuh"
 #include "query_kernel.cuh"
+#include "sync_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -131,6 +132,15 @@ struct pt_batch {
     HostBuf h_stage, h_results, h_text, h_spans, h_pool, h_misc, h_seq, h_ctoff, h_csoff;
     HostBuf h_chg_status, h_chg_desc, h_chg_insdel, h_chg_marks;   // the view of the last pt_batch_change
     HostBuf h_xch_totals, h_xch_status, h_xch_off, h_xch_delivered, h_xch_desc;   // the view of the last pt_batch_exchange
+    // pt_batch_upload_actors: each log's actor ids in the PT_POOL_ACTORS layout, and per log its first id and first byte
+    // ([n_logs + 1]) and whether its counters were re-ranked densely
+    bool have_actors = false;
+    DevBuf d_anames, d_aoff, d_afirst;
+    std::vector<uint64_t> h_afirst, h_abyte;
+    std::vector<char> h_adense;
+    HostBuf h_act_data, h_act_off, h_act_first;                          // the view of pt_batch_download_actors
+    HostBuf h_syn_totals, h_syn_status, h_syn_off, h_syn_aoff, h_syn_amap;   // the view of the last pt_batch_sync_pairs
+    HostBuf h_add_totals, h_add_rank, h_add_aoff, h_add_amap;               // the view of the last pt_batch_add_actors
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -367,7 +377,7 @@ int install_plan(pt_batch* b, const pt_packed_ops& ops, ptp::Plan&& plan, bool o
 int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
     PT_CUDA(cudaSetDevice(b->device));
     PT_CUDA(cudaStreamSynchronize(b->stream));
-    b->have_batch = false; b->merged = false; b->dl_begun = false; b->have_changes = false;
+    b->have_batch = false; b->merged = false; b->dl_begun = false; b->have_changes = false; b->have_actors = false;
     drop_graph(b);
     ptp::Plan plan;
     if (const char* err = ptp::make_plan(ops, b->limits, b->num_sms, plan)) { g_last_error = err; return PT_ERR_INVALID; }
@@ -863,6 +873,10 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
     PT_CUDA(cudaStreamSynchronize(b->stream));              // also: the caller's arrays may be freed on return
     if (bad) { g_last_error = std::string(fn) + "a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
     // Accepted: the new records and change table replace the old ones (freed with the locals), and the batch is re-planned.
+    // The actor tables stay only while no log's actor set can have changed: no actor or counter map, every n_actors kept.
+    bool keep_actors = !(R.actor_off && R.actor_off[n] > R.actor_off[0]) && !(R.ctr_off && R.ctr_off[n] > R.ctr_off[0]);
+    for (uint32_t i = 0; keep_actors && i < n; i++) keep_actors = nd[i].n_actors == b->h_desc[i].n_actors;
+    b->have_actors = b->have_actors && keep_actors;
     b->have_batch = false; b->merged = false; b->dl_begun = false;
     drop_graph(b);
     b->d_insdel.swap(nins); b->d_marks.swap(nmarks);
@@ -1031,9 +1045,22 @@ int pt_batch_change(pt_batch* b, const pt_change_input* in, const pt_change_tabl
 
 // pt_batch_exchange's host checks of the pairs and their maps (include/peritext_b200.h).  On success slot_off holds each
 // pair's scratch slot (exclusive scan of its src's n_changes).  Returns the problem, or an empty string.
+static std::string pair_at(uint32_t p) { return "pair " + std::to_string(p) + ": "; }   // an error's prefix
+
+// The rules every pair of pt_batch_exchange and pt_batch_sync_pairs follows: both logs in the batch, src != dst, no dst named
+// twice (is_dst: the dsts of the earlier pairs).  Returns the problem, or an empty string.
+static std::string check_pair(const pt_batch* b, uint32_t p, pt_exchange_pair pr, std::vector<char>& is_dst) {
+    const uint32_t n = b->n_logs, src = pr.src, dst = pr.dst;
+    if (src >= n || dst >= n) return pair_at(p) + "log " + std::to_string(src >= n ? src : dst) + " is outside the batch's " + std::to_string(n) + " logs";
+    if (src == dst) return pair_at(p) + "src and dst are both log " + std::to_string(src);
+    if (is_dst[dst]) return pair_at(p) + "log " + std::to_string(dst) + " is the dst of an earlier pair";
+    is_dst[dst] = 1;
+    return std::string();
+}
+
 static std::string check_exchange(const pt_batch* b, const pt_exchange_input& in, std::vector<unsigned long long>& slot_off) {
     const uint32_t n = b->n_logs, np = in.n_pairs;
-    auto at = [](uint32_t p) { return "pair " + std::to_string(p) + ": "; };
+    auto at = pair_at;
     if (!in.pairs || !in.actor_off) return "null pairs or actor_off";
     if (in.actor_off[np] > in.actor_off[0] && !in.actor_map) return "null actor_map with a nonzero length";
     if (in.ctr_off && in.ctr_off[np] > in.ctr_off[0] && !in.ctr_map) return "null ctr_map with a nonzero length";
@@ -1041,10 +1068,8 @@ static std::string check_exchange(const pt_batch* b, const pt_exchange_input& in
     slot_off.assign((size_t)np + 1, 0);
     for (uint32_t p = 0; p < np; p++) {
         const uint32_t src = in.pairs[p].src, dst = in.pairs[p].dst;
-        if (src >= n || dst >= n) return at(p) + "log " + std::to_string(src >= n ? src : dst) + " is outside the batch's " + std::to_string(n) + " logs";
-        if (src == dst) return at(p) + "src and dst are both log " + std::to_string(src);
-        if (is_dst[dst]) return at(p) + "log " + std::to_string(dst) + " is the dst of an earlier pair";
-        is_dst[dst] = 1;
+        std::string e = check_pair(b, p, in.pairs[p], is_dst);
+        if (!e.empty()) return e;
         if (in.actor_off[p + 1] < in.actor_off[p]) return "actor_off decreases";
         const uint64_t na = in.actor_off[p + 1] - in.actor_off[p];
         if (na != b->h_desc[src].n_actors)
@@ -1069,15 +1094,25 @@ static std::string check_exchange(const pt_batch* b, const pt_exchange_input& in
     return std::string();
 }
 
+static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pairs, uint32_t np, const std::vector<unsigned long long>& slot_off,
+                         const unsigned long long* actor_off, const uint16_t* actor_map, const unsigned long long* ctr_off, const uint32_t* ctr_map,
+                         pt_exchange_view* out);
+
+// The pinned buffers of an exchange view for np pairs.
+static int reserve_exchange_view(pt_batch* b, uint32_t np) {
+    int rc;
+    if ((rc = reserve_n<ptx::PairTotals>(b->h_xch_totals, np)) || (rc = reserve_n<uint32_t>(b->h_xch_status, np)) ||
+        (rc = reserve_n<uint64_t>(b->h_xch_off, (uint64_t)np + 1)) || (rc = reserve_n<pt_log_desc>(b->h_xch_desc, b->n_logs))) return rc;
+    return PT_OK;
+}
+
 int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view* out) {
     if (!b || !in || !out) { g_last_error = "pt_batch_exchange: null argument"; return PT_ERR_INVALID; }
     if (!b->have_batch) { g_last_error = "pt_batch_exchange before pt_batch_upload"; return PT_ERR_STATE; }
     if (!b->have_changes) { g_last_error = "pt_batch_exchange: the handle has no change table"; return PT_ERR_STATE; }
     const uint32_t n = b->n_logs, np = in->n_pairs;
     int rc;
-    if ((rc = reserve_n<ptx::PairTotals>(b->h_xch_totals, np)) || (rc = reserve_n<uint32_t>(b->h_xch_status, np)) ||
-        (rc = reserve_n<uint64_t>(b->h_xch_off, (uint64_t)np + 1)) || (rc = reserve_n<pt_log_desc>(b->h_xch_desc, n))) return rc;
-    ptx::PairTotals* tot = (ptx::PairTotals*)b->h_xch_totals.p;
+    if ((rc = reserve_exchange_view(b, np))) return rc;
     uint32_t* status = (uint32_t*)b->h_xch_status.p;
     uint64_t* doff = (uint64_t*)b->h_xch_off.p;
     pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
@@ -1093,21 +1128,37 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     std::vector<unsigned long long> slot_off;
     std::string err = check_exchange(b, *in, slot_off);
     if (!err.empty()) { g_last_error = "pt_batch_exchange: " + err; return PT_ERR_INVALID; }
-    const uint64_t n_slot = slot_off[np];
     PT_CUDA(cudaSetDevice(b->device));
     PT_CUDA(cudaStreamSynchronize(b->stream));
-    // the pairs, their maps and the select kernel's scratch: freed on return
-    DevBuf dpairs, daoff, damap, dcoff, dcmap, dslot, dqueue, dpos, ddlv, dtot, ddoff, dbase, dgi, dgm, dgc, dgd, dgx;
+    DevBuf daoff, damap, dcoff, dcmap;                          // the maps: freed on return
     const uint64_t n_amap = in->actor_off[np], n_cmap = in->ctr_off ? in->ctr_off[np] : 0;
-    if ((rc = upload_n(b, dpairs, in->pairs, np)) || (rc = upload_n(b, daoff, in->actor_off, (uint64_t)np + 1)) ||
-        (rc = upload_n(b, damap, in->actor_map, n_amap)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)np + 1)) ||
+    if ((rc = upload_n(b, daoff, in->actor_off, (uint64_t)np + 1)) || (rc = upload_n(b, damap, in->actor_map, n_amap))) return rc;
+    if (in->ctr_off && ((rc = upload_n(b, dcoff, in->ctr_off, (uint64_t)np + 1)) || (rc = upload_n(b, dcmap, in->ctr_map, n_cmap)))) return rc;
+    return exchange_core(b, "pt_batch_exchange: ", in->pairs, np, slot_off, (const unsigned long long*)daoff.p, (const uint16_t*)damap.p,
+                         in->ctr_off ? (const unsigned long long*)dcoff.p : nullptr, (const uint32_t*)dcmap.p, out);
+}
+
+// pt_batch_exchange after its host checks (pt_batch_sync_pairs after deriving its maps): the pairs (host memory) and their maps
+// (device memory; ctr_off null = identity), the scratch slots of check_exchange.  Writes the view into the h_xch_* buffers.
+static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pairs, uint32_t np, const std::vector<unsigned long long>& slot_off,
+                         const unsigned long long* actor_off, const uint16_t* actor_map, const unsigned long long* ctr_off, const uint32_t* ctr_map,
+                         pt_exchange_view* out) {
+    const uint32_t n = b->n_logs;
+    int rc;
+    ptx::PairTotals* tot = (ptx::PairTotals*)b->h_xch_totals.p;
+    uint32_t* status = (uint32_t*)b->h_xch_status.p;
+    uint64_t* doff = (uint64_t*)b->h_xch_off.p;
+    pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
+    const uint64_t n_slot = slot_off[np];
+    // the pairs and the select kernel's scratch: freed on return
+    DevBuf dpairs, dslot, dqueue, dpos, ddlv, dtot, ddoff, dbase, dgi, dgm, dgc, dgd, dgx;
+    if ((rc = upload_n(b, dpairs, pairs, np)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)np + 1)) ||
         (rc = reserve_n<uint32_t>(dqueue, n_slot)) || (rc = reserve_n<uint32_t>(dpos, n_slot)) ||
         (rc = reserve_n<ptx::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptx::PairTotals>(dtot, np))) return rc;
-    if (in->ctr_off && ((rc = upload_n(b, dcoff, in->ctr_off, (uint64_t)np + 1)) || (rc = upload_n(b, dcmap, in->ctr_map, n_cmap)))) return rc;
     ptx::ExchangeParams P{};
     P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = np; P.maxR = b->adm_maxR;
-    P.actor_off = (const unsigned long long*)daoff.p; P.actor_map = (const uint16_t*)damap.p;
-    P.ctr_off = in->ctr_off ? (const unsigned long long*)dcoff.p : nullptr; P.ctr_map = (const uint32_t*)dcmap.p;
+    P.actor_off = actor_off; P.actor_map = actor_map;
+    P.ctr_off = ctr_off; P.ctr_map = ctr_map;
     P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
     P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
     P.insdel = b->dp_insdel; P.marks = b->dp_marks;
@@ -1151,7 +1202,7 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     doff[0] = 0;
     for (uint32_t p = 0; p < np; p++) {
         status[p] = tot[p].status;
-        const uint32_t dst = in->pairs[p].dst, cnt = status[p] == PT_EXCHANGE_OK ? tot[p].n_changes : 0u;
+        const uint32_t dst = pairs[p].dst, cnt = status[p] == PT_EXCHANGE_OK ? tot[p].n_changes : 0u;
         if (cnt) {
             dd[dst] = pt_log_desc{base[p].insdel, base[p].mark, tot[p].n_insdel, tot[p].n_mark, b->h_desc[dst].n_actors, std::max(b->h_desc[dst].max_ctr, tot[p].max_ctr)};
             cdesc[dst] = pt_change_desc{base[p].change, base[p].dep, tot[p].n_changes, tot[p].n_deps};
@@ -1161,8 +1212,309 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     }
     const pt_packed_ops delta{n, dd, (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
     const pt_change_table ct{n, cdesc.data(), (const pt_change_rec*)dgc.p, n_ch, (const pt_dep_rec*)dgd.p, n_dp};
-    if ((rc = splice_append(b, "pt_batch_exchange: ", &delta, true, pt_append_remap{}, &ct, true))) return rc;
+    if ((rc = splice_append(b, fn, &delta, true, pt_append_remap{}, &ct, true))) return rc;
     *out = pt_exchange_view{np, status, doff, delivered, dd};
+    return PT_OK;
+}
+
+// UTF-16 code-unit order of two UTF-16LE strings (JS string order): <0, 0, >0.
+static int js_cmp_host(const uint8_t* a, uint64_t na, const uint8_t* b, uint64_t nb) {
+    for (uint64_t i = 0; i + 1 < std::min(na, nb); i += 2) {
+        const uint32_t x = a[i] | (uint32_t)a[i + 1] << 8, y = b[i] | (uint32_t)b[i + 1] << 8;
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return na < nb ? -1 : na > nb ? 1 : 0;
+}
+
+// pt_batch_upload_actors' host checks (include/peritext_b200.h).  Returns the problem, or an empty string.
+static std::string check_actor_tables(const pt_batch* b, const pt_actor_tables& t) {
+    const uint32_t n = b->n_logs;
+    if (t.n_logs != n) return "the tables have " + std::to_string(t.n_logs) + " logs and the batch " + std::to_string(n);
+    if (!t.per_log_first || !t.off) return "null per_log_first or off";
+    if (t.count && t.off[t.count] > t.off[0] && !t.data) return "null data with a nonzero length";
+    if (t.per_log_first[0] != 0 || t.per_log_first[n] != t.count) return "per_log_first does not run from 0 to count";
+    for (uint64_t k = 0; k < t.count; k++) if (t.off[k + 1] < t.off[k]) return "the byte offsets decrease at id " + std::to_string(k);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t lo = t.per_log_first[i], hi = t.per_log_first[i + 1];
+        if (hi < lo || hi > t.count) return at(i) + "per_log_first decreases or passes count";
+        const uint64_t cnt = hi - lo, R = b->h_desc[i].n_actors;
+        if (cnt != R && !(cnt == 0 && R == 1)) return at(i) + std::to_string(cnt) + " actor ids and n_actors " + std::to_string(R);
+        for (uint64_t k = lo; k < hi; k++) {
+            if ((t.off[k + 1] - t.off[k]) & 1) return at(i) + "actor " + std::to_string(k - lo) + " has an odd byte length";
+            if (k > lo && js_cmp_host(t.data + t.off[k - 1], t.off[k] - t.off[k - 1], t.data + t.off[k], t.off[k + 1] - t.off[k]) >= 0)
+                return at(i) + "actor " + std::to_string(k - lo) + " does not sort after actor " + std::to_string(k - lo - 1) + " (UTF-16 code-unit order)";
+        }
+        if (t.counters_first && t.counters_first[i + 1] < t.counters_first[i]) return at(i) + "counters_first decreases";
+    }
+    return std::string();
+}
+
+int pt_batch_upload_actors(pt_batch* b, const pt_actor_tables* t) {
+    if (!b || !t) { g_last_error = "pt_batch_upload_actors: null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_upload_actors before pt_batch_upload"; return PT_ERR_STATE; }
+    const std::string err = check_actor_tables(b, *t);
+    if (!err.empty()) { g_last_error = "pt_batch_upload_actors: " + err; return PT_ERR_INVALID; }
+    const uint32_t n = b->n_logs;
+    const uint64_t lo = t->count ? t->off[0] : 0, bytes = t->count ? t->off[t->count] - lo : 0;
+    std::vector<uint64_t> off(t->count + 1), abyte(n + 1);
+    for (uint64_t k = 0; k <= t->count; k++) off[k] = t->count ? t->off[k] - lo : 0;
+    for (uint32_t i = 0; i <= n; i++) abyte[i] = off[t->per_log_first[i]];
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    int rc;
+    if ((rc = upload_n(b, b->d_anames, bytes ? t->data + lo : nullptr, bytes)) || (rc = upload_n(b, b->d_aoff, off.data(), off.size())) ||
+        (rc = upload_n(b, b->d_afirst, t->per_log_first, (uint64_t)n + 1))) { b->have_actors = false; return rc; }
+    PT_CUDA(cudaStreamSynchronize(b->stream));            // the caller's arrays may be freed on return
+    b->h_afirst.assign(t->per_log_first, t->per_log_first + n + 1);
+    b->h_abyte = std::move(abyte);
+    b->h_adense.assign(n, 0);
+    for (uint32_t i = 0; t->counters_first && i < n; i++) b->h_adense[i] = t->counters_first[i + 1] > t->counters_first[i];
+    b->have_actors = true;
+    return PT_OK;
+}
+
+int pt_batch_download_actors(pt_batch* b, pt_actor_tables* out) {
+    if (!b || !out) { g_last_error = "pt_batch_download_actors: null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch || !b->have_actors) { g_last_error = "pt_batch_download_actors: the handle has no actor tables"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs;
+    const uint64_t count = b->h_afirst[n], bytes = b->h_abyte[n];
+    int rc;
+    if ((rc = reserve_n<uint8_t>(b->h_act_data, bytes)) || (rc = reserve_n<uint64_t>(b->h_act_off, count + 1)) ||
+        (rc = reserve_n<uint64_t>(b->h_act_first, (uint64_t)n + 1))) return rc;
+    PT_CUDA(cudaSetDevice(b->device));
+    if (bytes) PT_CUDA(cudaMemcpyAsync(b->h_act_data.p, b->d_anames.p, bytes, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(b->h_act_off.p, b->d_aoff.p, (count + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    memcpy(b->h_act_first.p, b->h_afirst.data(), ((size_t)n + 1) * 8);
+    *out = pt_actor_tables{n, (const uint8_t*)b->h_act_data.p, (const uint64_t*)b->h_act_off.p, count, (const uint64_t*)b->h_act_first.p, nullptr};
+    return PT_OK;
+}
+
+// Grows every log i with grow[i] != ~0 by the n_new names of slot grow[i] (tot[slot]: n_new, new_bytes, moves), which are the
+// ids new_id[new_off[slot] ..] of the pool (new_data, new_byte_off), in JS order, none in the log's table: the merge kernel
+// writes the grown tables and the old -> new rank maps of the logs whose ranks move; when a rank moves or an n_actors grows,
+// one splice of an empty delta with those maps applies it (identity counters).  Then the grown tables replace the old.  The
+// per-log maps go to haoff ([n_logs + 1]) / hamap.
+static int grow_tables(pt_batch* b, const char* fn, const std::vector<uint32_t>& grow, const pty::SyncTotals* tot, uint32_t n_slots,
+                       const uint8_t* new_data, const unsigned long long* new_byte_off, const unsigned long long* new_off, const unsigned long long* new_id,
+                       HostBuf& haoff, HostBuf& hamap, bool* spliced = nullptr) {
+    const uint32_t n = b->n_logs;
+    int rc;
+    if ((rc = reserve_n<uint64_t>(haoff, (uint64_t)n + 1))) return rc;
+    uint64_t* aoff = (uint64_t*)haoff.p;
+    std::vector<uint32_t> n_new(n_slots, 0);
+    for (uint32_t g = 0; g < n_slots; g++) n_new[g] = tot[g].n_new;
+    std::vector<unsigned long long> map_off(n, ~0ull), new_first((size_t)n + 1, 0), new_byte((size_t)n + 1, 0);
+    std::vector<uint32_t> new_actors(n);
+    bool grows = false, splice = false;
+    uint64_t n_map = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t g = grow[i];
+        const uint64_t cnt = b->h_afirst[i + 1] - b->h_afirst[i] + (g == 0xFFFFFFFFu ? 0 : n_new[g]);
+        new_first[i + 1] = new_first[i] + cnt;
+        new_byte[i + 1] = new_byte[i] + (b->h_abyte[i + 1] - b->h_abyte[i]) + (g == 0xFFFFFFFFu ? 0 : tot[g].new_bytes);
+        new_actors[i] = (uint32_t)std::max<uint64_t>(std::max<uint64_t>(1, cnt), b->h_desc[i].n_actors);
+        if (cnt > 0xFFFF) { g_last_error = std::string(fn) + at(i) + "more than 65535 actors"; return PT_ERR_INVALID; }
+        if (g == 0xFFFFFFFFu) continue;
+        grows = true;
+        if (tot[g].moves) { map_off[i] = n_map; n_map += b->h_desc[i].n_actors; }
+        splice = splice || tot[g].moves || new_actors[i] != b->h_desc[i].n_actors;
+    }
+    DevBuf nnames, noff, nfirst, nbyte, dgrow, dnn, dmoff, dmap, dsrc;   // the grown tables (swapped in once accepted) and scratch
+    if (grows) {
+        if ((rc = reserve_n<uint8_t>(nnames, new_byte[n])) || (rc = reserve_n<unsigned long long>(noff, new_first[n] + 1)) ||
+            (rc = upload_n(b, nfirst, new_first.data(), (uint64_t)n + 1)) || (rc = upload_n(b, nbyte, new_byte.data(), n)) ||
+            (rc = upload_n(b, dgrow, grow.data(), n)) || (rc = upload_n(b, dnn, n_new.data(), n_slots)) || (rc = upload_n(b, dmoff, map_off.data(), n)) ||
+            (rc = reserve_n<uint16_t>(dmap, n_map)) || (rc = reserve_n<const uint8_t*>(dsrc, new_first[n]))) return rc;
+        PT_CUDA(cudaMemsetAsync(noff.p, 0, 8, b->stream));
+        pty::MergeParams M{};
+        M.n_logs = n;
+        M.old_t = pty::Tables{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+        M.data = (uint8_t*)nnames.p; M.off = (unsigned long long*)noff.p; M.first = (const unsigned long long*)nfirst.p;
+        M.byte_base = (const unsigned long long*)nbyte.p; M.grow = (const uint32_t*)dgrow.p;
+        M.new_data = new_data; M.new_byte_off = new_byte_off; M.new_off = new_off; M.new_id = new_id; M.n_new = (const uint32_t*)dnn.p;
+        M.map_off = (const unsigned long long*)dmoff.p; M.map = (uint16_t*)dmap.p; M.src_at = (const uint8_t**)dsrc.p;
+        pty::actor_merge_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(M);
+        PT_CUDA(launched(b));
+    }
+    if ((rc = reserve_n<uint16_t>(hamap, n_map))) return rc;
+    aoff[0] = 0;
+    for (uint32_t i = 0; i < n; i++) aoff[i + 1] = aoff[i] + (map_off[i] == ~0ull ? 0 : b->h_desc[i].n_actors);
+    if (n_map) PT_CUDA(cudaMemcpyAsync(hamap.p, dmap.p, n_map * 2, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    if (spliced) *spliced = splice;
+    if (splice) {
+        std::vector<pt_log_desc> dd(n);
+        for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, new_actors[i], b->h_desc[i].max_ctr};
+        std::vector<pt_change_desc> cd(n, pt_change_desc{0, 0, 0, 0});
+        const pt_packed_ops delta{n, dd.data(), nullptr, 0, nullptr, 0};
+        const pt_change_table ct{n, cd.data(), nullptr, 0, nullptr, 0};
+        const pt_append_remap R{n_map ? aoff : nullptr, (const uint16_t*)hamap.p, nullptr, nullptr, nullptr, 0};
+        if ((rc = splice_append(b, fn, &delta, true, R, b->have_changes ? &ct : nullptr, false))) return rc;
+    }
+    if (grows) {
+        b->d_anames.swap(nnames); b->d_aoff.swap(noff); b->d_afirst.swap(nfirst);
+        b->h_afirst.assign(new_first.begin(), new_first.end()); b->h_abyte.assign(new_byte.begin(), new_byte.end());
+        b->have_actors = true;
+    }
+    return PT_OK;
+}
+
+int pt_batch_sync_pairs(pt_batch* b, const pt_exchange_pair* pairs, uint32_t np, pt_sync_view* out) {
+    const char* fn = "pt_batch_sync_pairs: ";
+    if (!b || !out || (np && !pairs)) { g_last_error = std::string(fn) + "null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_sync_pairs before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = std::string(fn) + "the handle has no change table"; return PT_ERR_STATE; }
+    if (!b->have_actors) { g_last_error = std::string(fn) + "the handle has no actor tables"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs;
+    int rc;
+    if ((rc = reserve_exchange_view(b, np)) || (rc = reserve_n<uint32_t>(b->h_syn_status, np)) || (rc = reserve_n<uint64_t>(b->h_syn_off, (uint64_t)np + 1)) ||
+        (rc = reserve_n<uint64_t>(b->h_syn_aoff, (uint64_t)n + 1)) || (rc = reserve_n<pty::SyncTotals>(b->h_syn_totals, np))) return rc;
+    uint32_t* status = (uint32_t*)b->h_syn_status.p;
+    uint64_t* soff = (uint64_t*)b->h_syn_off.p;
+    pty::SyncTotals* tot = (pty::SyncTotals*)b->h_syn_totals.p;
+    std::vector<char> is_dst(n, 0);
+    for (uint32_t p = 0; p < np; p++) {
+        const std::string e = check_pair(b, p, pairs[p], is_dst);
+        if (!e.empty()) { g_last_error = fn + e; return PT_ERR_INVALID; }
+    }
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // the pinned view buffers may still be the target of an earlier copy
+    // ---- derive: a pair with a densely ranked log is DENSE outright; the others go to the derive kernel ----
+    std::vector<uint32_t> live;
+    std::vector<pt_exchange_pair> lp;
+    std::vector<unsigned long long> slot_off(1, 0), new_off(1, 0);
+    for (uint32_t p = 0; p < np; p++) {
+        status[p] = PT_EXCHANGE_DENSE;
+        if (b->h_adense[pairs[p].src] || b->h_adense[pairs[p].dst]) continue;
+        live.push_back(p); lp.push_back(pairs[p]);
+        slot_off.push_back(slot_off.back() + b->h_cdesc[pairs[p].src].n_changes);
+        new_off.push_back(new_off.back() + (b->h_afirst[pairs[p].src + 1] - b->h_afirst[pairs[p].src]));
+    }
+    const uint32_t nl = (uint32_t)live.size();
+    const pty::Tables T0{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+    DevBuf dlp, dslot, dpos, dnoff, dnew, dtot;                 // freed on return
+    if (nl) {
+        if ((rc = upload_n(b, dlp, lp.data(), nl)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)nl + 1)) ||
+            (rc = upload_n(b, dnoff, new_off.data(), (uint64_t)nl + 1)) || (rc = reserve_n<uint32_t>(dpos, slot_off[nl])) ||
+            (rc = reserve_n<unsigned long long>(dnew, new_off[nl])) || (rc = reserve_n<pty::SyncTotals>(dtot, nl))) return rc;
+        pty::DeriveParams D{};
+        D.pairs = (const pt_exchange_pair*)dlp.p; D.n_pairs = nl; D.maxR = b->adm_maxR; D.T = T0;
+        D.desc = (const pt_log_desc*)b->d_desc.p; D.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+        D.changes = (const pt_change_rec*)b->d_changes.p; D.deps = (const pt_dep_rec*)b->d_deps.p; D.insdel = b->dp_insdel; D.marks = b->dp_marks;
+        D.slot_off = (const unsigned long long*)dslot.p; D.pos = (uint32_t*)dpos.p;
+        D.new_off = (const unsigned long long*)dnoff.p; D.new_id = (unsigned long long*)dnew.p; D.totals = (pty::SyncTotals*)dtot.p;
+        const auto [wpb, smem] = actor_shape(b->adm_maxR);
+        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(pty::sync_derive_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        pty::sync_derive_kernel<<<warp_grid(b, nl, wpb * 32), wpb * 32, smem, b->stream>>>(D);
+        PT_CUDA(launched(b));
+        PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)nl * sizeof(pty::SyncTotals), cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    // ---- growth and pre-append ----
+    std::vector<uint32_t> grow(n, 0xFFFFFFFFu);
+    for (uint32_t k = 0; k < nl; k++) {
+        if (tot[k].verdict == pty::kDeriveDense) continue;
+        status[live[k]] = PT_EXCHANGE_OK;
+        if (tot[k].verdict == pty::kDeriveGrow && tot[k].n_new) grow[lp[k].dst] = k;
+    }
+    if ((rc = grow_tables(b, fn, grow, tot, nl, T0.data, T0.off, (const unsigned long long*)dnoff.p, (const unsigned long long*)dnew.p,
+                          b->h_syn_aoff, b->h_syn_amap))) return rc;
+    // ---- the exchange of the pairs that are not DENSE, with the maps of the grown tables ----
+    std::vector<pt_exchange_pair> xp;
+    std::vector<unsigned long long> xslot(1, 0), xaoff(1, 0);
+    for (uint32_t p = 0; p < np; p++) {
+        if (status[p] == PT_EXCHANGE_DENSE) continue;
+        xp.push_back(pairs[p]);
+        xslot.push_back(xslot.back() + b->h_cdesc[pairs[p].src].n_changes);
+        xaoff.push_back(xaoff.back() + b->h_desc[pairs[p].src].n_actors);
+    }
+    const uint32_t nx = (uint32_t)xp.size();
+    pt_exchange_view xv{};
+    if (nx) {
+        DevBuf dxp, dxaoff, dxmap;
+        if ((rc = upload_n(b, dxp, xp.data(), nx)) || (rc = upload_n(b, dxaoff, xaoff.data(), (uint64_t)nx + 1)) || (rc = reserve_n<uint16_t>(dxmap, xaoff[nx]))) return rc;
+        const pty::Tables T{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+        pty::sync_maps_kernel<<<warp_grid(b, nx, 128), 128, 0, b->stream>>>((const pt_exchange_pair*)dxp.p, nx, T, (const pt_log_desc*)b->d_desc.p,
+                                                                            (const unsigned long long*)dxaoff.p, (uint16_t*)dxmap.p);
+        PT_CUDA(launched(b));
+        if ((rc = exchange_core(b, fn, xp.data(), nx, xslot, (const unsigned long long*)dxaoff.p, (const uint16_t*)dxmap.p, nullptr, nullptr, &xv))) return rc;
+    } else {
+        if ((rc = b->h_xch_delivered.reserve(4))) return rc;
+        pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
+        for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
+        ((uint64_t*)b->h_xch_off.p)[0] = 0;
+        xv = pt_exchange_view{0, (const uint32_t*)b->h_xch_status.p, (const uint64_t*)b->h_xch_off.p, (const uint32_t*)b->h_xch_delivered.p, dd};
+    }
+    // the view: the exchange's, with the DENSE pairs (nothing delivered) in their places
+    soff[0] = 0;
+    for (uint32_t p = 0, x = 0; p < np; p++) {
+        if (status[p] == PT_EXCHANGE_DENSE) { soff[p + 1] = soff[p]; continue; }
+        status[p] = xv.status[x];
+        soff[p + 1] = soff[p] + (xv.delivered_off[x + 1] - xv.delivered_off[x]);
+        x++;
+    }
+    *out = pt_sync_view{np, status, soff, xv.delivered, xv.delta, (const uint64_t*)b->h_syn_aoff.p, (const uint16_t*)b->h_syn_amap.p};
+    return PT_OK;
+}
+
+int pt_batch_add_actors(pt_batch* b, const pt_actor_input* in, pt_actor_view* out) {
+    const char* fn = "pt_batch_add_actors: ";
+    if (!b || !in || !out) { g_last_error = std::string(fn) + "null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_add_actors before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_actors) { g_last_error = std::string(fn) + "the handle has no actor tables"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs;
+    std::string err;
+    if (in->n_logs != n) err = "the input has " + std::to_string(in->n_logs) + " logs and the batch " + std::to_string(n);
+    else if (!in->per_log_first || (in->count && !in->off)) err = "null per_log_first or off";
+    else if (in->count && in->off[in->count] > in->off[0] && !in->data) err = "null data with a nonzero length";
+    else if (in->per_log_first[0] != 0 || in->per_log_first[n] != in->count) err = "per_log_first does not run from 0 to count";
+    for (uint32_t i = 0; err.empty() && i < n; i++) {
+        if (in->per_log_first[i + 1] < in->per_log_first[i] || in->per_log_first[i + 1] > in->count) err = at(i) + "per_log_first decreases or passes count";
+        for (uint64_t k = in->per_log_first[i]; err.empty() && k < in->per_log_first[i + 1]; k++) {
+            if (in->off[k + 1] < in->off[k]) err = "the byte offsets decrease at id " + std::to_string(k);
+            else if ((in->off[k + 1] - in->off[k]) & 1) err = at(i) + "id " + std::to_string(k - in->per_log_first[i]) + " has an odd byte length";
+        }
+    }
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    const uint64_t count = in->count, lo = count ? in->off[0] : 0, bytes = count ? in->off[count] - lo : 0;
+    int rc;
+    if ((rc = reserve_n<uint16_t>(b->h_add_rank, count)) || (rc = reserve_n<pty::SyncTotals>(b->h_add_totals, n))) return rc;
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // the pinned view buffers may still be the target of an earlier copy
+    std::vector<unsigned long long> off(count + 1);
+    for (uint64_t k = 0; k <= count; k++) off[k] = count ? in->off[k] - lo : 0;
+    DevBuf ddata, doff, dfirst, dfresh, dnew, dtot, drank;      // freed on return
+    if ((rc = upload_n(b, ddata, bytes ? in->data + lo : nullptr, bytes)) || (rc = upload_n(b, doff, off.data(), count + 1)) ||
+        (rc = upload_n(b, dfirst, in->per_log_first, (uint64_t)n + 1)) || (rc = reserve_n<uint32_t>(dfresh, count)) ||
+        (rc = reserve_n<unsigned long long>(dnew, count)) || (rc = reserve_n<pty::SyncTotals>(dtot, n)) || (rc = reserve_n<uint16_t>(drank, count))) return rc;
+    pty::SyncTotals* tot = (pty::SyncTotals*)b->h_add_totals.p;
+    std::vector<uint32_t> grow(n, 0xFFFFFFFFu);
+    bool spliced = false;
+    if (count) {
+        pty::AddParams A{};
+        A.n_logs = n; A.T = pty::Tables{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+        A.data = (const uint8_t*)ddata.p; A.off = (const unsigned long long*)doff.p; A.first = (const unsigned long long*)dfirst.p;
+        A.fresh = (uint32_t*)dfresh.p; A.new_id = (unsigned long long*)dnew.p; A.totals = (pty::SyncTotals*)dtot.p;
+        pty::add_select_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(A);
+        PT_CUDA(launched(b));
+        PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)n * sizeof(pty::SyncTotals), cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+        for (uint32_t i = 0; i < n; i++) if (tot[i].n_new) grow[i] = i;
+    } else {
+        for (uint32_t i = 0; i < n; i++) tot[i] = pty::SyncTotals{};
+    }
+    if ((rc = grow_tables(b, fn, grow, tot, n, (const uint8_t*)ddata.p, (const unsigned long long*)doff.p, (const unsigned long long*)dfirst.p,
+                          (const unsigned long long*)dnew.p, b->h_add_aoff, b->h_add_amap, &spliced))) return rc;
+    if (count) {
+        const pty::Tables T{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+        pty::add_ranks_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(n, T, (const uint8_t*)ddata.p, (const unsigned long long*)doff.p,
+                                                                           (const unsigned long long*)dfirst.p, (uint16_t*)drank.p);
+        PT_CUDA(launched(b));
+        PT_CUDA(cudaMemcpyAsync(b->h_add_rank.p, drank.p, count * 2, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    *out = pt_actor_view{n, count, (const uint16_t*)b->h_add_rank.p, (const uint64_t*)b->h_add_aoff.p, (const uint16_t*)b->h_add_amap.p, spliced ? 1u : 0u};
     return PT_OK;
 }
 

@@ -12,14 +12,15 @@ import os
 import numpy as np
 
 from .packing import (CDESC_DT, CHANGE_DT, CLOCK_DT, CHANGES_REQUEST_DT, EXTRA_DT, ChangeExtras, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
-                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs)
+                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs,
+                      string_pools)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
 _lib = None
 
 EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
-           "pt_batch_append", "pt_batch_change", "pt_batch_exchange", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
+           "pt_batch_append", "pt_batch_change", "pt_batch_exchange", "pt_batch_upload_actors", "pt_batch_download_actors", "pt_batch_add_actors", "pt_batch_sync_pairs", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
            "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
            "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
            "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_render_changes_json", "pt_ingest_change_extras", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
@@ -134,6 +135,33 @@ class _ExchangeView(ctypes.Structure):
 PAIR_DT = np.dtype([("src", "<u4"), ("dst", "<u4")])
 
 
+class _ActorTables(ctypes.Structure):
+    _fields_ = [("n_logs", ctypes.c_uint32), ("data", ctypes.c_void_p), ("off", ctypes.c_void_p), ("count", ctypes.c_uint64),
+                ("per_log_first", ctypes.c_void_p), ("counters_first", ctypes.c_void_p)]
+
+
+class _ActorInput(ctypes.Structure):
+    _fields_ = [("n_logs", ctypes.c_uint32), ("data", ctypes.c_void_p), ("off", ctypes.c_void_p), ("count", ctypes.c_uint64),
+                ("per_log_first", ctypes.c_void_p)]
+
+
+class _ActorView(ctypes.Structure):
+    _fields_ = [("n_logs", ctypes.c_uint32), ("count", ctypes.c_uint64), ("rank", ctypes.c_void_p), ("actor_off", ctypes.c_void_p),
+                ("actor_map", ctypes.c_void_p), ("spliced", ctypes.c_uint32)]
+
+
+class _SyncView(ctypes.Structure):
+    _fields_ = [("n_pairs", ctypes.c_uint32), ("status", ctypes.c_void_p), ("delivered_off", ctypes.c_void_p), ("delivered", ctypes.c_void_p),
+                ("delta", ctypes.c_void_p), ("actor_off", ctypes.c_void_p), ("actor_map", ctypes.c_void_p)]
+
+
+def _view_array(p, count, dt):
+    """A copy of `count` elements of dtype `dt` at address p (engine-owned view memory)."""
+    if not count or not p:
+        return np.zeros(0, dt)
+    return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
+
+
 class _SpansView(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("results", ctypes.c_void_p), ("text_off", ctypes.c_void_p),
                 ("span_off", ctypes.c_void_p), ("text", ctypes.c_void_p), ("spans", ctypes.c_void_p),
@@ -200,6 +228,10 @@ def load_library() -> ctypes.CDLL:
     L.pt_batch_append.argtypes = [vp, vp, vp, vp]
     L.pt_batch_change.argtypes = [vp, vp, vp, vp]
     L.pt_batch_exchange.argtypes = [vp, vp, vp]
+    L.pt_batch_upload_actors.argtypes = [vp, vp]
+    L.pt_batch_download_actors.argtypes = [vp, vp]
+    L.pt_batch_sync_pairs.argtypes = [vp, vp, u32, vp]
+    L.pt_batch_add_actors.argtypes = [vp, vp, vp]
     L.pt_compact_ops.argtypes = [vp, vp, vp, ctypes.c_int]
     L.pt_batch_upload_compact.argtypes = [vp, vp]
     L.pt_ingest_create.argtypes = [ctypes.POINTER(vp)]
@@ -375,6 +407,73 @@ class BatchEngine:
         self._n_seq += got
         self.patch_window = None                                             # the splice resets the window
         return status, (off, flat), desc
+
+    def upload_actors(self, batch_or_pools):
+        """Attach the per-log actor ids (pt_batch_upload_actors): a PackedBatch (its ``string_pools``) or a dict with the keys
+        actors / actors_off / actors_first and optionally counters_first (``packing.string_pools``, or pt_ingest_pool kinds 4
+        and 5).  Every upload and any append that can change a log's actors drop them."""
+        p = string_pools(batch_or_pools) if isinstance(batch_or_pools, PackedBatch) else batch_or_pools
+        data = np.ascontiguousarray(p["actors"], np.uint8)
+        off = np.ascontiguousarray(p["actors_off"], np.uint64)
+        first = np.ascontiguousarray(p["actors_first"], np.uint64)
+        cf = p.get("counters_first")
+        cf = None if cf is None else np.ascontiguousarray(cf, np.uint64)
+        t = _ActorTables(len(first) - 1 if len(first) else 0, data.ctypes.data if len(data) else None, off.ctypes.data if len(off) else None,
+                         max(0, len(off) - 1), first.ctypes.data if len(first) else None, None if cf is None else cf.ctypes.data)
+        _check(self._L.pt_batch_upload_actors(self._h, ctypes.byref(t)), "pt_batch_upload_actors")
+
+    def actors(self) -> list[list[str]]:
+        """The handle's actor tables (pt_batch_download_actors), per log its ids in rank order."""
+        t = _ActorTables()
+        _check(self._L.pt_batch_download_actors(self._h, ctypes.byref(t)), "pt_batch_download_actors")
+        off = _view_array(t.off, int(t.count) + 1, np.uint64)
+        first = _view_array(t.per_log_first, t.n_logs + 1, np.uint64)
+        data = _view_array(t.data, int(off[-1]) if len(off) else 0, np.uint8).tobytes()
+        ids = [data[int(off[k]): int(off[k + 1])].decode("utf-16-le", "surrogatepass") for k in range(int(t.count))]
+        return [ids[int(first[i]): int(first[i + 1])] for i in range(t.n_logs)]
+
+    def add_actors(self, names):
+        """Introduce actor ids per log on the device (pt_batch_add_actors): ``names[i]`` = ids for log i, in any order.  Returns
+        (per log the rank of each given id afterwards, the per-log old -> new actor maps as (u64 offsets [n_logs + 1], u16
+        maps)).  The handle then holds what ``packing.add_actors`` specifies; where a rank moved or an n_actors grew, the
+        records were spliced and the batch needs a merge."""
+        enc = [x.encode("utf-16-le", "surrogatepass") for ids in names for x in ids]
+        data = np.frombuffer(b"".join(enc), np.uint8) if enc else np.zeros(0, np.uint8)
+        off = np.zeros(len(enc) + 1, np.uint64)
+        off[1:] = np.cumsum([len(x) for x in enc])
+        first = np.zeros(len(names) + 1, np.uint64)
+        first[1:] = np.cumsum([len(ids) for ids in names])
+        inp = _ActorInput(len(names), data.ctypes.data if len(data) else None, off.ctypes.data, len(enc), first.ctypes.data)
+        v = _ActorView()
+        _check(self._L.pt_batch_add_actors(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_add_actors")
+        rank = _view_array(v.rank, int(v.count), np.uint16)
+        aoff = _view_array(v.actor_off, self.n_logs + 1, np.uint64)
+        amap = _view_array(v.actor_map, int(aoff[-1]) if len(aoff) else 0, np.uint16)
+        if v.spliced:
+            self.patch_window = None                                         # the splice resets the window
+        return [rank[int(first[i]): int(first[i + 1])].tolist() for i in range(len(names))], (aoff, amap)
+
+    def sync_pairs(self, pairs):
+        """``exchange`` with the maps and the pre-append derived on the device from the actor tables (pt_batch_sync_pairs):
+        only the pairs cross PCIe.  Returns (per-pair status, EXCHANGE_DENSE included, the delivered indices as (offsets,
+        indices), the DESC_DT delta, the pre-append's per-log actor maps as (u64 offsets [n_logs + 1], u16 maps)).  The
+        handle then holds what ``packing.sync_maps`` specifies and needs a merge."""
+        a = np.asarray(pairs, np.int64).reshape(-1, 2)
+        pr = np.zeros(len(a), PAIR_DT)
+        pr["src"], pr["dst"] = a[:, 0], a[:, 1]
+        v = _SyncView()
+        _check(self._L.pt_batch_sync_pairs(self._h, pr.ctypes.data if len(pr) else None, len(pr), ctypes.byref(v)), "pt_batch_sync_pairs")
+        status = _view_array(v.status, v.n_pairs, np.uint32)
+        off = _view_array(v.delivered_off, v.n_pairs + 1, np.uint64)
+        flat = _view_array(v.delivered, int(off[-1]) if len(off) else 0, np.uint32)
+        desc = _view_array(v.delta, self.n_logs, DESC_DT)
+        aoff = _view_array(v.actor_off, self.n_logs + 1, np.uint64)
+        amap = _view_array(v.actor_map, int(aoff[-1]) if len(aoff) else 0, np.uint16)
+        got = int(desc["n_insdel"].astype(np.uint64).sum())
+        self._n_insdel += got
+        self._n_seq += got
+        self.patch_window = None                                             # the splices reset the window
+        return status, (off, flat), desc, (aoff, amap)
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion

@@ -479,6 +479,27 @@ def _grown_ids(prev: PackedBatch, i: int, new_actors, new_max_ctr: int, n_new_op
             cm if cm is not None and cm != list(range(len(cm))) else None)
 
 
+def add_actors(batch: PackedBatch, names: Sequence[Sequence[str]]) -> tuple[PackedBatch, AppendRemap, list[list[int]]]:
+    """The host specification of ``pt_batch_add_actors``: ``names[i]`` are ids for log i in any order (duplicates and known ids
+    allowed).  Returns (the empty delta and the remap of ``pt_batch_append`` that make each log's actor table the sorted union,
+    n_actors = max(1, count), counters untouched; per log the rank of every given id afterwards)."""
+    n = batch.n_logs
+    if len(names) != n:
+        raise ValueError(f"add_actors: {len(names)} id lists for a batch of {n} logs")
+    desc = np.zeros(n, DESC_DT)
+    actor_maps, log_actors, ranks = [], [], []
+    for i in range(n):
+        ranked, rank, amap, _, _, _, _ = _grown_ids(batch, i, names[i], 0, 0, set)
+        actor_maps.append(amap); log_actors.append(ranked)
+        ranks.append([rank[a] for a in names[i]])
+        desc[i]["n_actors"] = max(1, len(ranked)); desc[i]["max_ctr"] = batch.desc[i]["max_ctr"]
+    aoff, amaps = _flat_maps(actor_maps, np.uint16)
+    table = ChangeTable(np.zeros(n, CDESC_DT), np.zeros(0, CHANGE_DT), np.zeros(0, DEP_DT)) if batch.changes is not None else None
+    delta = PackedBatch(desc, np.zeros(0, INSDEL_DT), np.zeros(0, MARK_DT), batch.values, batch.link_attrs, batch.comment_ids, batch.other_attrs,
+                        dict(batch.meta), log_actors, list(batch.log_counters) if batch.log_counters else [None] * n, table, list(batch.log_lists))
+    return delta, AppendRemap(aoff, amaps), ranks
+
+
 def pack_append(prev: PackedBatch, new_logs: Sequence[Sequence[dict]], *, with_changes: bool = False,
                 list_ids: Sequence[str | None] | None = None) -> tuple[PackedBatch, AppendRemap]:
     """The delta and remap of ``pt_batch_append`` that extend every log of ``prev`` (a ``pack_logs`` batch) with the Change
@@ -692,6 +713,7 @@ def apply_append(prev: PackedBatch, delta: PackedBatch, remap: AppendRemap | Non
 # Exchange (include/peritext_b200.h pt_batch_exchange)
 # ------------------------------------------------------------------------------------------------------------------
 EXCHANGE_OK, EXCHANGE_BAD_TABLE, EXCHANGE_STUCK, EXCHANGE_UNMAPPED = 0, 1, 2, 3
+EXCHANGE_DENSE = 4           # pt_batch_sync_pairs only: see sync_maps
 ACTOR_UNMAPPED = 0xFFFF      # an actor-map entry for a src actor without a rank in dst
 
 
@@ -764,13 +786,43 @@ def _log_changes(batch: PackedBatch, i: int):
     return ch, dp
 
 
-def exchange_maps(batch: PackedBatch, pairs) -> tuple[ExchangeMaps, tuple[PackedBatch, AppendRemap] | None]:
+def _missing_ids(batch: PackedBatch, src: int, dst: int):
+    """What log src delivers to log dst, read from the change tables and src's records: (the actor ids the missing changes
+    name, their top opId counter, their record count, a callable giving every counter they name), or None if nothing is
+    missing or src's change table does not fit its records.  Counters are original ones."""
+    sch, sdp = _log_changes(batch, src)
+    dch, _ = _log_changes(batch, dst)
+    have: dict[str, int] = {}
+    for c in dch:
+        a = batch.log_actors[dst][int(c["actor"])]
+        have[a] = have.get(a, 0) + 1
+    sn = batch.log_actors[src]
+    miss = [k for k, c in enumerate(sch) if int(c["seq"]) > have.get(sn[int(c["actor"])], 0)]
+    rng = change_record_ranges(batch, src)
+    if not miss or rng is None:
+        return None
+    ins, mk = batch.log_slice(src)
+    ins = np.concatenate([ins[rng[k, 0]: rng[k, 1]] for k in miss]); mk = np.concatenate([mk[rng[k, 2]: rng[k, 3]] for k in miss])
+    st = batch.log_counters[src] if batch.log_counters else None      # src's records are in the batch's id space
+    orig = (lambda c: int(c)) if st is None else (lambda c, st=st: int(st[int(c)]) if int(c) < len(st) else int(c))
+    actors = {sn[int(sch[k]["actor"])] for k in miss}
+    actors |= {sn[int(q["actor"])] for k in miss for q in sdp[int(sch[k]["dep_off"]): int(sch[k]["dep_off"]) + int(sch[k]["n_deps"])]}
+    for recs, ids in ((ins, (("ctr", "actor"), ("ref_ctr", "ref_actor"))), (mk, (("ctr", "actor"), ("start_ctr", "start_actor"), ("end_ctr", "end_actor")))):
+        for cf, af in ids:
+            actors |= {sn[int(a)] for c, a in zip(recs[cf], recs[af]) if int(c)}
+    used = lambda: {orig(c) for recs, fs in ((ins, ("ctr", "ref_ctr")), (mk, ("ctr", "start_ctr", "end_ctr"))) for f in fs for c in recs[f] if int(c)}
+    top = max([0] + [orig(c) for c in ins["ctr"]] + [orig(c) for c in mk["ctr"]])
+    return actors, top, len(ins) + len(mk), used
+
+
+def exchange_maps(batch: PackedBatch, pairs, *, grow=None) -> tuple[ExchangeMaps, tuple[PackedBatch, AppendRemap] | None]:
     """The maps of ``pt_batch_exchange`` for `pairs` = [(src, dst), ...] on `batch` (a ``pack_logs(..., with_changes=True)``
     batch or one grown from it), and the empty pre-append that introduces what the deliveries bring to each dst: new actors
     (``log_actors``) and, where ``pack_logs`` would rank the grown log's counters densely (``log_counters``), its new counter
     ranks.  Returns (maps, (delta, remap)) or (maps, None) if no log's id space moves; the maps are in the id spaces AFTER
     ``apply_append(batch, delta, remap)`` / ``BatchEngine.append(delta, remap)``, so {A->B, B->A} sees both logs grown.
-    What a dst will receive is read from the change tables alone: src's changes by an actor past dst's count of that actor."""
+    What a dst will receive is read from the change tables alone: src's changes by an actor past dst's count of that actor.
+    ``grow(src, dst)`` False leaves that pair's dst as it is (default: every pair may grow its dst)."""
     n = batch.n_logs
     names = [list(a) for a in batch.log_actors]
     tables = list(batch.log_counters) if batch.log_counters else [None] * n
@@ -779,29 +831,11 @@ def exchange_maps(batch: PackedBatch, pairs) -> tuple[ExchangeMaps, tuple[Packed
     actor_maps_pre, ctr_maps_pre = [None] * n, [None] * n
     moved = False
     for src, dst in pairs:
-        sch, sdp = _log_changes(batch, src)
-        dch, _ = _log_changes(batch, dst)
-        have: dict[str, int] = {}
-        for c in dch:
-            a = batch.log_actors[dst][int(c["actor"])]
-            have[a] = have.get(a, 0) + 1
-        sn = batch.log_actors[src]
-        miss = [k for k, c in enumerate(sch) if int(c["seq"]) > have.get(sn[int(c["actor"])], 0)]
-        rng = change_record_ranges(batch, src)
-        if not miss or rng is None:
+        got = _missing_ids(batch, src, dst) if grow is None or grow(src, dst) else None
+        if got is None:
             continue
-        ins, mk = batch.log_slice(src)
-        ins = np.concatenate([ins[rng[k, 0]: rng[k, 1]] for k in miss]); mk = np.concatenate([mk[rng[k, 2]: rng[k, 3]] for k in miss])
-        st = batch.log_counters[src] if batch.log_counters else None      # src's records are in the batch's id space
-        orig = (lambda c: int(c)) if st is None else (lambda c, st=st: int(st[int(c)]) if int(c) < len(st) else int(c))
-        actors = {sn[int(sch[k]["actor"])] for k in miss}
-        actors |= {sn[int(q["actor"])] for k in miss for q in sdp[int(sch[k]["dep_off"]): int(sch[k]["dep_off"]) + int(sch[k]["n_deps"])]}
-        for recs, ids in ((ins, (("ctr", "actor"), ("ref_ctr", "ref_actor"))), (mk, (("ctr", "actor"), ("start_ctr", "start_actor"), ("end_ctr", "end_actor")))):
-            for cf, af in ids:
-                actors |= {sn[int(a)] for c, a in zip(recs[cf], recs[af]) if int(c)}
-        used = lambda: {orig(c) for recs, fs in ((ins, ("ctr", "ref_ctr")), (mk, ("ctr", "start_ctr", "end_ctr"))) for f in fs for c in recs[f] if int(c)}
-        top = max([0] + [orig(c) for c in ins["ctr"]] + [orig(c) for c in mk["ctr"]])
-        ranked, _, amap, table, _, _, cm = _grown_ids(batch, dst, actors, top, len(ins) + len(mk), used)
+        actors, top, n_ops, used = got
+        ranked, _, amap, table, _, _, cm = _grown_ids(batch, dst, actors, top, n_ops, used)
         old_max = int(batch.desc[dst]["max_ctr"])
         moved = moved or ranked != names[dst] or amap is not None or cm is not None or (table is None) != (tables[dst] is None) or \
             (table is not None and len(table) != len(tables[dst]))
@@ -834,6 +868,40 @@ def exchange_maps(batch: PackedBatch, pairs) -> tuple[ExchangeMaps, tuple[Packed
     delta = PackedBatch(desc, np.zeros(0, INSDEL_DT), np.zeros(0, MARK_DT), batch.values, batch.link_attrs, batch.comment_ids, batch.other_attrs,
                         dict(batch.meta), names, tables, ChangeTable(np.zeros(n, CDESC_DT), np.zeros(0, CHANGE_DT), np.zeros(0, DEP_DT)), list(batch.log_lists))
     return maps, (delta, AppendRemap(aoff, aflat, coff, cflat))
+
+
+def _clock_ok(batch: PackedBatch, i: int) -> bool:
+    """Log i's change table passes pt_batch_exchange's clock checks: actors < n_actors, seq == count + 1, deps inside."""
+    ch, dp = _log_changes(batch, i)
+    cnt: dict[int, int] = {}
+    for c in ch:
+        a = int(c["actor"])
+        if a >= int(batch.desc[i]["n_actors"]) or int(c["seq"]) != cnt.get(a, 0) + 1 or int(c["dep_off"]) + int(c["n_deps"]) > len(dp):
+            return False
+        cnt[a] = cnt.get(a, 0) + 1
+    return True
+
+
+def sync_maps(batch: PackedBatch, pairs) -> tuple[np.ndarray, list, ExchangeMaps, tuple[PackedBatch, AppendRemap] | None]:
+    """The host specification of ``pt_batch_sync_pairs``: (per-pair status, EXCHANGE_DENSE or 0, the pairs that are not DENSE,
+    and ``exchange_maps`` of those).  A pair is DENSE when src or dst has a dense counter table (``log_counters``) or when dst,
+    grown by what it is missing from src, would get one (``_wants_dense``); exactly then ``exchange_maps`` would give it a
+    counter table or a counter map.  A pair whose change tables fail the exchange's clock checks does not grow its dst (the
+    exchange reports it as EXCHANGE_BAD_TABLE).  The handle afterwards holds ``apply_exchange(apply_append(batch, *pre), live,
+    maps)``, with the DENSE pairs' statuses in their places."""
+    dense = lambda i: bool(batch.log_counters) and batch.log_counters[i] is not None
+    ok = lambda s, d: _clock_ok(batch, s) and _clock_ok(batch, d)
+    status = np.zeros(len(pairs), np.uint32)
+    live = []
+    for p, (src, dst) in enumerate(pairs):
+        got = None if dense(src) or dense(dst) or not ok(src, dst) else _missing_ids(batch, src, dst)
+        d = batch.desc[dst]
+        if dense(src) or dense(dst) or (got is not None and _wants_dense(max(int(d["max_ctr"]), got[1]), int(d["n_insdel"]) + int(d["n_mark"]) + got[2])):
+            status[p] = EXCHANGE_DENSE
+        else:
+            live.append((int(src), int(dst)))
+    maps, pre = exchange_maps(batch, live, grow=ok)
+    return status, live, maps, pre
 
 
 def _exchange_order(batch: PackedBatch, src: int, dst: int, amap: np.ndarray) -> tuple[int, list[int]]:
