@@ -348,7 +348,9 @@ int pt_compact_ops(const pt_packed_ops* ops, pt_insdel_c8* insdel_out, pt_mark_c
 int pt_batch_upload_compact(pt_batch*, const pt_packed_compact* host_compact);
 
 /* Adopt a batch that is ALREADY RESIDENT in device memory (pointers are device pointers owned by the
- * caller, e.g. torch tensors); only the descriptors are read on the host. */
+ * caller, e.g. torch tensors); only the descriptors are read on the host.  The records are also read at adopt time, on
+ * the handle's stream, to derive the warp kernel's half-width copy of them: after an in-place change to the adopted
+ * arrays, adopt them again before the next merge. */
 int pt_batch_adopt_device(pt_batch*, const pt_packed_ops* host_desc_device_arrays);
 
 /* ------------------------------------------------------------------------------------------------

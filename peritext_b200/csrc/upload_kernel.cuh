@@ -1,5 +1,5 @@
 // upload_kernel.cuh — expansion of the optional upload wire forms (pt_batch_upload_runs, pt_batch_upload_compact) into the
-// pt_insdel_rec / pt_mark_rec records the merge kernels read.
+// pt_insdel_rec / pt_mark_rec records the merge kernels read, and the warp kernel's half-width copy of those records.
 #pragma once
 #include <cstdint>
 
@@ -71,6 +71,34 @@ __global__ void expand_mark_c16_kernel(const pt_mark_c16* __restrict__ in, pt_ma
         b.x = ((q.w >> 4) & 0xFu) | (((q.w >> 8) & 0xFu) << 16);
         b.y = q.z; b.z = q.y >> 16; b.w = 0;
         reinterpret_cast<uint4*>(out)[2 * i] = a; reinterpret_cast<uint4*>(out)[2 * i + 1] = b;
+    }
+}
+
+// ---- the warp kernel's half-width copy of the resident records (warp_kernel.cuh reads it and nothing else on its streams) -----
+// Same record positions as the full arrays, so the descriptors' offsets index it unchanged.
+//   ins/del, 8 B (uint2):  x = ctr:16 | ref_ctr:16 << 16;  y = actor:8 | ref_actor:8 << 8 | kind:2 << 16   (no payload)
+//   mark, 16 B (uint4):    x = ctr:16 | start_ctr:16 << 16;  y = end_ctr:16 | arrival:16 << 16;  z = attr;
+//                          w = actor:8 | start_actor:8 << 8 | end_actor:8 << 16 | kind:3 << 24 | bounds:4 << 27
+// A counter or arrival too wide for its field saturates at 0xFFFF, an actor at 255.  The warp routes have C * R < 0xFFFF,
+// n < 0xFFFF and R <= 255 (ptp::route_of), so a saturated id fails the same range check as the original and a saturated
+// arrival still exceeds every record index: the copy changes no warp-kernel result.  The warp kernel reads no mark kind bit
+// above 2 and no bound bit above 3.
+__device__ __forceinline__ uint32_t sat16(uint32_t v) { return min(v, 0xFFFFu); }
+__device__ __forceinline__ uint32_t sat8(uint32_t v) { return min(v, 0xFFu); }
+__global__ void derive_half_records_kernel(const pt_insdel_rec* __restrict__ ins, const pt_mark_rec* __restrict__ mk,
+                                           uint2* __restrict__ hins, uint4* __restrict__ hmk, unsigned long long n, unsigned long long m) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n + m; i += (unsigned long long)gridDim.x * blockDim.x) {
+        if (i < n) {
+            const uint4 r = __ldg(reinterpret_cast<const uint4*>(ins + i));   // {ctr, ref_ctr, actor | ref_actor << 16, payload}
+            hins[i] = make_uint2(sat16(r.x) | (sat16(r.y) << 16), sat8(r.z & 0xFFFFu) | (sat8(r.z >> 16) << 8) | ((r.w >> 30) << 16));
+        } else {
+            const uint4* q = reinterpret_cast<const uint4*>(mk + (i - n));
+            // {ctr, actor | kind << 16 | bounds << 24, start_ctr, end_ctr} {start_actor | end_actor << 16, attr, arrival, reserved}
+            const uint4 a = __ldg(q), b = __ldg(q + 1);
+            hmk[i - n] = make_uint4(sat16(a.x) | (sat16(a.z) << 16), sat16(a.w) | (sat16(b.z) << 16), b.y,
+                                    sat8(a.y & 0xFFFFu) | (sat8(b.x & 0xFFFFu) << 8) | (sat8(b.x >> 16) << 16) |
+                                        (((a.y >> 16) & 7u) << 24) | (((a.y >> 24) & 0xFu) << 27));
+        }
     }
 }
 

@@ -112,17 +112,22 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     const unsigned long long mark_off = (unsigned long long)dsc0.z | ((unsigned long long)dsc0.w << 32);
     const uint32_t n = dsc1.x, m = dsc1.y, R = dsc1.z ? dsc1.z : 1u, C = dsc1.w;
     const unsigned long long KS64 = (unsigned long long)C * R;
-    if (KS64 >= 0xFFFFull || n >= 0xFFFFu || m >= 0xFFFFu) { ps.leave(); return 1; }     // 16-bit keys / indices only
+    // 16-bit keys / indices only, and actors that fit the 8-bit fields of the half-width records (the host routes no other log here)
+    if (KS64 >= 0xFFFFull || n >= 0xFFFFu || m >= 0xFFFFu || R > 255u) { ps.leave(); return 1; }
     const uint32_t KS = (uint32_t)KS64;
-    const pt_insdel_rec* __restrict__ ins = P.insdel + insdel_off;
-    const pt_mark_rec* __restrict__ mk = P.marks + mark_off;
+    // the record streams are read from the half-width copy (upload_kernel.cuh: ins {ctr | ref_ctr << 16, actor | ref_actor << 8 |
+    // kind << 16}, marks {ctr | start_ctr << 16, end_ctr | arrival << 16, attr, actor | start_actor << 8 | end_actor << 16 |
+    // kind << 24 | bounds << 27}); only phase F reads the full ins/del records, for the payloads of visible elements
+    const uint2* __restrict__ ins = P.half_insdel + insdel_off;
+    const uint4* __restrict__ mk = P.half_marks + mark_off;
+    const pt_insdel_rec* __restrict__ full_ins = P.insdel + insdel_off;
     uint32_t* text_out = P.text + P.text_off[li];
     pt_span* span_out = P.spans + P.span_off[li];
     pt_log_result* res = P.results + li;
 
     if ((P.warp_flags & 1u) && m) {       // this log's mark records are needed late: pull them into L2 now
         const char* p0 = reinterpret_cast<const char*>(mk);
-        const uint32_t lines = (m * (uint32_t)sizeof(pt_mark_rec) + 127u) >> 7;
+        const uint32_t lines = (m * 16u + 127u) >> 7;
         for (uint32_t l = lane; l < lines; l += 32) prefetch_l2(p0 + ((size_t)l << 7));
     }
 
@@ -180,7 +185,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         }
     };
 
-    // ---- A+B: one pass over the ins/del records, 32 per trip, two trips in flight ------------------------------------------
+    // ---- A+B: one pass over the ins/del records, 32 per trip (256 B), two trips in flight -----------------------------------
     // A: id table, insert bits, chain-link bits (reference element == the insert at record i-1: compare with the left
     //    neighbour's key, no lookup).  B: parents of non-chain inserts ("has another child" bits) and deletes (tombstones, OR).
     //    A referenced element must have arrived EARLIER in the log (src/micromerge.ts:752 throws otherwise).
@@ -189,24 +194,24 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         uint32_t carryK = 0xFFFFFFFFu;                         // key of the last record of the previous trip if it is an insert
         // records past the end are loaded from a clamped index and ignored (every use is guarded by i < n)
         const uint32_t nm1 = n ? n - 1u : 0u;
-        uint4 ra = make_uint4(0, 0, 0, 0);
-        if (n) ra = ld_rec(ins + min(lane, nm1));
-        // an L2 prefetch stream runs >= 10 trips (512 B each) ahead of the register loads: DRAM latency under load is longer than
-        // two trips.  Every 8th trip all 32 lanes fetch the 32 lines of 8 later trips (one uniform branch per trip otherwise).
+        uint2 ra = make_uint2(0, 0);
+        if (n) ra = __ldg(ins + min(lane, nm1));
+        // an L2 prefetch stream runs >= 18 trips (4.5 KB) ahead of the register loads: DRAM latency under load is longer than
+        // two trips.  Every 16th trip all 32 lanes fetch the 32 lines of 16 later trips (one uniform branch per trip otherwise).
         const char* insb = reinterpret_cast<const char*>(ins);
-        const uint32_t insBytes = n * 16u;
-        if (lane * 128u + 1024u < insBytes) prefetch_l2(insb + 1024u + lane * 128u);          // trips 2 .. 9
+        const uint32_t insBytes = n * 8u;
+        if (lane * 128u + 512u < insBytes) prefetch_l2(insb + 512u + lane * 128u);            // trips 2 .. 17
         PT_PHASE(kPhStart);
 #pragma unroll 2
         for (uint32_t base = 0; base < n; base += 32) {
             const uint32_t i = base + lane;
-            if ((base & 255u) == 0u) {                                                       // trips t+10 .. t+17
-                const uint32_t po = (base + 320u) * 16u + lane * 128u;
+            if ((base & 511u) == 0u) {                                                       // trips t+18 .. t+33
+                const uint32_t po = (base + 576u) * 8u + lane * 128u;
                 if (po < insBytes) prefetch_l2(insb + po);
             }
-            const uint4 rc = ld_rec(ins + min(i + 32u, nm1));           // one trip ahead (the lines are in L2 by now); unrolled by 2: no moves
-            const uint4 r = ra;
-            const uint32_t ctr = r.x, ref_ctr = r.y, actor = r.z & 0xFFFFu, ref_actor = r.z >> 16, kind = r.w >> 30;
+            const uint2 rc = __ldg(ins + min(i + 32u, nm1));            // one trip ahead (the lines are in L2 by now); unrolled by 2: no moves
+            const uint2 r = ra;
+            const uint32_t ctr = r.x & 0xFFFFu, ref_ctr = r.x >> 16, actor = r.y & 0xFFu, ref_actor = (r.y >> 8) & 0xFFu, kind = r.y >> 16;
             // straight-line form: predicates instead of nested branches
             const bool inb = i < n;
             const bool kbad = kind > 1u, ibad = badId(ctr, actor);
@@ -302,10 +307,9 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t pc = __popc(head) | (__popc(vis) << 16);
             const uint32_t inc = warp_incl_scan(pc, lane), ex = inc - pc, tot = __shfl_sync(kFull, inc, 31);
             if (w < NWr) WI[w] = make_uint4(insW, head, vis, (carryH + (ex & 0xFFFFu)) | ((carryV + (ex >> 16)) << 16));
-            // phase D reads every run head's record again: the 128-byte lines that hold heads go to L2 now, all at once
-#pragma unroll
-            for (uint32_t k = 0; k < 4; k++)
-                if ((head >> (8u * k)) & 0xFFu) prefetch_l2(ins + w * 32u + 8u * k);
+            // phase D reads every run head's record again: the 128-byte lines (16 records) that hold heads go to L2 now, all at once
+            if (head & 0xFFFFu) prefetch_l2(ins + w * 32u);
+            if (head >> 16) prefetch_l2(ins + w * 32u + 16u);
             carryH += tot & 0xFFFFu; carryV += tot >> 16;
             N += __reduce_add_sync(kFull, (uint32_t)__popc(insW));
         }
@@ -366,14 +370,14 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t r = rb + lane;
             if (r < M) {
                 const uint32_t i = HV[r], w = i >> 5, b = i & 31;
-                const uint4 rec = ld_rec(ins + i);                 // issued before the run-end scan: its latency overlaps the scan
+                const uint2 rec = __ldg(ins + i);                  // issued before the run-end scan: its latency overlaps the scan
                 const uint4 q0 = WI[w];
                 uint32_t stop = (q0.y | ~q0.x) & ~(0xFFFFFFFFu >> (31 - b));
                 uint32_t ww = w;
                 while (!stop) { ww++; const uint2 q1 = *reinterpret_cast<const uint2*>(&WI[ww]); stop = q1.y | ~q1.x; }   // pad word: insert bits == 0 -> stops
                 const uint32_t end = ww * 32 + (__ffs(stop) - 1);
-                const uint32_t key = keyOf(rec.x, rec.z & 0xFFFFu);
-                const uint32_t p = rec.y == 0 ? n : lookup(rec.y, rec.z >> 16);
+                const uint32_t key = keyOf(rec.x & 0xFFFFu, rec.y & 0xFFu), ref_ctr = rec.x >> 16;
+                const uint32_t p = ref_ctr == 0 ? n : lookup(ref_ctr, (rec.y >> 8) & 0xFFu);
                 const uint32_t q = p == n ? M : runOf(p);
                 const uint32_t hv = visBefore(i);
                 N16[2 * r + 1] = (uint16_t)(visBefore(end) - hv);
@@ -510,7 +514,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t isv = (vbits >> lane) & 1u;
             EV[i] = (uint16_t)(vr | (isv << 15));
             if (isv) {
-                const uint32_t tok = PT_PAYLOAD_TOKEN(__ldg(&ins[i].payload));
+                const uint32_t tok = PT_PAYLOAD_TOKEN(__ldg(&full_ins[i].payload));
                 text_out[vr] = tok;
                 digest_add(d0, d1, pt_term_text(vr, tok));
             }
@@ -521,15 +525,15 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     uint32_t nspans = 0;
     if ((P.warp_flags & 2u) && li_next != 0xFFFFFFFFu) {        // the next log's ins/del records -> L2 while this one does its marks
         const uint4 q0 = __ldg(reinterpret_cast<const uint4*>(P.desc + li_next)), q1 = __ldg(reinterpret_cast<const uint4*>(P.desc + li_next) + 1);
-        const char* p0 = reinterpret_cast<const char*>(P.insdel + ((unsigned long long)q0.x | ((unsigned long long)q0.y << 32)));
-        const uint32_t lines = (q1.x * (uint32_t)sizeof(pt_insdel_rec) + 127u) >> 7;
+        const char* p0 = reinterpret_cast<const char*>(P.half_insdel + ((unsigned long long)q0.x | ((unsigned long long)q0.y << 32)));
+        const uint32_t lines = (q1.x * 8u + 127u) >> 7;
         for (uint32_t l = lane; l < lines; l += 32) prefetch_l2(p0 + ((size_t)l << 7));
     }
 
-    // the first 6 trips of mark records -> L2 now, just before G: prefetched right after C, most lines were evicted from L2
-    // (thousands of logs in flight stream through it) before G read them (DESIGN.md §4.1)
+    // the first 12 trips (6 KB) of mark records -> L2 now, just before G: prefetched right after C, most lines were evicted from
+    // L2 (thousands of logs in flight stream through it) before G read them (DESIGN.md §4.1)
     if (m) {
-        const uint32_t pfb = min(m * 32u, 6u * 1024u);
+        const uint32_t pfb = min(m * 16u, 6u * 1024u);
         for (uint32_t o = lane * 128u; o < pfb; o += 32u * 128u) prefetch_l2(reinterpret_cast<const char*>(mk) + o);
     }
     PT_PHASE(kPhF);
@@ -549,22 +553,19 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         if (!A.fits()) { ps.leave(); return 1; }
         wfill<uint32_t>(KBits, KW + 1, 0u, lane);
         __syncwarp();
-        const uint4* mq = reinterpret_cast<const uint4*>(mk);
         const uint32_t mm1 = m - 1u;                               // m > 0 here; past-the-end lanes load a clamped record, unused
-        uint4 a0 = __ldg(mq + 2 * min(lane, mm1)), a1 = __ldg(mq + 2 * min(lane, mm1) + 1);
-        const uint32_t mkBytes = m * 32u;
+        uint4 a = __ldg(mk + min(lane, mm1));
+        const uint32_t mkBytes = m * 16u;
 #pragma unroll 2
         for (uint32_t kb = 0; kb < m; kb += 32) {
             const uint32_t k = kb + lane;
-            if ((kb & 127u) == 0u) {                               // every 4th trip: the 32 lines of trips t+6 .. t+9 (1 KB per trip)
-                const uint32_t po = (kb + 192u) * 32u + lane * 128u;
+            if ((kb & 255u) == 0u) {                               // every 8th trip: the 32 lines of trips t+12 .. t+19 (512 B per trip)
+                const uint32_t po = (kb + 384u) * 16u + lane * 128u;
                 if (po < mkBytes) prefetch_l2(reinterpret_cast<const char*>(mk) + po);
             }
-            const uint32_t kn = min(k + 32u, mm1);
-            const uint4 b0 = __ldg(mq + 2 * kn), b1 = __ldg(mq + 2 * kn + 1);   // one trip ahead (L2 hits); unrolled by 2: no moves
-            // a0 = {ctr, actor|kind<<16|bounds<<24, start_ctr, end_ctr}; a1 = {start_actor|end_actor<<16, attr, arrival, reserved}
-            const uint32_t ctr = a0.x, actor = a0.y & 0xFFFFu, kind = (a0.y >> 16) & 0xFFu, bounds = a0.y >> 24;
-            const uint32_t start_ctr = a0.z, end_ctr = a0.w, start_actor = a1.x & 0xFFFFu, end_actor = a1.x >> 16, attr = a1.y, arrival = a1.z;
+            const uint4 b = __ldg(mk + min(k + 32u, mm1));         // one trip ahead (L2 hits); unrolled by 2: no moves
+            const uint32_t ctr = a.x & 0xFFFFu, start_ctr = a.x >> 16, end_ctr = a.y & 0xFFFFu, arrival = a.y >> 16, attr = a.z;
+            const uint32_t actor = a.w & 0xFFu, start_actor = (a.w >> 8) & 0xFFu, end_actor = (a.w >> 16) & 0xFFu, kind = (a.w >> 24) & 7u, bounds = a.w >> 27;
             const uint32_t type = (kind >> 1) & 3u;
             // straight-line form (predicated loads instead of nested branches).  A boundary element must exist AND have arrived
             // before the mark op: the reference's walk never matches anything else (peritext.ts:236-241) — a missing start is a
@@ -605,7 +606,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                 }
             }
             nS += __popc(bal); nC += __popc(balC);
-            a0 = b0; a1 = b1;
+            a = b;
         }
         __syncwarp();
         st = __reduce_or_sync(kFull, st);
