@@ -11,28 +11,97 @@ import os
 
 import numpy as np
 
-from .packing import (CDESC_DT, CHANGE_DT, CLOCK_DT, CHANGES_REQUEST_DT, EXTRA_DT, ChangeExtras, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT, INSDEL_DT, MARK_DT,
-                      RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts, change_inputs, elem_refs,
-                      string_pools)
+from .packing import (CDESC_DT, CHANGE_DT, CLOCK_DT, CHANGES_REQUEST_DT, EXTRA_DT, ChangeExtras, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT,
+                      INPUT_OP_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts,
+                      change_inputs, elem_refs, json_pools, string_pools)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libperitext_b200.so")
 _lib = None
 
-EXPORTS = ["pt_batch_create", "pt_batch_upload", "pt_batch_upload_runs", "pt_compress_runs", "pt_compact_ops", "pt_batch_upload_compact", "pt_batch_adopt_device", "pt_batch_upload_changes",
-           "pt_batch_append", "pt_batch_change", "pt_batch_exchange", "pt_batch_upload_actors", "pt_batch_download_actors", "pt_batch_add_actors", "pt_batch_sync_pairs", "pt_ingest_create", "pt_ingest_parse", "pt_ingest_packed", "pt_ingest_pool", "pt_ingest_error", "pt_ingest_destroy", "pt_batch_merge", "pt_batch_sync",
-           "pt_batch_download", "pt_batch_download_begin", "pt_batch_download_results", "pt_batch_device_results", "pt_batch_launch_count", "pt_batch_stats",
-           "pt_batch_last_merge_ms", "pt_batch_set_comment_pool", "pt_batch_download_patches", "pt_batch_set_patch_pool", "pt_batch_set_patch_window", "pt_batch_query_elements", "pt_batch_find_elements",
-           "pt_batch_render_json", "pt_batch_render_patches_json", "pt_batch_render_changes_json", "pt_ingest_change_extras", "pt_batch_destroy", "pt_strerror", "pt_last_error", "pt_version"]
+_vp, _u32, _u64, _int, _str, _out = ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_int, ctypes.c_char_p, ctypes.POINTER
+# every export of include/peritext_b200.h: name -> (argtypes, restype); an int restype is a pt_status
+_ENTRY_POINTS = {
+    "pt_batch_create": ([_int, _vp, _vp, _out(_vp)], _int),
+    "pt_batch_upload": ([_vp, _vp], _int),
+    "pt_batch_upload_runs": ([_vp, _vp], _int),
+    "pt_compress_runs": ([_vp, _vp, _vp, _vp, _vp, _out(_u64), _out(_u64)], _int),
+    "pt_compact_ops": ([_vp, _vp, _vp, _int], _int),
+    "pt_batch_upload_compact": ([_vp, _vp], _int),
+    "pt_batch_adopt_device": ([_vp, _vp], _int),
+    "pt_batch_upload_changes": ([_vp, _vp], _int),
+    "pt_batch_append": ([_vp, _vp, _vp, _vp], _int),
+    "pt_batch_change": ([_vp, _vp, _vp, _vp], _int),
+    "pt_batch_exchange": ([_vp, _vp, _vp], _int),
+    "pt_batch_upload_actors": ([_vp, _vp], _int),
+    "pt_batch_download_actors": ([_vp, _vp], _int),
+    "pt_batch_add_actors": ([_vp, _vp, _vp], _int),
+    "pt_batch_sync_pairs": ([_vp, _vp, _u32, _vp], _int),
+    "pt_ingest_create": ([_out(_vp)], _int),
+    "pt_ingest_parse": ([_vp, _vp, _vp, _u32, _int], _int),
+    "pt_ingest_packed": ([_vp, _vp, _vp], _int),
+    "pt_ingest_pool": ([_vp, _int, _out(_vp), _out(_vp), _out(_u64), _out(_vp)], _int),
+    "pt_ingest_error": ([_vp], _str),
+    "pt_ingest_destroy": ([_vp], None),
+    "pt_batch_merge": ([_vp], _int),
+    "pt_batch_sync": ([_vp], _int),
+    "pt_batch_download": ([_vp, _vp], _int),
+    "pt_batch_download_begin": ([_vp], _int),
+    "pt_batch_download_results": ([_vp, _vp, _u32], _int),
+    "pt_batch_device_results": ([_vp, _out(_vp), _out(_u32)], _int),
+    "pt_batch_launch_count": ([_vp], _u64),
+    "pt_batch_stats": ([_vp, _out(_u64 * 4)], _int),
+    "pt_batch_last_merge_ms": ([_vp], ctypes.c_float),
+    "pt_batch_set_comment_pool": ([_vp, _u64], _int),
+    "pt_batch_download_patches": ([_vp, _vp], _int),
+    "pt_batch_set_patch_pool": ([_vp, _u64], _int),
+    "pt_batch_set_patch_window": ([_vp, _vp, _u32], _int),
+    "pt_batch_query_elements": ([_vp, _vp, _u32, _vp], _int),
+    "pt_batch_find_elements": ([_vp, _vp, _u32, _vp], _int),
+    "pt_batch_render_json": ([_vp, _vp, _vp], _int),
+    "pt_batch_render_patches_json": ([_vp, _vp, _vp], _int),
+    "pt_batch_render_changes_json": ([_vp, _vp, _vp], _int),
+    "pt_ingest_change_extras": ([_vp, _out(_vp), _out(_u64)], _int),
+    "pt_batch_destroy": ([_vp], None),
+    "pt_strerror": ([_int], _str),
+    "pt_last_error": ([], _str),
+    "pt_version": ([], _str),
+}
+EXPORTS = list(_ENTRY_POINTS)
 
 
 class EngineError(RuntimeError):
-    pass
+    """A failed engine call; ``status`` is the pt_status code it returned (None when no call was made)."""
+
+    def __init__(self, message: str, status: int | None = None):
+        super().__init__(message)
+        self.status = status
+
+
+def _ptr(a):
+    """The data pointer of a numpy array, or NULL (None) for None or an empty array."""
+    return None if a is None or not a.size else a.ctypes.data
+
+
+def _view(p, count, dt, copy: bool = True) -> np.ndarray:
+    """`count` elements of dtype `dt` at address `p` (memory a native library owns): a copy, or with ``copy=False`` a zero-copy
+    array over that memory, valid until the library reuses it.  Empty when `count` is 0 or `p` is NULL."""
+    dt, count = np.dtype(dt), int(count)
+    if not count or not p:
+        return np.zeros(0, dt)
+    a = np.frombuffer((ctypes.c_char * (count * dt.itemsize)).from_address(p), dtype=dt, count=count)
+    return a.copy() if copy else a
 
 
 class _PackedOps(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("logs", ctypes.c_void_p), ("insdel", ctypes.c_void_p),
                 ("n_insdel_total", ctypes.c_uint64), ("marks", ctypes.c_void_p), ("n_mark_total", ctypes.c_uint64)]
+
+
+def _packed_ops(desc, insdel, n_insdel, marks, n_mark) -> _PackedOps:
+    """pt_packed_ops, and pt_packed_compact (the same layout): `insdel` / `marks` are host arrays or device addresses."""
+    p = lambda a: _ptr(a) if isinstance(a, np.ndarray) else a
+    return _PackedOps(len(desc), _ptr(desc), p(insdel), n_insdel, p(marks), n_mark)
 
 
 class _PackedRuns(ctypes.Structure):
@@ -84,7 +153,7 @@ def compress_runs(batch: PackedBatch, pin=None) -> PackedRuns:
     desc = np.ascontiguousarray(batch.desc)
     insdel = np.ascontiguousarray(batch.insdel)
     marks = np.ascontiguousarray(batch.marks)
-    ops = _PackedOps(len(desc), desc.ctypes.data, insdel.ctypes.data, len(insdel), marks.ctypes.data, len(marks))
+    ops = _packed_ops(desc, insdel, len(insdel), marks, len(marks))
     n = len(desc)
     run_off = np.zeros(n + 1, np.uint64); tok_off = np.zeros(n + 1, np.uint64)
     nr, nt = ctypes.c_uint64(0), ctypes.c_uint64(0)
@@ -109,7 +178,16 @@ class _AppendRemap(ctypes.Structure):
 def _change_struct(table: ChangeTable):
     """(pt_change_table, the contiguous arrays it points into)."""
     d, c, p = np.ascontiguousarray(table.desc), np.ascontiguousarray(table.changes), np.ascontiguousarray(table.deps)
-    return _ChangeTable(len(d), d.ctypes.data, c.ctypes.data if len(c) else 0, len(c), p.ctypes.data if len(p) else 0, len(p)), (d, c, p)
+    return _ChangeTable(len(d), _ptr(d), _ptr(c), len(c), _ptr(p), len(p)), (d, c, p)
+
+
+# the map fields of pt_append_remap, in order; pt_exchange_input has the first four
+_MAP_FIELDS = (("actor_off", np.uint64), ("actor_map", np.uint16), ("ctr_off", np.uint64), ("ctr_map", np.uint32), ("comment_map", np.uint32))
+
+
+def _map_arrays(maps: AppendRemap | ExchangeMaps) -> list:
+    """The maps of an AppendRemap or ExchangeMaps as typed contiguous arrays (None stays None), in the struct's field order."""
+    return [None if getattr(maps, k) is None else np.ascontiguousarray(getattr(maps, k), dt) for k, dt in _MAP_FIELDS if hasattr(maps, k)]
 
 
 class _ChangeInput(ctypes.Structure):
@@ -135,6 +213,14 @@ class _ExchangeView(ctypes.Structure):
 PAIR_DT = np.dtype([("src", "<u4"), ("dst", "<u4")])
 
 
+def _pairs(pairs) -> np.ndarray:
+    """(src, dst) pairs (a list of tuples or an (n, 2) array) as PAIR_DT rows."""
+    a = np.asarray(pairs, np.int64).reshape(-1, 2)
+    pr = np.zeros(len(a), PAIR_DT)
+    pr["src"], pr["dst"] = a[:, 0], a[:, 1]
+    return pr
+
+
 class _ActorTables(ctypes.Structure):
     _fields_ = [("n_logs", ctypes.c_uint32), ("data", ctypes.c_void_p), ("off", ctypes.c_void_p), ("count", ctypes.c_uint64),
                 ("per_log_first", ctypes.c_void_p), ("counters_first", ctypes.c_void_p)]
@@ -153,13 +239,6 @@ class _ActorView(ctypes.Structure):
 class _SyncView(ctypes.Structure):
     _fields_ = [("n_pairs", ctypes.c_uint32), ("status", ctypes.c_void_p), ("delivered_off", ctypes.c_void_p), ("delivered", ctypes.c_void_p),
                 ("delta", ctypes.c_void_p), ("actor_off", ctypes.c_void_p), ("actor_map", ctypes.c_void_p)]
-
-
-def _view_array(p, count, dt):
-    """A copy of `count` elements of dtype `dt` at address p (engine-owned view memory)."""
-    if not count or not p:
-        return np.zeros(0, dt)
-    return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
 
 
 class _SpansView(ctypes.Structure):
@@ -183,6 +262,14 @@ class _JsonPools(ctypes.Structure):
     _fields_ = [("values", ctypes.c_void_p), ("values_off", ctypes.c_void_p), ("n_values", ctypes.c_uint64),
                 ("links", ctypes.c_void_p), ("links_off", ctypes.c_void_p), ("n_links", ctypes.c_uint64),
                 ("comments", ctypes.c_void_p), ("comments_off", ctypes.c_void_p), ("n_comments", ctypes.c_uint64)]
+
+
+def _json_pools(batch: PackedBatch, pools):
+    """(pt_json_pools of `pools` (values, values_off, links, links_off, comments, comments_off; default
+    ``packing.json_pools(batch)``), the contiguous arrays it points into)."""
+    a = [np.ascontiguousarray(x, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, x in enumerate(json_pools(batch) if pools is None else pools)]
+    n = lambda off: max(0, len(off) - 1)
+    return _JsonPools(_ptr(a[0]), _ptr(a[1]), n(a[1]), _ptr(a[2]), _ptr(a[3]), n(a[3]), _ptr(a[4]), _ptr(a[5]), n(a[5])), a
 
 
 class _JsonView(ctypes.Structure):
@@ -218,51 +305,9 @@ def load_library() -> ctypes.CDLL:
         raise EngineError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                           f"(make -C peritext_b200/csrc). There is no CPU fallback.")
     L = ctypes.CDLL(LIB_PATH)
-    vp, u32, u64 = ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint64
-    L.pt_batch_create.argtypes = [ctypes.c_int, vp, vp, ctypes.POINTER(vp)]
-    L.pt_batch_upload.argtypes = [vp, vp]
-    L.pt_batch_adopt_device.argtypes = [vp, vp]
-    L.pt_batch_upload_runs.argtypes = [vp, vp]
-    L.pt_compress_runs.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(u64), ctypes.POINTER(u64)]
-    L.pt_batch_upload_changes.argtypes = [vp, vp]
-    L.pt_batch_append.argtypes = [vp, vp, vp, vp]
-    L.pt_batch_change.argtypes = [vp, vp, vp, vp]
-    L.pt_batch_exchange.argtypes = [vp, vp, vp]
-    L.pt_batch_upload_actors.argtypes = [vp, vp]
-    L.pt_batch_download_actors.argtypes = [vp, vp]
-    L.pt_batch_sync_pairs.argtypes = [vp, vp, u32, vp]
-    L.pt_batch_add_actors.argtypes = [vp, vp, vp]
-    L.pt_compact_ops.argtypes = [vp, vp, vp, ctypes.c_int]
-    L.pt_batch_upload_compact.argtypes = [vp, vp]
-    L.pt_ingest_create.argtypes = [ctypes.POINTER(vp)]
-    L.pt_ingest_parse.argtypes = [vp, vp, vp, u32, ctypes.c_int]
-    L.pt_ingest_packed.argtypes = [vp, vp, vp]
-    L.pt_ingest_pool.argtypes = [vp, ctypes.c_int, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.POINTER(vp)]
-    L.pt_ingest_error.argtypes = [vp]; L.pt_ingest_error.restype = ctypes.c_char_p
-    L.pt_ingest_destroy.argtypes = [vp]; L.pt_ingest_destroy.restype = None
-    L.pt_batch_merge.argtypes = [vp]
-    L.pt_batch_sync.argtypes = [vp]
-    L.pt_batch_download.argtypes = [vp, vp]
-    L.pt_batch_download_begin.argtypes = [vp]
-    L.pt_batch_download_results.argtypes = [vp, vp, u32]
-    L.pt_batch_device_results.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u32)]
-    L.pt_batch_launch_count.argtypes = [vp]; L.pt_batch_launch_count.restype = u64
-    L.pt_batch_stats.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64 * 4)]
-    L.pt_batch_last_merge_ms.argtypes = [vp]; L.pt_batch_last_merge_ms.restype = ctypes.c_float
-    L.pt_batch_set_comment_pool.argtypes = [vp, u64]
-    L.pt_batch_download_patches.argtypes = [vp, vp]
-    L.pt_batch_set_patch_pool.argtypes = [vp, u64]
-    L.pt_batch_set_patch_window.argtypes = [vp, vp, u32]
-    L.pt_batch_query_elements.argtypes = [vp, vp, u32, vp]
-    L.pt_batch_find_elements.argtypes = [vp, vp, u32, vp]
-    L.pt_batch_render_json.argtypes = [vp, vp, vp]
-    L.pt_batch_render_patches_json.argtypes = [vp, vp, vp]
-    L.pt_batch_render_changes_json.argtypes = [vp, vp, vp]
-    L.pt_ingest_change_extras.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u64)]
-    L.pt_batch_destroy.argtypes = [vp]; L.pt_batch_destroy.restype = None
-    L.pt_strerror.argtypes = [ctypes.c_int]; L.pt_strerror.restype = ctypes.c_char_p
-    L.pt_last_error.restype = ctypes.c_char_p
-    L.pt_version.restype = ctypes.c_char_p
+    for name, (argtypes, restype) in _ENTRY_POINTS.items():
+        fn = getattr(L, name)
+        fn.argtypes, fn.restype = argtypes, restype
     _lib = L
     return L
 
@@ -270,7 +315,7 @@ def load_library() -> ctypes.CDLL:
 def _check(rc: int, what: str):
     if rc != 0:
         L = load_library()
-        raise EngineError(f"{what}: {L.pt_strerror(rc).decode()} ({L.pt_last_error().decode()})")
+        raise EngineError(f"{what}: {L.pt_strerror(rc).decode()} ({L.pt_last_error().decode()})", rc)
 
 
 class BatchEngine:
@@ -300,16 +345,30 @@ class BatchEngine:
         self._n_insdel = int(n_insdel_total)                                 # patch records: one per ins/del record
         self._n_seq = int(desc["n_insdel"].astype(np.uint64).sum())          # element sequences: the capacity layout
 
-    def _ops_struct(self, desc, insdel_ptr, n_insdel, marks_ptr, n_mark):
-        return _PackedOps(len(desc), desc.ctypes.data, insdel_ptr, n_insdel, marks_ptr, n_mark)
+    _ops_struct = staticmethod(_packed_ops)                                  # the builder under its earlier method name
+
+    def _spliced(self, delta_desc):
+        """Record a splice into the resident batch (append, change, exchange, sync, a re-ranking add_actors): the device rebuilds
+        the records tightly from the new descriptors, so it then holds exactly their n_insdel sum; a splice also resets the
+        patch window."""
+        self._n_seq += int(delta_desc["n_insdel"].astype(np.uint64).sum())
+        self._n_insdel = self._n_seq
+        self.patch_window = None
 
     def upload(self, batch: PackedBatch):
         desc = np.ascontiguousarray(batch.desc)
         insdel = np.ascontiguousarray(batch.insdel)
         marks = np.ascontiguousarray(batch.marks)
-        ops = self._ops_struct(desc, insdel.ctypes.data, len(insdel), marks.ctypes.data, len(marks))
+        ops = _packed_ops(desc, insdel, len(insdel), marks, len(marks))
         _check(self._L.pt_batch_upload(self._h, ctypes.byref(ops)), "pt_batch_upload")
         self._uploaded(desc, len(insdel))
+
+    def _upload_with_changes(self, batch, upload=None, *args):
+        """``upload(batch, *args)`` (default the plain form), then attach the batch's change table if it has one, so the next
+        merge runs the admission pre-pass."""
+        (upload or self.upload)(batch, *args)
+        if getattr(batch, "changes", None) is not None:
+            self.upload_changes(batch.changes)
 
     def upload_changes(self, table: ChangeTable):
         """Attach the batch's change table: the next merge runs the admission pre-pass (seq / deps checks of
@@ -322,20 +381,34 @@ class BatchEngine:
         handle holds what an upload of ``packing.apply_append(batch, delta, remap)`` would hold, and needs a merge.  `delta`
         and `remap` come from ``packing.pack_append``; `changes` is the delta's change table (default ``delta.changes``),
         required exactly when the resident batch has one.  Works after every upload form and after an earlier append."""
-        r = remap or AppendRemap()
         desc = np.ascontiguousarray(delta.desc)
         insdel = np.ascontiguousarray(delta.insdel); marks = np.ascontiguousarray(delta.marks)
-        ops = self._ops_struct(desc, insdel.ctypes.data if len(insdel) else 0, len(insdel), marks.ctypes.data if len(marks) else 0, len(marks))
-        arrs = [None if a is None else np.ascontiguousarray(a, dtype=dt)
-                for a, dt in ((r.actor_off, np.uint64), (r.actor_map, np.uint16), (r.ctr_off, np.uint64), (r.ctr_map, np.uint32), (r.comment_map, np.uint32))]
-        ptr = lambda a: None if a is None else a.ctypes.data
-        st = _AppendRemap(*[ptr(a) for a in arrs], 0 if arrs[4] is None else len(arrs[4]))
+        ops = _packed_ops(desc, insdel, len(insdel), marks, len(marks))
+        arrs = _map_arrays(remap or AppendRemap())
+        # not _ptr: an empty comment_map is no identity (NULL is), it maps no resident comment rank and the device refuses
+        st = _AppendRemap(*[None if a is None else a.ctypes.data for a in arrs], 0 if arrs[4] is None else len(arrs[4]))
         table = delta.changes if changes is None else changes
         ct = _change_struct(table) if table is not None else None
         _check(self._L.pt_batch_append(self._h, ctypes.byref(ops), ctypes.byref(st), ctypes.byref(ct[0]) if ct else None), "pt_batch_append")
-        self._n_insdel += len(insdel)
-        self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
-        self.patch_window = None                                             # so does an append
+        self._spliced(desc)
+
+    def change_packed(self, actor, input_off, ops, tokens, n_values: int, n_links: int, n_comments: int, changes: ChangeTable | None = None):
+        """pt_batch_change from its arrays (``packing.change_inputs``, ``workload.sync_round``): per log i the actor rank of its
+        change (CHANGE_NO_ACTOR: none) and its InputOperations ops[input_off[i]:input_off[i + 1]] (INPUT_OP_DT), the value
+        tokens they name, and the sizes of the value, link and comment pools their tokens and attrs index.  ``changes`` is the
+        change table of the new changes, required exactly when the resident batch has one.  Returns (the per-log
+        CHANGE_STATUS_DT rows, the DESC_DT delta, its ins/del records, its mark records); the handle needs a merge afterwards."""
+        actor, off = np.ascontiguousarray(actor, np.uint32), np.ascontiguousarray(input_off, np.uint64)
+        ops, tokens = np.ascontiguousarray(ops, INPUT_OP_DT), np.ascontiguousarray(tokens, np.uint32)
+        n = len(actor)
+        inp = _ChangeInput(n, _ptr(actor), _ptr(off), _ptr(ops), _ptr(tokens), len(tokens), n_values, n_links, n_comments, 0)
+        ct = _change_struct(changes) if changes is not None else None
+        v = _ChangeView()
+        _check(self._L.pt_batch_change(self._h, ctypes.byref(inp), ctypes.byref(ct[0]) if ct else None, ctypes.byref(v)), "pt_batch_change")
+        desc = _view(v.delta.logs, n, DESC_DT)
+        self._spliced(desc)
+        return (_view(v.status, n, CHANGE_STATUS_DT), desc, _view(v.delta.insdel, v.delta.n_insdel_total, INSDEL_DT),
+                _view(v.delta.marks, v.delta.n_mark_total, MARK_DT))
 
     def change(self, batch: PackedBatch, inputs, actor_ranks, changes: ChangeTable | None = None):
         """Micromerge.change for many documents on the device (pt_batch_change): ``inputs[i]`` is None (no change) or
@@ -345,21 +418,9 @@ class BatchEngine:
         (the batch the handle now holds = ``apply_append`` of the generated records, the Change objects (None where there is no
         change or it failed), the per-log CHANGE_STATUS_DT rows); a failed log ("List index out of bounds") appends nothing
         and its row names the failing InputOperation.  Needs emit_sequence; the handle needs a merge afterwards."""
-        n = batch.n_logs
         actor, off, ops, tokens, values, links, counters = change_inputs(batch, inputs, actor_ranks)
-        ptr = lambda a: a.ctypes.data if len(a) else None
-        inp = _ChangeInput(n, ptr(actor), ptr(off), ptr(ops), ptr(tokens), len(tokens), len(values), len(links), len(batch.comment_ids), 0)
-        ct = _change_struct(changes) if changes is not None else None
-        v = _ChangeView()
-        _check(self._L.pt_batch_change(self._h, ctypes.byref(inp), ctypes.byref(ct[0]) if ct else None, ctypes.byref(v)), "pt_batch_change")
-
-        def arr(p, count, dt):
-            if not count or not p:
-                return np.zeros(0, dt)
-            return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
-        status = arr(v.status, n, CHANGE_STATUS_DT)
-        desc = arr(v.delta.logs, n, DESC_DT)
-        failed = [i for i in range(n) if int(status[i]["status"]) != CHANGE_OK]
+        status, desc, insdel, marks = self.change_packed(actor, off, ops, tokens, len(values), len(links), len(batch.comment_ids), changes)
+        failed = [i for i in range(batch.n_logs) if int(status[i]["status"]) != CHANGE_OK]
         for i in failed:                                 # no records: the counter table stays as it was
             counters[i] = batch.log_counters[i] if batch.log_counters else None
         dch = None
@@ -367,12 +428,8 @@ class BatchEngine:
             cd = changes.desc.copy()
             cd["n_changes"][failed] = 0; cd["n_deps"][failed] = 0
             dch = ChangeTable(cd, changes.changes, changes.deps)
-        delta = PackedBatch(desc, arr(v.delta.insdel, int(v.delta.n_insdel_total), INSDEL_DT), arr(v.delta.marks, int(v.delta.n_mark_total), MARK_DT),
-                            values, links, batch.comment_ids, batch.other_attrs, dict(batch.meta), list(batch.log_actors), counters, dch,
+        delta = PackedBatch(desc, insdel, marks, values, links, batch.comment_ids, batch.other_attrs, dict(batch.meta), list(batch.log_actors), counters, dch,
                             list(batch.log_lists))
-        self._n_insdel += int(desc["n_insdel"].astype(np.uint64).sum())
-        self._n_seq += int(desc["n_insdel"].astype(np.uint64).sum())
-        self.patch_window = None                                             # the append resets the window
         return apply_append(batch, delta), change_dicts(batch, inputs, actor_ranks, status, delta), status
 
     def exchange(self, pairs, maps: ExchangeMaps):
@@ -384,28 +441,19 @@ class BatchEngine:
         per log the records it received, its n_actors and new max_ctr).  The handle then holds ``packing.apply_exchange`` of
         the batch and needs a merge; a log's old n_insdel + n_mark as its patch window gives the Patches applyChanges
         returned.  Needs a change table."""
-        a = np.asarray(pairs, np.int64).reshape(-1, 2)
-        pr = np.zeros(len(a), PAIR_DT)
-        pr["src"], pr["dst"] = a[:, 0], a[:, 1]
-        arrs = [None if a is None else np.ascontiguousarray(a, dtype=dt)
-                for a, dt in ((maps.actor_off, np.uint64), (maps.actor_map, np.uint16), (maps.ctr_off, np.uint64), (maps.ctr_map, np.uint32))]
-        ptr = lambda a: None if a is None or not len(a) else a.ctypes.data
-        inp = _ExchangeInput(len(pr), ptr(pr), *[ptr(a) for a in arrs])
+        pr = _pairs(pairs)
+        inp = _ExchangeInput(len(pr), _ptr(pr), *[_ptr(a) for a in _map_arrays(maps)])
         v = _ExchangeView()
         _check(self._L.pt_batch_exchange(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_exchange")
+        return self._delivered(v)
 
-        def arr(p, count, dt):
-            if not count or not p:
-                return np.zeros(0, dt)
-            return np.frombuffer((ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(p), dtype=dt, count=count).copy()
-        status = arr(v.status, v.n_pairs, np.uint32)
-        off = arr(v.delivered_off, v.n_pairs + 1, np.uint64)
-        flat = arr(v.delivered, int(off[-1]) if len(off) else 0, np.uint32)
-        desc = arr(v.delta, self.n_logs, DESC_DT)
-        got = int(desc["n_insdel"].astype(np.uint64).sum())
-        self._n_insdel += got
-        self._n_seq += got
-        self.patch_window = None                                             # the splice resets the window
+    def _delivered(self, v):
+        """(per-pair status, (delivered offsets, indices), DESC_DT delta) of an exchange or sync view; records the splice."""
+        status = _view(v.status, v.n_pairs, np.uint32)
+        off = _view(v.delivered_off, v.n_pairs + 1, np.uint64)
+        flat = _view(v.delivered, off[-1] if len(off) else 0, np.uint32)
+        desc = _view(v.delta, self.n_logs, DESC_DT)
+        self._spliced(desc)
         return status, (off, flat), desc
 
     def upload_actors(self, batch_or_pools):
@@ -418,17 +466,16 @@ class BatchEngine:
         first = np.ascontiguousarray(p["actors_first"], np.uint64)
         cf = p.get("counters_first")
         cf = None if cf is None else np.ascontiguousarray(cf, np.uint64)
-        t = _ActorTables(len(first) - 1 if len(first) else 0, data.ctypes.data if len(data) else None, off.ctypes.data if len(off) else None,
-                         max(0, len(off) - 1), first.ctypes.data if len(first) else None, None if cf is None else cf.ctypes.data)
+        t = _ActorTables(max(0, len(first) - 1), _ptr(data), _ptr(off), max(0, len(off) - 1), _ptr(first), _ptr(cf))
         _check(self._L.pt_batch_upload_actors(self._h, ctypes.byref(t)), "pt_batch_upload_actors")
 
     def actors(self) -> list[list[str]]:
         """The handle's actor tables (pt_batch_download_actors), per log its ids in rank order."""
         t = _ActorTables()
         _check(self._L.pt_batch_download_actors(self._h, ctypes.byref(t)), "pt_batch_download_actors")
-        off = _view_array(t.off, int(t.count) + 1, np.uint64)
-        first = _view_array(t.per_log_first, t.n_logs + 1, np.uint64)
-        data = _view_array(t.data, int(off[-1]) if len(off) else 0, np.uint8).tobytes()
+        off = _view(t.off, t.count + 1, np.uint64)
+        first = _view(t.per_log_first, t.n_logs + 1, np.uint64)
+        data = _view(t.data, off[-1] if len(off) else 0, np.uint8).tobytes()
         ids = [data[int(off[k]): int(off[k + 1])].decode("utf-16-le", "surrogatepass") for k in range(int(t.count))]
         return [ids[int(first[i]): int(first[i + 1])] for i in range(t.n_logs)]
 
@@ -443,14 +490,14 @@ class BatchEngine:
         off[1:] = np.cumsum([len(x) for x in enc])
         first = np.zeros(len(names) + 1, np.uint64)
         first[1:] = np.cumsum([len(ids) for ids in names])
-        inp = _ActorInput(len(names), data.ctypes.data if len(data) else None, off.ctypes.data, len(enc), first.ctypes.data)
+        inp = _ActorInput(len(names), _ptr(data), _ptr(off), len(enc), _ptr(first))
         v = _ActorView()
         _check(self._L.pt_batch_add_actors(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_add_actors")
-        rank = _view_array(v.rank, int(v.count), np.uint16)
-        aoff = _view_array(v.actor_off, self.n_logs + 1, np.uint64)
-        amap = _view_array(v.actor_map, int(aoff[-1]) if len(aoff) else 0, np.uint16)
-        if v.spliced:
-            self.patch_window = None                                         # the splice resets the window
+        rank = _view(v.rank, v.count, np.uint16)
+        aoff = _view(v.actor_off, self.n_logs + 1, np.uint64)
+        amap = _view(v.actor_map, aoff[-1] if len(aoff) else 0, np.uint16)
+        if v.spliced:                                                        # re-ranked records, none added
+            self._spliced(np.zeros(0, DESC_DT))
         return [rank[int(first[i]): int(first[i + 1])].tolist() for i in range(len(names))], (aoff, amap)
 
     def sync_pairs(self, pairs):
@@ -458,22 +505,12 @@ class BatchEngine:
         only the pairs cross PCIe.  Returns (per-pair status, EXCHANGE_DENSE included, the delivered indices as (offsets,
         indices), the DESC_DT delta, the pre-append's per-log actor maps as (u64 offsets [n_logs + 1], u16 maps)).  The
         handle then holds what ``packing.sync_maps`` specifies and needs a merge."""
-        a = np.asarray(pairs, np.int64).reshape(-1, 2)
-        pr = np.zeros(len(a), PAIR_DT)
-        pr["src"], pr["dst"] = a[:, 0], a[:, 1]
+        pr = _pairs(pairs)
         v = _SyncView()
-        _check(self._L.pt_batch_sync_pairs(self._h, pr.ctypes.data if len(pr) else None, len(pr), ctypes.byref(v)), "pt_batch_sync_pairs")
-        status = _view_array(v.status, v.n_pairs, np.uint32)
-        off = _view_array(v.delivered_off, v.n_pairs + 1, np.uint64)
-        flat = _view_array(v.delivered, int(off[-1]) if len(off) else 0, np.uint32)
-        desc = _view_array(v.delta, self.n_logs, DESC_DT)
-        aoff = _view_array(v.actor_off, self.n_logs + 1, np.uint64)
-        amap = _view_array(v.actor_map, int(aoff[-1]) if len(aoff) else 0, np.uint16)
-        got = int(desc["n_insdel"].astype(np.uint64).sum())
-        self._n_insdel += got
-        self._n_seq += got
-        self.patch_window = None                                             # the splices reset the window
-        return status, (off, flat), desc, (aoff, amap)
+        _check(self._L.pt_batch_sync_pairs(self._h, _ptr(pr), len(pr), ctypes.byref(v)), "pt_batch_sync_pairs")
+        status, delivered, desc = self._delivered(v)
+        aoff = _view(v.actor_off, self.n_logs + 1, np.uint64)
+        return status, delivered, desc, (aoff, _view(v.actor_map, aoff[-1] if len(aoff) else 0, np.uint16))
 
     def upload_compact(self, batch: PackedBatch, cins: np.ndarray | None = None, cmarks: np.ndarray | None = None, threads: int = 0):
         """Upload in the compact wire format (8-byte ins/del, 16-byte mark records; expanded on the device): the conversion
@@ -484,17 +521,16 @@ class BatchEngine:
             cins = np.zeros(max(1, len(insdel)), INSDEL_C8_DT)
         if cmarks is None:
             cmarks = np.zeros(max(1, len(marks)), MARK_C16_DT)
-        ops = self._ops_struct(desc, insdel.ctypes.data, len(insdel), marks.ctypes.data, len(marks))
-        _check(self._L.pt_compact_ops(ctypes.byref(ops), cins.ctypes.data, cmarks.ctypes.data, threads), "pt_compact_ops")
-        cc = _PackedOps(len(desc), desc.ctypes.data, cins.ctypes.data, len(insdel), cmarks.ctypes.data, len(marks))     # same field layout as pt_packed_compact
+        ops = _packed_ops(desc, insdel, len(insdel), marks, len(marks))
+        _check(self._L.pt_compact_ops(ctypes.byref(ops), _ptr(cins), _ptr(cmarks), threads), "pt_compact_ops")
+        cc = _packed_ops(desc, cins, len(insdel), cmarks, len(marks))
         self._keep = (desc, cins, cmarks)
         _check(self._L.pt_batch_upload_compact(self._h, ctypes.byref(cc)), "pt_batch_upload_compact")
         self._uploaded(desc, len(insdel))
 
     def upload_runs(self, r: PackedRuns):
         desc = np.ascontiguousarray(r.desc)
-        st = _PackedRuns(len(desc), desc.ctypes.data, r.run_off.ctypes.data, r.tok_off.ctypes.data, r.runs.ctypes.data if len(r.runs) else 0,
-                         r.tokens.ctypes.data if len(r.tokens) else 0, r.marks.ctypes.data if len(r.marks) else 0, r.n_insdel_total, len(r.marks))
+        st = _PackedRuns(len(desc), _ptr(desc), _ptr(r.run_off), _ptr(r.tok_off), _ptr(r.runs), _ptr(r.tokens), _ptr(r.marks), r.n_insdel_total, len(r.marks))
         self._keep = (desc, r)
         _check(self._L.pt_batch_upload_runs(self._h, ctypes.byref(st)), "pt_batch_upload_runs")
         self._uploaded(desc, r.n_insdel_total)
@@ -502,7 +538,7 @@ class BatchEngine:
     def adopt_device(self, desc: np.ndarray, insdel_dev_ptr: int, n_insdel: int, marks_dev_ptr: int, n_mark: int):
         """Use op arrays already resident in device memory (e.g. ``tensor.data_ptr()``); caller keeps them alive."""
         desc = np.ascontiguousarray(desc)
-        ops = self._ops_struct(desc, insdel_dev_ptr, n_insdel, marks_dev_ptr, n_mark)
+        ops = _packed_ops(desc, insdel_dev_ptr, n_insdel, marks_dev_ptr, n_mark)
         _check(self._L.pt_batch_adopt_device(self._h, ctypes.byref(ops)), "pt_batch_adopt_device")
         self._uploaded(desc, n_insdel)
 
@@ -533,7 +569,7 @@ class BatchEngine:
 
     def results(self) -> np.ndarray:
         out = np.zeros(self.n_logs, RESULT_DT)
-        _check(self._L.pt_batch_download_results(self._h, out.ctypes.data, self.n_logs), "pt_batch_download_results")
+        _check(self._L.pt_batch_download_results(self._h, _ptr(out), self.n_logs), "pt_batch_download_results")
         return out
 
     def download_begin(self):
@@ -543,14 +579,7 @@ class BatchEngine:
         v = _SpansView()
         _check(self._L.pt_batch_download(self._h, ctypes.byref(v)), "pt_batch_download")
         n = v.n_logs
-
-        def arr(ptr, count, dt):
-            if not count:
-                return np.zeros(0, dt)
-            buf = (ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(ptr)
-            a = np.frombuffer(buf, dtype=dt, count=count)
-            return a.copy() if copy else a
-
+        arr = lambda p, count, dt: _view(p, count, dt, copy)
         results = arr(v.results, n, RESULT_DT)
         text_off = arr(v.text_off, n + 1, np.uint64)      # packed on the device: offsets are the scan of the counts
         span_off = arr(v.span_off, n + 1, np.uint64)
@@ -560,20 +589,14 @@ class BatchEngine:
         self.comment_pool_needed = int(v.comment_pool_needed)
         self.comment_pool_used = int(v.comment_pool_used)
         return MergedBatch(results, text_off, span_off, arr(v.text, n_text, np.uint32), arr(v.spans, n_span, SPAN_DT),
-                           arr(v.comment_pool, int(v.comment_pool_used), np.uint32),
+                           arr(v.comment_pool, v.comment_pool_used, np.uint32),
                            arr(v.seq, n_seq, np.uint32) if v.seq else None, seq_off)
 
     def download_patches(self):
         """PT_FLAG_EMIT_PATCHES: (patch records per ins/del record, pool items, per-log status, items needed) of the last merge."""
         v = _PatchView()
         _check(self._L.pt_batch_download_patches(self._h, ctypes.byref(v)), "pt_batch_download_patches")
-
-        def arr(ptr, count, dt):
-            if not count or not ptr:
-                return np.zeros(0, dt)
-            buf = (ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(ptr)
-            return np.frombuffer(buf, dtype=dt, count=count).copy()
-        return arr(v.recs, self._n_insdel, PATCH_REC_DT), arr(v.items, int(v.n_items), PATCH_ITEM_DT), arr(v.status, self.n_logs, np.uint32), int(v.n_items_needed)
+        return _view(v.recs, self._n_insdel, PATCH_REC_DT), _view(v.items, v.n_items, PATCH_ITEM_DT), _view(v.status, self.n_logs, np.uint32), int(v.n_items_needed)
 
     def set_patch_window(self, first_ops=None):
         """Restrict the Patch stream of the following merges to a suffix of every log's list ops (pt_batch_set_patch_window):
@@ -586,7 +609,7 @@ class BatchEngine:
             self.patch_window = None
             return
         w = np.ascontiguousarray(first_ops, dtype=np.uint32)
-        _check(self._L.pt_batch_set_patch_window(self._h, w.ctypes.data if len(w) else None, len(w)), "pt_batch_set_patch_window")
+        _check(self._L.pt_batch_set_patch_window(self._h, _ptr(w), len(w)), "pt_batch_set_patch_window")
         self.patch_window = w.copy()
 
     def run_with_patches(self, batch: PackedBatch, first_ops=None):
@@ -595,15 +618,13 @@ class BatchEngine:
         if first_ops is None:
             out = self.run(batch)
         else:
-            self.upload(batch)
-            if getattr(batch, "changes", None) is not None:
-                self.upload_changes(batch.changes)
+            self._upload_with_changes(batch)
             self.set_patch_window(first_ops)
             self.merge()
             out = self._download_with_pool_retry()
         recs, items, status, needed = self.download_patches()
         if needed > len(items):
-            _check(self._L.pt_batch_set_patch_pool(self._h, needed + 16), "pt_batch_set_patch_pool")
+            self.set_patch_pool(needed + 16)
             self.merge(); out = self.download()
             recs, items, status, needed = self.download_patches()
         from .packing import DevicePatches
@@ -618,7 +639,7 @@ class BatchEngine:
         q["log"], q["index"] = logs, indices
         q["flags"] = np.asarray(look_after_tombstones, dtype=np.uint32) if not np.isscalar(look_after_tombstones) else (1 if look_after_tombstones else 0)
         out = np.zeros(len(q), np.uint32)
-        _check(self._L.pt_batch_query_elements(self._h, q.ctypes.data, len(q), out.ctypes.data), "pt_batch_query_elements")
+        _check(self._L.pt_batch_query_elements(self._h, _ptr(q), len(q), _ptr(out)), "pt_batch_query_elements")
         return out
 
     def find_elements(self, logs, ctrs, actors) -> np.ndarray:
@@ -630,7 +651,7 @@ class BatchEngine:
         q = np.zeros(len(logs), ELEM_REF_DT)
         q["log"], q["ctr"], q["actor"] = logs, ctrs, actors
         out = np.zeros(len(q), ELEM_POS_DT)
-        _check(self._L.pt_batch_find_elements(self._h, q.ctypes.data, len(q), out.ctypes.data), "pt_batch_find_elements")
+        _check(self._L.pt_batch_find_elements(self._h, _ptr(q), len(q), _ptr(out)), "pt_batch_find_elements")
         return out
 
     def resolve_cursors(self, batch: PackedBatch, logs, elem_ids) -> np.ndarray:
@@ -645,17 +666,10 @@ class BatchEngine:
         return out
 
     def _render(self, entry: str, batch: PackedBatch, pools) -> tuple[np.ndarray, np.ndarray]:
-        from .packing import json_pools
-        p = json_pools(batch) if pools is None else pools
-        arrs = [np.ascontiguousarray(a, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, a in enumerate(p)]
-        ptr = lambda a: a.ctypes.data if a.size else None
-        st = _JsonPools(ptr(arrs[0]), ptr(arrs[1]), max(0, len(arrs[1]) - 1), ptr(arrs[2]), ptr(arrs[3]), max(0, len(arrs[3]) - 1),
-                        ptr(arrs[4]), ptr(arrs[5]), max(0, len(arrs[5]) - 1))
+        st, _keep = _json_pools(batch, pools)
         v = _JsonView()
         _check(getattr(self._L, entry)(self._h, ctypes.byref(st), ctypes.byref(v)), entry)
-        off = np.frombuffer((ctypes.c_char * ((v.n_logs + 1) * 8)).from_address(v.off), np.uint64).copy()
-        data = np.frombuffer((ctypes.c_char * v.n_bytes).from_address(v.bytes), np.uint8).copy() if v.n_bytes else np.zeros(0, np.uint8)
-        return data, off
+        return _view(v.bytes, v.n_bytes, np.uint8), _view(v.off, v.n_logs + 1, np.uint64)
 
     @staticmethod
     def _split(data: np.ndarray, off: np.ndarray) -> list[bytes]:
@@ -691,30 +705,22 @@ class BatchEngine:
         and list-id tables); ``extras`` = the ``ChangeExtras`` of its changes (None: the list-op projection); ``pools`` as for
         ``render_json``.  Returns (uint8 bytes, uint64 offsets [n_requests + 1], uint32 status per request): request r is
         bytes[off[r]:off[r+1]], a Change[] array, empty for a request whose status is not CHANGES_OK."""
-        from .packing import json_pools, string_pools
         req, clock = requests if isinstance(requests, tuple) else (requests, np.zeros(0, CLOCK_DT))
         req = np.ascontiguousarray(req, CHANGES_REQUEST_DT); clock = np.ascontiguousarray(clock, CLOCK_DT)
-        p = json_pools(batch) if pools is None else pools
-        jp = [np.ascontiguousarray(a, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, a in enumerate(p)]
+        st, jp = _json_pools(batch, pools)
         sp = string_pools(batch)
         ex = extras if extras is not None else ChangeExtras(np.zeros(0, EXTRA_DT), [])
         rows = np.ascontiguousarray(ex.rows, EXTRA_DT)
         xdata, xoff = ex.pools()
         keep = [req, clock, jp, sp, rows, xdata, xoff]
-        ptr = lambda a: a.ctypes.data if a.size else None
-        st = _JsonPools(ptr(jp[0]), ptr(jp[1]), max(0, len(jp[1]) - 1), ptr(jp[2]), ptr(jp[3]), max(0, len(jp[3]) - 1),
-                        ptr(jp[4]), ptr(jp[5]), max(0, len(jp[5]) - 1))
-        inp = _ChangesJsonInput(len(req), 0, ptr(req), ptr(clock), len(clock), st, ptr(sp["actors"]), ptr(sp["actors_off"]), ptr(sp["actors_first"]),
-                                ptr(sp["counters"]), ptr(sp["counters_first"]), ptr(sp["list_ids"]), ptr(sp["list_ids_off"]),
-                                ptr(rows), len(rows), ptr(xdata), ptr(xoff), len(ex.ops))
+        inp = _ChangesJsonInput(len(req), 0, _ptr(req), _ptr(clock), len(clock), st, _ptr(sp["actors"]), _ptr(sp["actors_off"]), _ptr(sp["actors_first"]),
+                                _ptr(sp["counters"]), _ptr(sp["counters_first"]), _ptr(sp["list_ids"]), _ptr(sp["list_ids_off"]),
+                                _ptr(rows), len(rows), _ptr(xdata), _ptr(xoff), len(ex.ops))
         v = _ChangesJsonView()
         _check(self._L.pt_batch_render_changes_json(self._h, ctypes.byref(inp), ctypes.byref(v)), "pt_batch_render_changes_json")
         del keep
         nr = len(req)
-        off = np.frombuffer((ctypes.c_char * ((nr + 1) * 8)).from_address(v.off), np.uint64).copy()
-        data = np.frombuffer((ctypes.c_char * v.n_bytes).from_address(v.bytes), np.uint8).copy() if v.n_bytes else np.zeros(0, np.uint8)
-        status = np.frombuffer((ctypes.c_char * (nr * 4)).from_address(v.status), np.uint32).copy() if nr else np.zeros(0, np.uint32)
-        return data, off, status
+        return _view(v.bytes, v.n_bytes, np.uint8), _view(v.off, nr + 1, np.uint64), _view(v.status, nr, np.uint32)
 
     def render_changes_json_list(self, batch: PackedBatch, requests, extras: ChangeExtras | None = None, pools=None) -> list[bytes]:
         """``render_changes_json`` as one bytes object per request."""
@@ -724,13 +730,16 @@ class BatchEngine:
     def set_comment_pool(self, entries: int):
         _check(self._L.pt_batch_set_comment_pool(self._h, int(entries)), "pt_batch_set_comment_pool")
 
+    def set_patch_pool(self, items: int):
+        """The capacity of the Patch item pool (pt_batch_set_patch_pool) from the next merge on: a merge whose patches do not
+        fit reports the items it needed (``download_patches``), and one re-merge with a pool of that size fits them."""
+        _check(self._L.pt_batch_set_patch_pool(self._h, int(items)), "pt_batch_set_patch_pool")
+
     def run(self, batch: PackedBatch) -> MergedBatch:
         """upload -> merge -> download.  The comment pool has a default capacity; a log whose comment lists do not fit
         reports status 4 without consuming pool space and the engine reports the batch's exact demand, so one re-merge
         with a pool of that size always succeeds (documents with many overlapping comments are valid input)."""
-        self.upload(batch)
-        if getattr(batch, "changes", None) is not None:
-            self.upload_changes(batch.changes)
+        self._upload_with_changes(batch)
         self.merge()
         return self._download_with_pool_retry()
 
@@ -790,16 +799,13 @@ class PipelinedEngine:
         cuts = sorted(set(min(max(c, 0), n) for c in cuts))
         subs = [batch.slice_logs(a, b) for a, b in zip(cuts, cuts[1:]) if b > a]
         used = self.engines[: len(subs)]
-        for e, sb in zip(used, subs):
+        for k, (e, sb) in enumerate(zip(used, subs)):
             if isinstance(sb, PackedRuns):
-                e.upload_runs(sb)
+                e._upload_with_changes(sb, e.upload_runs)
             elif compact:
-                ci, cm = self._compact_buffers(used.index(e), len(sb.insdel), len(sb.marks))
-                e.upload_compact(sb, ci, cm, threads)
+                e._upload_with_changes(sb, e.upload_compact, *self._compact_buffers(k, len(sb.insdel), len(sb.marks)), threads)
             else:
-                e.upload(sb)
-            if sb.changes is not None:
-                e.upload_changes(sb.changes)
+                e._upload_with_changes(sb)
             e.merge(); e.download_begin()
         return [e._download_with_pool_retry(copy=copy) for e in used]
 
@@ -838,47 +844,35 @@ def _ingest(logs_json, threads: int = 0, with_extras: bool = False):
         ops, tab = _PackedOps(), _ChangeTable()
         _check(L.pt_ingest_packed(h, ctypes.byref(ops), ctypes.byref(tab)), "pt_ingest_packed")
 
-        def arr(ptr, count, dt):
-            if not count or not ptr:
-                return np.zeros(0, dt)
-            buf = (ctypes.c_char * (count * np.dtype(dt).itemsize)).from_address(ptr)
-            return np.frombuffer(buf, dtype=dt, count=count).copy()
-
         def pool(kind):
+            """pt_ingest_pool: (bytes, u64 offsets [count + 1], u64 per-log first [n + 1] or None)."""
             data, off, cnt, first = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_void_p()
             _check(L.pt_ingest_pool(h, kind, ctypes.byref(data), ctypes.byref(off), ctypes.byref(cnt), ctypes.byref(first)), "pt_ingest_pool")
-            o = arr(off.value, cnt.value + 1, np.uint64)
-            raw = bytes(arr(data.value, int(o[-1]), np.uint8)) if cnt.value else b""
-            items = [raw[int(o[k]): int(o[k + 1])] for k in range(cnt.value)]
-            f = arr(first.value, n + 1, np.uint64) if first.value else None
-            return items, f
+            o = _view(off.value, cnt.value + 1, np.uint64)
+            return (_view(data.value, o[-1], np.uint8).tobytes() if cnt.value else b""), o, (_view(first.value, n + 1, np.uint64) if first.value else None)
 
+        pools = {kind: pool(kind) for kind in (range(8) if with_extras else (0, 1, 3, 4, 5))}
+        items = lambda kind: [pools[kind][0][int(a): int(b)] for a, b in zip(pools[kind][1][:-1], pools[kind][1][1:])]
         u16 = lambda b: b.decode("utf-16-le", "surrogatepass")
-        values = [u16(b) for b in pool(0)[0]]
-        link_attrs = [json.loads(b.decode("utf-8", "surrogatepass")) for b in pool(1)[0]]
-        comment_attrs = [json.loads(b.decode("utf-8", "surrogatepass")) for b in pool(3)[0]]
-        actors, afirst = pool(4)
-        counters, cfirst = pool(5)
+        values = [u16(b) for b in items(0)]
+        link_attrs = [json.loads(b.decode("utf-8", "surrogatepass")) for b in items(1)]
+        comment_attrs = [json.loads(b.decode("utf-8", "surrogatepass")) for b in items(3)]
+        actors, afirst = items(4), pools[4][2]
+        counters, cfirst = items(5), pools[5][2]
         log_actors = [[u16(x) for x in actors[int(afirst[i]): int(afirst[i + 1])]] for i in range(n)]
         log_counters = []
         for i in range(n):
             c = counters[int(cfirst[i]): int(cfirst[i + 1])]
             log_counters.append(np.array([int.from_bytes(x, "little") for x in c], dtype=np.uint64) if c else None)
-        table = ChangeTable(arr(tab.logs, tab.n_logs, CDESC_DT), arr(tab.changes, tab.n_changes_total, CHANGE_DT), arr(tab.deps, tab.n_deps_total, DEP_DT))
-        batch = PackedBatch(arr(ops.logs, ops.n_logs, DESC_DT), arr(ops.insdel, ops.n_insdel_total, INSDEL_DT), arr(ops.marks, ops.n_mark_total, MARK_DT),
+        table = ChangeTable(_view(tab.logs, tab.n_logs, CDESC_DT), _view(tab.changes, tab.n_changes_total, CHANGE_DT), _view(tab.deps, tab.n_deps_total, DEP_DT))
+        batch = PackedBatch(_view(ops.logs, ops.n_logs, DESC_DT), _view(ops.insdel, ops.n_insdel_total, INSDEL_DT), _view(ops.marks, ops.n_mark_total, MARK_DT),
                             values, link_attrs, comment_attrs, [], log_actors=log_actors, log_counters=log_counters, changes=table)
         if not with_extras:
             return batch, None, None
-        raw = {}
-        for kind in range(8):
-            data, off, cnt, first = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_void_p()
-            _check(L.pt_ingest_pool(h, kind, ctypes.byref(data), ctypes.byref(off), ctypes.byref(cnt), ctypes.byref(first)), "pt_ingest_pool")
-            o = arr(off.value, cnt.value + 1, np.uint64)
-            raw[kind] = (bytes(arr(data.value, int(o[-1]), np.uint8)) if cnt.value else b"", o, arr(first.value, n + 1, np.uint64) if first.value else None)
-        batch.log_lists = [u16(x) or None for x in pool(6)[0]]
+        batch.log_lists = [u16(x) or None for x in items(6)]
         xp, xn = ctypes.c_void_p(), ctypes.c_uint64()
         _check(L.pt_ingest_change_extras(h, ctypes.byref(xp), ctypes.byref(xn)), "pt_ingest_change_extras")
-        extras = ChangeExtras(arr(xp.value, xn.value, EXTRA_DT), [b.decode("utf-8", "surrogatepass") for b in pool(7)[0]])
-        return batch, extras, raw
+        extras = ChangeExtras(_view(xp.value, xn.value, EXTRA_DT), [b.decode("utf-8", "surrogatepass") for b in items(7)])
+        return batch, extras, pools
     finally:
         L.pt_ingest_destroy(h)

@@ -11,6 +11,7 @@ import os
 
 import numpy as np
 
+from .engine import _view
 from .packing import CDESC_DT, CHANGE_DT, CHANGE_NO_ACTOR, DEP_DT, DESC_DT, INPUT_OP_DT, INSDEL_DT, MARK_DT, ChangeTable, ExchangeMaps, PackedBatch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -75,14 +76,7 @@ def generate(config: str, *, n_docs: int | None = None, ops_per_doc: int | None 
     if rc != 0:
         raise RuntimeError(f"ptw_generate failed: {rc}")
     b = out.contents
-
-    def arr(ptr, count, dt):
-        if not count:
-            return np.zeros(0, dt)
-        buf = (ctypes.c_char * (count * dt.itemsize)).from_address(ptr)
-        return np.frombuffer(buf, dtype=dt, count=count).copy()
-
-    batch = PackedBatch(arr(b.desc, b.n_logs, DESC_DT), arr(b.insdel, b.n_insdel, INSDEL_DT), arr(b.marks, b.n_marks, MARK_DT),
+    batch = PackedBatch(_view(b.desc, b.n_logs, DESC_DT), _view(b.insdel, b.n_insdel, INSDEL_DT), _view(b.marks, b.n_marks, MARK_DT),
                         values=[], link_attrs=[{"url": f"{ch}.com"} for ch in "ABCDEFGHIJKLMNOPQRSTUVWXYZ"],
                         comment_ids=_SyntheticComments(), other_attrs=[],
                         meta=dict(config=config, label=cfg["label"], n_docs=cfg["n_docs"], replicas=cfg["replicas"],

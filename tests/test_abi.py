@@ -3,6 +3,7 @@ include/peritext_b200.h declares; without a GPU it fails loudly instead of falli
 import ctypes
 import os
 import re
+import subprocess
 
 import pytest
 
@@ -27,11 +28,54 @@ def test_library_exports_every_declared_symbol():
     assert b"sm_90a" in lib.pt_version()
 
 
-def test_struct_layouts_match_header():
-    from peritext_b200 import packing as p
-    assert p.INSDEL_DT.itemsize == 16 and p.MARK_DT.itemsize == 32 and p.DESC_DT.itemsize == 32
-    assert p.RESULT_DT.itemsize == 32 and p.SPAN_DT.itemsize == 16
-    assert p.MARK_DT.fields["attr"][1] == 20 and p.MARK_DT.fields["arrival"][1] == 24
+# every layout the binding mirrors -> its header type (the mirrors' field names are the header's)
+HEADER_TYPES = {
+    "_PackedOps": ("pt_packed_ops", "pt_packed_compact"), "_PackedRuns": ("pt_packed_runs",), "_ChangeTable": ("pt_change_table",),
+    "_AppendRemap": ("pt_append_remap",), "_ChangeInput": ("pt_change_input",), "_ChangeView": ("pt_change_view",),
+    "_ExchangeInput": ("pt_exchange_input",), "_ExchangeView": ("pt_exchange_view",), "_ActorTables": ("pt_actor_tables",),
+    "_ActorInput": ("pt_actor_input",), "_ActorView": ("pt_actor_view",), "_SyncView": ("pt_sync_view",), "_SpansView": ("pt_spans_view",),
+    "_Limits": ("pt_limits",), "_PatchView": ("pt_patch_view",), "_JsonPools": ("pt_json_pools",), "_JsonView": ("pt_json_view",),
+    "_ChangesJsonInput": ("pt_changes_json_input",), "_ChangesJsonView": ("pt_changes_json_view",),
+    "INSDEL_DT": ("pt_insdel_rec",), "MARK_DT": ("pt_mark_rec",), "DESC_DT": ("pt_log_desc",), "RESULT_DT": ("pt_log_result",),
+    "SPAN_DT": ("pt_span",), "CHANGE_DT": ("pt_change_rec",), "DEP_DT": ("pt_dep_rec",), "CDESC_DT": ("pt_change_desc",),
+    "ELEM_REF_DT": ("pt_elem_ref",), "ELEM_POS_DT": ("pt_elem_pos",), "INPUT_OP_DT": ("pt_input_op",), "CHANGE_STATUS_DT": ("pt_change_status",),
+    "EXTRA_DT": ("pt_change_extra",), "CHANGES_REQUEST_DT": ("pt_changes_request",), "CLOCK_DT": ("pt_clock_entry",),
+    "INSDEL_C8_DT": ("pt_insdel_c8",), "MARK_C16_DT": ("pt_mark_c16",), "RUN_DT": ("pt_run_rec",), "PAIR_DT": ("pt_exchange_pair",),
+    "QUERY_DT": ("pt_elem_query",), "PATCH_REC_DT": ("pt_patch_rec",), "PATCH_ITEM_DT": ("pt_patch_item",),
+}
+
+
+def mirrored_layouts():
+    """name -> (size, [(field, offset, size)]) of every ctypes Structure defined in peritext_b200.engine and every *_DT dtype of
+    peritext_b200.packing and peritext_b200.engine."""
+    import numpy as np
+    from peritext_b200 import engine, packing
+    out = {}
+    for name, c in vars(engine).items():
+        if isinstance(c, type) and issubclass(c, ctypes.Structure) and c.__module__ == engine.__name__:
+            out[name] = (ctypes.sizeof(c), [(f, getattr(c, f).offset, getattr(c, f).size) for f, *_ in c._fields_])
+    for mod in (packing, engine):
+        for name, dt in vars(mod).items():
+            if name.endswith("_DT") and isinstance(dt, np.dtype):
+                out[name] = (dt.itemsize, [(f, dt.fields[f][1], dt.fields[f][0].itemsize) for f in dt.names])
+    return out
+
+
+def test_struct_layouts_match_header(tmp_path):
+    """Every mirrored struct has the header's size, and every field its offset and size, checked by the C compiler."""
+    layouts = mirrored_layouts()
+    assert sorted(layouts) == sorted(HEADER_TYPES), "mirrors without a header type, or header types without a mirror"
+    lines = ['#include "peritext_b200.h"']
+    for name, (size, fields) in sorted(layouts.items()):
+        for t in HEADER_TYPES[name]:
+            lines.append(f'_Static_assert(sizeof({t}) == {size}, "{name}: sizeof({t}) is not {size}");')
+            for f, off, fsize in fields:
+                lines.append(f'_Static_assert(offsetof({t}, {f}) == {off}, "{name}.{f}: offsetof({t}, {f}) is not {off}");')
+                lines.append(f'_Static_assert(sizeof((({t}*)0)->{f}) == {fsize}, "{name}.{f}: sizeof({t}.{f}) is not {fsize}");')
+    src = tmp_path / "layouts.c"
+    src.write_text("\n".join(lines) + "\n")
+    r = subprocess.run(["gcc", "-std=c11", "-fsyntax-only", "-I", os.path.join(ROOT, "include"), str(src)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
 
 
 def test_no_cpu_fallback():

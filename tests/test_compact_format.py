@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from peritext_b200 import workload
-from peritext_b200.engine import INSDEL_C8_DT, MARK_C16_DT, EngineError, _PackedOps, _check, load_library
+from peritext_b200.engine import INSDEL_C8_DT, MARK_C16_DT, EngineError, _check, _packed_ops, load_library
 from peritext_b200.packing import DESC_DT, INSDEL_DT, MARK_DT, TOKEN_POOLED, PackedBatch
 
 
@@ -15,7 +15,7 @@ def convert(batch, threads=3):
     L = load_library()
     desc = np.ascontiguousarray(batch.desc); ins = np.ascontiguousarray(batch.insdel); mk = np.ascontiguousarray(batch.marks)
     ci = np.zeros(max(1, len(ins)), INSDEL_C8_DT); cm = np.zeros(max(1, len(mk)), MARK_C16_DT)
-    ops = _PackedOps(len(desc), desc.ctypes.data, ins.ctypes.data, len(ins), mk.ctypes.data, len(mk))
+    ops = _packed_ops(desc, ins, len(ins), mk, len(mk))
     _check(L.pt_compact_ops(ctypes.byref(ops), ci.ctypes.data, cm.ctypes.data, threads), "pt_compact_ops")
     return ci[: len(ins)], cm[: len(mk)]
 

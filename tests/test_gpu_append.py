@@ -391,11 +391,59 @@ def test_refusals_leave_the_batch_untouched():
 def no_table_append(e, d, r):
     """pt_batch_append with no delta change table (NULL) on a handle that has one."""
     import ctypes
-    from peritext_b200.engine import _AppendRemap
+    from peritext_b200.engine import _AppendRemap, _packed_ops
     desc, ins, mk = np.ascontiguousarray(d.desc), np.ascontiguousarray(d.insdel), np.ascontiguousarray(d.marks)
-    ops = e._ops_struct(desc, ins.ctypes.data, len(ins), mk.ctypes.data, len(mk))
+    ops = _packed_ops(desc, ins, len(ins), mk, len(mk))
     st = _AppendRemap(None, None, None, None, None, 0)          # identity maps: only the missing table is wrong
     return e._L.pt_batch_append(e._h, ctypes.byref(ops), ctypes.byref(st), None)
+
+
+@pytest.mark.gpu
+def test_an_empty_comment_map_is_not_the_identity():
+    """pt_append_remap: a NULL comment_map is the identity, an empty one maps no comment rank, so on a batch with comment marks
+    the device refuses the append."""
+    from peritext_b200.engine import EngineError
+    logs, ks = comment_and_link_logs()
+    prev = pack_logs(split(logs, ks)[0], with_changes=True)
+    assert (prev.marks["kind"] >> 1 & 3 == 2).any()                   # a comment mark
+    delta, _ = pack_append(prev, [[] for _ in logs], with_changes=True)
+    e = engine()
+    try:
+        e.run(prev)
+        before = canon(merged(e))
+        with pytest.raises(EngineError) as err:
+            e.append(delta, AppendRemap(comment_map=np.zeros(0, np.uint32)))
+        assert err.value.status == PT_ERR_INVALID
+        assert canon(merged(e)) == before
+        e.append(delta, AppendRemap())
+        assert canon(merged(e)) == before
+    finally:
+        e.close()
+
+
+@pytest.mark.gpu
+def test_patch_records_after_splicing_an_upload_with_slack():
+    """An upload whose ins/del array holds one record no descriptor covers has one patch record per uploaded record; the splice
+    of an append rebuilds the records from the descriptors, so afterwards there is one per record of the spliced batch."""
+    import copy
+    logs, ks = comment_and_link_logs()
+    prefix, suffix = split(logs, ks)
+    prev = pack_logs(prefix)
+    delta, remap = pack_append(prev, suffix)
+    slack = copy.copy(prev)
+    slack.insdel = np.concatenate([prev.insdel, prev.insdel[-1:]])
+    want = apply_append(prev, delta, remap)
+    e, u = engine(patches=True), engine(patches=True)
+    try:
+        e.upload(slack); e.merge()
+        assert len(e.download_patches()[0]) == len(slack.insdel)
+        e.append(delta, remap); e.merge()
+        recs = e.download_patches()[0]
+        assert len(recs) == len(want.insdel)
+        u.upload(want); u.merge()
+        assert recs.tobytes() == u.download_patches()[0].tobytes()
+    finally:
+        e.close(); u.close()
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -5,7 +5,6 @@ oracle's after its change, and the Patch JSON of the new ops (patch window) equa
 
 Cases come from tests/test_change_spec.py (KAT inputOps, fuzz-shaped multi-op changes on the append corpora, the named
 corners); tests/test_change_spec.py pins the host specification ``packing.generate_change`` on the same cases."""
-import ctypes
 import json
 
 import numpy as np
@@ -268,14 +267,17 @@ def test_true_shape_c5_document():
 # ------------------------------------------------------------------------------------------------------------------
 # 6. Refusals and state rules
 # ------------------------------------------------------------------------------------------------------------------
-def raw_change(e, n, actor, off, ops, tokens=(), pools=(0, 0, 0), table=None):
-    from peritext_b200.engine import _ChangeInput, _ChangeView, _change_struct
-    actor = np.asarray(actor, np.uint32); off = np.asarray(off, np.uint64); ops = np.asarray(ops, INPUT_OP_DT); tokens = np.asarray(tokens, np.uint32)
-    ptr = lambda a: a.ctypes.data if len(a) else None
-    inp = _ChangeInput(n, ptr(actor), ptr(off), ptr(ops), ptr(tokens), len(tokens), *pools, 0)
-    ct = _change_struct(table) if table is not None else None
-    v = _ChangeView()
-    return e._L.pt_batch_change(e._h, ctypes.byref(inp), ctypes.byref(ct[0]) if ct else None, ctypes.byref(v))
+def change(e, actor, off, ops, tokens=(), pools=(0, 0, 0), table=None):
+    """``change_packed`` from lists: `ops` as op() tuples, `pools` the value, link and comment pool sizes."""
+    return e.change_packed(actor, off, np.array(ops, INPUT_OP_DT), tokens, *pools, table)
+
+
+def refusal(call):
+    """The pt_status of a call the engine refuses."""
+    from peritext_b200.engine import EngineError
+    with pytest.raises(EngineError) as err:
+        call()
+    return err.value.status
 
 
 def op(action, index=0, arg=0, first_ctr=0, mark_type=0, attr=0xFFFFFFFF, tok_off=0):
@@ -291,33 +293,33 @@ def test_refusals_leave_the_batch_unchanged_and_the_state_rules():
     e = engine()
     try:
         e.upload(batch)
-        assert raw_change(e, 4, [0] * 4, [0] * 5, []) == PT_ERR_STATE                  # no merge since the upload
+        assert refusal(lambda: change(e, [0] * 4, [0] * 5, [])) == PT_ERR_STATE                  # no merge since the upload
         before = merged(e)
         snap = everything(e, batch, before)
         mc = [int(x) for x in batch.desc["max_ctr"]]
         na = [int(x) for x in batch.desc["n_actors"]]
         none = 0xFFFFFFFF
         bad = {
-            "n_logs": lambda: raw_change(e, 3, [0] * 3, [0] * 4, []),
-            "actor": lambda: raw_change(e, 4, [na[0], none, none, none], [0] * 5, []),
-            "inputs-without-actor": lambda: raw_change(e, 4, [none] * 4, [0, 1, 1, 1, 1], [op(0, 0, 0, mc[0] + 1)]),
-            "first_ctr": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 1, mc[0])]),
-            "overlap": lambda: raw_change(e, 4, [0, none, none, none], [0, 2, 2, 2, 2], [op(1, 0, 2, mc[0] + 1), op(1, 0, 1, mc[0] + 2)]),
-            "backwards": lambda: raw_change(e, 4, [0, none, none, none], [0, 2, 2, 2, 2], [op(1, 0, 1, mc[0] + 5), op(1, 0, 1, mc[0] + 3)]),
-            "counter-past-32-bits": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 2, 0xFFFFFFFF)]),
-            "action": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(7, 0, 1, mc[0] + 1)]),
-            "mark-type": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=4)]),
-            "attr-link": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=3, attr=2)], pools=(0, 2, 0)),
-            "attr-strong": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=0, attr=0)]),
-            "token-range": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 2, mc[0] + 1)], tokens=[97]),
-            "token-pool": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 1, mc[0] + 1)], tokens=[0x20000000 | 3], pools=(3, 0, 0)),
-            "token-code-point": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 1, mc[0] + 1)], tokens=[0x110000]),
-            "negative-values": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, -1, mc[0] + 1)]),
-            "max_ctr-x-actors": lambda: raw_change(e, 4, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 1, 0x7FFFFFFF // na[0] + 1)]),
-            "table-on-one-side": lambda: raw_change(e, 4, [none] * 4, [0] * 5, [], table=change_table(batch, [], [])),
+            "n_logs": lambda: change(e, [0] * 3, [0] * 4, []),
+            "actor": lambda: change(e, [na[0], none, none, none], [0] * 5, []),
+            "inputs-without-actor": lambda: change(e, [none] * 4, [0, 1, 1, 1, 1], [op(0, 0, 0, mc[0] + 1)]),
+            "first_ctr": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 1, mc[0])]),
+            "overlap": lambda: change(e, [0, none, none, none], [0, 2, 2, 2, 2], [op(1, 0, 2, mc[0] + 1), op(1, 0, 1, mc[0] + 2)]),
+            "backwards": lambda: change(e, [0, none, none, none], [0, 2, 2, 2, 2], [op(1, 0, 1, mc[0] + 5), op(1, 0, 1, mc[0] + 3)]),
+            "counter-past-32-bits": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 2, 0xFFFFFFFF)]),
+            "action": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(7, 0, 1, mc[0] + 1)]),
+            "mark-type": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=4)]),
+            "attr-link": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=3, attr=2)], pools=(0, 2, 0)),
+            "attr-strong": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(2, 0, 1, mc[0] + 1, mark_type=0, attr=0)]),
+            "token-range": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 2, mc[0] + 1)], tokens=[97]),
+            "token-pool": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 1, mc[0] + 1)], tokens=[0x20000000 | 3], pools=(3, 0, 0)),
+            "token-code-point": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, 1, mc[0] + 1)], tokens=[0x110000]),
+            "negative-values": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(0, 0, -1, mc[0] + 1)]),
+            "max_ctr-x-actors": lambda: change(e, [0, none, none, none], [0, 1, 1, 1, 1], [op(1, 0, 1, 0x7FFFFFFF // na[0] + 1)]),
+            "table-on-one-side": lambda: change(e, [none] * 4, [0] * 5, [], table=change_table(batch, [], [])),
         }
         for name, call in bad.items():
-            assert call() == PT_ERR_INVALID, name
+            assert refusal(call) == PT_ERR_INVALID, name
         after = merged(e)
         assert canon(after) == canon(before) and everything(e, batch, after) == snap
         # a log whose merge failed: refused, the batch stays as it was
@@ -330,28 +332,28 @@ def test_refusals_leave_the_batch_unchanged_and_the_state_rules():
             f.upload(broken)
             fb = merged(f)
             assert int(fb.results[1]["status"]) != 0
-            assert raw_change(f, 4, [none, 0, none, none], [0, 0, 1, 1, 1], [op(1, 0, 1, int(broken.desc[1]["max_ctr"]) + 1)]) == PT_ERR_INVALID
-            assert raw_change(f, 4, [none, 0, none, none], [0] * 5, []) == PT_ERR_INVALID      # with an empty change too
+            assert refusal(lambda: change(f, [none, 0, none, none], [0, 0, 1, 1, 1], [op(1, 0, 1, int(broken.desc[1]["max_ctr"]) + 1)])) == PT_ERR_INVALID
+            assert refusal(lambda: change(f, [none, 0, none, none], [0] * 5, [])) == PT_ERR_INVALID      # with an empty change too
             assert canon(merged(f)) == canon(fb)
         finally:
             f.close()
         # the state rules: a change needs a merge after every upload, append and change
         inputs = [{**header(log, a), "ops": ops} for _, log, a, ops in cs]
         batch2 = introduce(e, batch, cs)
-        assert raw_change(e, 4, [none] * 4, [0] * 5, []) == PT_ERR_STATE             # no merge since the append
+        assert refusal(lambda: change(e, [none] * 4, [0] * 5, [])) == PT_ERR_STATE             # no merge since the append
         merged(e)
         ranks = [batch2.log_actors[i].index(a) for i, (_, _, a, _) in enumerate(cs)]
         new, _, status = e.change(batch2, inputs, ranks)
-        assert raw_change(e, 4, [none] * 4, [0] * 5, []) == PT_ERR_STATE             # no merge since the change
+        assert refusal(lambda: change(e, [none] * 4, [0] * 5, [])) == PT_ERR_STATE             # no merge since the change
         with pytest.raises(Exception):
             e.download()                                                              # views of the last merge are invalid
         merged(e)
-        assert raw_change(e, 4, [none] * 4, [0] * 5, []) == 0                         # an empty change: nothing appended
+        change(e, [none] * 4, [0] * 5, [])                                            # an empty change: nothing appended
         merged(e)
         g = BatchEngine(0)
         try:
             g.upload(batch); g.merge()
-            assert raw_change(g, 4, [none] * 4, [0] * 5, []) == PT_ERR_STATE         # no PT_FLAG_EMIT_SEQUENCE
+            assert refusal(lambda: change(g, [none] * 4, [0] * 5, [])) == PT_ERR_STATE         # no PT_FLAG_EMIT_SEQUENCE
         finally:
             g.close()
         with pytest.raises(ValueError, match="append it first|introduce it"):

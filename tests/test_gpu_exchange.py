@@ -232,14 +232,11 @@ def test_dense_counters_on_either_side():
 
 
 def raw_exchange(e, pairs, aoff, amap, coff=None, cmap=None, null=()):
-    from peritext_b200.engine import PAIR_DT, _ExchangeInput, _ExchangeView
-    pr = np.array([tuple(p) for p in pairs], PAIR_DT)
-    arrs = [pr, np.asarray(aoff, np.uint64), np.asarray(amap, np.uint16), None if coff is None else np.asarray(coff, np.uint64),
-            None if cmap is None else np.asarray(cmap, np.uint32)]
-    ptrs = [None if a is None or k in null else a.ctypes.data for k, a in enumerate(arrs)]
-    inp = _ExchangeInput(len(pr), *ptrs)
-    v = _ExchangeView()
-    return e._L.pt_batch_exchange(e._h, ctypes.byref(inp), ctypes.byref(v))
+    """pt_batch_exchange's status; `null` = the positions among (pairs, actor_off, actor_map, ctr_off, ctr_map) passed as NULL."""
+    from peritext_b200.engine import _ExchangeInput, _ExchangeView, _map_arrays, _pairs, _ptr
+    arrs = [_pairs(pairs), *_map_arrays(ExchangeMaps(aoff, amap, coff, cmap))]
+    inp = _ExchangeInput(len(arrs[0]), *[None if k in null else _ptr(a) for k, a in enumerate(arrs)])
+    return e._L.pt_batch_exchange(e._h, ctypes.byref(inp), ctypes.byref(_ExchangeView()))
 
 
 @pytest.mark.gpu
@@ -351,15 +348,10 @@ def test_exchanges_between_and_across_routes():
 # ------------------------------------------------------------------------------------------------------------------
 # 5. A c4-shaped batch of 300 000 logs: one change and one two-way sync per document
 # ------------------------------------------------------------------------------------------------------------------
-def raw_change(e, batch, actor, off, ops, tokens, table):
-    from peritext_b200.engine import _ChangeInput, _ChangeView, _change_struct, _check
-    inp = _ChangeInput(batch.n_logs, actor.ctypes.data, off.ctypes.data, ops.ctypes.data, tokens.ctypes.data, len(tokens), 0, len(batch.link_attrs), 0, 0)
-    ct = _change_struct(table)
-    v = _ChangeView()
-    _check(e._L.pt_batch_change(e._h, ctypes.byref(inp), ctypes.byref(ct[0]), ctypes.byref(v)), "pt_batch_change")
-    arr = lambda p, count, dt: np.frombuffer((ctypes.c_char * (count * dt.itemsize)).from_address(p), dtype=dt, count=count).copy() if count else np.zeros(0, dt)
-    return PackedBatch(arr(v.delta.logs, batch.n_logs, DESC_DT), arr(v.delta.insdel, int(v.delta.n_insdel_total), INSDEL_DT),
-                       arr(v.delta.marks, int(v.delta.n_mark_total), MARK_DT), changes=table)
+def packed_change(e, batch, actor, off, ops, tokens, table):
+    """``change_packed`` of a ``workload.sync_round``; returns its delta as a PackedBatch with the round's change table."""
+    _, desc, insdel, marks = e.change_packed(actor, off, ops, tokens, 0, len(batch.link_attrs), 0, table)
+    return PackedBatch(desc, insdel, marks, changes=table)
 
 
 @pytest.mark.gpu
@@ -373,7 +365,7 @@ def test_c4_300k_logs_one_change_and_one_two_way_sync_per_document():
     try:
         e.upload(base); e.upload_changes(base.changes)
         e.merge()
-        delta = raw_change(e, base, actor, off, ops, tokens, table)
+        delta = packed_change(e, base, actor, off, ops, tokens, table)
         changed = apply_append(base, delta)
         status, (doff, flat), desc = e.exchange(pairs, maps)
         assert (status == 0).all()

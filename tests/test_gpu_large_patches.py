@@ -16,7 +16,7 @@ from peritext_b200.packing import pack_logs, patch_stream
 from tests.harness import environ, fuzz_session
 from tests.test_gpu_admission import tampered_logs
 from tests.test_gpu_patch_bounds import (cap_cases, corner_cases, encode, exact_case, list_ops, log_changes, marks_then_edits, named_cases,
-                                         oracle_per_op, set_patch_pool, splice)
+                                         oracle_per_op, splice)
 from tests.test_gpu_patch_window import check_window, merge_all
 from tests.test_gpu_routes import COMMENT, EM, FAULTS, LINK, STRONG, batch_of, lamport_forward, with_fault
 
@@ -41,7 +41,7 @@ def large_pass(e, batch, warp=True):
         merged = e.run(batch)
     recs, items, status, needed = e.download_patches()
     if needed > len(items):
-        set_patch_pool(e, needed + 16)
+        e.set_patch_pool(needed + 16)
         e.merge(); merged = e.download()
         recs, items, status, needed = e.download_patches()
     return merged, recs, items, status, needed
@@ -176,7 +176,7 @@ def test_windows_on_declined_logs_equal_the_whole_log_tail():
             win = merge_all(e, batch)
             check_window(batch, whole, win, w)
             # a pool of exactly the window's demand
-            set_patch_pool(e, max(1, win[4]))
+            e.set_patch_pool(max(1, win[4]))
             e.merge(); e.download()
             _, items, _, needed = e.download_patches()
             assert needed == win[4] and len(items) == needed
@@ -221,12 +221,12 @@ def test_pool_overflow_reports_the_exact_demand_and_one_retry_succeeds():
     try:
         full = large_pass(e, batch)
         check_large(batch, logs, full)
-        set_patch_pool(e, full[4] // 3)
+        e.set_patch_pool(full[4] // 3)
         e.merge(); e.download()
         recs, items, status, needed = e.download_patches()
         assert needed == full[4] and len(items) == full[4] // 3 and recs.tobytes() == full[1].tobytes()
         assert not (Counter(map(tuple, items.tolist())) - Counter(map(tuple, full[2].tolist())))
-        set_patch_pool(e, needed)
+        e.set_patch_pool(needed)
         e.merge(); merged = e.download()
         check_large(batch, logs, (merged, *e.download_patches()))
     finally:

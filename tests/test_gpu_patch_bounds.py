@@ -466,17 +466,12 @@ def pengine():
     e.close()
 
 
-def set_patch_pool(e, items):
-    from peritext_b200.engine import _check
-    _check(e._L.pt_batch_set_patch_pool(e._h, items), "pt_batch_set_patch_pool")
-
-
 def patch_pass(e, batch, retry=True):
     """One device pass: (merged, recs, items, status, n_items_needed), re-merged once with the reported pool demand."""
     merged = e.run(batch)
     recs, items, status, needed = e.download_patches()
     if retry and needed > len(items):
-        set_patch_pool(e, needed + 16)
+        e.set_patch_pool(needed + 16)
         e.merge(); merged = e.download()
         recs, items, status, needed = e.download_patches()
     return merged, recs, items, status, needed
@@ -691,7 +686,7 @@ def test_truncated_pass_and_engine_reuse_after_set_patch_pool():
         _, frecs, fitems, fstatus, fneeded = full
         # a pool smaller than the demand: the pool is full, the records are untouched, the items are a sub-multiset
         cap = fneeded // 3
-        set_patch_pool(e, cap)
+        e.set_patch_pool(cap)
         e.merge(); e.download()
         recs, items, status, needed = e.download_patches()
         assert len(items) == cap and needed == fneeded

@@ -12,7 +12,7 @@ import pytest
 
 from peritext_b200.packing import _root_text_list, apply_append, json_pools, pack_append, pack_logs
 from tests.harness import fuzz_session
-from tests.test_gpu_patch_bounds import list_ops, set_patch_pool
+from tests.test_gpu_patch_bounds import list_ops
 from tests.test_gpu_render_json import dense_comments, kat_logs
 from tests.test_gpu_render_patches_json import O, oracle_per_change
 from tests.test_patch_window import cut_json, in_window, inner_spans, n_ops, window_split
@@ -33,7 +33,7 @@ def merge_all(e, batch):
     out = e._download_with_pool_retry()
     recs, items, status, needed = e.download_patches()
     if needed > len(items):
-        set_patch_pool(e, needed)
+        e.set_patch_pool(needed)
         e.merge(); out = e.download()
         recs, items, status, needed = e.download_patches()
     assert needed == len(items)
@@ -235,11 +235,11 @@ def test_c4_tail_window_fits_a_pool_of_its_demand():
         assert (whole[0]["status"] == 0).all() and (whole[3] == 0).all()
         e.upload(batch)
         e.set_patch_window(w)
-        set_patch_pool(e, 16)
+        e.set_patch_pool(16)
         e.merge(); e.download()
         _, items, _, needed = e.download_patches()
         assert len(items) == min(16, needed) and 16 < needed < whole[4] // 10, (needed, whole[4])
-        set_patch_pool(e, needed)
+        e.set_patch_pool(needed)
         win = merge_all(e, batch)
         assert win[4] == needed
         check_window(batch, whole, win, w)

@@ -284,7 +284,7 @@ def test_spec_emits_what_json_stringify_writes():
 def ingest_pools(logs):
     """pt_ingest_pool kinds 0 / 1 / 3 of the logs, raw (data, offsets) as the native ingest hands them out."""
     import ctypes
-    from peritext_b200.engine import _check, load_library
+    from peritext_b200.engine import _check, _view, load_library
     L = load_library()
     blobs = [json.dumps(l).encode("utf-8") for l in logs]
     ptrs = (ctypes.c_char_p * len(blobs))(*blobs)
@@ -297,8 +297,8 @@ def ingest_pools(logs):
         for kind in (0, 1, 3):
             data, off, cnt, first = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_void_p()
             _check(L.pt_ingest_pool(h, kind, ctypes.byref(data), ctypes.byref(off), ctypes.byref(cnt), ctypes.byref(first)), "pt_ingest_pool")
-            o = np.frombuffer((ctypes.c_char * (8 * (cnt.value + 1))).from_address(off.value), np.uint64).copy() if off.value else np.zeros(1, np.uint64)
-            d = np.frombuffer(ctypes.string_at(data.value, int(o[-1])), np.uint8).copy() if int(o[-1]) else np.zeros(0, np.uint8)
+            o = _view(off.value, cnt.value + 1, np.uint64) if off.value else np.zeros(1, np.uint64)
+            d = _view(data.value, o[-1], np.uint8)
             out += [d, o]
         return tuple(out)
     finally:
@@ -498,7 +498,7 @@ def test_failed_logs_render_as_nothing():
 @pytest.mark.gpu
 def test_render_edge_cases():
     import ctypes
-    from peritext_b200.engine import BatchEngine, EngineError, _JsonPools, _JsonView
+    from peritext_b200.engine import BatchEngine, EngineError, _JsonPools, _JsonView, _json_pools
     logs = unicode_logs()
     batch = pack_logs(logs)
     e = BatchEngine(0, emit_patches=True)
@@ -547,8 +547,8 @@ def test_render_edge_cases():
         assert len(p[0]) == 0
         ref, _ = replay_packed(plain)
         assert_render_matches(e, plain, ref, p)
-        lk, lo, cm, co = (np.ascontiguousarray(x) for x in p[2:])
-        st = _JsonPools(None, None, 0, lk.ctypes.data, lo.ctypes.data, len(lo) - 1, cm.ctypes.data if cm.size else None, co.ctypes.data, len(co) - 1)
+        st, _keep = _json_pools(plain, p)
+        st.values = st.values_off = None
         v = _JsonView()
         assert e._L.pt_batch_render_json(e._h, ctypes.byref(st), ctypes.byref(v)) == 0 and v.n_logs == plain.n_logs
         empty = batch.select([])

@@ -18,7 +18,7 @@ from oracle.oracle import Micromerge as O
 from peritext_b200.packing import (SPAN_COMMENT, SPAN_EM, SPAN_LINK, SPAN_STRONG, DevicePatches, _root_text_list, json_pools, pack_logs,
                                    patch_stream)
 from tests.harness import fuzz_session, generateDocs, load_kats
-from tests.test_gpu_patch_bounds import encode, list_ops, oracle_per_op, set_patch_pool
+from tests.test_gpu_patch_bounds import encode, list_ops, oracle_per_op
 from tests.test_gpu_render_json import (HI, LO, dense_comments, fragment, fuzz_logs, ingest_pools, json_string, kat_logs, token_units,
                                         unicode_logs)
 
@@ -421,7 +421,7 @@ def test_two_merges_render_identical_bytes():
 
 @pytest.mark.gpu
 def test_render_patches_edge_cases():
-    from peritext_b200.engine import BatchEngine, EngineError, _JsonPools, _JsonView, _PatchView, _check
+    from peritext_b200.engine import BatchEngine, EngineError, _JsonPools, _JsonView, _PatchView, _check, _json_pools
     logs = unicode_logs()
     batch = pack_logs(logs)
     # a handle without PT_FLAG_EMIT_PATCHES
@@ -441,13 +441,13 @@ def test_render_patches_edge_cases():
         with pytest.raises(EngineError, match="out of order"):
             e.render_patches_json(batch)
         # a truncated item pool: PT_ERR_STATE with the demand; one re-merge with that pool size renders
-        set_patch_pool(e, 4)
+        e.set_patch_pool(4)
         e.merge(); e.download()
         _, items, _, needed = e.download_patches()
         assert len(items) == 4 and needed > 4
         with pytest.raises(EngineError, match="out of order.*needs %d patch items" % needed):
             e.render_patches_json(batch)
-        set_patch_pool(e, needed)
+        e.set_patch_pool(needed)
         with pytest.raises(EngineError, match="out of order.*replaced after the last merge"):
             e.render_patches_json(batch)
         e.merge()
@@ -477,10 +477,7 @@ def test_render_patches_edge_cases():
         pv = _PatchView()
         _check(L.pt_batch_download_patches(e._h, ctypes.byref(pv)), "pt_batch_download_patches")
         pv_recs = ctypes.string_at(pv.recs, len(recs) * 16)
-        arrs = [np.ascontiguousarray(a, dtype=np.uint8 if k % 2 == 0 else np.uint64) for k, a in enumerate(full)]
-        ptr = lambda a: a.ctypes.data if a.size else None
-        st = _JsonPools(ptr(arrs[0]), ptr(arrs[1]), len(arrs[1]) - 1, ptr(arrs[2]), ptr(arrs[3]), len(arrs[3]) - 1,
-                        ptr(arrs[4]), ptr(arrs[5]), len(arrs[5]) - 1)
+        st, _keep = _json_pools(batch, full)
         vs, vp = _JsonView(), _JsonView()
         assert L.pt_batch_render_json(e._h, ctypes.byref(st), ctypes.byref(vs)) == 0
         spans_json = ctypes.string_at(vs.bytes, vs.n_bytes)

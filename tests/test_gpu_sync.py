@@ -14,7 +14,7 @@ from peritext_b200.packing import (CDESC_DT, CHANGE_DT, CHANGE_NO_ACTOR, DEP_DT,
                                    pack_logs, range_requests, string_pools)
 from tests.test_exchange_model import SESSIONS, dense_logs, record_session, replay, three_replicas
 from tests.test_gpu_append import canon, merged
-from tests.test_gpu_exchange import engine, raw_change, same_as_upload, upload
+from tests.test_gpu_exchange import engine, packed_change, same_as_upload, upload
 from tests.test_change_spec import replica
 from tests.test_sync_model import spec_sync, turning_dense
 
@@ -187,12 +187,9 @@ def test_dst_turning_dense_is_decided_on_the_device():
 # 4. Table lifetime
 # ------------------------------------------------------------------------------------------------------------------
 def raw_sync(e, pairs, null=False):
-    from peritext_b200.engine import PAIR_DT, _SyncView
-    pr = np.zeros(len(pairs), PAIR_DT)
-    for k, (s, d) in enumerate(pairs):
-        pr[k] = (s, d)
-    v = _SyncView()
-    return e._L.pt_batch_sync_pairs(e._h, None if null or not len(pr) else pr.ctypes.data, len(pr), ctypes.byref(v))
+    from peritext_b200.engine import _SyncView, _pairs, _ptr
+    pr = _pairs(pairs)
+    return e._L.pt_batch_sync_pairs(e._h, None if null else _ptr(pr), len(pr), ctypes.byref(_SyncView()))
 
 
 @pytest.mark.gpu
@@ -275,13 +272,13 @@ def test_add_actors_on_the_device():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# 5. A closed loop that keeps no records on the host: add_actors, raw pt_batch_change, two-way sync, merge
+# 5. A closed loop that keeps no records on the host: add_actors, change_packed, two-way sync, merge
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_records_free_closed_loop():
     """Documents with two replicas each, logs 2d and 2d + 1.  Per round one replica of every document inserts a character: its
     actor is introduced with pt_batch_add_actors (the second replica's id sorts before the first's, so ranks move), the change
-    goes through raw pt_batch_change (InputOperations, the change record, dep ranks from pt_batch_download_actors), then both
+    goes through pt_batch_change from arrays (InputOperations, the change record, dep ranks from pt_batch_download_actors), then both
     replicas sync both ways with pt_batch_sync_pairs and the batch merges.  The host keeps only the reference replicas, which
     replay the same calls; at the end the handle equals their pack_logs, the replicas' digests agree, and the Change JSON
     rendered with the downloaded tables equals the one rendered with string_pools of that batch."""
@@ -321,8 +318,7 @@ def test_records_free_closed_loop():
             cd["change_off"] = np.cumsum(cd["n_changes"]) - cd["n_changes"]; cd["dep_off"] = np.cumsum(cd["n_deps"]) - cd["n_deps"]
             table = ChangeTable(cd, ch, np.array(deps, DEP_DT) if deps else np.zeros(0, DEP_DT))
             tokens = np.array([ord("xyz"[rnd % 3])] * n_docs, np.uint32)
-            got = int(raw_change(e, _Shape(n), actor, off, ops, tokens, table).desc["n_insdel"].sum())
-            e._n_insdel += got; e._n_seq += got                          # the sizes BatchEngine.change would have recorded
+            e.change_packed(actor, off, ops, tokens, 0, 0, 0, table)
             pairs = [(2 * d + r, 2 * d + 1 - r) for d in range(n_docs)] + [(2 * d + 1 - r, 2 * d + r) for d in range(n_docs)]
             status, (doff, flat), _, _ = e.sync_pairs(pairs)
             assert (status == EXCHANGE_OK).all() and np.diff(doff.astype(np.int64)).tolist() == [1] * n_docs + [0] * n_docs
@@ -341,11 +337,6 @@ def test_records_free_closed_loop():
     finally:
         e.close(); u.close()
 
-
-class _Shape:
-    """What raw_change reads of a batch: its log count and link pool."""
-    def __init__(self, n):
-        self.n_logs, self.link_attrs = n, []
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -403,7 +394,7 @@ def test_c4_300k_logs_sync_pairs_equals_exchange_with_host_maps():
     try:
         for h in (e, f):
             h.upload(base); h.upload_changes(base.changes); h.merge()
-            raw_change(h, base, actor, off, ops, tokens, table)
+            packed_change(h, base, actor, off, ops, tokens, table)
         e.upload_actors(base)
         s1, (o1, d1), desc1, (aoff, _) = e.sync_pairs(pairs)
         s2, (o2, d2), desc2 = f.exchange(pairs, maps)

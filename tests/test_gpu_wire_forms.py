@@ -502,7 +502,7 @@ def patches_as(e, batch, form):
     e.merge(); out = e.download()
     recs, items, status, needed = e.download_patches()
     if needed > len(items):
-        e._L.pt_batch_set_patch_pool(e._h, needed + 16)
+        e.set_patch_pool(needed + 16)
         e.merge(); out = e.download()
         recs, items, status, needed = e.download_patches()
     items = np.sort(items, order=["log", "tag", "a", "b"])

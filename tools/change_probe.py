@@ -12,7 +12,6 @@ with the patch window set to the new ops.  Prints one JSON line per case, with t
 from __future__ import annotations
 
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -24,7 +23,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from peritext_b200 import workload  # noqa: E402
-from peritext_b200.engine import BatchEngine, _ChangeInput, _ChangeView, _check  # noqa: E402
+from peritext_b200.engine import BatchEngine  # noqa: E402
 from peritext_b200.packing import INPUT_OP_DT  # noqa: E402
 
 
@@ -57,16 +56,9 @@ def inputs_for(batch, res, per_log, seed=7):
 
 
 def call(e, batch, actor, off, ops, tokens):
-    ptr = lambda a: a.ctypes.data if len(a) else None
-    inp = _ChangeInput(batch.n_logs, ptr(actor), ptr(off), ptr(ops), ptr(tokens), len(tokens), 0, len(batch.link_attrs), 0, 0)
-    v = _ChangeView()
     t0 = time.perf_counter()
-    _check(e._L.pt_batch_change(e._h, ctypes.byref(inp), None, ctypes.byref(v)), "pt_batch_change")
-    dt = time.perf_counter() - t0
-    desc = np.frombuffer((ctypes.c_char * (batch.n_logs * 32)).from_address(v.delta.logs), np.uint8).view(np.dtype(
-        [("insdel_off", "<u8"), ("mark_off", "<u8"), ("n_insdel", "<u4"), ("n_mark", "<u4"), ("n_actors", "<u4"), ("max_ctr", "<u4")])).copy()
-    st = np.frombuffer((ctypes.c_char * (batch.n_logs * 8)).from_address(v.status), np.uint32).reshape(-1, 2).copy()
-    return dt, desc, st
+    st, desc, _, _ = e.change_packed(actor, off, ops, tokens, 0, len(batch.link_attrs), 0)
+    return time.perf_counter() - t0, desc, st
 
 
 def case(name, batch, per_log):
@@ -91,7 +83,7 @@ def case(name, batch, per_log):
             if getattr(ev, "device_time_total", 0):
                 kern[ev.key.split("(")[0][:80]] = round(ev.device_time_total / 1000.0, 3)
         torch.cuda.synchronize()
-        return {"case": name, "logs": batch.n_logs, "inputs": int(args[1][-1]), "failed_logs": int((st[:, 0] != 0).sum()),
+        return {"case": name, "logs": batch.n_logs, "inputs": int(args[1][-1]), "failed_logs": int((st["status"] != 0).sum()),
                 "new_records": int(desc["n_insdel"].sum() + desc["n_mark"].sum()), "call_ms": round(dt * 1000, 3),
                 "kernel_ms": kern, "window_merge_ms": round(float(merge_ms), 3)}
     finally:

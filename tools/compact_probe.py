@@ -2,7 +2,7 @@ import sys, time, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, ctypes
 from peritext_b200 import workload
-from peritext_b200.engine import PipelinedEngine, INSDEL_C8_DT, MARK_C16_DT, _PackedOps, load_library
+from peritext_b200.engine import PipelinedEngine, INSDEL_C8_DT, MARK_C16_DT, _packed_ops, load_library
 from peritext_b200.packing import INSDEL_DT, MARK_DT, PackedBatch
 b = workload.generate("c4", n_docs=int(sys.argv[1]) if len(sys.argv) > 1 else 30000)
 def pinned(a): return torch.from_numpy(a.view(np.uint8).reshape(-1)).pin_memory()
@@ -11,7 +11,7 @@ pb = PackedBatch(b.desc, p_ins.numpy()[: b.insdel.nbytes].view(INSDEL_DT), p_mk.
 L = load_library()
 ci = torch.empty(len(b.insdel) * 8, dtype=torch.uint8).pin_memory(); cm = torch.empty(len(b.marks) * 16, dtype=torch.uint8).pin_memory()
 desc = np.ascontiguousarray(b.desc)
-ops = _PackedOps(len(desc), desc.ctypes.data, pb.insdel.ctypes.data, len(pb.insdel), pb.marks.ctypes.data, len(pb.marks))
+ops = _packed_ops(desc, pb.insdel, len(pb.insdel), pb.marks, len(pb.marks))
 for T in (16, 32, 64, 128):
     L.pt_compact_ops(ctypes.byref(ops), ci.data_ptr(), cm.data_ptr(), T)
     t0 = time.perf_counter(); L.pt_compact_ops(ctypes.byref(ops), ci.data_ptr(), cm.data_ptr(), T); dt = time.perf_counter() - t0

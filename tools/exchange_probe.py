@@ -17,7 +17,6 @@ Prints one JSON line with the GPU's name and power limit; needs a GPU.
 from __future__ import annotations
 
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -30,20 +29,14 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from peritext_b200 import workload  # noqa: E402
-from peritext_b200.engine import BatchEngine, _ChangeInput, _ChangeView, _change_struct, _check  # noqa: E402
-from peritext_b200.packing import CDESC_DT, DESC_DT, INSDEL_DT, MARK_DT, ChangeTable, PackedBatch, _ranges  # noqa: E402
+from peritext_b200.engine import BatchEngine  # noqa: E402
+from peritext_b200.packing import CDESC_DT, DESC_DT, MARK_DT, ChangeTable, PackedBatch, _ranges  # noqa: E402
 
 
 def change(e, batch, actor, off, ops, tokens, table):
-    """pt_batch_change from arrays; returns the view's delta (descriptors and ins/del records; the probe's change has no marks)."""
-    inp = _ChangeInput(batch.n_logs, actor.ctypes.data, off.ctypes.data, ops.ctypes.data, tokens.ctypes.data, len(tokens), 0, len(batch.link_attrs), 0, 0)
-    ct = _change_struct(table)
-    v = _ChangeView()
-    _check(e._L.pt_batch_change(e._h, ctypes.byref(inp), ctypes.byref(ct[0]), ctypes.byref(v)), "pt_batch_change")
-    arr = lambda p, count, dt: np.frombuffer((ctypes.c_char * (count * dt.itemsize)).from_address(p), dtype=dt, count=count) if count else np.zeros(0, dt)
-    desc = arr(v.delta.logs, batch.n_logs, DESC_DT).copy()
-    e._n_insdel += int(desc["n_insdel"].sum()); e._n_seq += int(desc["n_insdel"].sum())
-    return desc, arr(v.delta.insdel, int(v.delta.n_insdel_total), INSDEL_DT)
+    """``change_packed`` of the round; returns the delta's descriptors and ins/del records (the probe's change has no marks)."""
+    _, desc, recs, _ = e.change_packed(actor, off, ops, tokens, 0, len(batch.link_attrs), 0, table)
+    return desc, recs
 
 
 def readdress(batch, desc, recs, table, src, dst):

@@ -49,7 +49,7 @@ def stats(ts):
 
 
 def case(name, full, reps, pool=None, whole_render=True):
-    from peritext_b200.engine import BatchEngine, EngineError, _check
+    from peritext_b200.engine import BatchEngine, EngineError
     from peritext_b200.packing import json_pools, split_records
     n_ins = full.desc["n_insdel"].astype(np.int64)
     prefix, delta = split_records(full, (n_ins * 99) // 100)
@@ -58,7 +58,7 @@ def case(name, full, reps, pool=None, whole_render=True):
     e = BatchEngine(0, emit_patches=True)
     note = "default patch pool"
     if pool is not None:
-        _check(e._L.pt_batch_set_patch_pool(e._h, int(pool)), "pt_batch_set_patch_pool")
+        e.set_patch_pool(pool)
         note = f"patch pool sized to {int(pool)} items"
     try:
         e.upload(prefix)
