@@ -128,7 +128,7 @@ struct pt_batch {
     uint32_t adm_maxR = 1;
     const pt_insdel_rec* dp_insdel = nullptr;
     const pt_mark_rec* dp_marks = nullptr;
-    DevBuf d_half_insdel, d_half_marks;   // the warp kernel's half-width copy of the records (derive_half_records); empty when
+    DevBuf d_key_insdel, d_key_marks;     // the warp kernel's key-record copy of the records (derive_key_records); empty when
                                           // no log is on a warp route
     // pinned host
     HostBuf h_stage, h_results, h_text, h_spans, h_pool, h_misc, h_seq, h_ctoff, h_csoff;
@@ -386,25 +386,24 @@ int begin_upload(pt_batch* b, const pt_packed_ops& ops, bool own_records) {
     return install_plan(b, ops, std::move(plan), own_records);
 }
 
-// The warp kernel's half-width copy of the records the merge reads (upload_kernel.cuh), derived on the batch's stream wherever
+// The warp kernel's key-record copy of the records the merge reads (upload_kernel.cuh), derived on the batch's stream wherever
 // those records change: at every upload and when pt_batch_append swaps in the spliced records.  A batch without a log on a
 // warp route keeps no copy.
-int derive_half_records(pt_batch* b) {
+int derive_key_records(pt_batch* b) {
     const uint32_t* nr = b->plan.n_route;
-    if (!(nr[ptp::kPacked3] + nr[ptp::kCompact] + nr[ptp::kDirect])) { b->d_half_insdel.release(); b->d_half_marks.release(); return PT_OK; }
+    if (!(nr[ptp::kPacked3] + nr[ptp::kCompact] + nr[ptp::kDirect])) { b->d_key_insdel.release(); b->d_key_marks.release(); return PT_OK; }
     int rc;
-    if ((rc = reserve_n<uint2>(b->d_half_insdel, b->n_insdel)) || (rc = reserve_n<uint4>(b->d_half_marks, b->n_mark))) return rc;
-    const uint64_t total = b->n_insdel + b->n_mark;
-    const uint32_t threads = 256;      // one thread per record
-    if (total) {
-        ptu::derive_half_records_kernel<<<warp_grid(b, total, threads, 1), threads, 0, b->stream>>>(
-            b->dp_insdel, b->dp_marks, (uint2*)b->d_half_insdel.p, (uint4*)b->d_half_marks.p, b->n_insdel, b->n_mark);
+    if ((rc = reserve_n<uint32_t>(b->d_key_insdel, b->n_insdel)) || (rc = reserve_n<uint2>(b->d_key_marks, b->n_mark))) return rc;
+    const uint32_t threads = 256;      // one warp per log
+    if (b->n_logs) {
+        ptu::derive_key_records_kernel<<<warp_grid(b, b->n_logs, threads), threads, 0, b->stream>>>(
+            (const pt_log_desc*)b->d_desc.p, b->dp_insdel, b->dp_marks, (uint32_t*)b->d_key_insdel.p, (uint2*)b->d_key_marks.p, b->n_logs);
         PT_CUDA(launched(b));
     }
     return PT_OK;
 }
 
-// Shared finish: the records the merge reads and their half-width copy, and a wait for the copies when one of the caller's
+// Shared finish: the records the merge reads and their key-record copy, and a wait for the copies when one of the caller's
 // sources (pointer, bytes read) is pageable, because such a buffer may be freed on return (pinned ones stay asynchronous).
 int finish_upload(pt_batch* b, const void* insdel, const void* marks, std::initializer_list<std::pair<const void*, uint64_t>> sources) {
     bool pageable = false;
@@ -416,7 +415,7 @@ int finish_upload(pt_batch* b, const void* insdel, const void* marks, std::initi
     }
     b->dp_insdel = (const pt_insdel_rec*)insdel; b->dp_marks = (const pt_mark_rec*)marks;
     int rc;
-    if ((rc = derive_half_records(b))) return rc;
+    if ((rc = derive_key_records(b))) return rc;
     if (pageable) PT_CUDA(cudaStreamSynchronize(b->stream));
     b->have_batch = true;
     return PT_OK;
@@ -909,7 +908,7 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
     if ((rc = install_plan(b, ops, std::move(plan), true))) return rc;
     PT_CUDA(cudaStreamSynchronize(b->stream));
     b->dp_insdel = (const pt_insdel_rec*)b->d_insdel.p; b->dp_marks = (const pt_mark_rec*)b->d_marks.p;
-    if ((rc = derive_half_records(b))) return rc;
+    if ((rc = derive_key_records(b))) return rc;
     b->have_batch = true;
     return PT_OK;
 }
@@ -1547,7 +1546,7 @@ static int enqueue_merge(pt_batch* b) {
     ptk::BatchParams P{};
     P.desc = (const pt_log_desc*)b->d_desc.p;
     P.insdel = b->dp_insdel; P.marks = b->dp_marks;
-    P.half_insdel = (const uint2*)b->d_half_insdel.p; P.half_marks = (const uint4*)b->d_half_marks.p;
+    P.key_insdel = (const uint32_t*)b->d_key_insdel.p; P.key_marks = (const uint2*)b->d_key_marks.p;
     P.results = (pt_log_result*)b->d_results.p;
     P.text_off = (const uint64_t*)b->d_text_off.p; P.span_off = (const uint64_t*)b->d_span_off.p;
     P.text = (uint32_t*)b->d_text.p; P.spans = (pt_span*)b->d_spans.p;

@@ -33,8 +33,8 @@ struct BatchParams {
     const pt_log_desc* __restrict__ desc;
     const pt_insdel_rec* __restrict__ insdel;
     const pt_mark_rec* __restrict__ marks;
-    const uint2* __restrict__ half_insdel;   // the warp kernel's half-width copy of insdel / marks (upload_kernel.cuh); null when
-    const uint4* __restrict__ half_marks;    // no log is on a warp route
+    const uint32_t* __restrict__ key_insdel;   // the warp kernel's key-record copy of insdel / marks (upload_kernel.cuh); null
+    const uint2* __restrict__ key_marks;       // when no log is on a warp route
     const uint32_t* __restrict__ order;   // log indices of this launch (bin), largest first
     uint32_t n_work;
     uint32_t* work_counter;               // persistent-CTA work queue head

@@ -32,7 +32,7 @@ Route route_of(const pt_log_desc& L, const RouteConfig& cfg, bool emit_sequence)
     // short logs: one warp per log.  Footprint estimate: id table (packed3: three actors, 2 bits per key; compact: >= 3
     // actors, one slot per counter + overflow) + bitmaps + run-tree temporaries for ~ n/3 runs; a low guess only costs a
     // device-side deferral
-    // (<= 255 actors: the warp kernel reads actors from 8-bit fields of the records' half-width copy, upload_kernel.cuh)
+    // (<= 255 actors: a log with more actors goes to the CTA kernel, the route tests/test_gpu_merge_copy.py pins)
     if (cfg.warp_on && key16 && R <= 255 && recs <= cfg.warp.max_recs) {
         const bool packed3 = R == 3 && n <= 1022, compact = R >= 3 && R <= 30 && n <= 2046;
         const uint64_t idbytes = packed3 ? 4ull * L.max_ctr : compact ? 2ull * L.max_ctr + 512 : 2 * KS;

@@ -1,5 +1,5 @@
 // upload_kernel.cuh — expansion of the optional upload wire forms (pt_batch_upload_runs, pt_batch_upload_compact) into the
-// pt_insdel_rec / pt_mark_rec records the merge kernels read, and the warp kernel's half-width copy of those records.
+// pt_insdel_rec / pt_mark_rec records the merge kernels read, and the warp kernel's key-record copy of those records.
 #pragma once
 #include <cstdint>
 
@@ -74,30 +74,55 @@ __global__ void expand_mark_c16_kernel(const pt_mark_c16* __restrict__ in, pt_ma
     }
 }
 
-// ---- the warp kernel's half-width copy of the resident records (warp_kernel.cuh reads it and nothing else on its streams) -----
-// Same record positions as the full arrays, so the descriptors' offsets index it unchanged.
-//   ins/del, 8 B (uint2):  x = ctr:16 | ref_ctr:16 << 16;  y = actor:8 | ref_actor:8 << 8 | kind:2 << 16   (no payload)
-//   mark, 16 B (uint4):    x = ctr:16 | start_ctr:16 << 16;  y = end_ctr:16 | arrival:16 << 16;  z = attr;
-//                          w = actor:8 | start_actor:8 << 8 | end_actor:8 << 16 | kind:3 << 24 | bounds:4 << 27
-// A counter or arrival too wide for its field saturates at 0xFFFF, an actor at 255.  The warp routes have C * R < 0xFFFF,
-// n < 0xFFFF and R <= 255 (ptp::route_of), so a saturated id fails the same range check as the original and a saturated
-// arrival still exceeds every record index: the copy changes no warp-kernel result.  The warp kernel reads no mark kind bit
-// above 2 and no bound bit above 3.
-__device__ __forceinline__ uint32_t sat16(uint32_t v) { return min(v, 0xFFFFu); }
-__device__ __forceinline__ uint32_t sat8(uint32_t v) { return min(v, 0xFFu); }
-__global__ void derive_half_records_kernel(const pt_insdel_rec* __restrict__ ins, const pt_mark_rec* __restrict__ mk,
-                                           uint2* __restrict__ hins, uint4* __restrict__ hmk, unsigned long long n, unsigned long long m) {
-    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n + m; i += (unsigned long long)gridDim.x * blockDim.x) {
-        if (i < n) {
-            const uint4 r = __ldg(reinterpret_cast<const uint4*>(ins + i));   // {ctr, ref_ctr, actor | ref_actor << 16, payload}
-            hins[i] = make_uint2(sat16(r.x) | (sat16(r.y) << 16), sat8(r.z & 0xFFFFu) | (sat8(r.z >> 16) << 8) | ((r.w >> 30) << 16));
-        } else {
-            const uint4* q = reinterpret_cast<const uint4*>(mk + (i - n));
+// ---- the warp kernel's key-record copy of the resident records (warp_kernel.cuh reads it and nothing else on its streams) -----
+// Same record positions as the full arrays, so the descriptors' offsets index it unchanged.  An id (c, a) of a log with
+// C * R < 0xFFFF is stored as its 16-bit opId key (c - 1) * R + a, which is at most 0xFFFD; the two values above it are never
+// keys and carry what the record passes branch on:
+//   ins/del, 4 B (uint32):  own:16 | ref:16 << 16
+//       kind > 1: own = ref = S1;  own id out of range: own = S1, ref = S0;  delete: own = S0;
+//       ref = S0 at the head (ref_ctr == 0), the key of the reference if it is in range, else S1
+//   mark, 8 B (uint2):      x = own:16 | start:16 << 16;  y = end:16 | arrival:11 << 16 | kind:3 << 27 | start bound:1 << 30 |
+//                           end bound:1 << 31
+//       own = S1: the id is out of range;  start / end = S1: the id is out of range or the bound is above PT_BOUND_AFTER (the
+//       op then covers nothing / never ends);  a bound bit is kept only for a valid bound;  arrival = min(arrival, n), which
+//       fits 11 bits on every log the warp kernel merges marks of (n <= 2047), and compares with every record index the same
+// The warp kernel reads no mark kind bit above 2.  One warp per log; a log with C * R >= 0xFFFF is not on a warp route and
+// is left unwritten.  The link and comment attrs stay in the full mark records (warp_kernel.cuh reads them for survivors).
+constexpr uint32_t kKeyS0 = 0xFFFEu, kKeyS1 = 0xFFFFu;
+__global__ void derive_key_records_kernel(const pt_log_desc* __restrict__ desc, const pt_insdel_rec* __restrict__ ins,
+                                          const pt_mark_rec* __restrict__ mk, uint32_t* __restrict__ kins, uint2* __restrict__ kmk,
+                                          uint32_t n_logs) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t li = warp; li < n_logs; li += nwarps) {
+        const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(desc + li)), d1 = __ldg(reinterpret_cast<const uint4*>(desc + li) + 1);
+        const uint32_t n = d1.x, m = d1.y, R = d1.z ? d1.z : 1u, C = d1.w;
+        if ((unsigned long long)C * R >= 0xFFFFull) continue;
+        const unsigned long long io = (unsigned long long)d0.x | ((unsigned long long)d0.y << 32);
+        const unsigned long long mo = (unsigned long long)d0.z | ((unsigned long long)d0.w << 32);
+        auto key = [&](uint32_t c, uint32_t a) -> uint32_t { return c - 1u < C && a < R ? (c - 1u) * R + a : kKeyS1; };
+        for (uint32_t i = lane; i < n; i += 32) {
+            const uint4 r = __ldg(reinterpret_cast<const uint4*>(ins + io + i));   // {ctr, ref_ctr, actor | ref_actor << 16, payload}
+            const uint32_t kind = r.w >> 30;
+            uint32_t own = kind > 1u ? kKeyS1 : key(r.x, r.z & 0xFFFFu), ref = kKeyS1;
+            if (kind <= 1u) {
+                if (own == kKeyS1) ref = kKeyS0;
+                else {
+                    if (kind == PT_KIND_DELETE) own = kKeyS0;
+                    ref = r.y == 0 ? kKeyS0 : key(r.y, r.z >> 16);
+                }
+            }
+            kins[io + i] = own | (ref << 16);
+        }
+        const uint32_t narr = min(n, 0x7FFu);
+        for (uint32_t k = lane; k < m; k += 32) {
+            const uint4* q = reinterpret_cast<const uint4*>(mk + mo + k);
             // {ctr, actor | kind << 16 | bounds << 24, start_ctr, end_ctr} {start_actor | end_actor << 16, attr, arrival, reserved}
             const uint4 a = __ldg(q), b = __ldg(q + 1);
-            hmk[i - n] = make_uint4(sat16(a.x) | (sat16(a.z) << 16), sat16(a.w) | (sat16(b.z) << 16), b.y,
-                                    sat8(a.y & 0xFFFFu) | (sat8(b.x & 0xFFFFu) << 8) | (sat8(b.x >> 16) << 16) |
-                                        (((a.y >> 16) & 7u) << 24) | (((a.y >> 24) & 0xFu) << 27));
+            const uint32_t sb = (a.y >> 24) & 3u, eb = (a.y >> 26) & 3u;
+            const uint32_t s = sb <= PT_BOUND_AFTER ? key(a.z, b.x & 0xFFFFu) : kKeyS1, e = eb <= PT_BOUND_AFTER ? key(a.w, b.x >> 16) : kKeyS1;
+            kmk[mo + k] = make_uint2(key(a.x, a.y & 0xFFFFu) | (s << 16),
+                                     e | (min(b.z, narr) << 16) | (((a.y >> 16) & 7u) << 27) |
+                                         ((sb <= PT_BOUND_AFTER ? sb : 0u) << 30) | ((eb <= PT_BOUND_AFTER ? eb : 0u) << 31));
         }
     }
 }

@@ -16,6 +16,7 @@
 // the device to the block kernel's bins (merge_kernel.cuh) — results are identical either way.
 #pragma once
 #include "merge_kernel.cuh"
+#include "upload_kernel.cuh"
 
 namespace ptk {
 
@@ -112,14 +113,17 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     const unsigned long long mark_off = (unsigned long long)dsc0.z | ((unsigned long long)dsc0.w << 32);
     const uint32_t n = dsc1.x, m = dsc1.y, R = dsc1.z ? dsc1.z : 1u, C = dsc1.w;
     const unsigned long long KS64 = (unsigned long long)C * R;
-    // 16-bit keys / indices only, and actors that fit the 8-bit fields of the half-width records (the host routes no other log here)
-    if (KS64 >= 0xFFFFull || n >= 0xFFFFu || m >= 0xFFFFu || R > 255u) { ps.leave(); return 1; }
+    // 16-bit keys / indices only, and arrivals that fit the 11-bit field of the key records (the host routes no other log here
+    // at the default max_recs)
+    if (KS64 >= 0xFFFFull || n >= 0xFFFFu || m >= 0xFFFFu || (m && n > 2047u)) { ps.leave(); return 1; }
     const uint32_t KS = (uint32_t)KS64;
-    // the record streams are read from the half-width copy (upload_kernel.cuh: ins {ctr | ref_ctr << 16, actor | ref_actor << 8 |
-    // kind << 16}, marks {ctr | start_ctr << 16, end_ctr | arrival << 16, attr, actor | start_actor << 8 | end_actor << 16 |
-    // kind << 24 | bounds << 27}); only phase F reads the full ins/del records, for the payloads of visible elements
-    const uint2* __restrict__ ins = P.half_insdel + insdel_off;
-    const uint4* __restrict__ mk = P.half_marks + mark_off;
+    // the record streams are read from the key-record copy (upload_kernel.cuh: ins own:16 | ref:16, marks {own | start << 16,
+    // end | arrival << 16 | kind << 27 | start bound << 30 | end bound << 31}, keys K = (ctr-1)*R + actor, kS0 / kS1 above every
+    // key); phase F reads the full ins/del records for the payloads of visible elements, and G's link and comment survivors
+    // their attrs from the full mark records
+    constexpr uint32_t kS0 = ptu::kKeyS0, kS1 = ptu::kKeyS1;
+    const uint32_t* __restrict__ ins = P.key_insdel + insdel_off;
+    const uint2* __restrict__ mk = P.key_marks + mark_off;
     const pt_insdel_rec* __restrict__ full_ins = P.insdel + insdel_off;
     uint32_t* text_out = P.text + P.text_off[li];
     pt_span* span_out = P.spans + P.span_off[li];
@@ -127,14 +131,12 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
 
     if ((P.warp_flags & 1u) && m) {       // this log's mark records are needed late: pull them into L2 now
         const char* p0 = reinterpret_cast<const char*>(mk);
-        const uint32_t lines = (m * 16u + 127u) >> 7;
+        const uint32_t lines = (m * 8u + 127u) >> 7;
         for (uint32_t l = lane; l < lines; l += 32) prefetch_l2(p0 + ((size_t)l << 7));
     }
 
     WArena A; A.base = slice_base; A.used = 0; A.cap = slice_bytes;
     uint32_t st = 0;                                           // lane-local failures, bit (1 << code); the checkpoints report the highest code
-    auto keyOf = [&](uint32_t ctr, uint32_t actor) -> uint32_t { return (ctr - 1u) * R + actor; };
-    auto badId = [&](uint32_t ctr, uint32_t actor) -> bool { return ctr - 1u >= C || actor >= R; };
     auto fail = [&](uint32_t code) { st |= 1u << code; };
     // a duplicate insert opId sets bit 0 (no status has code 0): it is reported as PT_LOG_BAD_OPID only when the record pass
     // found no other failure — the block and team kernels count duplicates only after their record pass (DESIGN.md §2)
@@ -170,14 +172,18 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     wfill<uint32_t>(reinterpret_cast<uint32_t*>(WI), 4 * NWr, 0u, lane);
     __syncwarp();
     auto ovHash = [&](uint32_t key) -> uint32_t { return ((key * 40503u) >> 7) & (kOvSlots - 1u); };
-    // index of the insert record with opId (ctr, actor), kNone16 if there is none; the id must be in range (!badId)
-    auto lookup = [&](uint32_t ctr, uint32_t actor) -> uint32_t {
-        if (packed) { const uint32_t f = (T32[ctr - 1u] >> (10u * actor)) & 1023u; return f ? f - 1u : kNone16; }
-        if (!compact) return T[keyOf(ctr, actor)];
-        const uint32_t e = T[ctr - 1u];
+    // key -> (ctr - 1, actor).  packed3: key / 3 as a multiply-high, exact for 16-bit keys.  compact: key / R with the log's
+    // reciprocal ceil(2^32 / R), exact for 16-bit keys (the error is below (R-1) * 2^16 / 2^32 < 1 / R)
+    const uint32_t invR = compact ? 0xFFFFFFFFu / R + 1u : 0u;
+    auto ctrOf = [&](uint32_t key) -> uint32_t { return packed ? (key * 0xAAABu) >> 17 : __umulhi(key, invR); };
+    // index of the insert record with opId key `key`, kNone16 if there is none; the key must be valid (< kS0)
+    auto lookup = [&](uint32_t key) -> uint32_t {
+        if (!packed && !compact) return T[key];
+        const uint32_t c = ctrOf(key), actor = key - c * (packed ? 3u : R);
+        if (packed) { const uint32_t f = (T32[c] >> (10u * actor)) & 1023u; return f ? f - 1u : kNone16; }
+        const uint32_t e = T[c];
         if (e == kNone16) return kNone16;                      // no insert with this counter at all
         if ((e >> 11) == actor) return e & 0x7FFu;
-        const uint32_t key = keyOf(ctr, actor);
         for (uint32_t h = ovHash(key);; h = (h + 1u) & (kOvSlots - 1u)) {
             const uint32_t v = OV[h];
             if (v == kOvEmpty) return kNone16;
@@ -185,7 +191,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         }
     };
 
-    // ---- A+B: one pass over the ins/del records, 32 per trip (256 B), two trips in flight -----------------------------------
+    // ---- A+B: one pass over the ins/del records, 32 per trip (128 B), two trips in flight -----------------------------------
     // A: id table, insert bits, chain-link bits (reference element == the insert at record i-1: compare with the left
     //    neighbour's key, no lookup).  B: parents of non-chain inserts ("has another child" bits) and deletes (tombstones, OR).
     //    A referenced element must have arrived EARLIER in the log (src/micromerge.ts:752 throws otherwise).
@@ -194,45 +200,40 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         uint32_t carryK = 0xFFFFFFFFu;                         // key of the last record of the previous trip if it is an insert
         // records past the end are loaded from a clamped index and ignored (every use is guarded by i < n)
         const uint32_t nm1 = n ? n - 1u : 0u;
-        uint2 ra = make_uint2(0, 0);
+        uint32_t ra = 0;
         if (n) ra = __ldg(ins + min(lane, nm1));
-        // an L2 prefetch stream runs >= 18 trips (4.5 KB) ahead of the register loads: DRAM latency under load is longer than
-        // two trips.  Every 16th trip all 32 lanes fetch the 32 lines of 16 later trips (one uniform branch per trip otherwise).
+        // the whole stream past the first two trips (a c4 log's is ~2 KB) goes to L2 up front: DRAM latency under load is longer
+        // than two trips
         const char* insb = reinterpret_cast<const char*>(ins);
-        const uint32_t insBytes = n * 8u;
-        if (lane * 128u + 512u < insBytes) prefetch_l2(insb + 512u + lane * 128u);            // trips 2 .. 17
+        const uint32_t insBytes = n * 4u;
+        for (uint32_t o = 256u + lane * 128u; o < insBytes; o += 32u * 128u) prefetch_l2(insb + o);
         PT_PHASE(kPhStart);
 #pragma unroll 2
         for (uint32_t base = 0; base < n; base += 32) {
             const uint32_t i = base + lane;
-            if ((base & 511u) == 0u) {                                                       // trips t+18 .. t+33
-                const uint32_t po = (base + 576u) * 8u + lane * 128u;
-                if (po < insBytes) prefetch_l2(insb + po);
-            }
-            const uint2 rc = __ldg(ins + min(i + 32u, nm1));            // one trip ahead (the lines are in L2 by now); unrolled by 2: no moves
-            const uint2 r = ra;
-            const uint32_t ctr = r.x & 0xFFFFu, ref_ctr = r.x >> 16, actor = r.y & 0xFFu, ref_actor = (r.y >> 8) & 0xFFu, kind = r.y >> 16;
-            // straight-line form: predicates instead of nested branches
+            const uint32_t rc = __ldg(ins + min(i + 32u, nm1));         // one trip ahead (the lines are in L2 by now); unrolled by 2: no moves
+            const uint32_t own = ra & 0xFFFFu, rkey = ra >> 16;
+            // straight-line form: predicates instead of nested branches.  own == kS1: a bad kind (rkey == kS1) or a bad opId;
+            // own == kS0: a delete; else an insert with key own.  rkey: kS0 = the head, kS1 = out of range, else a key
             const bool inb = i < n;
-            const bool kbad = kind > 1u, ibad = badId(ctr, actor);
-            const bool valid = inb && !kbad && !ibad;
-            if (inb && kbad) fail(PT_LOG_BAD_KIND);
-            if (inb && ibad) fail(PT_LOG_BAD_OPID);
-            const uint32_t key = keyOf(ctr, actor);
-            const bool isIns = valid && kind == PT_KIND_INSERT;
+            const bool valid = inb && own != kS1;
+            if (inb && !valid) fail(rkey == kS1 ? PT_LOG_BAD_KIND : PT_LOG_BAD_OPID);
+            const uint32_t key = own;
+            const bool isIns = valid && own != kS0;
             bool toOv = false, wrote = false;
             uint32_t mine = 0;
             if (isIns) {
                 if (packed) {
-                    const uint32_t sh = 10u * actor;
-                    if ((atomicOr(&T32[ctr - 1u], (i + 1u) << sh) >> sh) & 1023u) failDup();   // two inserts with one opId
+                    const uint32_t c = ctrOf(key), sh = 10u * (key - 3u * c);
+                    if ((atomicOr(&T32[c], (i + 1u) << sh) >> sh) & 1023u) failDup();   // two inserts with one opId
                 } else if (!compact) {
                     if (T[key] != kNone16) failDup();                  // two inserts with one opId (earlier trip)
                     T[key] = (uint16_t)i;
                 } else {
+                    const uint32_t c = ctrOf(key), actor = key - c * R;
                     mine = (actor << 11) | i;
-                    const uint32_t e = T[ctr - 1u];
-                    if (e == kNone16) { T[ctr - 1u] = (uint16_t)mine; wrote = true; }
+                    const uint32_t e = T[c];
+                    if (e == kNone16) { T[c] = (uint16_t)mine; wrote = true; }
                     else if ((e >> 11) == actor) failDup();
                     else toOv = true;
                 }
@@ -241,8 +242,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             uint32_t prevK = __shfl_up_sync(kFull, myK, 1);
             if (lane == 0) prevK = carryK;
             carryK = __shfl_sync(kFull, myK, 31);
-            const bool refOk = ref_ctr != 0 && !badId(ref_ctr, ref_actor);
-            const uint32_t rkey = keyOf(ref_ctr, ref_actor);
+            const bool refOk = rkey < kS0;
             bool cand = isIns && refOk && rkey == prevK;           // typing-chain link: the reference element is record i-1
             if (cand && rkey >= key) { fail(PT_LOG_CYCLE); cand = false; }
             const uint32_t insW = __ballot_sync(kFull, isIns), candW = __ballot_sync(kFull, cand);
@@ -252,8 +252,8 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                 if (isIns && T[key] != (uint16_t)i) failDup();               // two inserts with one opId (same trip)
             } else if (compact) {
                 if (wrote) {                                       // same counter twice in one trip: one lane owns the slot
-                    const uint32_t e2 = T[ctr - 1u];
-                    if (e2 != mine) { if ((e2 >> 11) == actor) failDup(); else toOv = true; }
+                    const uint32_t e2 = T[ctrOf(key)];
+                    if (e2 != mine) { if ((e2 >> 11) == (mine >> 11)) failDup(); else toOv = true; }
                 }
                 const uint32_t ovW = __ballot_sync(kFull, toOv);
                 if (ovW) {
@@ -269,10 +269,10 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                     __syncwarp();
                 }
             }
-            {   // B: the reference element of a non-chain record (ref_ctr == 0: an insert at the head of the list)
-                const bool need = valid && !cand, hasRef = ref_ctr != 0;
+            {   // B: the reference element of a non-chain record (rkey == kS0: an insert at the head of the list)
+                const bool need = valid && !cand, hasRef = rkey != kS0;
                 uint32_t j = kNone16;
-                if (need && refOk) j = lookup(ref_ctr, ref_actor);
+                if (need && refOk) j = lookup(rkey);
                 const bool found = j != kNone16 && j < i;              // must have arrived earlier
                 const bool cyc = isIns && rkey >= key;
                 if (need) {
@@ -307,9 +307,8 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t pc = __popc(head) | (__popc(vis) << 16);
             const uint32_t inc = warp_incl_scan(pc, lane), ex = inc - pc, tot = __shfl_sync(kFull, inc, 31);
             if (w < NWr) WI[w] = make_uint4(insW, head, vis, (carryH + (ex & 0xFFFFu)) | ((carryV + (ex >> 16)) << 16));
-            // phase D reads every run head's record again: the 128-byte lines (16 records) that hold heads go to L2 now, all at once
-            if (head & 0xFFFFu) prefetch_l2(ins + w * 32u);
-            if (head >> 16) prefetch_l2(ins + w * 32u + 16u);
+            // phase D reads every run head's record again: the 128-byte lines (32 records) that hold heads go to L2 now, all at once
+            if (head) prefetch_l2(ins + w * 32u);
             carryH += tot & 0xFFFFu; carryV += tot >> 16;
             N += __reduce_add_sync(kFull, (uint32_t)__popc(insW));
         }
@@ -370,14 +369,14 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t r = rb + lane;
             if (r < M) {
                 const uint32_t i = HV[r], w = i >> 5, b = i & 31;
-                const uint2 rec = __ldg(ins + i);                  // issued before the run-end scan: its latency overlaps the scan
+                const uint32_t rec = __ldg(ins + i);               // issued before the run-end scan: its latency overlaps the scan
                 const uint4 q0 = WI[w];
                 uint32_t stop = (q0.y | ~q0.x) & ~(0xFFFFFFFFu >> (31 - b));
                 uint32_t ww = w;
                 while (!stop) { ww++; const uint2 q1 = *reinterpret_cast<const uint2*>(&WI[ww]); stop = q1.y | ~q1.x; }   // pad word: insert bits == 0 -> stops
                 const uint32_t end = ww * 32 + (__ffs(stop) - 1);
-                const uint32_t key = keyOf(rec.x & 0xFFFFu, rec.y & 0xFFu), ref_ctr = rec.x >> 16;
-                const uint32_t p = ref_ctr == 0 ? n : lookup(ref_ctr, (rec.y >> 8) & 0xFFu);
+                const uint32_t key = rec & 0xFFFFu, rkey = rec >> 16;   // a run head is a valid insert: rkey is kS0 or a key
+                const uint32_t p = rkey == kS0 ? n : lookup(rkey);
                 const uint32_t q = p == n ? M : runOf(p);
                 const uint32_t hv = visBefore(i);
                 N16[2 * r + 1] = (uint16_t)(visBefore(end) - hv);
@@ -525,20 +524,20 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     uint32_t nspans = 0;
     if ((P.warp_flags & 2u) && li_next != 0xFFFFFFFFu) {        // the next log's ins/del records -> L2 while this one does its marks
         const uint4 q0 = __ldg(reinterpret_cast<const uint4*>(P.desc + li_next)), q1 = __ldg(reinterpret_cast<const uint4*>(P.desc + li_next) + 1);
-        const char* p0 = reinterpret_cast<const char*>(P.half_insdel + ((unsigned long long)q0.x | ((unsigned long long)q0.y << 32)));
-        const uint32_t lines = (q1.x * 8u + 127u) >> 7;
+        const char* p0 = reinterpret_cast<const char*>(P.key_insdel + ((unsigned long long)q0.x | ((unsigned long long)q0.y << 32)));
+        const uint32_t lines = (q1.x * 4u + 127u) >> 7;
         for (uint32_t l = lane; l < lines; l += 32) prefetch_l2(p0 + ((size_t)l << 7));
     }
 
-    // the first 12 trips (6 KB) of mark records -> L2 now, just before G: prefetched right after C, most lines were evicted from
+    // the first 24 trips (6 KB) of mark records -> L2 now, just before G: prefetched right after C, most lines were evicted from
     // L2 (thousands of logs in flight stream through it) before G read them (DESIGN.md §4.1)
     if (m) {
-        const uint32_t pfb = min(m * 16u, 6u * 1024u);
+        const uint32_t pfb = min(m * 8u, 6u * 1024u);
         for (uint32_t o = lane * 128u; o < pfb; o += 32u * 128u) prefetch_l2(reinterpret_cast<const char*>(mk) + o);
     }
     PT_PHASE(kPhF);
     uint32_t nS = 0, nC = 0;
-    uint4* Sv = nullptr;                                           // survivors: {va | vb << 16, priority:16 | kind << 16, attr, -}
+    uint4* Sv = nullptr;                                           // survivors: {va | vb << 16, priority:16 | kind << 16, attr, k}
     uint16_t* CIdx = nullptr;                                      // surviving comment ops (indices into Sv), arrival order
     if (m) {
         // ---- G: mark ops -> visible intervals [va, vb); only ops that cover a visible element survive ---------------------
@@ -554,42 +553,41 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         wfill<uint32_t>(KBits, KW + 1, 0u, lane);
         __syncwarp();
         const uint32_t mm1 = m - 1u;                               // m > 0 here; past-the-end lanes load a clamped record, unused
-        uint4 a = __ldg(mk + min(lane, mm1));
-        const uint32_t mkBytes = m * 16u;
+        uint2 a = __ldg(mk + min(lane, mm1));
+        const uint32_t mkBytes = m * 8u;
 #pragma unroll 2
         for (uint32_t kb = 0; kb < m; kb += 32) {
             const uint32_t k = kb + lane;
-            if ((kb & 255u) == 0u) {                               // every 8th trip: the 32 lines of trips t+12 .. t+19 (512 B per trip)
-                const uint32_t po = (kb + 384u) * 16u + lane * 128u;
+            if ((kb & 511u) == 0u) {                               // every 16th trip: the 32 lines of trips t+24 .. t+39 (256 B per trip)
+                const uint32_t po = (kb + 768u) * 8u + lane * 128u;
                 if (po < mkBytes) prefetch_l2(reinterpret_cast<const char*>(mk) + po);
             }
-            const uint4 b = __ldg(mk + min(k + 32u, mm1));         // one trip ahead (L2 hits); unrolled by 2: no moves
-            const uint32_t ctr = a.x & 0xFFFFu, start_ctr = a.x >> 16, end_ctr = a.y & 0xFFFFu, arrival = a.y >> 16, attr = a.z;
-            const uint32_t actor = a.w & 0xFFu, start_actor = (a.w >> 8) & 0xFFu, end_actor = (a.w >> 16) & 0xFFu, kind = (a.w >> 24) & 7u, bounds = a.w >> 27;
+            const uint2 b = __ldg(mk + min(k + 32u, mm1));         // one trip ahead (L2 hits); unrolled by 2: no moves
+            // own / start / end == kS1: the id is out of range (a start or end also when its bound is above PT_BOUND_AFTER)
+            const uint32_t key = a.x & 0xFFFFu, skey = a.x >> 16, ekey = a.y & 0xFFFFu, arrival = (a.y >> 16) & 0x7FFu;
+            const uint32_t kind = (a.y >> 27) & 7u, sb = (a.y >> 30) & 1u, eb = a.y >> 31;
             const uint32_t type = (kind >> 1) & 3u;
             // straight-line form (predicated loads instead of nested branches).  A boundary element must exist AND have arrived
             // before the mark op: the reference's walk never matches anything else (peritext.ts:236-241) — a missing start is a
             // no-op, a missing end never ends
             const bool inb = k < m;
-            const bool idok = inb && !badId(ctr, actor);
-            const uint32_t key = keyOf(ctr, actor);
+            const bool idok = inb && key != kS1;
             bool dup = false;
             if (idok) {
                 const uint32_t bit = 1u << (key & 31);
-                dup = (atomicOr(&KBits[key >> 5], bit) & bit) != 0 || lookup(ctr, actor) != kNone16;      // duplicate opId
+                dup = (atomicOr(&KBits[key >> 5], bit) & bit) != 0 || lookup(key) != kNone16;      // duplicate opId
             }
             if (inb && (!idok || dup)) fail(PT_LOG_BAD_OPID);
-            const uint32_t sb = bounds & 3u, eb = (bounds >> 2) & 3u;
-            const bool sOk = idok && sb <= PT_BOUND_AFTER && !badId(start_ctr, start_actor);
+            const bool sOk = idok && skey != kS1;
             uint32_t js = kNone16;
-            if (sOk) js = lookup(start_ctr, start_actor);
+            if (sOk) js = lookup(skey);
             const bool sHit = js != kNone16 && js < arrival;
             uint32_t es = 0;
             if (sHit) es = EV[js];
             const uint32_t va = (es & 0x7FFFu) + (sb & (es >> 15));
-            const bool eOk = sHit && eb <= PT_BOUND_AFTER && !badId(end_ctr, end_actor);
+            const bool eOk = sHit && ekey != kS1;
             uint32_t je = kNone16;
-            if (eOk) je = lookup(end_ctr, end_actor);
+            if (eOk) je = lookup(ekey);
             // same slot: the start branch wins and the op never ends (quirk Q2)
             const bool eHit = je != kNone16 && je < arrival && !(je == js && eb == sb);
             uint32_t vb = nvis;
@@ -601,7 +599,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                 const uint32_t idx = nS + __popc(bal & lt);
                 if (idx < capS) {
                     // priority: LWW types compare opIds (peritext.ts:304-313) = keys; comments fold in arrival order (Q4)
-                    Sv[idx] = make_uint4(va | (vb << 16), (type == PT_MARK_COMMENT ? k : key) | (kind << 16), attr, 0u);
+                    Sv[idx] = make_uint4(va | (vb << 16), (type == PT_MARK_COMMENT ? k : key) | (kind << 16), PT_ATTR_NONE, k);
                     if (isC) { const uint32_t ci = nC + __popc(balC & lt); if (ci <= kMaxCommentSurvivors) CIdx[ci] = (uint16_t)idx; }
                 }
             }
@@ -613,6 +611,15 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         if (st) { bail(31u - __clz(st)); ps.leave(); return 0; }
         if (nS > capS) { ps.leave(); return 1; }
         A.used = svStart + ((nS * 16u + 15u) & ~15u);               // keep only the survivors
+        // the attrs of the link and comment survivors (phase I reads no other) from the full records, all loads in flight at once
+        const pt_mark_rec* __restrict__ full_mk = P.marks + (mk - P.key_marks);
+#pragma unroll 1
+        for (uint32_t s = lane; s < nS; s += 32) {
+            const uint4 sv = Sv[s];
+            const uint32_t t = (sv.y >> 17) & 3u;
+            if (t == PT_MARK_LINK || t == PT_MARK_COMMENT) Sv[s].z = __ldg(&full_mk[sv.w].attr);
+        }
+        __syncwarp();
     }
 
     ps.pass();                                                     // (5) marks resolved
