@@ -396,7 +396,7 @@ typedef struct pt_append_remap {      /* NULL pointer = identity everywhere */
  * length or is not strictly increasing; ctr_map[0] != 0; a mapped old bound (identity included; for the counter map, the
  * image of the old max_ctr) exceeds the new n_actors / max_ctr; a delta descriptor or arrival is out of range; a log would exceed 2^32 - 1 records; a change table on one side
  * only.  No batch: PT_ERR_STATE.  The device refuses too: a resident comment rank (other than PT_ATTR_NONE) outside
- * comment_map gives PT_ERR_INVALID with the batch untouched, because the splice writes new record buffers and only a
+ * comment_map, or mapped to 0xFFFFFFFF, gives PT_ERR_INVALID with the batch untouched, because the splice writes new record buffers and only a
  * successful one replaces the old.
  * On success: the batch is re-planned like an upload (routes, capacities and the patch kernel's shared memory can change),
  * there is no merge (views of the last merge are invalid, as after an upload), comment-pool and patch-pool settings persist
@@ -475,7 +475,7 @@ typedef struct pt_change_view {
  * NULL iff the handle has no change table); the records of failed logs are dropped.  A new actor or comment id shifts packed
  * ranks: introduce it first with a pt_batch_append of an empty delta and its remap, then call this with the new ranks.
  * Refused before anything changes:
- *   PT_ERR_STATE    no completed merge since the last upload, append or change; a handle without PT_FLAG_EMIT_SEQUENCE
+ *   PT_ERR_STATE    no completed merge since the last upload, append, change or select; a handle without PT_FLAG_EMIT_SEQUENCE
  *   PT_ERR_INVALID  (pt_last_error names the first offender) n_logs differs; input_off not increasing from 0 or past the ops; a log
  *                   with inputs and no actor; an actor rank >= the log's n_actors; a log with a change whose merge status is not
  *                   PT_LOG_OK; an unknown action or mark type; first_ctr not above the log's max_ctr, or below the previous
@@ -592,7 +592,7 @@ typedef struct pt_actor_tables {
  * count or decreases; a log's count is not its n_actors (0 is allowed only when n_actors == 1); an id of odd byte length; ids
  * not strictly increasing in UTF-16 code-unit order (JS string order, compareOpIds).  No batch: PT_ERR_STATE.
  * Lifetime: every upload form and pt_batch_adopt_device drop the tables (as they drop the change table); pt_batch_change and
- * pt_batch_exchange keep them; pt_batch_append keeps them only when its remap has no actor map, no counter map and no log's
+ * pt_batch_exchange keep them; pt_batch_select_logs gathers them with their logs; pt_batch_append keeps them only when its remap has no actor map, no counter map and no log's
  * n_actors changes (a comment-only remap keeps them).  Synchronises; the caller's arrays may be freed on return. */
 int pt_batch_upload_actors(pt_batch*, const pt_actor_tables* tables);
 
@@ -666,6 +666,45 @@ typedef struct pt_sync_view {
  * a map kernel (one warp per pair), then pt_batch_exchange's kernels.  Besides the pairs, 32 B per pair and the moved logs'
  * rank maps cross PCIe. */
 int pt_batch_sync_pairs(pt_batch*, const pt_exchange_pair* pairs, uint32_t n_pairs, pt_sync_view* out);
+
+/* ------------------------------------------------------------------------------------------------
+ * Select: change WHICH logs the resident batch holds, on the device.  A server that opens and closes documents, or a sync
+ * session in which a new replica joins (a fresh Micromerge that applies the initial change, then syncs), keeps every log that
+ * stays resident, including what pt_batch_change, pt_batch_exchange and pt_batch_sync_pairs wrote there, and uploads only the
+ * logs it adds.
+ * ---------------------------------------------------------------------------------------------- */
+#define PT_SELECT_ADDED 0xFFFFFFFFu
+/* New log i = resident log from[i], or, where from[i] == PT_SELECT_ADDED, the next log of `added` (in order).  `from` may drop
+ * logs, reorder them and name one log several times (a fork: a replica with the same state and arrival order).
+ * A kept log keeps its records, descriptor fields, change and dep records and actor table; only the comment ranks of its
+ * comment marks move, through comment_map (old rank -> new rank, n_comment_map entries; NULL = identity).  The mapped entries
+ * (all but 0xFFFFFFFF) strictly increase; 0xFFFFFFFF drops a rank that no kept log names, so retiring documents can shrink the
+ * batch-wide comment order.  An added log's records, change table (added_changes, dep_off relative to the log's deps, as for
+ * an upload) and actor ids (added_actors, pt_batch_upload_actors' layout and rules) are in the new id space and are copied
+ * verbatim: value-pool indices and link ids carry no order and never move, and counters and actor ranks are per log.
+ * added is NULL or has 0 logs iff no entry is PT_SELECT_ADDED; then added_changes and added_actors are NULL.  Otherwise
+ * added_changes is NULL iff the handle has no change table, and added_actors NULL iff it has no actor tables.
+ * On success the handle holds exactly what pt_batch_upload of the selected batch, pt_batch_upload_changes of its change table
+ * and pt_batch_upload_actors of its actor tables would hold: the batch is re-planned and its key records derived again, there
+ * is no merge (views of the last merge are invalid), the patch window is reset, and comment-pool and patch-pool settings
+ * persist.  n_logs == 0 is accepted, as by pt_batch_upload.
+ * Refused with nothing changed:
+ *   PT_ERR_STATE    no batch
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) from[i] >= the old n_logs and not PT_SELECT_ADDED; the number of
+ *                   PT_SELECT_ADDED entries is not added->n_logs; an added descriptor or change descriptor out of range; a
+ *                   change table or actor tables on one side only, or added actor tables that pt_batch_upload_actors refuses;
+ *                   comment_map not strictly increasing over its mapped entries; a new batch that an upload refuses (make_plan)
+ * The device refuses too: a kept comment mark whose rank is outside comment_map or maps to 0xFFFFFFFF gives PT_ERR_INVALID with
+ * the batch untouched, because the splice writes new buffers and only a successful one replaces the old.
+ * Synchronises; the caller's arrays may be freed on return.
+ * Device: pt_batch_append's splice with a gather index (one warp per new log, up to 64 for a log with many records, 16-byte
+ * coalesced copies; a log without a comment map is a straight copy) and a warp-per-log gather of the actor tables.  Peak
+ * device memory: old + added + new records (and change and actor tables). */
+int pt_batch_select_logs(pt_batch*, const uint32_t* from, uint32_t n_logs,
+                         const pt_packed_ops* added,            /* NULL iff no entry is PT_SELECT_ADDED           */
+                         const pt_change_table* added_changes,  /* NULL iff the handle has no change table          */
+                         const pt_actor_tables* added_actors,   /* NULL iff the handle has no actor tables          */
+                         const uint32_t* comment_map, uint64_t n_comment_map);   /* NULL = identity              */
 
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */

@@ -8,6 +8,9 @@
 // the boundary actors and the attr, with the fields it needs from its partner by one shuffle.  A log whose maps are all
 // identity is a straight copy.  splice_changes_kernel does the same for the change and dep tables (actor ranks only; the
 // delta changes' dep_off moves past the log's old deps).
+//
+// Both kernels also run pt_batch_select_logs: `from` names the resident log each new log copies (nullptr: log i itself, as in
+// an append; PT_SELECT_ADDED: none, so the log's records are all the delta's).  A select passes only the comment map.
 #pragma once
 #include <cstdint>
 
@@ -40,15 +43,22 @@ __device__ __forceinline__ LogMaps log_maps(const Remap& R, uint32_t li) {
     return m;
 }
 
+// The resident descriptor new log li copies: its own, log from[li]'s, or an empty one for an added log.
+template <class Desc>
+__device__ __forceinline__ Desc source_desc(const Desc* __restrict__ old, const uint32_t* __restrict__ from, uint32_t li) {
+    const uint32_t s = from ? __ldg(from + li) : li;
+    return s == PT_SELECT_ADDED ? Desc{} : old[s];
+}
+
 __global__ void splice_records_kernel(const pt_log_desc* __restrict__ old_desc, const pt_log_desc* __restrict__ new_desc,
-                                      const pt_log_desc* __restrict__ delta_desc, uint32_t n_logs, Remap R,
+                                      const pt_log_desc* __restrict__ delta_desc, const uint32_t* __restrict__ from, uint32_t n_logs, Remap R,
                                       const pt_insdel_rec* __restrict__ old_ins, const pt_mark_rec* __restrict__ old_marks,
                                       const pt_insdel_rec* __restrict__ delta_ins, const pt_mark_rec* __restrict__ delta_marks,
                                       pt_insdel_rec* __restrict__ new_ins, pt_mark_rec* __restrict__ new_marks, uint32_t* __restrict__ bad) {
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
     const uint32_t first = blockIdx.y * 32u + lane, step = gridDim.y * 32u;     // this warp's slice of each log
     for (uint32_t li = warp; li < n_logs; li += nwarps) {
-        const pt_log_desc O = old_desc[li], N = new_desc[li], D = delta_desc[li];
+        const pt_log_desc O = source_desc(old_desc, from, li), N = new_desc[li], D = delta_desc[li];
         const LogMaps m = log_maps(R, li);
         const bool ident = !m.na && !m.nc && !R.comment_map;       // warp-uniform
         // ins/del records: {ctr, ref_ctr, actor | ref_actor << 16, payload}
@@ -86,8 +96,8 @@ __global__ void splice_records_kernel(const pt_log_desc* __restrict__ old_desc, 
                     const uint32_t sa = m.id_actor(pz, q.x & 0xFFFFu), ea = m.id_actor(pw, q.x >> 16);
                     q.x = (sa & 0xFFFFu) | (ea << 16);
                     if (R.comment_map && ((py >> 17) & 3u) == PT_MARK_COMMENT && q.y != PT_ATTR_NONE) {
-                        if (q.y < R.n_comment) q.y = __ldg(R.comment_map + q.y);
-                        else atomicOr(bad, 1u);                    // refused: the new buffers are not used
+                        q.y = q.y < R.n_comment ? __ldg(R.comment_map + q.y) : PT_ATTR_NONE;
+                        if (q.y == PT_ATTR_NONE) atomicOr(bad, 1u);   // refused: the new buffers are not used
                     }
                 }
                 md[k] = q;
@@ -101,13 +111,13 @@ __global__ void splice_records_kernel(const pt_log_desc* __restrict__ old_desc, 
 // Change table splice: per log, the old change records (actor mapped), the delta's (dep_off rebased past the log's old
 // deps), the old dep records (actor mapped), the delta's.
 __global__ void splice_changes_kernel(const pt_change_desc* __restrict__ old_cd, const pt_change_desc* __restrict__ new_cd,
-                                      const pt_change_desc* __restrict__ delta_cd, uint32_t n_logs, Remap R,
+                                      const pt_change_desc* __restrict__ delta_cd, const uint32_t* __restrict__ from, uint32_t n_logs, Remap R,
                                       const pt_change_rec* __restrict__ old_ch, const pt_dep_rec* __restrict__ old_dp,
                                       const pt_change_rec* __restrict__ delta_ch, const pt_dep_rec* __restrict__ delta_dp,
                                       pt_change_rec* __restrict__ new_ch, pt_dep_rec* __restrict__ new_dp) {
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t li = warp; li < n_logs; li += nwarps) {
-        const pt_change_desc O = old_cd[li], N = new_cd[li], D = delta_cd[li];
+        const pt_change_desc O = source_desc(old_cd, from, li), N = new_cd[li], D = delta_cd[li];
         const LogMaps m = log_maps(R, li);
         // change records: {seq, actor | n_deps << 16, dep_off, n_ops}
         const uint4* cs = reinterpret_cast<const uint4*>(old_ch + O.change_off);

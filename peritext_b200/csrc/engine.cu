@@ -816,31 +816,30 @@ static std::string check_append(const pt_batch* b, const pt_packed_ops& delta, b
     return std::string();
 }
 
-// pt_batch_append after its host checks, and the append of pt_batch_change and pt_batch_exchange (`fn` prefixes the error text):
-// `delta`'s records are host memory, or device memory the caller keeps alive (delta_on_device); so are the change and dep
-// records of `dch` (table_on_device).  The delta's descriptors, the remap and the change table's descriptors are host memory.
-static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R,
-                         const pt_change_table* dch, bool table_on_device) {
-    std::vector<pt_log_desc> nd;
-    std::vector<pt_change_desc> ncd;
-    uint32_t maxR = 1;
-    std::string err = check_append(b, *delta, delta_on_device, R, dch, nd, ncd, maxR);
-    const uint32_t n = b->n_logs;
-    const bool sized = err.empty() && n;                      // nd is filled only when the checks passed
-    const uint64_t n_ins = sized ? nd[n - 1].insdel_off + nd[n - 1].n_insdel : 0, n_mk = sized ? nd[n - 1].mark_off + nd[n - 1].n_mark : 0;
+// The splice of pt_batch_append and pt_batch_select_logs once their host checks pass: new log i (nd[i], ncd[i]) is the resident
+// log from[i] (from == nullptr: log i; PT_SELECT_ADDED: none) with its ids through R's maps, followed by delta log i's records,
+// and likewise for the change table.  `delta`'s records are host memory, or device memory the caller keeps alive
+// (delta_on_device); so are the change and dep records of `dch` (table_on_device).  The delta's descriptors, the remap, `from`
+// and the change table's descriptors are host memory.  keep_actors: the actor tables still describe the new logs.
+static int splice(pt_batch* b, const char* fn, std::vector<pt_log_desc>&& nd, std::vector<pt_change_desc>&& ncd, uint32_t maxR,
+                  const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R, const uint32_t* from,
+                  const pt_change_table* dch, bool table_on_device, bool keep_actors) {
+    const uint32_t n = (uint32_t)nd.size();
+    const uint64_t n_ins = n ? nd[n - 1].insdel_off + nd[n - 1].n_insdel : 0, n_mk = n ? nd[n - 1].mark_off + nd[n - 1].n_mark : 0;
     const pt_packed_ops ops{n, nd.data(), nullptr, n_ins, nullptr, n_mk};
     ptp::Plan plan;
-    if (err.empty()) if (const char* e = ptp::make_plan(ops, b->limits, b->num_sms, plan)) err = e;
-    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    if (const char* e = ptp::make_plan(ops, b->limits, b->num_sms, plan)) { g_last_error = std::string(fn) + e; return PT_ERR_INVALID; }
     PT_CUDA(cudaSetDevice(b->device));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge and downloads of the resident batch are done
     // The delta and the remap go to the device; the splice writes NEW buffers, so the resident batch stays intact until the
     // device has accepted every record.
     int rc;
     DevBuf ndesc, nins, nmarks, ncdesc, nch, ndp;              // the new batch's descriptors, records and change table
-    DevBuf ddesc, dins, dmarks, dcdesc, dchg, ddep, amap[5], abad;   // the delta, its remap and the refusal flag: freed on return
+    DevBuf ddesc, dins, dmarks, dcdesc, dchg, ddep, amap[5], abad, dfrom;   // the delta, its remap, the index, the refusal flag: freed on return
     if ((rc = upload_n(b, ddesc, delta->logs, n)) || (rc = upload_n(b, ndesc, nd.data(), n)) || (rc = abad.reserve(4)) ||
         (rc = reserve_n<pt_insdel_rec>(nins, n_ins)) || (rc = reserve_n<pt_mark_rec>(nmarks, n_mk))) return rc;
+    if (from && (rc = upload_n(b, dfrom, from, n))) return rc;
+    const uint32_t* d_from = from ? (const uint32_t*)dfrom.p : nullptr;
     const pt_insdel_rec* d_dins = delta->insdel;
     const pt_mark_rec* d_dmarks = delta->marks;
     if (!delta_on_device) {
@@ -867,7 +866,7 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
         uint64_t most = 0;
         for (uint32_t i = 0; i < n; i++) most = std::max<uint64_t>(most, (uint64_t)nd[i].n_insdel + 2ull * nd[i].n_mark);
         pta::splice_records_kernel<<<slice_grid(b, n, most, threads), threads, 0, b->stream>>>(
-            (const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, n, DR, b->dp_insdel, b->dp_marks,
+            (const pt_log_desc*)b->d_desc.p, (const pt_log_desc*)ndesc.p, (const pt_log_desc*)ddesc.p, d_from, n, DR, b->dp_insdel, b->dp_marks,
             d_dins, d_dmarks, (pt_insdel_rec*)nins.p, (pt_mark_rec*)nmarks.p, (uint32_t*)abad.p);
         PT_CUDA(launched(b));
     }
@@ -884,19 +883,17 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
         }
         if (n) {
             pta::splice_changes_kernel<<<warp_grid(b, n, threads), threads, 0, b->stream>>>(
-                (const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p, n, DR,
+                (const pt_change_desc*)b->d_cdesc.p, (const pt_change_desc*)ncdesc.p, (const pt_change_desc*)dcdesc.p, d_from, n, DR,
                 (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p, d_dchg, d_ddep, (pt_change_rec*)nch.p, (pt_dep_rec*)ndp.p);
             PT_CUDA(launched(b));
         }
+        if ((rc = reserve_n<uint32_t>(b->d_admit, n))) return rc;
     }
     uint32_t bad = 0;
     PT_CUDA(cudaMemcpyAsync(&bad, abad.p, 4, cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));              // also: the caller's arrays may be freed on return
-    if (bad) { g_last_error = std::string(fn) + "a resident comment rank is outside comment_map"; return PT_ERR_INVALID; }
+    if (bad) { g_last_error = std::string(fn) + "a resident comment rank is outside comment_map or maps to 0xFFFFFFFF"; return PT_ERR_INVALID; }
     // Accepted: the new records and change table replace the old ones (freed with the locals), and the batch is re-planned.
-    // The actor tables stay only while no log's actor set can have changed: no actor or counter map, every n_actors kept.
-    bool keep_actors = !(R.actor_off && R.actor_off[n] > R.actor_off[0]) && !(R.ctr_off && R.ctr_off[n] > R.ctr_off[0]);
-    for (uint32_t i = 0; keep_actors && i < n; i++) keep_actors = nd[i].n_actors == b->h_desc[i].n_actors;
     b->have_actors = b->have_actors && keep_actors;
     b->have_batch = false; b->merged = false; b->dl_begun = false;
     drop_graph(b);
@@ -911,6 +908,21 @@ static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta
     if ((rc = derive_key_records(b))) return rc;
     b->have_batch = true;
     return PT_OK;
+}
+
+// pt_batch_append after its host checks, and the append of pt_batch_change and pt_batch_exchange (`fn` prefixes the error text).
+static int splice_append(pt_batch* b, const char* fn, const pt_packed_ops* delta, bool delta_on_device, const pt_append_remap& R,
+                         const pt_change_table* dch, bool table_on_device) {
+    std::vector<pt_log_desc> nd;
+    std::vector<pt_change_desc> ncd;
+    uint32_t maxR = 1;
+    const std::string err = check_append(b, *delta, delta_on_device, R, dch, nd, ncd, maxR);
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    // The actor tables stay only while no log's actor set can have changed: no actor or counter map, every n_actors kept.
+    const uint32_t n = b->n_logs;
+    bool keep_actors = !(R.actor_off && R.actor_off[n] > R.actor_off[0]) && !(R.ctr_off && R.ctr_off[n] > R.ctr_off[0]);
+    for (uint32_t i = 0; keep_actors && i < n; i++) keep_actors = nd[i].n_actors == b->h_desc[i].n_actors;
+    return splice(b, fn, std::move(nd), std::move(ncd), maxR, delta, delta_on_device, R, nullptr, dch, table_on_device, keep_actors);
 }
 
 int pt_batch_append(pt_batch* b, const pt_packed_ops* delta, const pt_append_remap* remap, const pt_change_table* dch) {
@@ -1248,9 +1260,9 @@ static int js_cmp_host(const uint8_t* a, uint64_t na, const uint8_t* b, uint64_t
     return na < nb ? -1 : na > nb ? 1 : 0;
 }
 
-// pt_batch_upload_actors' host checks (include/peritext_b200.h).  Returns the problem, or an empty string.
-static std::string check_actor_tables(const pt_batch* b, const pt_actor_tables& t) {
-    const uint32_t n = b->n_logs;
+// pt_batch_upload_actors' host checks (include/peritext_b200.h) of tables for the n logs `desc`.  Returns the problem, or an
+// empty string.
+static std::string check_actor_tables(const pt_log_desc* desc, uint32_t n, const pt_actor_tables& t) {
     if (t.n_logs != n) return "the tables have " + std::to_string(t.n_logs) + " logs and the batch " + std::to_string(n);
     if (!t.per_log_first || !t.off) return "null per_log_first or off";
     if (t.count && t.off[t.count] > t.off[0] && !t.data) return "null data with a nonzero length";
@@ -1259,7 +1271,7 @@ static std::string check_actor_tables(const pt_batch* b, const pt_actor_tables& 
     for (uint32_t i = 0; i < n; i++) {
         const uint64_t lo = t.per_log_first[i], hi = t.per_log_first[i + 1];
         if (hi < lo || hi > t.count) return at(i) + "per_log_first decreases or passes count";
-        const uint64_t cnt = hi - lo, R = b->h_desc[i].n_actors;
+        const uint64_t cnt = hi - lo, R = desc[i].n_actors;
         if (cnt != R && !(cnt == 0 && R == 1)) return at(i) + std::to_string(cnt) + " actor ids and n_actors " + std::to_string(R);
         for (uint64_t k = lo; k < hi; k++) {
             if ((t.off[k + 1] - t.off[k]) & 1) return at(i) + "actor " + std::to_string(k - lo) + " has an odd byte length";
@@ -1274,7 +1286,7 @@ static std::string check_actor_tables(const pt_batch* b, const pt_actor_tables& 
 int pt_batch_upload_actors(pt_batch* b, const pt_actor_tables* t) {
     if (!b || !t) { g_last_error = "pt_batch_upload_actors: null argument"; return PT_ERR_INVALID; }
     if (!b->have_batch) { g_last_error = "pt_batch_upload_actors before pt_batch_upload"; return PT_ERR_STATE; }
-    const std::string err = check_actor_tables(b, *t);
+    const std::string err = check_actor_tables(b->h_desc.data(), b->n_logs, *t);
     if (!err.empty()) { g_last_error = "pt_batch_upload_actors: " + err; return PT_ERR_INVALID; }
     const uint32_t n = b->n_logs;
     const uint64_t lo = t->count ? t->off[0] : 0, bytes = t->count ? t->off[t->count] - lo : 0;
@@ -1537,6 +1549,141 @@ int pt_batch_add_actors(pt_batch* b, const pt_actor_input* in, pt_actor_view* ou
         PT_CUDA(cudaStreamSynchronize(b->stream));
     }
     *out = pt_actor_view{n, count, (const uint16_t*)b->h_add_rank.p, (const uint64_t*)b->h_add_aoff.p, (const uint16_t*)b->h_add_amap.p, spliced ? 1u : 0u};
+    return PT_OK;
+}
+
+// pt_batch_select_logs' host checks (include/peritext_b200.h).  On success nd / dd / ncd / dcd hold the new batch's
+// descriptors and the per-new-log delta descriptors of the splice (an added log's records, empty for a kept one) and
+// add_idx[i] the added log new log i is (or ~0u).  Returns the problem, or an empty string.
+static std::string check_select(const pt_batch* b, const uint32_t* from, uint32_t n, const pt_packed_ops* added, const pt_change_table* ach,
+                                const pt_actor_tables* aact, const uint32_t* comment_map, uint64_t n_comment_map,
+                                std::vector<pt_log_desc>& nd, std::vector<pt_log_desc>& dd, std::vector<pt_change_desc>& ncd,
+                                std::vector<pt_change_desc>& dcd, std::vector<uint32_t>& add_idx, uint32_t& maxR) {
+    if (n && !from) return "null from with n_logs > 0";
+    const uint32_t na = added ? added->n_logs : 0;
+    if (added && na && !added->logs) return "null added descriptors with a nonzero n_logs";
+    add_idx.assign(n, ~0u);
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (from[i] == PT_SELECT_ADDED) { add_idx[i] = k++; continue; }
+        if (from[i] >= b->n_logs) return "from[" + std::to_string(i) + "] = " + std::to_string(from[i]) + " names no resident log (the batch has " + std::to_string(b->n_logs) + ")";
+    }
+    if (k != na) return std::to_string(k) + " entries are PT_SELECT_ADDED and added has " + std::to_string(na) + " logs";
+    if (!na && (ach || aact)) return "added change or actor tables without added logs";
+    if (na && (ach != nullptr) != b->have_changes)
+        return b->have_changes ? "the batch has a change table and the added logs none" : "the added logs have a change table and the batch none";
+    if (na && (aact != nullptr) != b->have_actors)
+        return b->have_actors ? "the batch has actor tables and the added logs none" : "the added logs have actor tables and the batch none";
+    if (na && ((added->n_insdel_total && !added->insdel) || (added->n_mark_total && !added->marks))) return "null added records with a nonzero count";
+    if (n_comment_map && !comment_map) return "null comment_map with a nonzero length";
+    uint64_t last = 0;
+    bool any = false;
+    for (uint64_t c = 0; comment_map && c < n_comment_map; c++) {
+        if (comment_map[c] == 0xFFFFFFFFu) continue;
+        if (any && comment_map[c] <= last) return "comment_map is not strictly increasing at entry " + std::to_string(c);
+        last = comment_map[c]; any = true;
+    }
+    for (uint32_t j = 0; j < na; j++) {
+        const pt_log_desc& A = added->logs[j];
+        if (A.insdel_off + A.n_insdel > added->n_insdel_total || A.mark_off + A.n_mark > added->n_mark_total) return "added log " + std::to_string(j) + ": descriptor out of range";
+    }
+    if (ach) {
+        if (ach->n_logs != na || !ach->logs) return "the added change table does not match the added logs";
+        if ((ach->n_changes_total && !ach->changes) || (ach->n_deps_total && !ach->deps)) return "null added change records with a nonzero count";
+        for (uint32_t j = 0; j < na; j++) {
+            const pt_change_desc& D = ach->logs[j];
+            if (D.change_off + D.n_changes > ach->n_changes_total || D.dep_off + D.n_deps > ach->n_deps_total) return "added log " + std::to_string(j) + ": change descriptor out of range";
+        }
+    }
+    if (aact) {
+        const std::string e = check_actor_tables(added->logs, na, *aact);
+        if (!e.empty()) return "added actor tables: " + e;
+    }
+    nd.resize(n); dd.assign(n, pt_log_desc{}); ncd.clear(); dcd.clear();
+    if (b->have_changes) { ncd.resize(n); dcd.assign(n, pt_change_desc{}); }
+    uint64_t io = 0, mo = 0, co = 0, po = 0;
+    maxR = 1;
+    for (uint32_t i = 0; i < n; i++) {
+        const bool add = add_idx[i] != ~0u;
+        const pt_log_desc S = add ? added->logs[add_idx[i]] : b->h_desc[from[i]];
+        if (add) dd[i] = pt_log_desc{S.insdel_off, S.mark_off, S.n_insdel, S.n_mark, S.n_actors, S.max_ctr};
+        nd[i] = pt_log_desc{io, mo, S.n_insdel, S.n_mark, S.n_actors, S.max_ctr};
+        io += S.n_insdel; mo += S.n_mark;
+        maxR = std::max<uint32_t>(maxR, S.n_actors);
+        if (!b->have_changes) continue;
+        const pt_change_desc C = add ? ach->logs[add_idx[i]] : b->h_cdesc[from[i]];
+        if (add) dcd[i] = C;
+        ncd[i] = pt_change_desc{co, po, C.n_changes, C.n_deps};
+        co += C.n_changes; po += C.n_deps;
+    }
+    if (b->have_changes && actor_table_bytes(maxR) > kAdmitMaxBytes) return "more than 25600 actors in one log: not supported by the admission pre-pass";
+    return std::string();
+}
+
+int pt_batch_select_logs(pt_batch* b, const uint32_t* from, uint32_t n, const pt_packed_ops* added, const pt_change_table* added_changes,
+                         const pt_actor_tables* added_actors, const uint32_t* comment_map, uint64_t n_comment_map) {
+    const char* fn = "pt_batch_select_logs: ";
+    if (!b) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_select_logs before pt_batch_upload"; return PT_ERR_STATE; }
+    std::vector<pt_log_desc> nd, dd;
+    std::vector<pt_change_desc> ncd, dcd;
+    std::vector<uint32_t> add_idx;
+    uint32_t maxR = 1;
+    const std::string err = check_select(b, from, n, added, added_changes, added_actors, comment_map, n_comment_map, nd, dd, ncd, dcd, add_idx, maxR);
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    // the splice's delta: the added logs' records, described per new log
+    const pt_packed_ops delta{n, dd.data(), added ? added->insdel : nullptr, added ? added->n_insdel_total : 0, added ? added->marks : nullptr,
+                              added ? added->n_mark_total : 0};
+    const pt_change_table dch{n, dcd.data(), added_changes ? added_changes->changes : nullptr, added_changes ? added_changes->n_changes_total : 0,
+                              added_changes ? added_changes->deps : nullptr, added_changes ? added_changes->n_deps_total : 0};
+    const pt_append_remap R{nullptr, nullptr, nullptr, nullptr, comment_map, comment_map ? n_comment_map : 0};
+    PT_CUDA(cudaSetDevice(b->device));
+    // The actor tables are gathered first, into new buffers that replace the old ones once the splice is accepted.
+    int rc;
+    DevBuf nnames, noff, nfirst, nbyte, dfrom, adata, aoff, afirst;
+    std::vector<unsigned long long> new_first, new_byte;
+    std::vector<char> new_dense;
+    if (b->have_actors) {
+        const uint64_t lo = added_actors && added_actors->count ? added_actors->off[0] : 0;
+        const uint64_t abytes = added_actors && added_actors->count ? added_actors->off[added_actors->count] - lo : 0, acount = added_actors ? added_actors->count : 0;
+        std::vector<unsigned long long> add_first(n, 0), add_off(acount + 1, 0);
+        for (uint64_t k = 0; k <= acount && added_actors; k++) add_off[k] = acount ? added_actors->off[k] - lo : 0;
+        new_first.assign((size_t)n + 1, 0); new_byte.assign((size_t)n + 1, 0); new_dense.assign(n, 0);
+        for (uint32_t i = 0; i < n; i++) {
+            uint64_t cnt, bytes;
+            if (add_idx[i] != ~0u) {
+                const uint64_t* pf = added_actors->per_log_first + add_idx[i];
+                add_first[i] = pf[0]; cnt = pf[1] - pf[0]; bytes = add_off[pf[1]] - add_off[pf[0]];
+                new_dense[i] = added_actors->counters_first && added_actors->counters_first[add_idx[i] + 1] > added_actors->counters_first[add_idx[i]];
+            } else {
+                const uint32_t s = from[i];
+                cnt = b->h_afirst[s + 1] - b->h_afirst[s]; bytes = b->h_abyte[s + 1] - b->h_abyte[s];
+                new_dense[i] = b->h_adense[s];
+            }
+            new_first[i + 1] = new_first[i] + cnt; new_byte[i + 1] = new_byte[i] + bytes;
+        }
+        if ((rc = reserve_n<uint8_t>(nnames, new_byte[n])) || (rc = reserve_n<unsigned long long>(noff, new_first[n] + 1)) ||
+            (rc = upload_n(b, nfirst, new_first.data(), (uint64_t)n + 1)) || (rc = upload_n(b, nbyte, new_byte.data(), (uint64_t)n + 1)) ||
+            (rc = upload_n(b, dfrom, from, n)) || (rc = upload_n(b, adata, abytes ? added_actors->data + lo : nullptr, abytes)) ||
+            (rc = upload_n(b, aoff, add_off.data(), acount + 1)) || (rc = upload_n(b, afirst, add_first.data(), n))) return rc;
+        PT_CUDA(cudaMemsetAsync(noff.p, 0, 8, b->stream));
+        if (n) {
+            pty::GatherParams G{};
+            G.n_logs = n; G.from = (const uint32_t*)dfrom.p;
+            G.old_t = pty::Tables{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+            G.add_data = (const uint8_t*)adata.p; G.add_off = (const unsigned long long*)aoff.p; G.add_first = (const unsigned long long*)afirst.p;
+            G.data = (uint8_t*)nnames.p; G.off = (unsigned long long*)noff.p;
+            G.first = (const unsigned long long*)nfirst.p; G.byte_base = (const unsigned long long*)nbyte.p;
+            pty::actor_gather_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(G);
+            PT_CUDA(launched(b));
+        }
+    }
+    if ((rc = splice(b, fn, std::move(nd), std::move(ncd), maxR, &delta, false, R, from, b->have_changes ? &dch : nullptr, false, true))) return rc;
+    if (b->have_actors) {
+        b->d_anames.swap(nnames); b->d_aoff.swap(noff); b->d_afirst.swap(nfirst);
+        b->h_afirst.assign(new_first.begin(), new_first.end()); b->h_abyte.assign(new_byte.begin(), new_byte.end());
+        b->h_adense = std::move(new_dense);
+    }
     return PT_OK;
 }
 

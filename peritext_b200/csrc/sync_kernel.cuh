@@ -22,6 +22,8 @@
 // add_select_kernel (pt_batch_add_actors): one warp per log sorts and deduplicates the caller's ids for it by counting, per id,
 // the distinct ids before it (O(m^2) compares: a log names few ids per call, and a long list is slower but exact), and keeps the
 // ones the table lacks; actor_merge_kernel then merges them in.  add_ranks_kernel: each given id's rank in the grown table.
+// actor_gather_kernel (pt_batch_select_logs): one warp per new log copies its ids' bytes and rebased offsets from the old
+// tables or the added ones.
 #pragma once
 #include <cstdint>
 
@@ -283,6 +285,30 @@ __global__ void actor_merge_kernel(MergeParams P) {
             const uint8_t* s = P.src_at[f + r];
             for (unsigned long long b = lo; b < hi; b++) P.data[b] = s[b - lo];
         }
+    }
+}
+
+// pt_batch_select_logs: new log i's table is resident log from[i]'s, or (PT_SELECT_ADDED) the ids of the added tables from
+// id add_first[i] on.  The host knows every log's id and byte counts, so first / byte_base (the new layout) come from it.
+struct GatherParams {
+    uint32_t n_logs;
+    const uint32_t* from;
+    Tables old_t;
+    const uint8_t* add_data; const unsigned long long* add_off; const unsigned long long* add_first;   // add_first: [n_logs]
+    uint8_t* data; unsigned long long* off;                      // the new tables; off[0] is set by the host
+    const unsigned long long* first; const unsigned long long* byte_base;   // [n_logs + 1] each
+};
+
+__global__ void actor_gather_kernel(GatherParams P) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t i = warp; i < P.n_logs; i += nwarps) {
+        const uint32_t s = P.from[i];
+        const bool added = s == PT_SELECT_ADDED;
+        const uint8_t* src = added ? P.add_data : P.old_t.data;
+        const unsigned long long* so = (added ? P.add_off : P.old_t.off) + (added ? P.add_first[i] : P.old_t.first[s]);
+        const unsigned long long f = P.first[i], cnt = P.first[i + 1] - f, b0 = so[0], nb = P.byte_base[i];
+        for (unsigned long long r = lane; r < cnt; r += 32) P.off[f + r + 1] = so[r + 1] - b0 + nb;
+        for (unsigned long long k = lane; k < P.byte_base[i + 1] - nb; k += 32) P.data[nb + k] = src[b0 + k];
     }
 }
 

@@ -12,7 +12,7 @@ import os
 import numpy as np
 
 from .packing import (CDESC_DT, CHANGE_DT, CLOCK_DT, CHANGES_REQUEST_DT, EXTRA_DT, ChangeExtras, CHANGE_OK, CHANGE_STATUS_DT, DEP_DT, DESC_DT, ELEM_NOT_FOUND, ELEM_POS_DT, ELEM_REF_DT,
-                      INPUT_OP_DT, INSDEL_DT, MARK_DT, RESULT_DT, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts,
+                      INPUT_OP_DT, INSDEL_DT, MARK_DT, RESULT_DT, SELECT_ADDED, SPAN_DT, AppendRemap, ChangeTable, ExchangeMaps, MergedBatch, PackedBatch, apply_append, change_dicts,
                       change_inputs, elem_refs, json_pools, string_pools)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -37,6 +37,7 @@ _ENTRY_POINTS = {
     "pt_batch_download_actors": ([_vp, _vp], _int),
     "pt_batch_add_actors": ([_vp, _vp, _vp], _int),
     "pt_batch_sync_pairs": ([_vp, _vp, _u32, _vp], _int),
+    "pt_batch_select_logs": ([_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u64], _int),
     "pt_ingest_create": ([_out(_vp)], _int),
     "pt_ingest_parse": ([_vp, _vp, _vp, _u32, _int], _int),
     "pt_ingest_packed": ([_vp, _vp, _vp], _int),
@@ -343,7 +344,10 @@ class BatchEngine:
         self.n_logs = len(desc)
         self.patch_window = None                                             # every upload resets the window to whole logs
         self._n_insdel = int(n_insdel_total)                                 # patch records: one per ins/del record
-        self._n_seq = int(desc["n_insdel"].astype(np.uint64).sum())          # element sequences: the capacity layout
+        self._log_insdel = desc["n_insdel"].astype(np.uint64)                # per log, and its n_actors: what a select moves
+        self._log_n_actors = desc["n_actors"].astype(np.uint32)
+        self._n_seq = int(self._log_insdel.sum())                            # element sequences: the capacity layout
+        self._has_changes = self._has_actors = False                         # every upload drops both tables
 
     _ops_struct = staticmethod(_packed_ops)                                  # the builder under its earlier method name
 
@@ -351,7 +355,10 @@ class BatchEngine:
         """Record a splice into the resident batch (append, change, exchange, sync, a re-ranking add_actors): the device rebuilds
         the records tightly from the new descriptors, so it then holds exactly their n_insdel sum; a splice also resets the
         patch window."""
-        self._n_seq += int(delta_desc["n_insdel"].astype(np.uint64).sum())
+        if len(delta_desc):
+            self._log_insdel = self._log_insdel + delta_desc["n_insdel"].astype(np.uint64)
+            self._log_n_actors = delta_desc["n_actors"].astype(np.uint32)
+        self._n_seq = int(self._log_insdel.sum())
         self._n_insdel = self._n_seq
         self.patch_window = None
 
@@ -375,6 +382,7 @@ class BatchEngine:
         Micromerge.applyChange, reference src/micromerge.ts:501-509) and rejected logs report status 6 / 7."""
         t, _keep = _change_struct(table)
         _check(self._L.pt_batch_upload_changes(self._h, ctypes.byref(t)), "pt_batch_upload_changes")
+        self._has_changes = True
 
     def append(self, delta: PackedBatch, remap: AppendRemap | None = None, changes: ChangeTable | None = None):
         """Extend every log of the resident batch with the delta's records on the device (pt_batch_append): afterwards the
@@ -390,7 +398,47 @@ class BatchEngine:
         table = delta.changes if changes is None else changes
         ct = _change_struct(table) if table is not None else None
         _check(self._L.pt_batch_append(self._h, ctypes.byref(ops), ctypes.byref(st), ctypes.byref(ct[0]) if ct else None), "pt_batch_append")
+        # the engine drops the actor tables where a log's actor set can have changed (pt_batch_upload_actors' lifetime rule)
+        if arrs[1] is not None and len(arrs[1]) or arrs[3] is not None and len(arrs[3]) or (desc["n_actors"] != self._log_n_actors).any():
+            self._has_actors = False
         self._spliced(desc)
+
+    def select_logs(self, from_, added: PackedBatch | None = None, comment_map=None):
+        """Change which logs the resident batch holds, on the device (pt_batch_select_logs): new log i is resident log
+        ``from_[i]``, or, where ``from_[i]`` is SELECT_ADDED, the next log of `added` (``packing.pack_select``).  Kept logs keep
+        everything they hold on the device; `comment_map` (old comment rank -> new rank, SELECT_DROPPED for a rank no kept log
+        names; None = identity) moves their comment ranks.  `added` brings its change table when the handle has one and its
+        ``log_actors`` when the handle has actor tables.  The handle then holds what an upload of ``packing.apply_select``
+        would hold, and needs a merge."""
+        frm = np.ascontiguousarray(from_, np.uint32)
+        ops = ct = at = None
+        keep = []
+        if added is not None:
+            desc = np.ascontiguousarray(added.desc)
+            insdel = np.ascontiguousarray(added.insdel); marks = np.ascontiguousarray(added.marks)
+            ops = _packed_ops(desc, insdel, len(insdel), marks, len(marks))
+            keep += [desc, insdel, marks]
+            if self._has_changes and added.changes is not None:
+                ct, arrs = _change_struct(added.changes)
+                keep.append(arrs)
+            if self._has_actors:
+                p = string_pools(added)
+                data, off, first = (np.ascontiguousarray(p[k], dt) for k, dt in (("actors", np.uint8), ("actors_off", np.uint64), ("actors_first", np.uint64)))
+                cf = np.ascontiguousarray(p["counters_first"], np.uint64)
+                at = _ActorTables(len(desc), _ptr(data), _ptr(off), max(0, len(off) - 1), _ptr(first), _ptr(cf))
+                keep += [data, off, first, cf]
+        cm = None if comment_map is None else np.ascontiguousarray(comment_map, np.uint32)
+        ref = lambda st: ctypes.byref(st) if st is not None else None
+        _check(self._L.pt_batch_select_logs(self._h, _ptr(frm), len(frm), ref(ops), ref(ct), ref(at),
+                                            None if cm is None else cm.ctypes.data, 0 if cm is None else len(cm)), "pt_batch_select_logs")
+        add = added.desc if added is not None else np.zeros(0, DESC_DT)
+        kept = frm != SELECT_ADDED
+        ins, act = np.zeros(len(frm), np.uint64), np.zeros(len(frm), np.uint32)
+        ins[kept], act[kept] = self._log_insdel[frm[kept]], self._log_n_actors[frm[kept]]
+        ins[~kept], act[~kept] = add["n_insdel"], add["n_actors"]
+        self.n_logs = len(frm)
+        self._log_insdel, self._log_n_actors = ins, act
+        self._spliced(np.zeros(0, DESC_DT))
 
     def change_packed(self, actor, input_off, ops, tokens, n_values: int, n_links: int, n_comments: int, changes: ChangeTable | None = None):
         """pt_batch_change from its arrays (``packing.change_inputs``, ``workload.sync_round``): per log i the actor rank of its
@@ -468,6 +516,7 @@ class BatchEngine:
         cf = None if cf is None else np.ascontiguousarray(cf, np.uint64)
         t = _ActorTables(max(0, len(first) - 1), _ptr(data), _ptr(off), max(0, len(off) - 1), _ptr(first), _ptr(cf))
         _check(self._L.pt_batch_upload_actors(self._h, ctypes.byref(t)), "pt_batch_upload_actors")
+        self._has_actors = True
 
     def actors(self) -> list[list[str]]:
         """The handle's actor tables (pt_batch_download_actors), per log its ids in rank order."""

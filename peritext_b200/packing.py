@@ -373,7 +373,15 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
 
     comment_sorted = sorted(pools.comment_objs, key=js_key)       # sortBy(..., c => c.id), src/peritext.ts:318
     comment_rank = {cid: i for i, cid in enumerate(comment_sorted)}
+    desc, insdel, marks, counters, ranks = _emit_logs(builders, comment_rank)
+    table = _change_table(builders, ranks) if with_changes else None
+    return PackedBatch(desc, insdel, marks, pools.values, pools.link_attrs, [pools.comment_objs[c] for c in comment_sorted], pools.other_attrs,
+                       log_actors=[sorted(b.actors, key=js_key) for b in builders], log_counters=counters, changes=table, log_lists=lids)
 
+
+def _emit_logs(builders: Sequence[_LogBuilder], comment_rank: dict):
+    """Whole logs in the packed id space (``pack_logs``' rules per log): (descriptors, ins/del records, mark records, per log
+    None or the dense counter table, per log actor -> rank)."""
     n_ins = sum(len(b.insdel) for b in builders)
     n_mk = sum(len(b.marks) for b in builders)
     desc = np.zeros(len(builders), DESC_DT)
@@ -400,9 +408,7 @@ def pack_logs(logs: Sequence[Sequence[dict]], *, list_ids: Sequence[str | None] 
         desc[li] = (io, mo, len(b.insdel), len(b.marks), max(1, len(ranked)), dc(b.max_ctr) if dense is not None else b.max_ctr)
         _emit_log(b, rank, dc, comment_rank, insdel, io, marks, mo)
         io += len(b.insdel); mo += len(b.marks)
-    table = _change_table(builders, ranks) if with_changes else None
-    return PackedBatch(desc, insdel, marks, pools.values, pools.link_attrs, [pools.comment_objs[c] for c in comment_sorted], pools.other_attrs,
-                       log_actors=[sorted(b.actors, key=js_key) for b in builders], log_counters=counters, changes=table, log_lists=lids)
+    return desc, insdel, marks, counters, ranks
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -707,6 +713,93 @@ def apply_append(prev: PackedBatch, delta: PackedBatch, remap: AppendRemap | Non
                               cat(oc.deps, dcg.deps, "dep_off", "n_deps", DEP_DT, map_actor, lambda d, lg: None))
     return PackedBatch(desc, insdel, marks, delta.values, delta.link_attrs, delta.comment_ids, delta.other_attrs, dict(prev.meta),
                        delta.log_actors, delta.log_counters, changes, delta.log_lists)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Select (include/peritext_b200.h pt_batch_select_logs)
+# ------------------------------------------------------------------------------------------------------------------
+SELECT_ADDED = 0xFFFFFFFF    # a `from_` entry: the next log of `added`
+SELECT_DROPPED = 0xFFFFFFFF  # a comment-map entry: a rank that no kept log names
+
+
+def pack_select(prev: PackedBatch, from_: Sequence[int], new_logs: Sequence[Sequence[dict]], *, with_changes: bool) -> tuple[PackedBatch, np.ndarray | None]:
+    """The added logs and comment map of ``pt_batch_select_logs``: ``new_logs`` are the Change logs of the entries of ``from_``
+    that are SELECT_ADDED, in order, packed as ``pack_logs`` would pack them against ``prev``'s pools.  Known strings keep their
+    pool index and new ones take the next; the batch-wide comment order is ``prev``'s ids and the new ones in JS order, and the
+    comment map says where each old rank moves (None when none moves).  Only ``prev``'s pools are read, so this also works when
+    the kept logs' records live only on the device.  ``with_changes`` builds the added logs' change table."""
+    n_add = sum(1 for f in from_ if int(f) == SELECT_ADDED)
+    if len(new_logs) != n_add:
+        raise ValueError(f"pack_select: {len(new_logs)} new logs for {n_add} SELECT_ADDED entries")
+    pools = _Pools(prev.values, prev.link_attrs, prev.comment_ids, prev.other_attrs)
+    lids = [_root_text_list(changes) for changes in new_logs]
+    builders = [_collect_log(changes, lid, with_changes, pools) for changes, lid in zip(new_logs, lids)]
+    comment_sorted = sorted(pools.comment_objs, key=js_key)
+    comment_rank = {cid: i for i, cid in enumerate(comment_sorted)}
+    cmap = [comment_rank[a["id"]] for a in prev.comment_ids]
+    desc, insdel, marks, counters, ranks = _emit_logs(builders, comment_rank)
+    added = PackedBatch(desc, insdel, marks, pools.values, pools.link_attrs, [pools.comment_objs[c] for c in comment_sorted], pools.other_attrs,
+                        dict(prev.meta), [sorted(b.actors, key=js_key) for b in builders], counters,
+                        _change_table(builders, ranks) if with_changes else None, lids)
+    return added, (np.array(cmap, np.uint32) if cmap != list(range(len(cmap))) else None)
+
+
+def apply_select(prev: PackedBatch, from_: Sequence[int], added: PackedBatch | None = None, comment_map=None) -> PackedBatch:
+    """The readable host specification of ``pt_batch_select_logs``: new log i is ``prev``'s log ``from_[i]``, or, where it is
+    SELECT_ADDED, the next log of ``added``.  Kept logs keep their records, change tables, ``log_actors``, ``log_counters`` and
+    ``log_lists``; their comment marks' ranks go through ``comment_map`` (None = identity), and a kept rank outside it or mapped
+    to SELECT_DROPPED raises ValueError, as the device refuses it.  Added logs are copied verbatim.  The pools are ``added``'s,
+    or without added logs ``prev``'s with the comment ids moved through the map."""
+    from_ = [int(f) for f in from_]
+    n_prev, n_add = prev.n_logs, (added.n_logs if added is not None else 0)
+    if sum(1 for f in from_ if f == SELECT_ADDED) != n_add:
+        raise ValueError("apply_select: the SELECT_ADDED entries do not match the added logs")
+    if any(f != SELECT_ADDED and not 0 <= f < n_prev for f in from_):
+        raise ValueError("apply_select: an entry names no log of prev")
+    if added is not None and n_add and (prev.changes is None) != (added.changes is None):
+        raise ValueError("apply_select: a change table on one side only")
+    marks = prev.marks.copy()
+    if comment_map is not None:
+        cm = np.asarray(comment_map, np.int64)
+        li = np.repeat(np.arange(n_prev), prev.desc["n_mark"].astype(np.int64))
+        at = _ranges(prev.desc["mark_off"], prev.desc["n_mark"])
+        kept = np.isin(li, [f for f in from_ if f != SELECT_ADDED])
+        m = marks[at]
+        com = kept & (((m["kind"] >> 1) & 3) == 2) & (m["attr"] != ATTR_NONE)
+        rank = m["attr"][com].astype(np.int64)
+        new = np.full(len(rank), SELECT_DROPPED, np.int64)
+        new[rank < len(cm)] = cm[rank[rank < len(cm)]]
+        if (new == SELECT_DROPPED).any():
+            raise ValueError("apply_select: a kept comment rank is outside comment_map or dropped")
+        m["attr"][com] = new
+        marks[at] = m
+    both = PackedBatch(prev.desc.copy(), prev.insdel, marks)
+    if added is not None:
+        d = added.desc.copy()
+        d["insdel_off"] += len(prev.insdel); d["mark_off"] += len(prev.marks)
+        both = PackedBatch(np.concatenate([prev.desc, d]), np.concatenate([prev.insdel, added.insdel]), np.concatenate([marks, added.marks]))
+    cat = lambda x, y: list(x or []) + list(y or []) if (x or not n_prev) and (not n_add or y) else []
+    src = added if added is not None else prev
+    both.log_actors = cat(prev.log_actors, added.log_actors if added is not None else [])
+    both.log_counters = cat(prev.log_counters, added.log_counters if added is not None else [])
+    both.log_lists = cat(prev.log_lists, added.log_lists if added is not None else [])
+    if prev.changes is not None:
+        ct = prev.changes
+        if added is not None and added.changes is not None:
+            cd = added.changes.desc.copy()
+            cd["change_off"] += len(ct.changes); cd["dep_off"] += len(ct.deps)
+            ct = ChangeTable(np.concatenate([ct.desc, cd]), np.concatenate([ct.changes, added.changes.changes]), np.concatenate([ct.deps, added.changes.deps]))
+        both.changes = ct
+    idx = [f if f != SELECT_ADDED else n_prev + k for k, f in zip(np.cumsum([f == SELECT_ADDED for f in from_]) - 1, from_)]
+    out = both.select(idx)
+    comment_ids = src.comment_ids
+    if added is None and comment_map is not None:
+        comment_ids = [None] * (max([int(c) for c in comment_map if int(c) != SELECT_DROPPED] + [-1]) + 1)
+        for r, c in enumerate(comment_map):
+            if int(c) != SELECT_DROPPED:
+                comment_ids[int(c)] = prev.comment_ids[r]
+    out.values, out.link_attrs, out.comment_ids, out.other_attrs, out.meta = src.values, src.link_attrs, comment_ids, src.other_attrs, dict(prev.meta)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------
