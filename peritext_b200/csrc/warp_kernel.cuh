@@ -126,7 +126,6 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     const uint2* __restrict__ mk = P.key_marks + mark_off;
     const pt_insdel_rec* __restrict__ full_ins = P.insdel + insdel_off;
     uint32_t* text_out = P.text + P.text_off[li];
-    pt_span* span_out = P.spans + P.span_off[li];
     pt_log_result* res = P.results + li;
 
     if ((P.warp_flags & 1u) && m) {       // this log's mark records are needed late: pull them into L2 now
@@ -164,10 +163,15 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     uint4* WI = A.alloc<uint4>(NWr);
     uint16_t* T = A.alloc<uint16_t>(packed ? 2u * C : compact ? C : KS);
     uint32_t* T32 = reinterpret_cast<uint32_t*>(T);              // packed3 view
+    // key-space bitmap of the opIds seen: A+B sets every insert key, G every mark key, so G's duplicate-opId test is the old
+    // bit of its one atomicOr (no id-table lookup)
+    const uint32_t KW = (KS + 31) / 32;
+    uint32_t* KSeen = A.alloc<uint32_t>(KW + 1);
     if (!A.fits()) { ps.leave(); return 1; }
     if (packed) wfill<uint32_t>(T32, C, 0u, lane);
     else wfill<uint16_t>(T, compact ? C : KS, (uint16_t)kNone16, lane);
     if (compact) wfill<uint32_t>(OV, kOvSlots, kOvEmpty, lane);
+    wfill<uint32_t>(KSeen, KW + 1, 0u, lane);
     // during A+B the z / w fields of WI collect the "element has a child that is not its log successor" and tombstone bits (atomicOr)
     wfill<uint32_t>(reinterpret_cast<uint32_t*>(WI), 4 * NWr, 0u, lane);
     __syncwarp();
@@ -223,6 +227,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             bool toOv = false, wrote = false;
             uint32_t mine = 0;
             if (isIns) {
+                atomicOr(&KSeen[key >> 5], 1u << (key & 31));
                 if (packed) {
                     const uint32_t c = ctrOf(key), sh = 10u * (key - 3u * c);
                     if ((atomicOr(&T32[c], (i + 1u) << sh) >> sh) & 1023u) failDup();   // two inserts with one opId
@@ -336,10 +341,12 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         // Euler tour nodes: enter(r) = r, exit(r) = (M+1) + r, r in 0..M (M = HEAD).  One 32-bit word per node: low half =
         // successor (later: owner splitter), high half = visible weight of the node (later: weight prefix inside the owner's
         // sublist); exits weigh 0.  Splitter ids: k < SPEND: node 8k; SPEND: the terminator; SPEND + 1: the tour's first node.
-        const uint32_t SPEND = END >> 3, nSp = SPEND + 2, KW = (KS + 31) / 32;
+        const uint32_t SPEND = END >> 3, nSp = SPEND + 2;
         uint32_t* Node = A.alloc<uint32_t>(E);
         uint16_t* N16 = reinterpret_cast<uint16_t*>(Node);         // N16[2x] = successor of x, N16[2x + 1] = weight of x
-        uint16_t* HV = A.alloc<uint16_t>(M + 1);                   // run head record index, then visBefore(head)
+        // run head record index, then visBefore(head); it lives in VisBase, which the last loop of E writes over it entry by
+        // entry (D's footprint bounds the runs a slice holds)
+        uint16_t* HV = VisBase;
         uint16_t* Prun = A.alloc<uint16_t>(M + 1);
         uint16_t* RKey = A.alloc<uint16_t>(M + 2);                 // key of the run head; dead after the ranking, then:
         uint16_t* Last = RKey;                                     // last threaded child of run q (q = M: HEAD)
@@ -499,6 +506,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     // boundary below is then one table read instead of run / prefix arithmetic.
     uint16_t* EV = A.alloc<uint16_t>(n + 1);
     if (!A.fits() || nvis >= 0x8000u) { ps.leave(); return 1; }
+    if (lane == 0) EV[n] = 0;                                      // what G reads for a boundary that has no insert record
     unsigned long long d0 = 0, d1 = 0;
 #pragma unroll 1
     for (uint32_t w = 0; w + 1 < NWr; w++) {
@@ -541,8 +549,6 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     uint16_t* CIdx = nullptr;                                      // surviving comment ops (indices into Sv), arrival order
     if (m) {
         // ---- G: mark ops -> visible intervals [va, vb); only ops that cover a visible element survive ---------------------
-        const uint32_t KW = (KS + 31) / 32;
-        uint32_t* KBits = A.alloc<uint32_t>(KW + 1);               // duplicate mark opIds
         CIdx = A.alloc<uint16_t>(kMaxCommentSurvivors + 32);
         if (!A.fits()) { ps.leave(); return 1; }
         const uint32_t room = A.cap - A.used, svStart = A.used;
@@ -550,9 +556,8 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         if (capS > m) capS = m;
         Sv = A.alloc<uint4>(capS + 1);
         if (!A.fits()) { ps.leave(); return 1; }
-        wfill<uint32_t>(KBits, KW + 1, 0u, lane);
-        __syncwarp();
         const uint32_t mm1 = m - 1u;                               // m > 0 here; past-the-end lanes load a clamped record, unused
+        const uint32_t ksMax = KS ? KS - 1u : 0u;                  // boundary keys are clamped to a valid slot for the lookups
         uint2 a = __ldg(mk + min(lane, mm1));
         const uint32_t mkBytes = m * 8u;
 #pragma unroll 2
@@ -567,31 +572,23 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
             const uint32_t key = a.x & 0xFFFFu, skey = a.x >> 16, ekey = a.y & 0xFFFFu, arrival = (a.y >> 16) & 0x7FFu;
             const uint32_t kind = (a.y >> 27) & 7u, sb = (a.y >> 30) & 1u, eb = a.y >> 31;
             const uint32_t type = (kind >> 1) & 3u;
-            // straight-line form (predicated loads instead of nested branches).  A boundary element must exist AND have arrived
-            // before the mark op: the reference's walk never matches anything else (peritext.ts:236-241) — a missing start is a
-            // no-op, a missing end never ends
+            // straight-line form: both boundary chains (lookup, then EV read) are issued unconditionally, on keys clamped to a
+            // valid slot and on EV's entry n for "no insert record", so they overlap; the hit rules are selects after the loads.
+            // A boundary element must exist AND have arrived before the mark op: the reference's walk never matches anything
+            // else (peritext.ts:236-241) — a missing start is a no-op, a missing end never ends
             const bool inb = k < m;
             const bool idok = inb && key != kS1;
+            const uint32_t js = lookup(min(skey, ksMax)), je = lookup(min(ekey, ksMax));
+            const uint32_t es = EV[min(js, n)], ee = EV[min(je, n)];
             bool dup = false;
-            if (idok) {
-                const uint32_t bit = 1u << (key & 31);
-                dup = (atomicOr(&KBits[key >> 5], bit) & bit) != 0 || lookup(key) != kNone16;      // duplicate opId
-            }
+            if (idok) { const uint32_t bit = 1u << (key & 31); dup = (atomicOr(&KSeen[key >> 5], bit) & bit) != 0; }   // an insert's or an earlier mark's opId
             if (inb && (!idok || dup)) fail(PT_LOG_BAD_OPID);
-            const bool sOk = idok && skey != kS1;
-            uint32_t js = kNone16;
-            if (sOk) js = lookup(skey);
-            const bool sHit = js != kNone16 && js < arrival;
-            uint32_t es = 0;
-            if (sHit) es = EV[js];
-            const uint32_t va = (es & 0x7FFFu) + (sb & (es >> 15));
-            const bool eOk = sHit && ekey != kS1;
-            uint32_t je = kNone16;
-            if (eOk) je = lookup(ekey);
+            // kNone16 is above every arrival (11 bits)
+            const bool sHit = idok && skey != kS1 && js < arrival;
             // same slot: the start branch wins and the op never ends (quirk Q2)
-            const bool eHit = je != kNone16 && je < arrival && !(je == js && eb == sb);
-            uint32_t vb = nvis;
-            if (eHit) { const uint32_t ee = EV[je]; vb = (ee & 0x7FFFu) + (eb & (ee >> 15)); }
+            const bool eHit = ekey != kS1 && je < arrival && !(je == js && eb == sb);
+            const uint32_t va = (es & 0x7FFFu) + (sb & (es >> 15));
+            const uint32_t vb = eHit ? (ee & 0x7FFFu) + (eb & (ee >> 15)) : nvis;
             const bool surv = sHit && va < vb;
             const bool isC = surv && type == PT_MARK_COMMENT;
             const uint32_t bal = __ballot_sync(kFull, surv), balC = __ballot_sync(kFull, isC);
@@ -602,6 +599,8 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
                     Sv[idx] = make_uint4(va | (vb << 16), (type == PT_MARK_COMMENT ? k : key) | (kind << 16), PT_ATTR_NONE, k);
                     if (isC) { const uint32_t ci = nC + __popc(balC & lt); if (ci <= kMaxCommentSurvivors) CIdx[ci] = (uint16_t)idx; }
                 }
+                // the attr that the batch after the loop loads: its line goes to L2 now, off the end of the pass
+                if (type == PT_MARK_LINK || type == PT_MARK_COMMENT) prefetch_l2(&P.marks[(mk + k) - P.key_marks].attr);
             }
             nS += __popc(bal); nC += __popc(balC);
             a = b;
@@ -625,6 +624,7 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     ps.pass();                                                     // (5) marks resolved
     PT_PHASE(kPhG);
     unsigned long long pool_base = 0;
+    pt_span* span_out = P.spans + P.span_off[li];               // derived here, not at the log's start: A+B to G need the registers
     if (nvis == 0) nspans = 0;
     else if (nS == 0) {
         // no mark op touches a visible element: one span {} (peritext.ts:392)
