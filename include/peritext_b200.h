@@ -706,6 +706,70 @@ int pt_batch_select_logs(pt_batch*, const uint32_t* from, uint32_t n_logs,
                          const pt_actor_tables* added_actors,   /* NULL iff the handle has no actor tables          */
                          const uint32_t* comment_map, uint64_t n_comment_map);   /* NULL = identity              */
 
+/* ------------------------------------------------------------------------------------------------
+ * Checkout: an EARLIER version of a resident log as a new log, on the device.  A history slider, "what does peer P see" (the
+ * version named by P's vector clock, getMissingChanges' input, reference test/merge.ts:25-38) and the last clock two diverged
+ * replicas shared are all a version: what a fresh Micromerge holds after applyChange of exactly the changes it covers.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_clock_entry { uint32_t actor; uint32_t seq; } pt_clock_entry;   /* actor rank in the request's log */
+#define PT_CHECKOUT_OK 0u
+#define PT_CHECKOUT_BAD_TABLE 1u   /* the source's change table fails pt_batch_exchange's BAD_TABLE rules for a src: not
+                                      seq-contiguous per actor, an actor >= n_actors, deps outside the log's, n_ops that do not
+                                      sum to its n_insdel + n_mark, or mark arrivals that do not fit those positions          */
+#define PT_CHECKOUT_UNKNOWN 2u     /* clock mode: clock[a] > the log's number of changes by a (the version holds changes this
+                                      log does not)                                                                          */
+#define PT_CHECKOUT_NOT_CLOSED 3u  /* a fresh replica applying the covered changes in table order would reject one           */
+/* Request k adds new log old n_logs + k, holding log logs[k] at a version:
+ *   covered   prefix mode (n_changes non-NULL): the first min(n_changes[k], table size) changes of the log's table.  Clock mode
+ *             (clock_off non-NULL): the changes with seq <= clock[actor], request k's clock being the entries
+ *             clock[clock_off[k] .. clock_off[k+1]) (actor ranks of log logs[k]); an absent actor counts as 0 and a seq of 0 is
+ *             allowed.  In a seq-contiguous table prefix j is the clock mode of the prefix's per-actor counts.
+ *   records   the covered changes' ins/del records, concatenated in table order, then their mark records likewise; record
+ *             ranges come from the list-op positions (pt_batch_exchange step 4).  A mark's arrival is the number of covered
+ *             ins/del records before it.  Change records keep seq and n_ops; dep_off is rebased and the deps are copied.
+ *   ids       the source's: actor ranks, counters, comment ranks, value and link ids, and the descriptor's n_actors and
+ *             max_ctr.  With actor tables attached the new log gets the source's table and its dense-counter bit.
+ *   status    status_out[k] = PT_CHECKOUT_*.  NOT_CLOSED is applyChange's check (src/micromerge.ts:505-509) in table order: a
+ *             covered change c fails it when a dep (a, d) of c has fewer than max(d, 1) covered changes by a before c, so a
+ *             zero clock entry fails and a source that admission rejected is reported as such.  A request that is not OK still
+ *             adds its log, with no records and no changes, so the indices stay stable.
+ * Several requests may name one log.  Afterwards the handle holds exactly what pt_batch_select_logs(from = [0 .. n_logs)
+ * followed by PT_SELECT_ADDED x n, added = the new logs) would hold: the batch is re-planned and its key records derived again,
+ * there is no merge (views of the last merge are invalid), the patch window is reset, pool settings persist, and a later
+ * pt_batch_select_logs([0 .. old n_logs)) retires the checkouts.  No merge is needed before the call.
+ * Refused with nothing changed:
+ *   PT_ERR_STATE    no batch, or a handle without a change table
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) null arguments; a log >= n_logs; both modes or neither; clock_off
+ *                   not non-decreasing from 0; a clock actor >= the log's n_actors; an actor named twice in one request; what
+ *                   an upload refuses for the resulting batch (make_plan)
+ * n == 0: PT_OK, nothing launched, nothing changed.  Synchronises; the caller's arrays may be freed on return.
+ * Device: a select kernel, one warp per request (the clocks in shared memory, then one pass over the table and an in-order
+ * pass that checks closure and places the covered changes' records, 32 changes per trip), the per-request totals back to the
+ * host (32 B per request), pt_batch_exchange's gather kernel with identity maps into empty logs, then pt_batch_select_logs'
+ * splice and actor-table gather.  No record and no change record crosses PCIe: only the requests, the totals and the
+ * statuses.  Peak device memory: old + delta + new records and change tables, plus 40 B of scratch per change of every
+ * request's source. */
+int pt_batch_checkout(pt_batch*, const uint32_t* logs, uint32_t n,
+                      const uint32_t* n_changes,      /* [n] prefix mode, or NULL                                           */
+                      const uint64_t* clock_off,      /* [n + 1] clock mode, or NULL; exactly one of the two is non-NULL       */
+                      const pt_clock_entry* clock,    /* request k's clock = clock[clock_off[k] .. clock_off[k+1])             */
+                      uint32_t* status_out);          /* [n] caller-owned, PT_CHECKOUT_*                                       */
+
+/* Every log's clock: seq[off[i] + a] = the number of changes by actor rank a in log i's change table (Micromerge.clock by
+ * rank), off = the exclusive scan of n_actors ([n_logs + 1]).  status[i] is PT_CHECKOUT_BAD_TABLE where the table fails
+ * pt_batch_exchange's clock checks (not seq-contiguous per actor, an actor >= n_actors, deps outside the log's); that log's
+ * entries are 0.  This names the version a log holds now, also after pt_batch_change, pt_batch_exchange or
+ * pt_batch_sync_pairs, so that it can be checked out later.  No batch or no change table: PT_ERR_STATE; null arguments:
+ * PT_ERR_INVALID.  Synchronises.  The view is engine-owned pinned memory, valid until the next call of it, upload or
+ * destroy.  Device: one warp per log counting its table (ptx::count_clock) into the output. */
+int pt_batch_download_clocks(pt_batch*, const uint64_t** off, const uint32_t** seq, const uint32_t** status);
+
+/* The handle's per-log descriptors ([n_logs]; offsets into the engine's records): the shape of the resident batch after calls
+ * that build logs on the device, such as pt_batch_checkout, whose record counts the caller does not know.  No batch:
+ * PT_ERR_STATE; null out: PT_ERR_INVALID.  The view is engine-owned host memory, valid until the next call that changes the
+ * batch (upload, append, change, exchange, sync, select, checkout) or destroy.  No device work. */
+int pt_batch_download_descs(pt_batch*, const pt_log_desc** out);
+
 /* Enqueue the merge: op-log apply + flatten for every log of the batch (the replacement for the
  * applyOp loop src/micromerge.ts:513 and getTextWithFormatting src/peritext.ts:337). Asynchronous. */
 int pt_batch_merge(pt_batch*);
@@ -866,7 +930,6 @@ typedef struct pt_changes_request {   /* 32 B */
     uint64_t clock_off;                /* MISSING: the peer's clock is clock[clock_off .. clock_off + n_clock)             */
     uint32_t n_clock, reserved;
 } pt_changes_request;
-typedef struct pt_clock_entry { uint32_t actor; uint32_t seq; } pt_clock_entry;   /* actor rank in the request's log */
 typedef struct pt_changes_json_input {
     uint32_t n_requests, reserved;
     const pt_changes_request* requests;

@@ -29,6 +29,7 @@
 #include "admit_kernel.cuh"
 #include "query_kernel.cuh"
 #include "sync_kernel.cuh"
+#include "checkout_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -143,6 +144,7 @@ struct pt_batch {
     HostBuf h_act_data, h_act_off, h_act_first;                          // the view of pt_batch_download_actors
     HostBuf h_syn_totals, h_syn_status, h_syn_off, h_syn_aoff, h_syn_amap;   // the view of the last pt_batch_sync_pairs
     HostBuf h_add_totals, h_add_rank, h_add_aoff, h_add_amap;               // the view of the last pt_batch_add_actors
+    HostBuf h_clk_off, h_clk_seq, h_clk_status;                             // the view of the last pt_batch_download_clocks
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -1220,7 +1222,7 @@ static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pa
     uint32_t* delivered = (uint32_t*)b->h_xch_delivered.p;
     if (n_ch) {
         if ((rc = upload_n(b, ddoff, dlv_off.data(), (uint64_t)np + 1)) || (rc = upload_n(b, dbase, base.data(), np))) return rc;
-        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p;
+        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p; P.dst_desc = P.desc;
         P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
         P.out_delivered = (uint32_t*)dgx.p;
         // one warp per delivered change; a pair's records are an upper bound of its longest change
@@ -1620,6 +1622,60 @@ static std::string check_select(const pt_batch* b, const uint32_t* from, uint32_
     return std::string();
 }
 
+// New actor tables for the n logs of a select or a checkout: new log i takes resident log from[i]'s table, or (from[i] ==
+// PT_SELECT_ADDED) added log add_idx[i]'s of `added`.  They are gathered into buffers of their own, which replace the handle's
+// (install_actor_tables) once the splice is accepted.
+struct NewActorTables {
+    DevBuf names, off, first, byte, from, adata, aoff, afirst;   // the tables, and the gather's inputs
+    std::vector<unsigned long long> h_first, h_byte;
+    std::vector<char> dense;
+};
+
+static int gather_actor_tables(pt_batch* b, const uint32_t* from, uint32_t n, const pt_actor_tables* added, const std::vector<uint32_t>& add_idx,
+                               NewActorTables& T) {
+    int rc;
+    const uint64_t lo = added && added->count ? added->off[0] : 0;
+    const uint64_t abytes = added && added->count ? added->off[added->count] - lo : 0, acount = added ? added->count : 0;
+    std::vector<unsigned long long> add_first(n, 0), add_off(acount + 1, 0);
+    for (uint64_t k = 0; k <= acount && added; k++) add_off[k] = acount ? added->off[k] - lo : 0;
+    T.h_first.assign((size_t)n + 1, 0); T.h_byte.assign((size_t)n + 1, 0); T.dense.assign(n, 0);
+    for (uint32_t i = 0; i < n; i++) {
+        uint64_t cnt, bytes;
+        if (add_idx[i] != ~0u) {
+            const uint64_t* pf = added->per_log_first + add_idx[i];
+            add_first[i] = pf[0]; cnt = pf[1] - pf[0]; bytes = add_off[pf[1]] - add_off[pf[0]];
+            T.dense[i] = added->counters_first && added->counters_first[add_idx[i] + 1] > added->counters_first[add_idx[i]];
+        } else {
+            const uint32_t s = from[i];
+            cnt = b->h_afirst[s + 1] - b->h_afirst[s]; bytes = b->h_abyte[s + 1] - b->h_abyte[s];
+            T.dense[i] = b->h_adense[s];
+        }
+        T.h_first[i + 1] = T.h_first[i] + cnt; T.h_byte[i + 1] = T.h_byte[i] + bytes;
+    }
+    if ((rc = reserve_n<uint8_t>(T.names, T.h_byte[n])) || (rc = reserve_n<unsigned long long>(T.off, T.h_first[n] + 1)) ||
+        (rc = upload_n(b, T.first, T.h_first.data(), (uint64_t)n + 1)) || (rc = upload_n(b, T.byte, T.h_byte.data(), (uint64_t)n + 1)) ||
+        (rc = upload_n(b, T.from, from, n)) || (rc = upload_n(b, T.adata, abytes ? added->data + lo : nullptr, abytes)) ||
+        (rc = upload_n(b, T.aoff, add_off.data(), acount + 1)) || (rc = upload_n(b, T.afirst, add_first.data(), n))) return rc;
+    PT_CUDA(cudaMemsetAsync(T.off.p, 0, 8, b->stream));
+    if (n) {
+        pty::GatherParams G{};
+        G.n_logs = n; G.from = (const uint32_t*)T.from.p;
+        G.old_t = pty::Tables{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
+        G.add_data = (const uint8_t*)T.adata.p; G.add_off = (const unsigned long long*)T.aoff.p; G.add_first = (const unsigned long long*)T.afirst.p;
+        G.data = (uint8_t*)T.names.p; G.off = (unsigned long long*)T.off.p;
+        G.first = (const unsigned long long*)T.first.p; G.byte_base = (const unsigned long long*)T.byte.p;
+        pty::actor_gather_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(G);
+        PT_CUDA(launched(b));
+    }
+    return PT_OK;
+}
+
+static void install_actor_tables(pt_batch* b, NewActorTables& T) {
+    b->d_anames.swap(T.names); b->d_aoff.swap(T.off); b->d_afirst.swap(T.first);
+    b->h_afirst.assign(T.h_first.begin(), T.h_first.end()); b->h_abyte.assign(T.h_byte.begin(), T.h_byte.end());
+    b->h_adense = std::move(T.dense);
+}
+
 int pt_batch_select_logs(pt_batch* b, const uint32_t* from, uint32_t n, const pt_packed_ops* added, const pt_change_table* added_changes,
                          const pt_actor_tables* added_actors, const uint32_t* comment_map, uint64_t n_comment_map) {
     const char* fn = "pt_batch_select_logs: ";
@@ -1640,50 +1696,171 @@ int pt_batch_select_logs(pt_batch* b, const uint32_t* from, uint32_t n, const pt
     PT_CUDA(cudaSetDevice(b->device));
     // The actor tables are gathered first, into new buffers that replace the old ones once the splice is accepted.
     int rc;
-    DevBuf nnames, noff, nfirst, nbyte, dfrom, adata, aoff, afirst;
-    std::vector<unsigned long long> new_first, new_byte;
-    std::vector<char> new_dense;
-    if (b->have_actors) {
-        const uint64_t lo = added_actors && added_actors->count ? added_actors->off[0] : 0;
-        const uint64_t abytes = added_actors && added_actors->count ? added_actors->off[added_actors->count] - lo : 0, acount = added_actors ? added_actors->count : 0;
-        std::vector<unsigned long long> add_first(n, 0), add_off(acount + 1, 0);
-        for (uint64_t k = 0; k <= acount && added_actors; k++) add_off[k] = acount ? added_actors->off[k] - lo : 0;
-        new_first.assign((size_t)n + 1, 0); new_byte.assign((size_t)n + 1, 0); new_dense.assign(n, 0);
-        for (uint32_t i = 0; i < n; i++) {
-            uint64_t cnt, bytes;
-            if (add_idx[i] != ~0u) {
-                const uint64_t* pf = added_actors->per_log_first + add_idx[i];
-                add_first[i] = pf[0]; cnt = pf[1] - pf[0]; bytes = add_off[pf[1]] - add_off[pf[0]];
-                new_dense[i] = added_actors->counters_first && added_actors->counters_first[add_idx[i] + 1] > added_actors->counters_first[add_idx[i]];
-            } else {
-                const uint32_t s = from[i];
-                cnt = b->h_afirst[s + 1] - b->h_afirst[s]; bytes = b->h_abyte[s + 1] - b->h_abyte[s];
-                new_dense[i] = b->h_adense[s];
-            }
-            new_first[i + 1] = new_first[i] + cnt; new_byte[i + 1] = new_byte[i] + bytes;
-        }
-        if ((rc = reserve_n<uint8_t>(nnames, new_byte[n])) || (rc = reserve_n<unsigned long long>(noff, new_first[n] + 1)) ||
-            (rc = upload_n(b, nfirst, new_first.data(), (uint64_t)n + 1)) || (rc = upload_n(b, nbyte, new_byte.data(), (uint64_t)n + 1)) ||
-            (rc = upload_n(b, dfrom, from, n)) || (rc = upload_n(b, adata, abytes ? added_actors->data + lo : nullptr, abytes)) ||
-            (rc = upload_n(b, aoff, add_off.data(), acount + 1)) || (rc = upload_n(b, afirst, add_first.data(), n))) return rc;
-        PT_CUDA(cudaMemsetAsync(noff.p, 0, 8, b->stream));
-        if (n) {
-            pty::GatherParams G{};
-            G.n_logs = n; G.from = (const uint32_t*)dfrom.p;
-            G.old_t = pty::Tables{(const uint8_t*)b->d_anames.p, (const unsigned long long*)b->d_aoff.p, (const unsigned long long*)b->d_afirst.p};
-            G.add_data = (const uint8_t*)adata.p; G.add_off = (const unsigned long long*)aoff.p; G.add_first = (const unsigned long long*)afirst.p;
-            G.data = (uint8_t*)nnames.p; G.off = (unsigned long long*)noff.p;
-            G.first = (const unsigned long long*)nfirst.p; G.byte_base = (const unsigned long long*)nbyte.p;
-            pty::actor_gather_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>(G);
-            PT_CUDA(launched(b));
-        }
-    }
+    NewActorTables T;
+    if (b->have_actors && (rc = gather_actor_tables(b, from, n, added_actors, add_idx, T))) return rc;
     if ((rc = splice(b, fn, std::move(nd), std::move(ncd), maxR, &delta, false, R, from, b->have_changes ? &dch : nullptr, false, true))) return rc;
-    if (b->have_actors) {
-        b->d_anames.swap(nnames); b->d_aoff.swap(noff); b->d_afirst.swap(nfirst);
-        b->h_afirst.assign(new_first.begin(), new_first.end()); b->h_abyte.assign(new_byte.begin(), new_byte.end());
-        b->h_adense = std::move(new_dense);
+    if (b->have_actors) install_actor_tables(b, T);
+    return PT_OK;
+}
+
+// pt_batch_checkout's host checks (include/peritext_b200.h).  Returns the problem, or an empty string.
+static std::string check_checkout(const pt_batch* b, const uint32_t* logs, uint32_t n, const uint32_t* n_changes, const uint64_t* clock_off,
+                                  const pt_clock_entry* clock, const uint32_t* status_out) {
+    if (!logs || !status_out) return "null logs or status_out";
+    if ((n_changes != nullptr) == (clock_off != nullptr)) return "exactly one of n_changes (prefix mode) and clock_off (clock mode) must be given";
+    if ((uint64_t)b->n_logs + n > 0xFFFFFFFFull) return "the batch would have more than 2^32 - 1 logs";
+    if (clock_off && clock_off[0] != 0) return "clock_off[0] is not 0";
+    std::vector<uint32_t> seen;                           // seen[a] = k + 1: request k names actor a
+    for (uint32_t k = 0; k < n; k++) {
+        const std::string here = "request " + std::to_string(k) + ": ";
+        if (logs[k] >= b->n_logs) return here + "log " + std::to_string(logs[k]) + " is outside the batch's " + std::to_string(b->n_logs) + " logs";
+        if (!clock_off) continue;
+        if (clock_off[k + 1] < clock_off[k]) return "clock_off decreases at request " + std::to_string(k);
+        if (clock_off[k + 1] > clock_off[k] && !clock) return "null clock with a nonzero length";
+        const uint32_t R = b->h_desc[logs[k]].n_actors;
+        if (seen.size() < R) seen.resize(R, 0);
+        for (uint64_t e = clock_off[k]; e < clock_off[k + 1]; e++) {
+            const uint32_t a = clock[e].actor;
+            if (a >= R) return here + "clock actor " + std::to_string(a) + " >= log " + std::to_string(logs[k]) + "'s " + std::to_string(R) + " actors";
+            if (seen[a] == k + 1) return here + "actor " + std::to_string(a) + " is named twice";
+            seen[a] = k + 1;
+        }
     }
+    return std::string();
+}
+
+int pt_batch_checkout(pt_batch* b, const uint32_t* logs, uint32_t n, const uint32_t* n_changes, const uint64_t* clock_off,
+                      const pt_clock_entry* clock, uint32_t* status_out) {
+    const char* fn = "pt_batch_checkout: ";
+    if (!b) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_checkout before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = std::string(fn) + "the handle has no change table"; return PT_ERR_STATE; }
+    if (!n) return PT_OK;
+    const std::string err = check_checkout(b, logs, n, n_changes, clock_off, clock, status_out);
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    const uint32_t n0 = b->n_logs, nn = n0 + n;
+    std::vector<unsigned long long> slot_off((size_t)n + 1, 0);
+    for (uint32_t k = 0; k < n; k++) slot_off[k + 1] = slot_off[k] + b->h_cdesc[logs[k]].n_changes;
+    const uint64_t n_slot = slot_off[n];
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    int rc;
+    // ---- select: which changes each request covers, its status and its records' places ----
+    DevBuf dlogs, dnch, dcoff, dclk, dslot, dpos, dcov, ddlv, dtot;   // freed on return
+    if ((rc = upload_n(b, dlogs, logs, n)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)n + 1)) ||
+        (rc = reserve_n<uint32_t>(dpos, n_slot)) || (rc = reserve_n<uint32_t>(dcov, n_slot)) ||
+        (rc = reserve_n<ptx::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptx::PairTotals>(dtot, n))) return rc;
+    if (n_changes && (rc = upload_n(b, dnch, n_changes, n))) return rc;
+    if (clock_off && ((rc = upload_n(b, dcoff, clock_off, (uint64_t)n + 1)) || (rc = upload_n(b, dclk, clock, clock_off[n])))) return rc;
+    ptck::CheckoutParams C{};
+    C.logs = (const uint32_t*)dlogs.p; C.n = n; C.maxR = b->adm_maxR;
+    C.n_changes = n_changes ? (const uint32_t*)dnch.p : nullptr;
+    C.clock_off = (const unsigned long long*)dcoff.p; C.clock = (const pt_clock_entry*)dclk.p;
+    C.desc = (const pt_log_desc*)b->d_desc.p; C.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    C.changes = (const pt_change_rec*)b->d_changes.p; C.deps = (const pt_dep_rec*)b->d_deps.p; C.marks = b->dp_marks;
+    C.slot_off = (const unsigned long long*)dslot.p; C.pos = (uint32_t*)dpos.p; C.cov = (uint32_t*)dcov.p; C.dlv = (ptx::Delivered*)ddlv.p;
+    C.totals = (ptx::PairTotals*)dtot.p;
+    const auto [wpb, smem] = actor_shape(b->adm_maxR);
+    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptck::checkout_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ptck::checkout_select_kernel<<<warp_grid(b, n, wpb * 32), wpb * 32, smem, b->stream>>>(C);
+    PT_CUDA(launched(b));
+    std::vector<ptx::PairTotals> tot(n);
+    PT_CUDA(cudaMemcpyAsync(tot.data(), dtot.p, (size_t)n * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    // ---- the new batch: the resident logs, then one log per request (a request that is not OK has zero totals) ----
+    std::vector<uint32_t> from(nn), tables_from(nn);
+    std::vector<pt_log_desc> nd(nn), dd(nn, pt_log_desc{});
+    std::vector<pt_change_desc> ncd(nn), dcd(nn, pt_change_desc{});
+    std::vector<ptx::PairBase> base(n);
+    std::vector<pt_exchange_pair> pairs(n);
+    std::vector<unsigned long long> dlv_off((size_t)n + 1, 0);
+    uint64_t io = 0, mo = 0, co = 0, po = 0, n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0, most = 0;
+    for (uint32_t i = 0; i < nn; i++) {
+        const bool old = i < n0;
+        const uint32_t s = old ? i : logs[i - n0];
+        const pt_log_desc S = b->h_desc[s];
+        const pt_change_desc CS = b->h_cdesc[s];
+        from[i] = old ? i : PT_SELECT_ADDED; tables_from[i] = s;
+        pt_log_desc L = S;
+        pt_change_desc LC = CS;
+        if (!old) {
+            const uint32_t k = i - n0;
+            const ptx::PairTotals& t = tot[k];
+            status_out[k] = t.status;
+            L = pt_log_desc{n_ins, n_mk, t.n_insdel, t.n_mark, S.n_actors, S.max_ctr};
+            LC = pt_change_desc{n_ch, n_dp, t.n_changes, t.n_deps};
+            dd[i] = L; dcd[i] = LC;
+            base[k] = ptx::PairBase{n_ins, n_mk, n_ch, n_dp};
+            pairs[k] = pt_exchange_pair{s, k};
+            n_ins += t.n_insdel; n_mk += t.n_mark; n_ch += t.n_changes; n_dp += t.n_deps;
+            dlv_off[k + 1] = n_ch;
+            most = std::max<uint64_t>(most, (uint64_t)t.n_insdel + 2ull * t.n_mark);
+        }
+        nd[i] = pt_log_desc{io, mo, L.n_insdel, L.n_mark, L.n_actors, L.max_ctr};
+        ncd[i] = pt_change_desc{co, po, LC.n_changes, LC.n_deps};
+        io += L.n_insdel; mo += L.n_mark; co += LC.n_changes; po += LC.n_deps;
+    }
+    // ---- gather: the covered changes' records, change and dep records into the delta, identity maps, arrivals from 0 ----
+    DevBuf dpairs, ddoff, dbase, dempty, dgi, dgm, dgc, dgd;
+    if ((rc = reserve_n<pt_insdel_rec>(dgi, n_ins)) || (rc = reserve_n<pt_mark_rec>(dgm, n_mk)) ||
+        (rc = reserve_n<pt_change_rec>(dgc, n_ch)) || (rc = reserve_n<pt_dep_rec>(dgd, n_dp))) return rc;
+    if (n_ch) {
+        if ((rc = upload_n(b, dpairs, pairs.data(), n)) || (rc = upload_n(b, ddoff, dlv_off.data(), (uint64_t)n + 1)) ||
+            (rc = upload_n(b, dbase, base.data(), n)) || (rc = reserve_n<pt_log_desc>(dempty, n))) return rc;
+        PT_CUDA(cudaMemsetAsync(dempty.p, 0, (size_t)n * sizeof(pt_log_desc), b->stream));
+        ptx::ExchangeParams P{};
+        P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = n;
+        P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+        P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
+        P.insdel = b->dp_insdel; P.marks = b->dp_marks;
+        P.slot_off = (const unsigned long long*)dslot.p; P.dlv = (ptx::Delivered*)ddlv.p; P.totals = (ptx::PairTotals*)dtot.p;
+        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p;
+        P.dst_desc = (const pt_log_desc*)dempty.p;
+        P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
+        ptx::exchange_gather_kernel<<<slice_grid(b, n_ch, most, 128), 128, 0, b->stream>>>(P);
+        PT_CUDA(launched(b));
+    }
+    // ---- splice: the delta as added logs behind the kept ones, and the sources' actor tables ----
+    const pt_packed_ops delta{nn, dd.data(), (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
+    const pt_change_table dch{nn, dcd.data(), (const pt_change_rec*)dgc.p, n_ch, (const pt_dep_rec*)dgd.p, n_dp};
+    NewActorTables T;
+    if (b->have_actors && (rc = gather_actor_tables(b, tables_from.data(), nn, nullptr, std::vector<uint32_t>(nn, ~0u), T))) return rc;
+    if ((rc = splice(b, fn, std::move(nd), std::move(ncd), b->adm_maxR, &delta, true, pt_append_remap{}, from.data(), &dch, true, true))) return rc;
+    if (b->have_actors) install_actor_tables(b, T);
+    return PT_OK;
+}
+
+int pt_batch_download_clocks(pt_batch* b, const uint64_t** off, const uint32_t** seq, const uint32_t** status) {
+    if (!b || !off || !seq || !status) { g_last_error = "pt_batch_download_clocks: null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_download_clocks before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = "pt_batch_download_clocks: the handle has no change table"; return PT_ERR_STATE; }
+    const uint32_t n = b->n_logs;
+    int rc;
+    if ((rc = reserve_n<uint64_t>(b->h_clk_off, (uint64_t)n + 1)) || (rc = reserve_n<uint32_t>(b->h_clk_status, n))) return rc;
+    uint64_t* hoff = (uint64_t*)b->h_clk_off.p;
+    hoff[0] = 0;
+    for (uint32_t i = 0; i < n; i++) hoff[i + 1] = hoff[i] + b->h_desc[i].n_actors;
+    if ((rc = reserve_n<uint32_t>(b->h_clk_seq, hoff[n]))) return rc;
+    PT_CUDA(cudaSetDevice(b->device));
+    if (n) {
+        DevBuf doff, dseq, dst;                              // freed on return
+        if ((rc = upload_n(b, doff, hoff, (uint64_t)n + 1)) || (rc = reserve_n<uint32_t>(dseq, hoff[n])) || (rc = reserve_n<uint32_t>(dst, n))) return rc;
+        ptck::clocks_kernel<<<warp_grid(b, n, 128), 128, 0, b->stream>>>((const pt_change_desc*)b->d_cdesc.p, (const pt_change_rec*)b->d_changes.p,
+                                                                         (const pt_log_desc*)b->d_desc.p, n, (const unsigned long long*)doff.p,
+                                                                         (uint32_t*)dseq.p, (uint32_t*)dst.p);
+        PT_CUDA(launched(b));
+        if (hoff[n]) PT_CUDA(cudaMemcpyAsync(b->h_clk_seq.p, dseq.p, hoff[n] * 4, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaMemcpyAsync(b->h_clk_status.p, dst.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    *off = hoff; *seq = (const uint32_t*)b->h_clk_seq.p; *status = (const uint32_t*)b->h_clk_status.p;
+    return PT_OK;
+}
+
+int pt_batch_download_descs(pt_batch* b, const pt_log_desc** out) {
+    if (!b || !out) { g_last_error = "pt_batch_download_descs: null argument"; return PT_ERR_INVALID; }
+    if (!b->have_batch) { g_last_error = "pt_batch_download_descs before pt_batch_upload"; return PT_ERR_STATE; }
+    *out = b->h_desc.data();
     return PT_OK;
 }
 

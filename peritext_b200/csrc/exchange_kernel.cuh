@@ -22,7 +22,8 @@
 // exchange_gather_kernel: one warp per delivered change (blockIdx.y slices a long change, as splice_records_kernel slices a
 // long log): 16-byte coalesced copies with the pair's actor and counter maps applied (a mark is a lane pair, as in the
 // splice), mark arrivals rebased onto dst's records; slice 0 also writes the change record, its deps and the delivered index.
-// An id without an image sets the pair's status, and the host drops that pair's delta.
+// An id without an image sets the pair's status, and the host drops that pair's delta.  pt_batch_checkout runs it too, with
+// identity maps and empty dst logs (checkout_kernel.cuh).
 #pragma once
 #include <cstdint>
 
@@ -40,12 +41,12 @@ struct Delivered {          // one per delivered change, in delivery order.  32 
 };
 struct PairBase { unsigned long long insdel, mark, change, dep; };   // where a pair's records start in the delta arrays
 
-// One pair's maps, src id space -> dst id space.  The actor map has exactly src's n_actors entries; nc == 0 is the identity
-// counter map.  No image: 0xFFFF / 0xFFFFFFFF.
+// One pair's maps, src id space -> dst id space.  The actor map has exactly src's n_actors entries; a == null (pt_batch_checkout)
+// is the identity actor map and nc == 0 the identity counter map.  No image: 0xFFFF / 0xFFFFFFFF.
 struct PairMaps {
     const uint16_t* a; uint32_t na;
     const uint32_t* c; uint32_t nc;
-    __device__ __forceinline__ uint32_t actor(uint32_t x) const { return x < na ? (uint32_t)__ldg(a + x) : 0xFFFFu; }
+    __device__ __forceinline__ uint32_t actor(uint32_t x) const { return a ? (x < na ? (uint32_t)__ldg(a + x) : 0xFFFFu) : x; }
     __device__ __forceinline__ uint32_t ctr(uint32_t x) const { return nc ? (x < nc ? __ldg(c + x) : 0xFFFFFFFFu) : x; }
     // the actor of an id whose counter is ctr_old: counter 0 is HEAD / a text boundary and names no actor
     __device__ __forceinline__ uint32_t id_actor(uint32_t ctr_old, uint32_t x) const { return ctr_old ? actor(x) : x; }
@@ -53,7 +54,7 @@ struct PairMaps {
 
 struct ExchangeParams {
     const pt_exchange_pair* pairs; uint32_t n_pairs; uint32_t maxR;
-    const unsigned long long* actor_off; const uint16_t* actor_map;
+    const unsigned long long* actor_off; const uint16_t* actor_map;    // actor_off null: identity for every pair (gather only)
     const unsigned long long* ctr_off;  const uint32_t* ctr_map;       // ctr_off null: identity for every pair
     const pt_log_desc* desc; const pt_change_desc* cdesc; const pt_change_rec* changes; const pt_dep_rec* deps;
     const pt_insdel_rec* insdel; const pt_mark_rec* marks;
@@ -64,13 +65,14 @@ struct ExchangeParams {
     const unsigned long long* dlv_off;    // [n_pairs + 1] exclusive scan of the pairs' delivered changes
     unsigned long long n_dlv;
     const PairBase* base;
-    pt_insdel_rec* out_insdel; pt_mark_rec* out_marks; pt_change_rec* out_changes; pt_dep_rec* out_deps; uint32_t* out_delivered;
+    const pt_log_desc* dst_desc;          // the descriptors a pair's dst indexes: desc, or a checkout's empty logs
+    pt_insdel_rec* out_insdel; pt_mark_rec* out_marks; pt_change_rec* out_changes; pt_dep_rec* out_deps;
+    uint32_t* out_delivered;              // may be null
 };
 
 __device__ __forceinline__ PairMaps pair_maps(const ExchangeParams& P, uint32_t p) {
     PairMaps m{nullptr, 0u, nullptr, 0u};
-    const unsigned long long ao = P.actor_off[p];
-    m.a = P.actor_map + ao; m.na = (uint32_t)(P.actor_off[p + 1] - ao);
+    if (P.actor_off) { const unsigned long long ao = P.actor_off[p]; m.a = P.actor_map + ao; m.na = (uint32_t)(P.actor_off[p + 1] - ao); }
     if (P.ctr_off) { const unsigned long long o = P.ctr_off[p]; m.c = P.ctr_map + o; m.nc = (uint32_t)(P.ctr_off[p + 1] - o); }
     return m;
 }
@@ -265,7 +267,7 @@ __global__ void exchange_gather_kernel(ExchangeParams P) {
         while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (P.dlv_off[mid] <= j) lo = mid; else hi = mid; }
         const uint32_t p = lo, k = (uint32_t)(j - P.dlv_off[p]);
         const pt_exchange_pair pr = P.pairs[p];
-        const pt_log_desc S = P.desc[pr.src], D = P.desc[pr.dst];
+        const pt_log_desc S = P.desc[pr.src], D = P.dst_desc[pr.dst];
         const PairMaps m = pair_maps(P, p);
         const PairBase B = P.base[p];
         const Delivered d = P.dlv[P.slot_off[p] + k];
@@ -325,7 +327,7 @@ __global__ void exchange_gather_kernel(ExchangeParams P) {
                 unmapped |= a == 0xFFFFu;
                 r.y = (r.y & 0xFFFF0000u) | a; r.z = d.dep_off;
                 reinterpret_cast<uint4*>(P.out_changes + B.change)[k] = r;
-                P.out_delivered[j] = d.change;
+                if (P.out_delivered) P.out_delivered[j] = d.change;
             }
         }
         for (int o = 16; o > 0; o >>= 1) top = max(top, __shfl_xor_sync(0xffffffffu, top, o));

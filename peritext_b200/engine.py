@@ -38,6 +38,9 @@ _ENTRY_POINTS = {
     "pt_batch_add_actors": ([_vp, _vp, _vp], _int),
     "pt_batch_sync_pairs": ([_vp, _vp, _u32, _vp], _int),
     "pt_batch_select_logs": ([_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u64], _int),
+    "pt_batch_checkout": ([_vp, _vp, _u32, _vp, _vp, _vp, _vp], _int),
+    "pt_batch_download_clocks": ([_vp, _out(_vp), _out(_vp), _out(_vp)], _int),
+    "pt_batch_download_descs": ([_vp, _out(_vp)], _int),
     "pt_ingest_create": ([_out(_vp)], _int),
     "pt_ingest_parse": ([_vp, _vp, _vp, _u32, _int], _int),
     "pt_ingest_packed": ([_vp, _vp, _vp], _int),
@@ -439,6 +442,39 @@ class BatchEngine:
         self.n_logs = len(frm)
         self._log_insdel, self._log_n_actors = ins, act
         self._spliced(np.zeros(0, DESC_DT))
+
+    def checkout(self, logs, n_changes=None, clock=None) -> np.ndarray:
+        """Fork resident logs at an earlier version, on the device (pt_batch_checkout): request k appends a new log holding log
+        ``logs[k]`` at the version of its first ``n_changes[k]`` changes (prefix mode) or of a vector clock (clock mode:
+        ``clock`` = (u64 offsets [n + 1], CLOCK_DT entries by actor rank), ``packing.checkout_clocks``).  Exactly one of the two
+        is given.  Returns the per-request status CHECKOUT_*; a request that is not OK adds an empty log.  The handle then
+        holds what an upload of ``packing.apply_checkout`` would hold, and needs a merge.  Needs a change table."""
+        lg = np.ascontiguousarray(logs, np.uint32)
+        nch = None if n_changes is None else np.ascontiguousarray(n_changes, np.uint32)
+        off = ent = None
+        if clock is not None:
+            off, ent = np.ascontiguousarray(clock[0], np.uint64), np.ascontiguousarray(clock[1], CLOCK_DT)
+        status = np.zeros(len(lg), np.uint32)
+        ptr = lambda a: None if a is None else a.ctypes.data                 # not _ptr: an empty array still names its mode
+        _check(self._L.pt_batch_checkout(self._h, _ptr(lg), len(lg), ptr(nch), ptr(off), _ptr(ent), _ptr(status)), "pt_batch_checkout")
+        if len(lg):
+            d = ctypes.c_void_p()
+            _check(self._L.pt_batch_download_descs(self._h, ctypes.byref(d)), "pt_batch_download_descs")
+            desc = _view(d.value, self.n_logs + len(lg), DESC_DT)
+            self.n_logs = len(desc)
+            self._log_insdel = desc["n_insdel"].astype(np.uint64)
+            self._log_n_actors = desc["n_actors"].astype(np.uint32)
+            self._spliced(np.zeros(0, DESC_DT))
+        return status
+
+    def clocks(self):
+        """Every log's clock (pt_batch_download_clocks): (u64 offsets [n_logs + 1], u32 seq, u32 status), log i's number of
+        changes by actor rank a at seq[off[i] + a]; status CHECKOUT_BAD_TABLE (and zeros) where the table is not
+        seq-contiguous.  ``packing.clocks`` is its host specification.  Needs a change table."""
+        off, seq, st = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        _check(self._L.pt_batch_download_clocks(self._h, ctypes.byref(off), ctypes.byref(seq), ctypes.byref(st)), "pt_batch_download_clocks")
+        o = _view(off.value, self.n_logs + 1, np.uint64)
+        return o, _view(seq.value, int(o[-1]), np.uint32), _view(st.value, self.n_logs, np.uint32)
 
     def change_packed(self, actor, input_off, ops, tokens, n_values: int, n_links: int, n_comments: int, changes: ChangeTable | None = None):
         """pt_batch_change from its arrays (``packing.change_inputs``, ``workload.sync_round``): per log i the actor rank of its

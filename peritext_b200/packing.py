@@ -1119,6 +1119,156 @@ def apply_exchange(batch: PackedBatch, pairs, maps: ExchangeMaps) -> tuple[Packe
     return apply_append(batch, delta), status, delivered, ddesc
 
 
+# ------------------------------------------------------------------------------------------------------------------
+# Checkout (include/peritext_b200.h pt_batch_checkout, pt_batch_download_clocks)
+# ------------------------------------------------------------------------------------------------------------------
+CHECKOUT_OK, CHECKOUT_BAD_TABLE, CHECKOUT_UNKNOWN, CHECKOUT_NOT_CLOSED = 0, 1, 2, 3
+
+
+def _checkout_table_ok(batch: PackedBatch, i: int) -> bool:
+    """pt_batch_exchange's BAD_TABLE rules for log i as a src: the clock checks, every dep actor < n_actors, and record ranges
+    that fit the log."""
+    if not _clock_ok(batch, i):
+        return False
+    ch, dp = _log_changes(batch, i)
+    deps = [q for c in ch for q in dp[int(c["dep_off"]): int(c["dep_off"]) + int(c["n_deps"])]]
+    if any(int(q["actor"]) >= int(batch.desc[i]["n_actors"]) for q in deps):
+        return False
+    return change_record_ranges(batch, i) is not None
+
+
+def _request_clocks(batch: PackedBatch, logs: Sequence[int], n_changes, clock) -> list[dict]:
+    """Per request the clock {actor rank: seq} it names, after pt_batch_checkout's host checks (ValueError)."""
+    if (n_changes is None) == (clock is None):
+        raise ValueError("apply_checkout: exactly one of n_changes and clock must be given")
+    if any(not 0 <= s < batch.n_logs for s in logs):
+        raise ValueError("apply_checkout: a request names no log of the batch")
+    out = []
+    if n_changes is not None:
+        n_changes = [int(x) for x in n_changes]
+        if len(n_changes) != len(logs):
+            raise ValueError("apply_checkout: one n_changes entry per request")
+        for s, m in zip(logs, n_changes):
+            ch, _ = _log_changes(batch, s)
+            req: dict[int, int] = {}
+            for c in ch[:m]:
+                req[int(c["actor"])] = req.get(int(c["actor"]), 0) + 1
+            out.append(req)
+        return out
+    off, ent = np.asarray(clock[0], np.int64), np.asarray(clock[1], CLOCK_DT)
+    if len(off) != len(logs) + 1 or off[0] != 0 or (np.diff(off) < 0).any() or off[-1] > len(ent):
+        raise ValueError("apply_checkout: clock offsets are not non-decreasing from 0 within the clock array")
+    for k, s in enumerate(logs):
+        req = {}
+        for e in ent[int(off[k]): int(off[k + 1])]:
+            a = int(e["actor"])
+            if a >= int(batch.desc[s]["n_actors"]):
+                raise ValueError(f"apply_checkout: request {k}: clock actor {a} >= the log's n_actors")
+            if a in req:
+                raise ValueError(f"apply_checkout: request {k}: actor {a} is named twice")
+            req[a] = int(e["seq"])
+        out.append(req)
+    return out
+
+
+def apply_checkout(batch: PackedBatch, logs: Sequence[int], n_changes=None, clock=None) -> tuple[PackedBatch, np.ndarray]:
+    """The readable host specification of ``pt_batch_checkout``: request k appends a new log holding log ``logs[k]`` at a
+    version, covering the first ``n_changes[k]`` changes of its table (prefix mode) or the changes with seq <= the clock's entry
+    for their actor (clock mode, ``clock`` = (u64 offsets [n + 1], CLOCK_DT entries by actor rank); an absent actor counts as
+    0).  The new log holds the covered changes' ins/del records in table order, then their mark records, a mark's arrival being
+    the covered ins/del records before it; their change records with dep_off rebased, and their deps; the source's id space,
+    ``log_actors``, ``log_counters`` and ``log_lists``.  Returns (``apply_select`` of the batch with the new logs added, the
+    per-request status CHECKOUT_*); a request that is not OK adds a log without records or changes.  NOT_CLOSED is
+    applyChange's dep check (reference src/micromerge.ts:505-509) against the covered changes before each one in table order."""
+    logs = [int(x) for x in logs]
+    if batch.changes is None:
+        raise ValueError("apply_checkout: the batch has no change table")
+    reqs = _request_clocks(batch, logs, n_changes, clock)
+    n = len(logs)
+    status = np.zeros(n, np.uint32)
+    desc, cdesc = np.zeros(n, DESC_DT), np.zeros(n, CDESC_DT)
+    parts = []
+    for k, (s, req) in enumerate(zip(logs, reqs)):
+        ch, dp = _log_changes(batch, s)
+        desc[k]["n_actors"], desc[k]["max_ctr"] = batch.desc[s]["n_actors"], batch.desc[s]["max_ctr"]
+        have: dict[int, int] = {}
+        for c in ch:
+            have[int(c["actor"])] = have.get(int(c["actor"]), 0) + 1
+        covered = [int(c["seq"]) <= req.get(int(c["actor"]), 0) for c in ch]
+        if not _checkout_table_ok(batch, s):
+            status[k] = CHECKOUT_BAD_TABLE
+        elif any(seq > have.get(a, 0) for a, seq in req.items()):
+            status[k] = CHECKOUT_UNKNOWN
+        else:
+            run: dict[int, int] = {}
+            for c, cov in zip(ch, covered):
+                if not cov:
+                    continue
+                if any(run.get(int(q["actor"]), 0) < max(int(q["seq"]), 1) for q in dp[int(c["dep_off"]): int(c["dep_off"]) + int(c["n_deps"])]):
+                    status[k] = CHECKOUT_NOT_CLOSED
+                    break
+                run[int(c["actor"])] = run.get(int(c["actor"]), 0) + 1
+        order = [j for j, cov in enumerate(covered) if cov] if status[k] == CHECKOUT_OK else []
+        rng = change_record_ranges(batch, s) if order else None
+        sins, smk = batch.log_slice(s)
+        ins = np.concatenate([sins[rng[j, 0]: rng[j, 1]] for j in order] + [sins[:0]]).copy()
+        mk = np.concatenate([smk[rng[j, 2]: rng[j, 3]] for j in order] + [smk[:0]]).copy()
+        before = np.cumsum([0] + [rng[j, 1] - rng[j, 0] for j in order])
+        mk["arrival"] = np.concatenate([before[t] + np.clip(smk["arrival"][rng[j, 2]: rng[j, 3]].astype(np.int64) - rng[j, 0], 0, rng[j, 1] - rng[j, 0])
+                                        for t, j in enumerate(order)] + [np.zeros(0, np.int64)])
+        c2 = ch[order].copy()
+        d2 = np.concatenate([dp[int(c["dep_off"]): int(c["dep_off"]) + int(c["n_deps"])] for c in c2] + [dp[:0]]).copy()
+        c2["dep_off"] = _excl_scan(c2["n_deps"]) if len(c2) else c2["dep_off"]
+        desc[k]["n_insdel"], desc[k]["n_mark"] = len(ins), len(mk)
+        cdesc[k]["n_changes"], cdesc[k]["n_deps"] = len(c2), len(d2)
+        parts.append((ins, mk, c2, d2))
+    desc["insdel_off"], desc["mark_off"] = _excl_scan(desc["n_insdel"]), _excl_scan(desc["n_mark"])
+    cdesc["change_off"], cdesc["dep_off"] = _excl_scan(cdesc["n_changes"]), _excl_scan(cdesc["n_deps"])
+    cat = lambda j, dt: np.concatenate([p[j] for p in parts] + [np.zeros(0, dt)])
+    pick = lambda t: [t[s] for s in logs] if t else []
+    added = PackedBatch(desc, cat(0, INSDEL_DT), cat(1, MARK_DT), batch.values, batch.link_attrs, batch.comment_ids, batch.other_attrs, dict(batch.meta),
+                        pick(batch.log_actors), pick(batch.log_counters), ChangeTable(cdesc, cat(2, CHANGE_DT), cat(3, DEP_DT)), pick(batch.log_lists))
+    return apply_select(batch, list(range(batch.n_logs)) + [SELECT_ADDED] * n, added), status
+
+
+def checkout_clocks(batch: PackedBatch, logs: Sequence[int], clocks_by_actor_id: Sequence[dict]) -> tuple[np.ndarray, np.ndarray]:
+    """The clock-mode arrays of ``pt_batch_checkout``: request k's clock {actor id: seq} (``Micromerge.clock``) in log
+    ``logs[k]``'s actor ranks, as (u64 offsets [n + 1], CLOCK_DT entries in rank order).  An id the log does not know is dropped
+    when its seq is 0 and raises ValueError otherwise (the version would hold changes the log cannot name)."""
+    off = np.zeros(len(logs) + 1, np.uint64)
+    rows = []
+    for k, (s, clk) in enumerate(zip(logs, clocks_by_actor_id)):
+        rank = {a: r for r, a in enumerate(batch.log_actors[int(s)])}
+        ent = []
+        for a, seq in clk.items():
+            if a not in rank:
+                if int(seq):
+                    raise ValueError(f"checkout_clocks: request {k}: log {int(s)} does not know actor {a!r}")
+                continue
+            ent.append((rank[a], int(seq)))
+        rows += sorted(ent)
+        off[k + 1] = len(rows)
+    return off, np.array(rows, CLOCK_DT) if rows else np.zeros(0, CLOCK_DT)
+
+
+def clocks(batch: PackedBatch) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The host specification of ``pt_batch_download_clocks``: (u64 offsets [n_logs + 1] = the exclusive scan of n_actors, u32
+    seq, u32 status): log i's number of changes by actor rank a at seq[off[i] + a], and CHECKOUT_BAD_TABLE with zeros where its
+    table fails pt_batch_exchange's clock checks."""
+    n_act = batch.desc["n_actors"].astype(np.uint64)
+    off = np.zeros(batch.n_logs + 1, np.uint64)
+    off[1:] = np.cumsum(n_act)
+    seq = np.zeros(int(off[-1]), np.uint32)
+    status = np.zeros(batch.n_logs, np.uint32)
+    for i in range(batch.n_logs):
+        if not _clock_ok(batch, i):
+            status[i] = CHECKOUT_BAD_TABLE
+            continue
+        ch, _ = _log_changes(batch, i)
+        np.add.at(seq, int(off[i]) + ch["actor"].astype(np.int64), 1)
+    return off, seq, status
+
+
 def elem_refs(batch: PackedBatch, logs: Sequence[int], elem_ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
     """elemIds ``"ctr@actor"`` of the logs ``logs[k]`` -> packed ids for ``pt_batch_find_elements``: (ELEM_REF_DT array,
     bool mask of the ids that can exist in their log).  The actor becomes its rank in ``batch.log_actors[log]``; the counter
