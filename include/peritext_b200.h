@@ -843,6 +843,69 @@ typedef struct pt_elem_pos {
 #define PT_ELEM_LOG_FAILED 4u
 int pt_batch_find_elements(pt_batch*, const pt_elem_ref* refs, uint32_t n, pt_elem_pos* out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Attribution: which change inserted, and which change deleted, every element of a merged log, and what changed since a
+ * version.  Blame ("written by"), highlighting what collaborators changed while one was away (the reference's essay demo does
+ * it for live patches, src/essay-demo.ts:47-75) and showing deleted text in a review view all read it.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_attr_run {   /* 32 B: a maximal run of consecutive elements (element-sequence order, tombstones included) with
+                                  equal (ins_actor, ins_seq, del_actor, del_seq, flags) */
+    uint32_t elem;       /* index of its first element in the element sequence (the reference's metadata index)          */
+    uint32_t visible;    /* visible elements before it (resolveCursor's answer for its first element)                    */
+    uint32_t n;          /* elements in the run; all visible iff del_seq == 0                                            */
+    uint32_t flags;      /* PT_ATTR_INSERTED_SINCE, PT_ATTR_DELETED_SINCE (clock requests only, else 0)                   */
+    uint32_t ins_seq;    /* Change.seq of the change whose op inserted the elements                                      */
+    uint32_t del_seq;    /* 0: not deleted; else Change.seq of the change holding the elements' attributed delete        */
+    uint16_t ins_actor;  /* that change's actor rank in the log                                                          */
+    uint16_t del_actor;  /* the deleting change's actor rank (0 when del_seq == 0)                                       */
+    uint32_t reserved;   /* 0 */
+} pt_attr_run;
+#define PT_ATTR_INSERTED_SINCE 1u   /* the inserting change is not covered by the request's clock                       */
+#define PT_ATTR_DELETED_SINCE 2u    /* deleted now, and no delete of the element is in a covered change                 */
+#define PT_ATTR_OK 0u
+#define PT_ATTR_LOG_FAILED 1u       /* the log's merge status is not PT_LOG_OK (admission-rejected logs included)       */
+#define PT_ATTR_BAD_TABLE 2u        /* the table fails pt_batch_exchange's BAD_TABLE rules for a src (as PT_CHECKOUT_BAD_TABLE) */
+typedef struct pt_attr_view {
+    uint32_t n;
+    const uint32_t* status;         /* [n] PT_ATTR_*; a request that is not OK has no runs                              */
+    const uint64_t* off;            /* [n + 1] request k's runs are runs[off[k] .. off[k+1])                            */
+    const pt_attr_run* runs; uint64_t n_runs;
+} pt_attr_view;
+/* Request k attributes every element of log logs[k] in the element sequence of the last merge:
+ *   insert    the element's insert record lies at list-op position p (pt_batch_set_patch_window's order); its change is the c
+ *             with P_c <= p < P_c + n_ops_c, P_c = the sum of the earlier n_ops.  ins_actor / ins_seq are c's.  In Change terms:
+ *             the change whose actor is the elemId's actor and whose [startOp, startOp + ops.length) holds its counter.
+ *   delete    of the delete records that target the element, the one with the smallest opId in compareOpIds order (packed
+ *             (ctr, actor rank) order, src/micromerge.ts:812-827) is attributed, and its change gives del_actor / del_seq.  The
+ *             first delete by arrival would depend on the replica; the smallest opId makes converged replicas give identical
+ *             runs once actor ranks are mapped to ids.
+ *   clock     (clock_off non-NULL) request k's clock = clock[clock_off[k] .. clock_off[k+1]) (actor ranks of log logs[k]); a
+ *             change is covered iff seq <= clock[actor], an absent actor counting as 0 (pt_batch_checkout's clock mode; no
+ *             closure check).  INSERTED_SINCE: the inserting change is not covered.  DELETED_SINCE: the element is deleted and
+ *             none of its deletes is covered (a concurrent uncovered delete can have a smaller opId than a covered one).  An
+ *             element was visible at the clock's version iff !INSERTED_SINCE && (del_seq == 0 || DELETED_SINCE).
+ *   status    PT_ATTR_LOG_FAILED before PT_ATTR_BAD_TABLE; a request that is not OK has no runs.
+ * Several requests may name one log.  A log without elements has no runs.
+ * Refused with nothing changed:
+ *   PT_ERR_STATE    no batch, no change table, a handle without PT_FLAG_EMIT_SEQUENCE, or no completed merge since the last call
+ *                   that changed the batch (pt_batch_find_elements' rules)
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) null arguments; a log >= n_logs; clock_off not non-decreasing from 0;
+ *                   a clock actor >= the log's n_actors; an actor named twice in one request (pt_batch_checkout's clock rules)
+ * n == 0: PT_OK with an empty view, nothing launched.  Synchronises.  The view is engine-owned pinned memory, valid until the
+ * next pt_batch_attribute, upload or destroy; every other view stays valid.
+ * Device: a resolve kernel, one warp per request (the clocks in shared memory; ptx::count_clock and ptw::marks_before_lane give
+ * each change's first ins/del record; each record finds its change by bisection over those, 32 records per trip; each delete
+ * finds its target through an open-addressing opId table over the log's inserts and takes part in an atomicMin of its opId,
+ * and a second pass lets the winner write its change), then a count pass and a write pass over the element sequence (one warp
+ * per request, 32 words per trip, one function for both), with the runs sized exactly by the exclusive scan of the counts in
+ * between.  Only the requests, the total, the statuses, the offsets and the runs cross PCIe.  Cost per request:
+ * O(n_changes + n_insdel x (log n_changes + probes) + n_elems).  Peak scratch: 28 B per ins/del record (the opId table at half
+ * load is 8 of them) and 8 B per change of every request's log (a log named twice counts twice), plus 32 B per run. */
+int pt_batch_attribute(pt_batch*, const uint32_t* logs, uint32_t n,
+                       const uint64_t* clock_off,     /* [n + 1] or NULL: no clock, flags are 0                           */
+                       const pt_clock_entry* clock,   /* request k's clock = clock[clock_off[k] .. clock_off[k+1])         */
+                       pt_attr_view* out);
+
 /* getTextWithFormatting's return value (FormatSpanWithText[], src/peritext.ts:35-38, 337-455) of every merged log as UTF-8
  * JSON text, rendered on the device.  Log i's text is bytes[off[i] .. off[i+1]):
  *   [{"marks":M,"text":T},...]      one object per span, keys sorted; no visible text gives []

@@ -26,6 +26,19 @@
 
 namespace ptck {
 
+// Step 3's checks of change r (its record: seq, actor | n_deps << 16, dep_off, n_ops) at list-op position x0 of a table that
+// passed count_clock: true if a dep names an actor >= R or its record ranges do not fit log S (marks mk).  *ins_lo = its first
+// ins/del record.
+__device__ __forceinline__ bool change_unfit(uint4 r, uint32_t x0, const pt_dep_rec* __restrict__ d0, uint32_t R, const pt_mark_rec* __restrict__ mk,
+                                             const pt_log_desc& S, uint32_t* ins_lo) {
+    bool bad = false;
+    for (uint32_t d = 0; d < (r.y >> 16); d++) bad |= d0[r.z + d].actor >= R;
+    const uint32_t x1 = x0 + r.w;
+    const uint32_t k0 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x0), k1 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x1);
+    *ins_lo = x0 - k0;
+    return bad || k0 > x0 || k1 > x1 || k1 < k0 || x1 - k1 > S.n_insdel || x1 - k1 < x0 - k0;   // arrivals that do not fit the table
+}
+
 struct CheckoutParams {
     const uint32_t* logs; uint32_t n; uint32_t maxR;
     const uint32_t* n_changes;                                          // [n] prefix mode, or null
@@ -82,10 +95,8 @@ __global__ void checkout_select_kernel(CheckoutParams P) {
             if (c >= n) continue;
             const uint4 r = __ldg(reinterpret_cast<const uint4*>(c0 + c));
             cov[c] = r.x <= B[r.y & 0xFFFFu];
-            for (uint32_t d = 0; d < (r.y >> 16); d++) bad |= d0[r.z + d].actor >= R;
-            const uint32_t x0 = pos[c], x1 = x0 + r.w;
-            const uint32_t k0 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x0), k1 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x1);
-            bad |= k0 > x0 || k1 > x1 || k1 < k0 || x1 - k1 > S.n_insdel || x1 - k1 < x0 - k0;   // arrivals that do not fit the table
+            uint32_t ins_lo;
+            bad |= change_unfit(r, pos[c], d0, R, mk, S, &ins_lo);
         }
         if (__any_sync(0xffffffffu, bad)) status = PT_CHECKOUT_BAD_TABLE;
         else if (unknown) status = PT_CHECKOUT_UNKNOWN;

@@ -30,6 +30,7 @@
 #include "query_kernel.cuh"
 #include "sync_kernel.cuh"
 #include "checkout_kernel.cuh"
+#include "attribute_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -145,6 +146,7 @@ struct pt_batch {
     HostBuf h_syn_totals, h_syn_status, h_syn_off, h_syn_aoff, h_syn_amap;   // the view of the last pt_batch_sync_pairs
     HostBuf h_add_totals, h_add_rank, h_add_aoff, h_add_amap;               // the view of the last pt_batch_add_actors
     HostBuf h_clk_off, h_clk_seq, h_clk_status;                             // the view of the last pt_batch_download_clocks
+    HostBuf h_attr_status, h_attr_off, h_attr_runs;                         // the view of the last pt_batch_attribute
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -1703,12 +1705,9 @@ int pt_batch_select_logs(pt_batch* b, const uint32_t* from, uint32_t n, const pt
     return PT_OK;
 }
 
-// pt_batch_checkout's host checks (include/peritext_b200.h).  Returns the problem, or an empty string.
-static std::string check_checkout(const pt_batch* b, const uint32_t* logs, uint32_t n, const uint32_t* n_changes, const uint64_t* clock_off,
-                                  const pt_clock_entry* clock, const uint32_t* status_out) {
-    if (!logs || !status_out) return "null logs or status_out";
-    if ((n_changes != nullptr) == (clock_off != nullptr)) return "exactly one of n_changes (prefix mode) and clock_off (clock mode) must be given";
-    if ((uint64_t)b->n_logs + n > 0xFFFFFFFFull) return "the batch would have more than 2^32 - 1 logs";
+// The request checks of pt_batch_checkout and pt_batch_attribute: logs inside the batch and, with clock_off, their clocks.
+// Returns the problem, or an empty string.
+static std::string check_clock_requests(const pt_batch* b, const uint32_t* logs, uint32_t n, const uint64_t* clock_off, const pt_clock_entry* clock) {
     if (clock_off && clock_off[0] != 0) return "clock_off[0] is not 0";
     std::vector<uint32_t> seen;                           // seen[a] = k + 1: request k names actor a
     for (uint32_t k = 0; k < n; k++) {
@@ -1727,6 +1726,15 @@ static std::string check_checkout(const pt_batch* b, const uint32_t* logs, uint3
         }
     }
     return std::string();
+}
+
+// pt_batch_checkout's host checks (include/peritext_b200.h).  Returns the problem, or an empty string.
+static std::string check_checkout(const pt_batch* b, const uint32_t* logs, uint32_t n, const uint32_t* n_changes, const uint64_t* clock_off,
+                                  const pt_clock_entry* clock, const uint32_t* status_out) {
+    if (!logs || !status_out) return "null logs or status_out";
+    if ((n_changes != nullptr) == (clock_off != nullptr)) return "exactly one of n_changes (prefix mode) and clock_off (clock mode) must be given";
+    if ((uint64_t)b->n_logs + n > 0xFFFFFFFFull) return "the batch would have more than 2^32 - 1 logs";
+    return check_clock_requests(b, logs, n, clock_off, clock);
 }
 
 int pt_batch_checkout(pt_batch* b, const uint32_t* logs, uint32_t n, const uint32_t* n_changes, const uint64_t* clock_off,
@@ -2169,6 +2177,73 @@ int pt_batch_find_elements(pt_batch* b, const pt_elem_ref* refs, uint32_t n, pt_
         ptq::find_elements_kernel<<<grid, threads, 0, b->stream>>>(dq, n, (const pt_log_desc*)b->d_desc.p, b->dp_insdel, (const pt_log_result*)b->d_results.p,
                                                                   (const uint64_t*)b->d_text_off.p, (const uint32_t*)b->d_seq.p, b->n_logs, da);
     });
+}
+
+int pt_batch_attribute(pt_batch* b, const uint32_t* logs, uint32_t n, const uint64_t* clock_off, const pt_clock_entry* clock, pt_attr_view* out) {
+    const char* fn = "pt_batch_attribute: ";
+    if (!b) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_attribute before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = std::string(fn) + "the handle has no change table"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = std::string(fn) + "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
+    if (!b->merged) { g_last_error = "attribute before merge"; return PT_ERR_STATE; }
+    if (!out || (n && !logs)) { g_last_error = std::string(fn) + "null logs or out"; return PT_ERR_INVALID; }
+    const std::string err = check_clock_requests(b, logs, n, clock_off, clock);
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    int rc;
+    if ((rc = reserve_n<uint32_t>(b->h_attr_status, n)) || (rc = reserve_n<uint64_t>(b->h_attr_off, (uint64_t)n + 1)) ||
+        (rc = reserve_n<pt_attr_run>(b->h_attr_runs, 0))) return rc;
+    uint64_t* hoff = (uint64_t*)b->h_attr_off.p;
+    hoff[0] = 0;
+    if (!n) { *out = pt_attr_view{0, (const uint32_t*)b->h_attr_status.p, hoff, (const pt_attr_run*)b->h_attr_runs.p, 0}; return PT_OK; }
+    std::vector<unsigned long long> chg_slot((size_t)n + 1, 0), rec_slot((size_t)n + 1, 0);
+    for (uint32_t k = 0; k < n; k++) {
+        chg_slot[k + 1] = chg_slot[k] + b->h_cdesc[logs[k]].n_changes;
+        rec_slot[k + 1] = rec_slot[k] + b->h_desc[logs[k]].n_insdel;
+    }
+    const uint64_t nc = chg_slot[n], nr = rec_slot[n];
+    PT_CUDA(cudaSetDevice(b->device));
+    // ---- resolve: each request's table checks, each record's change, each element's attributed delete ----
+    DevBuf dlogs, dcoff, dclk, dcs, drs, dfirst, dcov, dchg, ddchg, ddcov, ddkey, dtab, dst, dcnt, dbsum, doff, druns;   // freed on return
+    if ((rc = upload_n(b, dlogs, logs, n)) || (rc = upload_n(b, dcs, chg_slot.data(), (uint64_t)n + 1)) ||
+        (rc = upload_n(b, drs, rec_slot.data(), (uint64_t)n + 1)) || (rc = reserve_n<uint32_t>(dfirst, nc)) || (rc = reserve_n<uint32_t>(dcov, nc)) ||
+        (rc = reserve_n<uint32_t>(dchg, nr)) || (rc = reserve_n<uint32_t>(ddchg, nr)) || (rc = reserve_n<uint32_t>(ddcov, nr)) ||
+        (rc = reserve_n<unsigned long long>(ddkey, nr)) || (rc = reserve_n<uint32_t>(dtab, 2 * nr)) || (rc = reserve_n<uint32_t>(dst, n)) ||
+        (rc = reserve_n<unsigned long long>(dcnt, n)) || (rc = reserve_n<unsigned long long>(doff, (uint64_t)n + 1))) return rc;
+    if (clock_off && ((rc = upload_n(b, dcoff, clock_off, (uint64_t)n + 1)) || (rc = upload_n(b, dclk, clock, clock_off[n])))) return rc;
+    pta::AttrParams P{};
+    P.logs = (const uint32_t*)dlogs.p; P.n = n; P.maxR = b->adm_maxR;
+    P.clock_off = clock_off ? (const unsigned long long*)dcoff.p : nullptr; P.clock = clock_off ? (const pt_clock_entry*)dclk.p : nullptr;
+    P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
+    P.insdel = b->dp_insdel; P.marks = b->dp_marks;
+    P.res = (const pt_log_result*)b->d_results.p; P.seq_off = (const uint64_t*)b->d_text_off.p; P.seq = (const uint32_t*)b->d_seq.p;
+    P.chg_slot = (const unsigned long long*)dcs.p; P.rec_slot = (const unsigned long long*)drs.p;
+    P.first = (uint32_t*)dfirst.p; P.cov = (uint32_t*)dcov.p;
+    P.chg = (uint32_t*)dchg.p; P.dchg = (uint32_t*)ddchg.p; P.dcov = (uint32_t*)ddcov.p; P.dkey = (unsigned long long*)ddkey.p; P.table = (uint32_t*)dtab.p;
+    P.status = (uint32_t*)dst.p; P.count = (unsigned long long*)dcnt.p; P.off = (const unsigned long long*)doff.p;
+    const auto [wpb, smem] = actor_shape(b->adm_maxR);
+    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(pta::attribute_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    pta::attribute_resolve_kernel<<<warp_grid(b, n, wpb * 32), wpb * 32, smem, b->stream>>>(P);
+    PT_CUDA(launched(b));
+    // ---- count, scan, one total back, write ----
+    const uint32_t threads = 128, grid = warp_grid(b, n, threads);
+    pta::attribute_runs_kernel<false><<<grid, threads, 0, b->stream>>>(P);
+    PT_CUDA(launched(b));
+    if ((rc = scan_offsets(b, pts::PlainCounts{P.count}, n, dbsum, (unsigned long long*)doff.p, nullptr))) return rc;
+    PT_CUDA(cudaMemcpyAsync(hoff, doff.p, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(b->h_attr_status.p, dst.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    const uint64_t total = hoff[n];
+    if ((rc = reserve_n<pt_attr_run>(druns, total)) || (rc = reserve_n<pt_attr_run>(b->h_attr_runs, total))) return rc;
+    if (total) {
+        P.runs = (pt_attr_run*)druns.p;
+        pta::attribute_runs_kernel<true><<<grid, threads, 0, b->stream>>>(P);
+        PT_CUDA(launched(b));
+        PT_CUDA(cudaMemcpyAsync(b->h_attr_runs.p, druns.p, total * sizeof(pt_attr_run), cudaMemcpyDeviceToHost, b->stream));
+        PT_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    *out = pt_attr_view{n, (const uint32_t*)b->h_attr_status.p, hoff, (const pt_attr_run*)b->h_attr_runs.p, total};
+    return PT_OK;
 }
 
 // JSON render of the spans (render_kernel.cuh).

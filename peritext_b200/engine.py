@@ -62,6 +62,7 @@ _ENTRY_POINTS = {
     "pt_batch_set_patch_window": ([_vp, _vp, _u32], _int),
     "pt_batch_query_elements": ([_vp, _vp, _u32, _vp], _int),
     "pt_batch_find_elements": ([_vp, _vp, _u32, _vp], _int),
+    "pt_batch_attribute": ([_vp, _vp, _u32, _vp, _vp, _vp], _int),
     "pt_batch_render_json": ([_vp, _vp, _vp], _int),
     "pt_batch_render_patches_json": ([_vp, _vp, _vp], _int),
     "pt_batch_render_changes_json": ([_vp, _vp, _vp], _int),
@@ -738,6 +739,23 @@ class BatchEngine:
         out = np.zeros(len(q), ELEM_POS_DT)
         _check(self._L.pt_batch_find_elements(self._h, _ptr(q), len(q), _ptr(out)), "pt_batch_find_elements")
         return out
+
+    def attribute(self, logs, clock=None):
+        """Attribute every element of the resident logs ``logs[k]`` to the changes that inserted and deleted it, on the device
+        (pt_batch_attribute), after a merge with ``emit_sequence``: (u32 status [n], u64 offsets [n + 1], ATTR_RUN_DT runs),
+        request k's runs at runs[off[k]:off[k + 1]].  ``clock`` (u64 offsets [n + 1], CLOCK_DT entries by actor rank;
+        ``packing.checkout_clocks``) also flags what was inserted or deleted since that version.  ``attribution.attribution_runs``
+        is its host specification.  Needs a change table."""
+        from .attribution import ATTR_RUN_DT, _AttrView
+        lg = np.ascontiguousarray(logs, np.uint32)
+        off = ent = None
+        if clock is not None:
+            off, ent = np.ascontiguousarray(clock[0], np.uint64), np.ascontiguousarray(clock[1], CLOCK_DT)
+        v = _AttrView()
+        _check(self._L.pt_batch_attribute(self._h, _ptr(lg), len(lg), None if off is None else off.ctypes.data, _ptr(ent), ctypes.byref(v)),
+               "pt_batch_attribute")
+        o = _view(v.off, len(lg) + 1, np.uint64) if len(lg) else np.zeros(1, np.uint64)
+        return _view(v.status, len(lg), np.uint32), o, _view(v.runs, v.n_runs, ATTR_RUN_DT)
 
     def resolve_cursors(self, batch: PackedBatch, logs, elem_ids) -> np.ndarray:
         """resolveCursor (reference src/micromerge.ts:475-477) for many documents in one device pass: the number of visible
