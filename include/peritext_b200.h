@@ -761,7 +761,7 @@ int pt_batch_checkout(pt_batch*, const uint32_t* logs, uint32_t n,
  * entries are 0.  This names the version a log holds now, also after pt_batch_change, pt_batch_exchange or
  * pt_batch_sync_pairs, so that it can be checked out later.  No batch or no change table: PT_ERR_STATE; null arguments:
  * PT_ERR_INVALID.  Synchronises.  The view is engine-owned pinned memory, valid until the next call of it, upload or
- * destroy.  Device: one warp per log counting its table (ptx::count_clock) into the output. */
+ * destroy.  Device: one warp per log counting its table (ptct::count_clock) into the output. */
 int pt_batch_download_clocks(pt_batch*, const uint64_t** off, const uint32_t** seq, const uint32_t** status);
 
 /* The handle's per-log descriptors ([n_logs]; offsets into the engine's records): the shape of the resident batch after calls
@@ -893,7 +893,7 @@ typedef struct pt_attr_view {
  *                   a clock actor >= the log's n_actors; an actor named twice in one request (pt_batch_checkout's clock rules)
  * n == 0: PT_OK with an empty view, nothing launched.  Synchronises.  The view is engine-owned pinned memory, valid until the
  * next pt_batch_attribute, upload or destroy; every other view stays valid.
- * Device: a resolve kernel, one warp per request (the clocks in shared memory; ptx::count_clock and ptw::marks_before_lane give
+ * Device: a resolve kernel, one warp per request (the clocks in shared memory; ptct::count_clock and ptw::marks_before_lane give
  * each change's first ins/del record; each record finds its change by bisection over those, 32 records per trip; each delete
  * finds its target through an open-addressing opId table over the log's inserts and takes part in an atomicMin of its opId,
  * and a second pass lets the winner write its change), then a count pass and a write pass over the element sequence (one warp

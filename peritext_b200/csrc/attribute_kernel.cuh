@@ -4,10 +4,10 @@
 // attribute_resolve_kernel: one warp per request, grid-stride.  Per-warp shared memory holds two words per actor of the log
 // (actor_shape's budget), A and B.  Each request has its own scratch slot: per change first and cov, per ins/del record chg,
 // dkey, dcov and dchg, and an opId table of 2 slots per ins/del record.
-//   1. A = the log's clock: ptx::count_clock over its table, writing each change's list-op position into first; a table that
-//      fails it, whose n_ops do not sum to the log's records, or that fails ptck::change_unfit is BAD_TABLE.  first[c] becomes
-//      change c's first ins/del record (ptw::marks_before_lane) and cov[c] = seq_c <= B[actor_c], B being the request clock
-//      (no clock: every change is covered).
+//   1. A = the log's clock: ptct::source_clock, writing each change's list-op position into first; a table that fails it, has
+//      a dep actor >= n_actors or a change whose records do not fit (ptct::change_records) is BAD_TABLE (DESIGN.md §4.3's
+//      change-table rules, as for pt_batch_checkout).  first[c] becomes change c's first ins/del record and
+//      cov[c] = seq_c <= B[actor_c], B being the request clock (no clock: every change is covered).
 //   2. records, 32 per trip: chg[r] = the last change whose first record is <= r (bisection over first); inserts go into the
 //      opId table, open addressing keyed by (ctr, actor), holding the record index (the key is read back from the record).
 //   3. deletes: the target's insert record through the table, then atomicMin of the delete's packed opId (ctr << 16 | actor,
@@ -23,7 +23,7 @@
 #include <cstdint>
 
 #include "../../include/peritext_b200.h"
-#include "checkout_kernel.cuh"
+#include "change_table.cuh"
 
 namespace pta {
 
@@ -82,25 +82,20 @@ __global__ void attribute_resolve_kernel(AttrParams P) {
         } else {
             for (uint32_t a = lane; a < R; a += 32) { A[a] = 0; B[a] = 0; }
             __syncwarp();
-            unsigned long long ops = 0;
-            if (!ptx::count_clock(c0, n, C.n_deps, R, A, first, &ops, lane) || ops != (unsigned long long)nI + S.n_mark || ops > 0xFFFFFFFFull)
-                status = PT_ATTR_BAD_TABLE;
-            if (status == PT_ATTR_OK && P.clock) {
-                for (unsigned long long e = P.clock_off[k] + lane; e < P.clock_off[k + 1]; e += 32) {   // actors < R and distinct (host)
-                    const pt_clock_entry q = P.clock[e];
-                    B[q.actor] = q.seq;
-                }
-            }
+            if (!ptct::source_clock(c0, C, S, A, first, lane)) status = PT_ATTR_BAD_TABLE;
+            if (status == PT_ATTR_OK && P.clock) ptct::load_clock(B, P.clock, P.clock_off[k], P.clock_off[k + 1], lane);
             __syncwarp();
+            const pt_dep_rec* d0 = P.deps + C.dep_off;
             bool bad = false;
             for (uint32_t base = 0; status == PT_ATTR_OK && base < n; base += 32) {
                 const uint32_t c = base + lane;
                 if (c >= n) continue;
                 const uint4 r = __ldg(reinterpret_cast<const uint4*>(c0 + c));
                 cov[c] = !P.clock || r.x <= B[r.y & 0xFFFFu];
-                uint32_t lo;
-                bad |= ptck::change_unfit(r, first[c], P.deps + C.dep_off, R, P.marks + S.mark_off, S, &lo);
-                first[c] = lo;
+                for (uint32_t d = 0; d < (r.y >> 16); d++) bad |= d0[r.z + d].actor >= R;
+                const ptct::Records x = ptct::change_records(P.marks + S.mark_off, S, first[c], r.w);
+                bad |= !x.fits;
+                first[c] = x.ins_lo;
             }
             if (__any_sync(0xffffffffu, bad)) status = PT_ATTR_BAD_TABLE;
             __syncwarp();

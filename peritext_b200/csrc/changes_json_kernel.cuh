@@ -3,11 +3,10 @@
 // (include/peritext_b200.h has the contract, DESIGN.md §4.8d the design).
 //
 // changes_select_kernel: one warp per request.  Every request first takes the list-op position of each change of its log's table
-// (running sum of n_ops, as pt_batch_exchange's clock pass does) and checks that they sum to the log's records.  RANGE selects a
-// clipped range of the table.  MISSING counts the log's clock with ptx::count_clock (seq-contiguous per actor, else
-// PT_CHANGES_BAD_TABLE), loads the peer's clock into shared memory by rank and builds the queue in getMissingChanges order the
-// with exchange_select_kernel's step 2 (ptx::missing_queue, one copy of the rule): one pass in table order gives every actor the
-// slot of its first missing change, and change (actor, seq) goes to slot[actor] + seq - clock - 1.  The selected changes are cut into WORK ITEMS of at most kSlice list
+// (ptct::count_clock without a clock: the positions and the dep-range check) and checks that they sum to the log's records.
+// RANGE selects a clipped range of the table.  MISSING counts the log's clock with ptct::count_clock (seq-contiguous per actor,
+// else PT_CHANGES_BAD_TABLE), loads the peer's clock into shared memory by rank and builds the queue in getMissingChanges order
+// with ptct::missing_queue (DESIGN.md §4.3's change-table rules).  The selected changes are cut into WORK ITEMS of at most kSlice list
 // ops each, so one c5-sized change is not left to a single warp; an OK request without changes gets one item, which writes "[]".
 //
 // changes_json_size_kernel / changes_json_write_kernel: one warp per item, both through render_item<W>.  Slice 0 of a change
@@ -23,7 +22,7 @@
 #include "../../include/peritext_b200.h"
 #include "render_kernel.cuh"
 #include "patch_json_kernel.cuh"
-#include "exchange_kernel.cuh"
+#include "change_table.cuh"
 #include "patch_window.cuh"
 
 namespace ptcj {
@@ -211,30 +210,6 @@ __device__ __forceinline__ uint32_t extras_upto(const pt_change_extra* x, uint32
     return lo;
 }
 
-// List-op positions: pos[k] = sum of n_ops over changes [0, k); returns the sum over the table.  *deps_ok = every change's deps
-// lie inside the log's n_deps dep records (the header reads them in every mode; count_clock checks the same for MISSING).
-// Warp-collective.
-__device__ __forceinline__ unsigned long long list_positions(const pt_change_rec* __restrict__ c0, uint32_t n, uint32_t n_deps, uint32_t* __restrict__ pos,
-                                                             bool* deps_ok, uint32_t lane) {
-    unsigned long long run = 0;
-    bool bad = false;
-    for (uint32_t base = 0; base < n; base += 32) {
-        const uint32_t k = base + lane;
-        uint4 r = make_uint4(0, 0, 0, 0);
-        if (k < n) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
-        const uint32_t w = r.w;
-        bad |= (unsigned long long)r.z + (r.y >> 16) > n_deps;
-        uint32_t tot;
-        const uint32_t ex = ptx::warp_excl_scan(w, lane, tot);   // a trip's sum can wrap only in a table the total check refuses
-        unsigned long long wide = w;
-        for (int o = 16; o > 0; o >>= 1) wide += __shfl_xor_sync(kFull, wide, o);
-        if (k < n) pos[k] = (uint32_t)run + ex;
-        run += wide;
-    }
-    *deps_ok = !__any_sync(kFull, bad);
-    return run;
-}
-
 __global__ void changes_select_kernel(ChangesParams C) {
     extern __shared__ uint32_t cj_smem[];
     const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
@@ -247,8 +222,8 @@ __global__ void changes_select_kernel(ChangesParams C) {
         const pt_change_rec* c0 = C.changes + CD.change_off;
         uint32_t* pos = C.pos + C.slot_off[r];
         Sel* sel = C.sel + C.slot_off[r];
-        bool deps_ok;
-        const unsigned long long ops = list_positions(c0, CD.n_changes, CD.n_deps, pos, &deps_ok, lane);
+        unsigned long long ops = 0;   // the header reads a change's deps in every mode
+        const bool deps_ok = ptct::count_clock(c0, CD.n_changes, CD.n_deps, 0u, nullptr, pos, &ops, lane);
         uint32_t status = deps_ok && ops == (unsigned long long)L.n_insdel + L.n_mark ? PT_CHANGES_OK : PT_CHANGES_BAD_TABLE;
         uint32_t ns = 0;
         if (status == PT_CHANGES_OK && q.mode == PT_CHANGES_RANGE) {
@@ -261,11 +236,11 @@ __global__ void changes_select_kernel(ChangesParams C) {
             __syncwarp();
             for (uint32_t k = lane; k < q.n_clock; k += 32) { const pt_clock_entry e = C.clock[q.clock_off + k]; atomicMax(&clk[e.actor], e.seq); }
             __syncwarp();
-            if (!ptx::count_clock(c0, CD.n_changes, CD.n_deps, R, cs, nullptr, nullptr, lane)) {
+            if (!ptct::count_clock(c0, CD.n_changes, CD.n_deps, R, cs, nullptr, nullptr, lane)) {
                 status = PT_CHANGES_BAD_TABLE;
             } else {
-                ns = ptx::missing_queue(c0, CD.n_changes, cs, [&](uint32_t actor) { return clk[actor]; },
-                                        [&](uint32_t k, uint4, uint32_t slot) { sel[slot].change = k; }, lane);
+                ns = ptct::missing_queue(c0, CD.n_changes, cs, [&](uint32_t actor) { return clk[actor]; },
+                                         [&](uint32_t k, uint4, uint32_t slot) { sel[slot].change = k; }, lane);
             }
         }
         if (status != PT_CHANGES_OK) ns = 0;
@@ -285,7 +260,7 @@ __global__ void changes_select_kernel(ChangesParams C) {
                 else if (x1 > x0 && C.extras[x0].op != PT_EXTRA_NONE && C.extras[x1 - 1].pos >= (unsigned long long)n_ops + (x1 - x0)) atomicMin(&C.bad[1], key);
             }
             uint32_t tot;
-            const uint32_t ex = ptx::warp_excl_scan(it, lane, tot);
+            const uint32_t ex = ptct::warp_excl_scan(it, lane, tot);
             if (valid) sel[k] = Sel{c, pos[c], (uint32_t)nitems + ex, 0u};
             nitems += tot;
         }

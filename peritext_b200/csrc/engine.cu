@@ -208,6 +208,16 @@ std::pair<uint32_t, size_t> actor_shape(uint32_t maxR) {
     return {wpb, per_warp * wpb};
 }
 
+// One warp per item over n_items items of a kernel with those tables, on the batch's stream: the launch's error, else PT_OK.
+template <class... Params, class... Args>
+int launch_actor_kernel(pt_batch* b, void (*kernel)(Params...), uint64_t n_items, Args... args) {
+    const auto [wpb, smem] = actor_shape(b->adm_maxR);
+    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<warp_grid(b, n_items, wpb * 32), wpb * 32, smem, b->stream>>>(args...);
+    PT_CUDA(launched(b));
+    return PT_OK;
+}
+
 // The scan triple over n per-log counts of src (scan_kernel.cuh): block sums into bsum, their scan, then each log's
 // exclusive offset in off0 (channel a) and off1 (channel c; may be null), the totals at [n].
 template <class Src>
@@ -1139,8 +1149,59 @@ static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pa
 // The pinned buffers of an exchange view for np pairs.
 static int reserve_exchange_view(pt_batch* b, uint32_t np) {
     int rc;
-    if ((rc = reserve_n<ptx::PairTotals>(b->h_xch_totals, np)) || (rc = reserve_n<uint32_t>(b->h_xch_status, np)) ||
+    if ((rc = reserve_n<ptct::PairTotals>(b->h_xch_totals, np)) || (rc = reserve_n<uint32_t>(b->h_xch_status, np)) ||
         (rc = reserve_n<uint64_t>(b->h_xch_off, (uint64_t)np + 1)) || (rc = reserve_n<pt_log_desc>(b->h_xch_desc, b->n_logs))) return rc;
+    return PT_OK;
+}
+
+// The exchange view of no pairs, in the reserved buffers: every log's delta empty, with its n_actors and max_ctr.
+static int empty_exchange_view(pt_batch* b, pt_exchange_view* out) {
+    int rc;
+    if ((rc = b->h_xch_delivered.reserve(4))) return rc;
+    pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
+    for (uint32_t i = 0; i < b->n_logs; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
+    ((uint64_t*)b->h_xch_off.p)[0] = 0;
+    *out = pt_exchange_view{0, (const uint32_t*)b->h_xch_status.p, (const uint64_t*)b->h_xch_off.p, (const uint32_t*)b->h_xch_delivered.p, dd};
+    return PT_OK;
+}
+
+// The changes a select kernel (exchange_select_kernel, checkout_select_kernel) delivered, as one delta: the pairs' records,
+// change records and deps back to back in pair order.
+struct Delta {
+    std::vector<ptct::PairBase> base;          // [np] where pair p's start
+    std::vector<unsigned long long> dlv_off;   // [np + 1] exclusive scan of the pairs' delivered changes
+    uint64_t n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0;
+    DevBuf insdel, marks, changes, deps, d_dlv_off, d_base;
+};
+
+// Lays out the delta of the pairs' totals tot (host; a pair that is not OK has zero counts) and gathers it with
+// exchange_gather_kernel: P holds the pairs and their maps, the select's scratch and totals (device), and the pairs' dsts index
+// dst_desc.  delivered (may be null) gets each delivered change's index in its src's table.
+static int gather_delta(pt_batch* b, ptx::ExchangeParams& P, const ptct::PairTotals* tot, const pt_log_desc* dst_desc, DevBuf* delivered, Delta& D) {
+    const uint32_t np = P.n_pairs;
+    D.base.resize(np);
+    D.dlv_off.assign((size_t)np + 1, 0);
+    uint64_t most = 0;                         // the largest pair's records: an upper bound of its longest change
+    for (uint32_t p = 0; p < np; p++) {
+        D.base[p] = ptct::PairBase{D.n_ins, D.n_mk, D.n_ch, D.n_dp};
+        D.n_ins += tot[p].n_insdel; D.n_mk += tot[p].n_mark; D.n_ch += tot[p].n_changes; D.n_dp += tot[p].n_deps;
+        D.dlv_off[p + 1] = D.n_ch;
+        most = std::max<uint64_t>(most, (uint64_t)tot[p].n_insdel + 2ull * tot[p].n_mark);
+    }
+    int rc;
+    if ((rc = reserve_n<pt_insdel_rec>(D.insdel, D.n_ins)) || (rc = reserve_n<pt_mark_rec>(D.marks, D.n_mk)) ||
+        (rc = reserve_n<pt_change_rec>(D.changes, D.n_ch)) || (rc = reserve_n<pt_dep_rec>(D.deps, D.n_dp)) ||
+        (delivered && (rc = reserve_n<uint32_t>(*delivered, D.n_ch)))) return rc;
+    if (!D.n_ch) return PT_OK;
+    if ((rc = upload_n(b, D.d_dlv_off, D.dlv_off.data(), (uint64_t)np + 1)) || (rc = upload_n(b, D.d_base, D.base.data(), np))) return rc;
+    P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
+    P.insdel = b->dp_insdel; P.marks = b->dp_marks;
+    P.dlv_off = (const unsigned long long*)D.d_dlv_off.p; P.n_dlv = D.n_ch; P.base = (const ptct::PairBase*)D.d_base.p; P.dst_desc = dst_desc;
+    P.out_insdel = (pt_insdel_rec*)D.insdel.p; P.out_marks = (pt_mark_rec*)D.marks.p; P.out_changes = (pt_change_rec*)D.changes.p; P.out_deps = (pt_dep_rec*)D.deps.p;
+    P.out_delivered = delivered ? (uint32_t*)delivered->p : nullptr;
+    ptx::exchange_gather_kernel<<<slice_grid(b, D.n_ch, most, 128), 128, 0, b->stream>>>(P);   // one warp per delivered change
+    PT_CUDA(launched(b));
     return PT_OK;
 }
 
@@ -1148,20 +1209,13 @@ int pt_batch_exchange(pt_batch* b, const pt_exchange_input* in, pt_exchange_view
     if (!b || !in || !out) { g_last_error = "pt_batch_exchange: null argument"; return PT_ERR_INVALID; }
     if (!b->have_batch) { g_last_error = "pt_batch_exchange before pt_batch_upload"; return PT_ERR_STATE; }
     if (!b->have_changes) { g_last_error = "pt_batch_exchange: the handle has no change table"; return PT_ERR_STATE; }
-    const uint32_t n = b->n_logs, np = in->n_pairs;
+    const uint32_t np = in->n_pairs;
     int rc;
     if ((rc = reserve_exchange_view(b, np))) return rc;
-    uint32_t* status = (uint32_t*)b->h_xch_status.p;
-    uint64_t* doff = (uint64_t*)b->h_xch_off.p;
-    pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
     if (!np) {
         PT_CUDA(cudaSetDevice(b->device));
         PT_CUDA(cudaStreamSynchronize(b->stream));          // the pinned view buffers may still be the target of an earlier copy
-        if ((rc = b->h_xch_delivered.reserve(4))) return rc;
-        for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
-        doff[0] = 0;
-        *out = pt_exchange_view{0, status, doff, (const uint32_t*)b->h_xch_delivered.p, dd};
-        return PT_OK;
+        return empty_exchange_view(b, out);
     }
     std::vector<unsigned long long> slot_off;
     std::string err = check_exchange(b, *in, slot_off);
@@ -1183,16 +1237,16 @@ static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pa
                          pt_exchange_view* out) {
     const uint32_t n = b->n_logs;
     int rc;
-    ptx::PairTotals* tot = (ptx::PairTotals*)b->h_xch_totals.p;
+    ptct::PairTotals* tot = (ptct::PairTotals*)b->h_xch_totals.p;
     uint32_t* status = (uint32_t*)b->h_xch_status.p;
     uint64_t* doff = (uint64_t*)b->h_xch_off.p;
     pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
     const uint64_t n_slot = slot_off[np];
     // the pairs and the select kernel's scratch: freed on return
-    DevBuf dpairs, dslot, dqueue, dpos, ddlv, dtot, ddoff, dbase, dgi, dgm, dgc, dgd, dgx;
+    DevBuf dpairs, dslot, dqueue, dpos, ddlv, dtot, dgx;
     if ((rc = upload_n(b, dpairs, pairs, np)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)np + 1)) ||
         (rc = reserve_n<uint32_t>(dqueue, n_slot)) || (rc = reserve_n<uint32_t>(dpos, n_slot)) ||
-        (rc = reserve_n<ptx::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptx::PairTotals>(dtot, np))) return rc;
+        (rc = reserve_n<ptct::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptct::PairTotals>(dtot, np))) return rc;
     ptx::ExchangeParams P{};
     P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = np; P.maxR = b->adm_maxR;
     P.actor_off = actor_off; P.actor_map = actor_map;
@@ -1200,38 +1254,17 @@ static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pa
     P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
     P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
     P.insdel = b->dp_insdel; P.marks = b->dp_marks;
-    P.slot_off = (const unsigned long long*)dslot.p; P.queue = (uint32_t*)dqueue.p; P.pos = (uint32_t*)dpos.p; P.dlv = (ptx::Delivered*)ddlv.p;
-    P.totals = (ptx::PairTotals*)dtot.p;
-    const auto [wpb, smem] = actor_shape(b->adm_maxR);
-    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptx::exchange_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ptx::exchange_select_kernel<<<warp_grid(b, np, wpb * 32), wpb * 32, smem, b->stream>>>(P);
-    PT_CUDA(launched(b));
-    PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));
+    P.slot_off = (const unsigned long long*)dslot.p; P.queue = (uint32_t*)dqueue.p; P.pos = (uint32_t*)dpos.p; P.dlv = (ptct::Delivered*)ddlv.p;
+    P.totals = (ptct::PairTotals*)dtot.p;
+    if ((rc = launch_actor_kernel(b, ptx::exchange_select_kernel, np, P))) return rc;
+    PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptct::PairTotals), cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
-    // the delta's layout: the pairs' records, change and dep records back to back in pair order
-    std::vector<ptx::PairBase> base(np);
-    std::vector<unsigned long long> dlv_off((size_t)np + 1, 0);
-    uint64_t n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0, most = 0;
-    for (uint32_t p = 0; p < np; p++) {
-        base[p] = ptx::PairBase{n_ins, n_mk, n_ch, n_dp};
-        n_ins += tot[p].n_insdel; n_mk += tot[p].n_mark; n_ch += tot[p].n_changes; n_dp += tot[p].n_deps;
-        dlv_off[p + 1] = n_ch;
-        most = std::max<uint64_t>(most, (uint64_t)tot[p].n_insdel + 2ull * tot[p].n_mark);
-    }
-    if ((rc = reserve_n<pt_insdel_rec>(dgi, n_ins)) || (rc = reserve_n<pt_mark_rec>(dgm, n_mk)) ||
-        (rc = reserve_n<pt_change_rec>(dgc, n_ch)) || (rc = reserve_n<pt_dep_rec>(dgd, n_dp)) ||
-        (rc = reserve_n<uint32_t>(dgx, n_ch)) || (rc = reserve_n<uint32_t>(b->h_xch_delivered, n_ch))) return rc;
+    Delta D;
+    if ((rc = gather_delta(b, P, tot, P.desc, &dgx, D)) || (rc = reserve_n<uint32_t>(b->h_xch_delivered, D.n_ch))) return rc;
     uint32_t* delivered = (uint32_t*)b->h_xch_delivered.p;
-    if (n_ch) {
-        if ((rc = upload_n(b, ddoff, dlv_off.data(), (uint64_t)np + 1)) || (rc = upload_n(b, dbase, base.data(), np))) return rc;
-        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p; P.dst_desc = P.desc;
-        P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
-        P.out_delivered = (uint32_t*)dgx.p;
-        // one warp per delivered change; a pair's records are an upper bound of its longest change
-        ptx::exchange_gather_kernel<<<slice_grid(b, n_ch, most, 128), 128, 0, b->stream>>>(P);
-        PT_CUDA(launched(b));
-        PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));   // status and max_ctr
-        PT_CUDA(cudaMemcpyAsync(delivered, dgx.p, n_ch * 4, cudaMemcpyDeviceToHost, b->stream));
+    if (D.n_ch) {
+        PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)np * sizeof(ptct::PairTotals), cudaMemcpyDeviceToHost, b->stream));   // status and max_ctr
+        PT_CUDA(cudaMemcpyAsync(delivered, dgx.p, D.n_ch * 4, cudaMemcpyDeviceToHost, b->stream));
         PT_CUDA(cudaStreamSynchronize(b->stream));
     }
     // the delta per log; a pair that found an id without an image delivers nothing: its records are never spliced
@@ -1242,14 +1275,14 @@ static int exchange_core(pt_batch* b, const char* fn, const pt_exchange_pair* pa
         status[p] = tot[p].status;
         const uint32_t dst = pairs[p].dst, cnt = status[p] == PT_EXCHANGE_OK ? tot[p].n_changes : 0u;
         if (cnt) {
-            dd[dst] = pt_log_desc{base[p].insdel, base[p].mark, tot[p].n_insdel, tot[p].n_mark, b->h_desc[dst].n_actors, std::max(b->h_desc[dst].max_ctr, tot[p].max_ctr)};
-            cdesc[dst] = pt_change_desc{base[p].change, base[p].dep, tot[p].n_changes, tot[p].n_deps};
-            if (doff[p] != dlv_off[p]) memmove(delivered + doff[p], delivered + dlv_off[p], (size_t)cnt * 4);
+            dd[dst] = pt_log_desc{D.base[p].insdel, D.base[p].mark, tot[p].n_insdel, tot[p].n_mark, b->h_desc[dst].n_actors, std::max(b->h_desc[dst].max_ctr, tot[p].max_ctr)};
+            cdesc[dst] = pt_change_desc{D.base[p].change, D.base[p].dep, tot[p].n_changes, tot[p].n_deps};
+            if (doff[p] != D.dlv_off[p]) memmove(delivered + doff[p], delivered + D.dlv_off[p], (size_t)cnt * 4);
         }
         doff[p + 1] = doff[p] + cnt;
     }
-    const pt_packed_ops delta{n, dd, (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
-    const pt_change_table ct{n, cdesc.data(), (const pt_change_rec*)dgc.p, n_ch, (const pt_dep_rec*)dgd.p, n_dp};
+    const pt_packed_ops delta{n, dd, (const pt_insdel_rec*)D.insdel.p, D.n_ins, (const pt_mark_rec*)D.marks.p, D.n_mk};
+    const pt_change_table ct{n, cdesc.data(), (const pt_change_rec*)D.changes.p, D.n_ch, (const pt_dep_rec*)D.deps.p, D.n_dp};
     if ((rc = splice_append(b, fn, &delta, true, pt_append_remap{}, &ct, true))) return rc;
     *out = pt_exchange_view{np, status, doff, delivered, dd};
     return PT_OK;
@@ -1442,10 +1475,7 @@ int pt_batch_sync_pairs(pt_batch* b, const pt_exchange_pair* pairs, uint32_t np,
         D.changes = (const pt_change_rec*)b->d_changes.p; D.deps = (const pt_dep_rec*)b->d_deps.p; D.insdel = b->dp_insdel; D.marks = b->dp_marks;
         D.slot_off = (const unsigned long long*)dslot.p; D.pos = (uint32_t*)dpos.p;
         D.new_off = (const unsigned long long*)dnoff.p; D.new_id = (unsigned long long*)dnew.p; D.totals = (pty::SyncTotals*)dtot.p;
-        const auto [wpb, smem] = actor_shape(b->adm_maxR);
-        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(pty::sync_derive_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        pty::sync_derive_kernel<<<warp_grid(b, nl, wpb * 32), wpb * 32, smem, b->stream>>>(D);
-        PT_CUDA(launched(b));
+        if ((rc = launch_actor_kernel(b, pty::sync_derive_kernel, nl, D))) return rc;
         PT_CUDA(cudaMemcpyAsync(tot, dtot.p, (size_t)nl * sizeof(pty::SyncTotals), cudaMemcpyDeviceToHost, b->stream));
         PT_CUDA(cudaStreamSynchronize(b->stream));
     }
@@ -1477,13 +1507,7 @@ int pt_batch_sync_pairs(pt_batch* b, const pt_exchange_pair* pairs, uint32_t np,
                                                                             (const unsigned long long*)dxaoff.p, (uint16_t*)dxmap.p);
         PT_CUDA(launched(b));
         if ((rc = exchange_core(b, fn, xp.data(), nx, xslot, (const unsigned long long*)dxaoff.p, (const uint16_t*)dxmap.p, nullptr, nullptr, &xv))) return rc;
-    } else {
-        if ((rc = b->h_xch_delivered.reserve(4))) return rc;
-        pt_log_desc* dd = (pt_log_desc*)b->h_xch_desc.p;
-        for (uint32_t i = 0; i < n; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
-        ((uint64_t*)b->h_xch_off.p)[0] = 0;
-        xv = pt_exchange_view{0, (const uint32_t*)b->h_xch_status.p, (const uint64_t*)b->h_xch_off.p, (const uint32_t*)b->h_xch_delivered.p, dd};
-    }
+    } else if ((rc = empty_exchange_view(b, &xv))) return rc;
     // the view: the exchange's, with the DENSE pairs (nothing delivered) in their places
     soff[0] = 0;
     for (uint32_t p = 0, x = 0; p < np; p++) {
@@ -1757,7 +1781,7 @@ int pt_batch_checkout(pt_batch* b, const uint32_t* logs, uint32_t n, const uint3
     DevBuf dlogs, dnch, dcoff, dclk, dslot, dpos, dcov, ddlv, dtot;   // freed on return
     if ((rc = upload_n(b, dlogs, logs, n)) || (rc = upload_n(b, dslot, slot_off.data(), (uint64_t)n + 1)) ||
         (rc = reserve_n<uint32_t>(dpos, n_slot)) || (rc = reserve_n<uint32_t>(dcov, n_slot)) ||
-        (rc = reserve_n<ptx::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptx::PairTotals>(dtot, n))) return rc;
+        (rc = reserve_n<ptct::Delivered>(ddlv, n_slot)) || (rc = reserve_n<ptct::PairTotals>(dtot, n))) return rc;
     if (n_changes && (rc = upload_n(b, dnch, n_changes, n))) return rc;
     if (clock_off && ((rc = upload_n(b, dcoff, clock_off, (uint64_t)n + 1)) || (rc = upload_n(b, dclk, clock, clock_off[n])))) return rc;
     ptck::CheckoutParams C{};
@@ -1766,23 +1790,28 @@ int pt_batch_checkout(pt_batch* b, const uint32_t* logs, uint32_t n, const uint3
     C.clock_off = (const unsigned long long*)dcoff.p; C.clock = (const pt_clock_entry*)dclk.p;
     C.desc = (const pt_log_desc*)b->d_desc.p; C.cdesc = (const pt_change_desc*)b->d_cdesc.p;
     C.changes = (const pt_change_rec*)b->d_changes.p; C.deps = (const pt_dep_rec*)b->d_deps.p; C.marks = b->dp_marks;
-    C.slot_off = (const unsigned long long*)dslot.p; C.pos = (uint32_t*)dpos.p; C.cov = (uint32_t*)dcov.p; C.dlv = (ptx::Delivered*)ddlv.p;
-    C.totals = (ptx::PairTotals*)dtot.p;
-    const auto [wpb, smem] = actor_shape(b->adm_maxR);
-    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptck::checkout_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ptck::checkout_select_kernel<<<warp_grid(b, n, wpb * 32), wpb * 32, smem, b->stream>>>(C);
-    PT_CUDA(launched(b));
-    std::vector<ptx::PairTotals> tot(n);
-    PT_CUDA(cudaMemcpyAsync(tot.data(), dtot.p, (size_t)n * sizeof(ptx::PairTotals), cudaMemcpyDeviceToHost, b->stream));
+    C.slot_off = (const unsigned long long*)dslot.p; C.pos = (uint32_t*)dpos.p; C.cov = (uint32_t*)dcov.p; C.dlv = (ptct::Delivered*)ddlv.p;
+    C.totals = (ptct::PairTotals*)dtot.p;
+    if ((rc = launch_actor_kernel(b, ptck::checkout_select_kernel, n, C))) return rc;
+    std::vector<ptct::PairTotals> tot(n);
+    PT_CUDA(cudaMemcpyAsync(tot.data(), dtot.p, (size_t)n * sizeof(ptct::PairTotals), cudaMemcpyDeviceToHost, b->stream));
     PT_CUDA(cudaStreamSynchronize(b->stream));
+    // ---- gather: the covered changes' records, change and dep records into the delta, identity maps, arrivals from 0 ----
+    std::vector<pt_exchange_pair> pairs(n);
+    for (uint32_t k = 0; k < n; k++) pairs[k] = pt_exchange_pair{logs[k], k};
+    DevBuf dpairs, dempty;
+    if ((rc = upload_n(b, dpairs, pairs.data(), n)) || (rc = reserve_n<pt_log_desc>(dempty, n))) return rc;
+    PT_CUDA(cudaMemsetAsync(dempty.p, 0, (size_t)n * sizeof(pt_log_desc), b->stream));
+    ptx::ExchangeParams P{};
+    P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = n;
+    P.slot_off = (const unsigned long long*)dslot.p; P.dlv = (ptct::Delivered*)ddlv.p; P.totals = (ptct::PairTotals*)dtot.p;
+    Delta D;
+    if ((rc = gather_delta(b, P, tot.data(), (const pt_log_desc*)dempty.p, nullptr, D))) return rc;
     // ---- the new batch: the resident logs, then one log per request (a request that is not OK has zero totals) ----
     std::vector<uint32_t> from(nn), tables_from(nn);
     std::vector<pt_log_desc> nd(nn), dd(nn, pt_log_desc{});
     std::vector<pt_change_desc> ncd(nn), dcd(nn, pt_change_desc{});
-    std::vector<ptx::PairBase> base(n);
-    std::vector<pt_exchange_pair> pairs(n);
-    std::vector<unsigned long long> dlv_off((size_t)n + 1, 0);
-    uint64_t io = 0, mo = 0, co = 0, po = 0, n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0, most = 0;
+    uint64_t io = 0, mo = 0, co = 0, po = 0;
     for (uint32_t i = 0; i < nn; i++) {
         const bool old = i < n0;
         const uint32_t s = old ? i : logs[i - n0];
@@ -1793,44 +1822,20 @@ int pt_batch_checkout(pt_batch* b, const uint32_t* logs, uint32_t n, const uint3
         pt_change_desc LC = CS;
         if (!old) {
             const uint32_t k = i - n0;
-            const ptx::PairTotals& t = tot[k];
+            const ptct::PairTotals& t = tot[k];
+            const ptct::PairBase& B = D.base[k];
             status_out[k] = t.status;
-            L = pt_log_desc{n_ins, n_mk, t.n_insdel, t.n_mark, S.n_actors, S.max_ctr};
-            LC = pt_change_desc{n_ch, n_dp, t.n_changes, t.n_deps};
+            L = pt_log_desc{B.insdel, B.mark, t.n_insdel, t.n_mark, S.n_actors, S.max_ctr};
+            LC = pt_change_desc{B.change, B.dep, t.n_changes, t.n_deps};
             dd[i] = L; dcd[i] = LC;
-            base[k] = ptx::PairBase{n_ins, n_mk, n_ch, n_dp};
-            pairs[k] = pt_exchange_pair{s, k};
-            n_ins += t.n_insdel; n_mk += t.n_mark; n_ch += t.n_changes; n_dp += t.n_deps;
-            dlv_off[k + 1] = n_ch;
-            most = std::max<uint64_t>(most, (uint64_t)t.n_insdel + 2ull * t.n_mark);
         }
         nd[i] = pt_log_desc{io, mo, L.n_insdel, L.n_mark, L.n_actors, L.max_ctr};
         ncd[i] = pt_change_desc{co, po, LC.n_changes, LC.n_deps};
         io += L.n_insdel; mo += L.n_mark; co += LC.n_changes; po += LC.n_deps;
     }
-    // ---- gather: the covered changes' records, change and dep records into the delta, identity maps, arrivals from 0 ----
-    DevBuf dpairs, ddoff, dbase, dempty, dgi, dgm, dgc, dgd;
-    if ((rc = reserve_n<pt_insdel_rec>(dgi, n_ins)) || (rc = reserve_n<pt_mark_rec>(dgm, n_mk)) ||
-        (rc = reserve_n<pt_change_rec>(dgc, n_ch)) || (rc = reserve_n<pt_dep_rec>(dgd, n_dp))) return rc;
-    if (n_ch) {
-        if ((rc = upload_n(b, dpairs, pairs.data(), n)) || (rc = upload_n(b, ddoff, dlv_off.data(), (uint64_t)n + 1)) ||
-            (rc = upload_n(b, dbase, base.data(), n)) || (rc = reserve_n<pt_log_desc>(dempty, n))) return rc;
-        PT_CUDA(cudaMemsetAsync(dempty.p, 0, (size_t)n * sizeof(pt_log_desc), b->stream));
-        ptx::ExchangeParams P{};
-        P.pairs = (const pt_exchange_pair*)dpairs.p; P.n_pairs = n;
-        P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
-        P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
-        P.insdel = b->dp_insdel; P.marks = b->dp_marks;
-        P.slot_off = (const unsigned long long*)dslot.p; P.dlv = (ptx::Delivered*)ddlv.p; P.totals = (ptx::PairTotals*)dtot.p;
-        P.dlv_off = (const unsigned long long*)ddoff.p; P.n_dlv = n_ch; P.base = (const ptx::PairBase*)dbase.p;
-        P.dst_desc = (const pt_log_desc*)dempty.p;
-        P.out_insdel = (pt_insdel_rec*)dgi.p; P.out_marks = (pt_mark_rec*)dgm.p; P.out_changes = (pt_change_rec*)dgc.p; P.out_deps = (pt_dep_rec*)dgd.p;
-        ptx::exchange_gather_kernel<<<slice_grid(b, n_ch, most, 128), 128, 0, b->stream>>>(P);
-        PT_CUDA(launched(b));
-    }
     // ---- splice: the delta as added logs behind the kept ones, and the sources' actor tables ----
-    const pt_packed_ops delta{nn, dd.data(), (const pt_insdel_rec*)dgi.p, n_ins, (const pt_mark_rec*)dgm.p, n_mk};
-    const pt_change_table dch{nn, dcd.data(), (const pt_change_rec*)dgc.p, n_ch, (const pt_dep_rec*)dgd.p, n_dp};
+    const pt_packed_ops delta{nn, dd.data(), (const pt_insdel_rec*)D.insdel.p, D.n_ins, (const pt_mark_rec*)D.marks.p, D.n_mk};
+    const pt_change_table dch{nn, dcd.data(), (const pt_change_rec*)D.changes.p, D.n_ch, (const pt_dep_rec*)D.deps.p, D.n_dp};
     NewActorTables T;
     if (b->have_actors && (rc = gather_actor_tables(b, tables_from.data(), nn, nullptr, std::vector<uint32_t>(nn, ~0u), T))) return rc;
     if ((rc = splice(b, fn, std::move(nd), std::move(ncd), b->adm_maxR, &delta, true, pt_append_remap{}, from.data(), &dch, true, true))) return rc;
@@ -1888,19 +1893,17 @@ static int enqueue_merge(pt_batch* b) {
     P.seq = (b->limits.flags & PT_FLAG_EMIT_SEQUENCE) ? (uint32_t*)b->d_seq.p : nullptr;
     P.stats = c->stats;
     P.admit = nullptr;
+    int rc;
     if (b->have_changes && b->n_logs) {
-        const auto [wpb, smem] = actor_shape(b->adm_maxR);     // admission pre-pass
-        if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptadm::admit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ptadm::admit_kernel<<<warp_grid(b, b->n_logs, wpb * 32), wpb * 32, smem, b->stream>>>(
-            (const pt_change_desc*)b->d_cdesc.p, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p, (const pt_log_desc*)b->d_desc.p,
-            b->n_logs, b->adm_maxR, (uint32_t*)b->d_admit.p, (pt_log_result*)b->d_results.p);
-        PT_CUDA(launched(b));
+        if ((rc = launch_actor_kernel(b, ptadm::admit_kernel, b->n_logs,     // admission pre-pass
+                                      (const pt_change_desc*)b->d_cdesc.p, (const pt_change_rec*)b->d_changes.p, (const pt_dep_rec*)b->d_deps.p,
+                                      (const pt_log_desc*)b->d_desc.p, b->n_logs, b->adm_maxR, (uint32_t*)b->d_admit.p, (pt_log_result*)b->d_results.p)))
+            return rc;
         P.admit = (const uint32_t*)b->d_admit.p;
     }
     { const char* e = getenv("PT_PREFETCH"); P.prefetch_next = e ? (uint32_t)atoi(e) : 0u; }
     { const char* e = getenv("PT_WARP_FLAGS"); P.warp_flags = e ? (uint32_t)atoi(e) : 0x704u; }   // default: phase-aligned rounds (bit 2), the in-log phase barriers 2-4 skipped (bits 8-10: measured), no extra L2 prefetch
     { const char* e = getenv("PT_TMA"); P.use_tma = e ? (uint32_t)atoi(e) : 1u; }
-    int rc;
     // ascending bins; a log whose working set does not fit bin k's shared memory is deferred (on the device) to bin k+1;
     // only the last bin can spill to the global slab
     // The CTA-per-log bins' own lists do not depend on the warp / team kernels: when both exist they are launched on a side
@@ -2221,10 +2224,7 @@ int pt_batch_attribute(pt_batch* b, const uint32_t* logs, uint32_t n, const uint
     P.first = (uint32_t*)dfirst.p; P.cov = (uint32_t*)dcov.p;
     P.chg = (uint32_t*)dchg.p; P.dchg = (uint32_t*)ddchg.p; P.dcov = (uint32_t*)ddcov.p; P.dkey = (unsigned long long*)ddkey.p; P.table = (uint32_t*)dtab.p;
     P.status = (uint32_t*)dst.p; P.count = (unsigned long long*)dcnt.p; P.off = (const unsigned long long*)doff.p;
-    const auto [wpb, smem] = actor_shape(b->adm_maxR);
-    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(pta::attribute_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    pta::attribute_resolve_kernel<<<warp_grid(b, n, wpb * 32), wpb * 32, smem, b->stream>>>(P);
-    PT_CUDA(launched(b));
+    if ((rc = launch_actor_kernel(b, pta::attribute_resolve_kernel, n, P))) return rc;
     // ---- count, scan, one total back, write ----
     const uint32_t threads = 128, grid = warp_grid(b, n, threads);
     pta::attribute_runs_kernel<false><<<grid, threads, 0, b->stream>>>(P);
@@ -2442,10 +2442,7 @@ int pt_batch_render_changes_json(pt_batch* b, const pt_changes_json_input* in, p
     unsigned long long* bad = (unsigned long long*)dbad.p;
     unsigned long long* miss = (unsigned long long*)dmiss.p;
     PT_CUDA(cudaMemsetAsync(bad, 0xFF, 16, b->stream));
-    const auto [wpb, smem] = actor_shape(b->adm_maxR);
-    if (smem > 48 * 1024) PT_CUDA(cudaFuncSetAttribute(ptcj::changes_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ptcj::changes_select_kernel<<<warp_grid(b, nr, wpb * 32), wpb * 32, smem, b->stream>>>(C);
-    PT_CUDA(launched(b));
+    if ((rc = launch_actor_kernel(b, ptcj::changes_select_kernel, nr, C))) return rc;
     if ((rc = scan_offsets(b, pts::PlainCounts{C.items}, nr, dbsum, (unsigned long long*)ditemoff.p, nullptr))) return rc;
     // read-back 1: the item count and the select kernel's findings
     uint64_t* hm = (uint64_t*)J.hmisc.p;

@@ -3,22 +3,17 @@
 //
 // exchange_select_kernel: one warp per pair, grid-stride.  Per-warp shared memory holds dst's clock (by dst actor rank) and a
 // per-src-actor word (first the actor's change count, then the queue slot of its first missing change).
-//   1. clocks: both change tables 32 changes per trip; match_any groups give each change its rank among the trip's changes of
-//      the same actor, so seq == count + 1 is checked per lane (admit_kernel's scheme).  The src pass also writes each change's
-//      list-op position (running sum of n_ops) into the pair's scratch slot.
-//   2. queue, getMissingChanges order (reference test/merge.ts:25-38): actors in the order src first saw them, ascending seq
-//      (missing_queue, shared with pt_batch_render_changes_json's select kernel).  In a seq-contiguous table an actor's first
-//      change is its seq 1, so one pass in table order gives every actor the slot of its first missing change (a warp scan over
-//      the trip's seq-1 lanes), and the change (actor, seq) goes to slot[actor] + seq - clock_dst - 1.
+//   1. clocks: ptct::count_clock over dst's table, ptct::source_clock over src's (with each change's list-op position into the
+//      pair's scratch slot).
+//   2. queue, getMissingChanges order: ptct::missing_queue, with dst's clock through the actor map.
 //   3. delivery, applyChanges order (test/merge.ts:4-23): repeated in-order passes over the queue, 32 candidates per trip.
 //      All lanes test seq and deps against the clock of the trip's start.  A pass is final (clocks only grow, and a
 //      seq-contiguous table has no second change with the same actor and seq); a lane that failed is tested again in lane
 //      order, after the clock bumps of the delivered lanes before it, so it sees exactly what the reference's queue front
 //      would.  Lanes that fail stay in the queue (compacted in place) for the next pass; a pass that delivers nothing ends
 //      the pair with PT_EXCHANGE_STUCK.
-//    A delivered change's record ranges come from its list-op positions: marks before position X = the first k with
-//    min(arrival_k, n) + k >= X (ptw::marks_before_lane, the per-lane form of the patch window's cut), ins/del records before
-//    it = X - k.  Running sums over the delivered changes give each its place in the delta.
+//    A delivered change's record ranges come from its list-op positions (ptct::change_records), and ptct::place_delivered
+//    gives it its place in the delta.
 // exchange_gather_kernel: one warp per delivered change (blockIdx.y slices a long change, as splice_records_kernel slices a
 // long log): 16-byte coalesced copies with the pair's actor and counter maps applied (a mark is a lane pair, as in the
 // splice), mark arrivals rebased onto dst's records; slice 0 also writes the change record, its deps and the delivered index.
@@ -28,18 +23,9 @@
 #include <cstdint>
 
 #include "../../include/peritext_b200.h"
-#include "patch_window.cuh"
+#include "change_table.cuh"
 
 namespace ptx {
-
-struct PairTotals { uint32_t n_insdel, n_mark, n_changes, n_deps, max_ctr, status, reserved0, reserved1; };   // 32 B per pair
-struct Delivered {          // one per delivered change, in delivery order.  32 B
-    uint32_t change;                    // index in src's change table
-    uint32_t ins_lo, mk_lo;             // its first ins/del and mark record in src's log
-    uint32_t n_insdel, n_mark;
-    uint32_t ins_off, mk_off, dep_off;  // its place among the pair's delivered records
-};
-struct PairBase { unsigned long long insdel, mark, change, dep; };   // where a pair's records start in the delta arrays
 
 // One pair's maps, src id space -> dst id space.  The actor map has exactly src's n_actors entries; a == null (pt_batch_checkout)
 // is the identity actor map and nc == 0 the identity counter map.  No image: 0xFFFF / 0xFFFFFFFF.
@@ -59,12 +45,12 @@ struct ExchangeParams {
     const pt_log_desc* desc; const pt_change_desc* cdesc; const pt_change_rec* changes; const pt_dep_rec* deps;
     const pt_insdel_rec* insdel; const pt_mark_rec* marks;
     const unsigned long long* slot_off;   // [n_pairs + 1] a pair's scratch slot: src's n_changes entries of queue, pos and dlv
-    uint32_t* queue; uint32_t* pos; Delivered* dlv;
-    PairTotals* totals;
+    uint32_t* queue; uint32_t* pos; ptct::Delivered* dlv;
+    ptct::PairTotals* totals;
     // gather only
     const unsigned long long* dlv_off;    // [n_pairs + 1] exclusive scan of the pairs' delivered changes
     unsigned long long n_dlv;
-    const PairBase* base;
+    const ptct::PairBase* base;
     const pt_log_desc* dst_desc;          // the descriptors a pair's dst indexes: desc, or a checkout's empty logs
     pt_insdel_rec* out_insdel; pt_mark_rec* out_marks; pt_change_rec* out_changes; pt_dep_rec* out_deps;
     uint32_t* out_delivered;              // may be null
@@ -75,74 +61,6 @@ __device__ __forceinline__ PairMaps pair_maps(const ExchangeParams& P, uint32_t 
     if (P.actor_off) { const unsigned long long ao = P.actor_off[p]; m.a = P.actor_map + ao; m.na = (uint32_t)(P.actor_off[p + 1] - ao); }
     if (P.ctr_off) { const unsigned long long o = P.ctr_off[p]; m.c = P.ctr_map + o; m.nc = (uint32_t)(P.ctr_off[p + 1] - o); }
     return m;
-}
-
-__device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, uint32_t& total) {
-    uint32_t s = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, d); if (lane >= (uint32_t)d) s += y; }
-    total = __shfl_sync(0xffffffffu, s, 31);
-    return s - v;
-}
-
-// Step 1 for one change table: cnt[actor] = the actor's changes (cnt zeroed by the caller); false if a change names an actor
-// >= R, breaks seq == count + 1, or its deps leave the log's dep records.  With pos: pos[k] = sum of n_ops before change k,
-// *ops = the sum over the table.
-__device__ __forceinline__ bool count_clock(const pt_change_rec* __restrict__ c0, uint32_t n, uint32_t n_deps, uint32_t R, uint32_t* cnt,
-                                            uint32_t* __restrict__ pos, unsigned long long* ops, uint32_t lane) {
-    const uint32_t lt = (1u << lane) - 1u;
-    unsigned long long run = 0;
-    bool ok = true;
-    for (uint32_t base = 0; base < n && ok; base += 32) {
-        const uint32_t k = base + lane;
-        const bool valid = k < n;
-        uint4 r = make_uint4(0, 0, 0, 0);
-        if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
-        const uint32_t actor = r.y & 0xFFFFu;
-        const bool aok = valid && actor < R;
-        const uint32_t mask = __match_any_sync(0xffffffffu, aok ? actor : (0x10000u + lane));
-        const bool bad = valid && (!aok || r.x != cnt[aok ? actor : 0] + __popc(mask & lt) + 1u || (unsigned long long)r.z + (r.y >> 16) > n_deps);
-        ok = !__any_sync(0xffffffffu, bad);
-        if (pos) {
-            uint32_t tot;
-            const uint32_t ex = warp_excl_scan(valid ? r.w : 0u, lane, tot);   // a trip's n_ops can wrap only in a table the total check refuses
-            unsigned long long wide = valid ? r.w : 0u;
-            for (int o = 16; o > 0; o >>= 1) wide += __shfl_xor_sync(0xffffffffu, wide, o);
-            if (valid) pos[k] = (uint32_t)run + ex;
-            run += wide;
-        }
-        __syncwarp();
-        if (aok && (mask & lt) == 0) cnt[actor] += __popc(mask);
-        __syncwarp();
-    }
-    if (ops) *ops = run;
-    return ok;
-}
-
-// getMissingChanges order (reference test/merge.ts:25-38) of a seq-contiguous table c0[0 .. n) whose clock count_clock left in
-// cs[actor]: actors in the order the table first shows them, then ascending seq.  have(actor) is the peer's clock entry for the
-// table's actor rank.  An actor's first change is its seq 1, so one pass in table order gives every actor the slot of its first
-// missing change (a warp scan over the trip's seq-1 lanes, overwriting cs), and change k = (actor, seq) with seq > have goes to
-// slot cs[actor] + seq - have - 1: queued(k, its record, slot).  Returns the queue length.  Warp-collective.
-template <class Have, class Queued>
-__device__ __forceinline__ uint32_t missing_queue(const pt_change_rec* __restrict__ c0, uint32_t n, uint32_t* cs, Have have_of, Queued queued, uint32_t lane) {
-    uint32_t nq = 0;
-    for (uint32_t base = 0; base < n; base += 32) {
-        const uint32_t k = base + lane;
-        const bool valid = k < n;
-        uint4 r = make_uint4(0, 0, 0, 0);
-        if (valid) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
-        const uint32_t actor = r.y & 0xFFFFu, have = valid ? have_of(actor) : 0u;
-        const bool first = valid && r.x == 1u;
-        uint32_t tot;
-        const uint32_t ex = warp_excl_scan(first && cs[actor] > have ? cs[actor] - have : 0u, lane, tot);
-        __syncwarp();
-        if (first) cs[actor] = nq + ex;
-        __syncwarp();
-        nq += tot;
-        if (valid && r.x > have) queued(k, r, cs[actor] + r.x - have - 1u);
-    }
-    return nq;
 }
 
 // applyChange's admission test (reference src/micromerge.ts:501-509) of a src change against dst's clock; the change's and
@@ -176,39 +94,37 @@ __global__ void exchange_select_kernel(ExchangeParams P) {
         const pt_dep_rec* d0 = P.deps + CS.dep_off;
         uint32_t* queue = P.queue + P.slot_off[p];
         uint32_t* pos = P.pos + P.slot_off[p];
-        Delivered* dlv = P.dlv + P.slot_off[p];
+        ptct::Delivered* dlv = P.dlv + P.slot_off[p];
         uint32_t status = PT_EXCHANGE_OK;
-        unsigned long long ops = 0;
-        if (!count_clock(P.changes + CD.change_off, CD.n_changes, CD.n_deps, Rd, clk, nullptr, nullptr, lane) ||
-            !count_clock(c0, CS.n_changes, CS.n_deps, Rs, cs, pos, &ops, lane) ||
-            ops != (unsigned long long)S.n_insdel + S.n_mark || ops > 0xFFFFFFFFull)
+        if (!ptct::count_clock(P.changes + CD.change_off, CD.n_changes, CD.n_deps, Rd, clk, nullptr, nullptr, lane) ||
+            !ptct::source_clock(c0, CS, S, cs, pos, lane))
             status = PT_EXCHANGE_BAD_TABLE;
         // ---- step 2: the queue ----
         uint32_t nq = 0;
         if (status == PT_EXCHANGE_OK) {
             bool bad = false, unmapped = false;
-            nq = missing_queue(c0, CS.n_changes, cs,
-                               [&](uint32_t actor) { const uint32_t ma = m.actor(actor); return ma < Rd ? clk[ma] : 0u; },   // no rank in dst: 0
-                               [&](uint32_t k, uint4 r, uint32_t slot) {
-                                   queue[slot] = k;
-                                   if (m.actor(r.y & 0xFFFFu) >= Rd) unmapped = true;
-                                   for (uint32_t d = 0; d < (r.y >> 16); d++) {
-                                       const uint32_t da = d0[r.z + d].actor;
-                                       if (da >= Rs) bad = true;
-                                       else if (m.actor(da) >= Rd) unmapped = true;
-                                   }
-                               }, lane);
+            nq = ptct::missing_queue(c0, CS.n_changes, cs,
+                                     [&](uint32_t actor) { const uint32_t ma = m.actor(actor); return ma < Rd ? clk[ma] : 0u; },   // no rank in dst: 0
+                                     [&](uint32_t k, uint4 r, uint32_t slot) {
+                                         queue[slot] = k;
+                                         if (m.actor(r.y & 0xFFFFu) >= Rd) unmapped = true;
+                                         for (uint32_t d = 0; d < (r.y >> 16); d++) {
+                                             const uint32_t da = d0[r.z + d].actor;
+                                             if (da >= Rs) bad = true;
+                                             else if (m.actor(da) >= Rd) unmapped = true;
+                                         }
+                                     }, lane);
             if (__any_sync(0xffffffffu, bad)) status = PT_EXCHANGE_BAD_TABLE;
             else if (__any_sync(0xffffffffu, unmapped)) status = PT_EXCHANGE_UNMAPPED;
         }
         // ---- step 3: delivery ----
-        uint32_t t_ins = 0, t_mk = 0, t_ch = 0, t_dep = 0;
+        ptct::PairTotals t{};                                 // the delivered changes' running totals; status PT_EXCHANGE_OK
         const pt_mark_rec* mk = P.marks + S.mark_off;
         uint32_t remaining = nq;
         __syncwarp();
         while (status == PT_EXCHANGE_OK && remaining) {
             uint32_t kept = 0;
-            const uint32_t before = t_ch;
+            const uint32_t before = t.n_changes;
             for (uint32_t base = 0; base < remaining && status == PT_EXCHANGE_OK; base += 32) {
                 const bool valid = base + lane < remaining;
                 const uint32_t c = valid ? queue[base + lane] : 0u;
@@ -229,32 +145,21 @@ __global__ void exchange_select_kernel(ExchangeParams P) {
                 }
                 if (((pass & ~applied) >> lane) & 1u) atomicMax(&clk[ma], r.x);
                 __syncwarp();
-                // the delivered lanes' record ranges and their places in the delta
-                uint32_t ins_lo = 0, ins_n = 0, mk_lo = 0, mk_n = 0;
-                bool broken = false;
-                if (ok) {
-                    const uint32_t x0 = pos[c], x1 = x0 + r.w;
-                    const uint32_t k0 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x0), k1 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x1);
-                    broken = k0 > x0 || k1 > x1 || k1 < k0 || x1 - k1 > S.n_insdel || x1 - k1 < x0 - k0;   // arrivals that do not fit the table
-                    if (!broken) { ins_lo = x0 - k0; ins_n = (x1 - k1) - ins_lo; mk_lo = k0; mk_n = k1 - k0; }
-                }
-                if (__any_sync(0xffffffffu, broken)) { status = PT_EXCHANGE_BAD_TABLE; break; }
-                uint32_t n_i, n_m, n_d;
-                const uint32_t e_i = warp_excl_scan(ins_n, lane, n_i), e_m = warp_excl_scan(mk_n, lane, n_m),
-                               e_d = warp_excl_scan(ok ? (r.y >> 16) : 0u, lane, n_d);
-                if (ok) dlv[t_ch + __popc(pass & lt)] = Delivered{c, ins_lo, mk_lo, ins_n, mk_n, t_ins + e_i, t_mk + e_m, t_dep + e_d};
-                t_ins += n_i; t_mk += n_m; t_dep += n_d; t_ch += __popc(pass);
+                // the delivered lanes' record ranges and their places in the delta (pass is ballot(ok))
+                ptct::Records x{};
+                if (ok) x = ptct::change_records(mk, S, pos[c], r.w);
+                if (__any_sync(0xffffffffu, ok && !x.fits)) { status = PT_EXCHANGE_BAD_TABLE; break; }
+                ptct::place_delivered(dlv, ok, c, x, r.y >> 16, lane, t);
                 // the others go back to the queue; slot kept + rank <= base + lane, which this trip has already read
                 if (valid && !ok) queue[kept + __popc(vmask & ~pass & lt)] = c;
                 kept += __popc(vmask & ~pass);
                 __syncwarp();
             }
-            if (status == PT_EXCHANGE_OK && t_ch == before) status = PT_EXCHANGE_STUCK;
+            if (status == PT_EXCHANGE_OK && t.n_changes == before) status = PT_EXCHANGE_STUCK;
             remaining = kept;
         }
         if (lane == 0)
-            P.totals[p] = status == PT_EXCHANGE_OK ? PairTotals{t_ins, t_mk, t_ch, t_dep, 0u, PT_EXCHANGE_OK, 0u, 0u}
-                                                   : PairTotals{0u, 0u, 0u, 0u, 0u, status, 0u, 0u};
+            P.totals[p] = status == PT_EXCHANGE_OK ? t : ptct::PairTotals{0u, 0u, 0u, 0u, 0u, status, 0u, 0u};
         __syncwarp();
     }
 }
@@ -269,8 +174,8 @@ __global__ void exchange_gather_kernel(ExchangeParams P) {
         const pt_exchange_pair pr = P.pairs[p];
         const pt_log_desc S = P.desc[pr.src], D = P.dst_desc[pr.dst];
         const PairMaps m = pair_maps(P, p);
-        const PairBase B = P.base[p];
-        const Delivered d = P.dlv[P.slot_off[p] + k];
+        const ptct::PairBase B = P.base[p];
+        const ptct::Delivered d = P.dlv[P.slot_off[p] + k];
         uint32_t top = 0;                                  // the largest mapped opId counter this lane wrote
         bool unmapped = false;
         auto ctr = [&](uint32_t c) { const uint32_t x = m.ctr(c); unmapped |= x == 0xFFFFFFFFu; return x; };

@@ -6,12 +6,12 @@
 // by bisection (js_cmp) and two tables join by name without a hash.
 //
 // sync_derive_kernel: one warp per pair.  Shared memory per warp, two words per src/dst rank (actor_shape's budget):
-//   1. clocks: ptx::count_clock over both change tables (dst's by dst rank into A, src's by src rank into B, with the src
-//      changes' list-op positions); a table that fails the checks leaves the pair to the exchange, which reports BAD_TABLE.
+//   1. clocks: ptct::count_clock over dst's change table by dst rank into A, ptct::source_clock over src's by src rank into B
+//      (with the list-op positions); a table that fails the checks leaves the pair to the exchange, which reports BAD_TABLE.
 //   2. have: B[r] = A[dst rank of src rank r's name] (0 without one): dst's clock keyed by actor NAME.  A becomes a bitmap over
 //      src ranks.
 //   3. missing set: src's changes with seq > B[actor].  Each marks its actor and its deps' actors in the bitmap; its records
-//      (ranges from its list-op positions, ptw::marks_before_lane, as the exchange's select kernel) are read by the whole warp,
+//      (ptct::change_records; records that do not fit leave the pair to the exchange too) are read by the whole warp,
 //      marking the actor of every id whose counter is non-zero, and giving the top opId counter and the op count.
 //   4. growth: the marked src names dst lacks, compacted in rank (= name) order into the pair's slot; their count and bytes,
 //      whether the first sorts before dst's last name (dst's ranks move), and the DENSE test of the grown dst.
@@ -28,8 +28,7 @@
 #include <cstdint>
 
 #include "../../include/peritext_b200.h"
-#include "exchange_kernel.cuh"
-#include "patch_window.cuh"
+#include "change_table.cuh"
 
 namespace pty {
 
@@ -113,10 +112,8 @@ __global__ void sync_derive_kernel(DeriveParams P) {
         const pt_change_rec* c0 = P.changes + CS.change_off;
         const pt_dep_rec* d0 = P.deps + CS.dep_off;
         uint32_t* pos = P.pos + P.slot_off[p];
-        unsigned long long ops = 0;
-        bool ok = ptx::count_clock(P.changes + CD.change_off, CD.n_changes, CD.n_deps, Rd, A, nullptr, nullptr, lane) &&
-                  ptx::count_clock(c0, CS.n_changes, CS.n_deps, Rs, B, pos, &ops, lane) &&
-                  ops == (unsigned long long)S.n_insdel + S.n_mark && ops <= 0xFFFFFFFFull;
+        bool ok = ptct::count_clock(P.changes + CD.change_off, CD.n_changes, CD.n_deps, Rd, A, nullptr, nullptr, lane) &&
+                  ptct::source_clock(c0, CS, S, B, pos, lane);
         // ---- 2: dst's clock by src rank, through the names ----
         if (ok) {
             for (uint32_t r = lane; r < Rs; r += 32) {
@@ -145,24 +142,22 @@ __global__ void sync_derive_kernel(DeriveParams P) {
             uint4 r = make_uint4(0, 0, 0, 0);
             if (k < CS.n_changes) r = __ldg(reinterpret_cast<const uint4*>(c0 + k));
             const bool miss = k < CS.n_changes && r.x > B[r.y & 0xFFFFu];
-            uint32_t ins_lo = 0, ins_n = 0, mk_lo = 0, mk_n = 0;
+            ptct::Records x{};
             if (miss) {
                 mark_actor(A, r.y & 0xFFFFu, Rs);
                 for (uint32_t d = 0; d < (r.y >> 16); d++) {
                     const uint32_t da = d0[r.z + d].actor;
                     if (da >= Rs) bad = true; else mark_actor(A, da, Rs);
                 }
-                const uint32_t x0 = pos[k], x1 = x0 + r.w;
-                const uint32_t k0 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x0), k1 = ptw::marks_before_lane(mk, S.n_insdel, S.n_mark, x1);
-                if (k0 > x0 || k1 > x1 || k1 < k0 || x1 - k1 > S.n_insdel || x1 - k1 < x0 - k0) bad = true;
-                else { ins_lo = x0 - k0; ins_n = (x1 - k1) - ins_lo; mk_lo = k0; mk_n = k1 - k0; }
+                x = ptct::change_records(mk, S, pos[k], r.w);
+                if (!x.fits) bad = true;
             }
             if (__any_sync(0xffffffffu, bad)) { ok = false; break; }
             // the whole warp reads each missing change's records in turn
             for (uint32_t todo = __ballot_sync(0xffffffffu, miss); todo; todo &= todo - 1) {
                 const uint32_t src = __ffs(todo) - 1;
-                const uint32_t il = __shfl_sync(0xffffffffu, ins_lo, src), in_ = __shfl_sync(0xffffffffu, ins_n, src);
-                const uint32_t ml = __shfl_sync(0xffffffffu, mk_lo, src), mn = __shfl_sync(0xffffffffu, mk_n, src);
+                const uint32_t il = __shfl_sync(0xffffffffu, x.ins_lo, src), in_ = __shfl_sync(0xffffffffu, x.n_insdel, src);
+                const uint32_t ml = __shfl_sync(0xffffffffu, x.mk_lo, src), mn = __shfl_sync(0xffffffffu, x.n_mark, src);
                 any = true;
                 n_ops += (unsigned long long)in_ + mn;
                 for (uint32_t i = lane; i < in_; i += 32) {
