@@ -906,6 +906,93 @@ int pt_batch_attribute(pt_batch*, const uint32_t* logs, uint32_t n,
                        const pt_clock_entry* clock,   /* request k's clock = clock[clock_off[k] .. clock_off[k+1])         */
                        pt_attr_view* out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Restore: make a resident log's visible text equal to an earlier version's, as a NEW local change.  In a CRDT a restore
+ * cannot truncate the log (peers already hold the later changes): it is a change an actor makes on top of the current
+ * document, which reaches peers through the normal sync (pt_batch_exchange / pt_batch_sync_pairs) like any other edit.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pt_restore_request {  /* 16 B */
+    uint32_t log;        /* the log that gets the new change                                                           */
+    uint32_t version;    /* a resident log in log's id space holding the target version (a pt_batch_checkout of log, or a
+                            pt_batch_select_logs fork of one)                                                           */
+    uint32_t actor;      /* the acting actor's rank in log (introduce a new actor first, as for pt_batch_change)         */
+    uint32_t first_ctr;  /* packed counter of the first generated op; op j gets first_ctr + j; must exceed log's max_ctr  */
+} pt_restore_request;
+#define PT_RESTORE_TEXT 1u          /* make log's visible text equal to version's                                        */
+#define PT_RESTORE_MARKS 2u         /* make log's formatting equal to version's (the visible texts must already be equal)  */
+#define PT_RESTORE_OK 0u
+#define PT_RESTORE_LOG_FAILED 1u    /* log's or version's merge status is not PT_LOG_OK                                  */
+#define PT_RESTORE_BAD_TABLE 2u     /* log's change table fails the change-table rules for a src (as PT_CHECKOUT_BAD_TABLE) */
+#define PT_RESTORE_FOREIGN 3u       /* TEXT: an element of version has no element of the same packed opId, in order, in log */
+#define PT_RESTORE_TEXT_DIFFERS 4u  /* MARKS: the two visible token sequences differ                                     */
+typedef struct pt_restore_view {
+    uint32_t n;
+    const uint32_t* status;   /* [n] PT_RESTORE_*; a request that is not OK appends nothing                              */
+    const uint32_t* n_ops;    /* [n] list ops of the appended change; 0 = nothing to do, no change appended              */
+    const uint32_t* seq;      /* [n] the appended change's seq (0 when none)                                             */
+} pt_restore_view;
+/* Request k appends to log req[k].log one change by actor req[k].actor that makes its visible text (mode PT_RESTORE_TEXT) or
+ * its formatting (PT_RESTORE_MARKS) equal to that of log req[k].version, both as of the last merge.  mode is exactly one of the
+ * two.  The full restore is TEXT, merge, MARKS, merge: MARKS compares the formatting the restored text inherits, and only a
+ * merge computes it.  TEXT:
+ *   join      log's element sequence is walked in order and merge-joined with version's by packed opId (ctr, actor of each
+ *             element's insert record): a log element matches when its opId is that of the next unmatched version element.  A
+ *             pt_batch_checkout keeps its source's packed ids and RGA never reorders elements, so a version of the log is a
+ *             subsequence of it; if the walk ends with version elements unmatched the status is FOREIGN.
+ *   classes   visible now and visible in version: keep; visible now, deleted in or absent from version: delete; deleted now,
+ *             visible in version: restore; deleted now and not visible in version: nothing (stays a tombstone).
+ *   runs      maximal sequences of one action in element order ("nothing" does not break a run, a kept element does).  With v
+ *             the visible index in the document as changed by the earlier InputOperations of the same change, a delete run of
+ *             k elements is {delete, index v, count k} and a restore run {insert, index v, values = its elements' value
+ *             tokens}, then v += k.  The change is by definition Micromerge.change of exactly these InputOperations (reference
+ *             src/micromerge.ts:308-441), lookAfterTombstones included: the inserted values are NEW elements (RGA cannot
+ *             revive a tombstone).
+ *   records   op j has ctr first_ctr + j and the actor's rank; a delete targets its element; an insert's first value
+ *             references HEAD at v == 0, else the last tombstone with a defined after slot (the sequence's bit 30) that follows
+ *             the (v - 1)-th visible element before the next element visible at that moment, else that element (elements this
+ *             change deleted count as tombstones); each further value references the one before.  These are the records
+ *             pt_batch_change generates from the same InputOperations with first_ctr advanced per op.
+ *   change    seq = the log's number of changes by actor + 1; deps = every actor with a nonzero count in the log's clock, in
+ *             the order the table first shows them (the key order of the reference's Object.assign({}, this.clock); the
+ *             acting actor is included iff it has earlier changes), each with that count; n_ops = the generated ops.  A
+ *             request with nothing to do appends no change and leaves seq unchanged (the reference's change([]) would still
+ *             bump its seq).
+ *   status    LOG_FAILED before BAD_TABLE before FOREIGN / TEXT_DIFFERS; a request that is not OK appends nothing.
+ * MARKS (the change record and statuses as above; FOREIGN does not occur):
+ *   compare   the visible token sequences must be equal (else TEXT_DIFFERS).  At every visible position compare strong, em, the
+ *             link attr and the set of comment ranks (PT_SPAN_COMMENT with no ids, quirk Q3, is not compared: no op can remove
+ *             the empty `comment` key).
+ *   ops       one per maximal range of positions differing the same way: strong / em addMark where only version has it,
+ *             removeMark where only log has it; link addMark with version's attr where version's link is present and differs,
+ *             removeMark (no attrs, attr PT_ATTR_NONE) where it is absent; comment, per rank, addMark where only version has it,
+ *             removeMark where only log has it (attr = the rank).  Ordered by startIndex, then mark type in ALL_MARKS order, then
+ *             comment rank.  Boundaries are pt_batch_change's for mark InputOperations: start before(elem[start]); end
+ *             endOfText for strong / em ending at the visible length, else before(elem[end]); after(elem[end - 1]) for comment
+ *             and link.  Op j has ctr first_ctr + j; every mark arrives after all of log's ins/del records.
+ * Preconditions: pt_batch_find_elements' (PT_FLAG_EMIT_SEQUENCE and a completed merge since the last call that changed the
+ * batch), and a change table.  All requests read the batch as it is before the call.
+ * Refused with nothing changed:
+ *   PT_ERR_STATE    no batch, no change table, a handle without PT_FLAG_EMIT_SEQUENCE, or no completed merge since the last call
+ *                   that changed the batch
+ *   PT_ERR_INVALID  (pt_last_error names the first offender) null arguments; mode not exactly one flag; a log or version
+ *                   >= n_logs; a log named twice; an actor >= the log's n_actors; first_ctr <= the log's max_ctr, or a counter past
+ *                   2^32 - 1; a log that would hold 2^22 elements or more, or whose max_ctr x n_actors would reach 2^31; whatever
+ *                   pt_batch_append refuses for the resulting batch.  The count pass runs before the splice, so the limits that
+ *                   depend on the generated counts are refused with nothing changed too.
+ * n == 0: PT_OK, nothing launched.  On success the handle holds exactly what pt_batch_append of the generated delta (identity
+ * maps) would give: re-planned, no merge, the patch window reset, pools persisting; pt_batch_set_patch_window(first_op = old
+ * n_insdel + n_mark) then gives the Patches change() returned.  Synchronises; req may be freed on return.  The view is
+ * engine-owned pinned memory, valid until the next pt_batch_restore or destroy.
+ * Device: restore_kernel<false> (count) and <true> (write), one warp per request, through one function: the log's clock in
+ * shared memory (ptct::source_clock, then ptct::first_shown for the deps), then TEXT's element walk, 32 elements of the log
+ * per trip, the version cursor advanced by ballot / popcount over a 32-element window of version's sequence, or MARKS' walk: a
+ * warp-built visible -> record table of log, then one lane merging the two span lists with the open ranges (comment ranks in
+ * scratch).  The records go straight into the delta that pt_batch_append's splice reads on the device.  Only the requests, the
+ * per-request counts and the view cross PCIe.  Cost per request: TEXT O(n_changes + n_elems(log) + n_elems(version)); MARKS
+ * O(n_changes + n_elems(log) + n_visible + (n_spans(log) + n_spans(version)) x the comment ids per span).  Scratch: 4 B per change
+ * of each request's log; MARKS also 4 B per ins/del record of log and 32 B per mark record of log and version. */
+int pt_batch_restore(pt_batch*, const pt_restore_request* req, uint32_t n, uint32_t mode, pt_restore_view* out);
+
 /* getTextWithFormatting's return value (FormatSpanWithText[], src/peritext.ts:35-38, 337-455) of every merged log as UTF-8
  * JSON text, rendered on the device.  Log i's text is bytes[off[i] .. off[i+1]):
  *   [{"marks":M,"text":T},...]      one object per span, keys sorted; no visible text gives []

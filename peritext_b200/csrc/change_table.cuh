@@ -124,6 +124,24 @@ __device__ __forceinline__ void place_delivered(Delivered* dlv, bool in, uint32_
     t.n_insdel += n_i; t.n_mark += n_m; t.n_deps += n_d; t.n_changes += __popc(pass);
 }
 
+// The actors of a seq-contiguous table c0[0 .. n) in the order it first shows them (the insertion order of Micromerge.clock): an
+// actor's first change is its seq 1, so that is the table order of the seq-1 changes (missing_queue's rule).  shown(actor, k) is
+// called for the k-th; returns their number.  Warp-collective.
+template <class Shown>
+__device__ __forceinline__ uint32_t first_shown(const pt_change_rec* __restrict__ c0, uint32_t n, Shown shown, uint32_t lane) {
+    uint32_t k = 0;
+    for (uint32_t base = 0; base < n; base += 32) {
+        const uint32_t c = base + lane;
+        uint4 r = make_uint4(0, 0, 0, 0);
+        if (c < n) r = __ldg(reinterpret_cast<const uint4*>(c0 + c));
+        const bool first = c < n && r.x == 1u;
+        const uint32_t fm = __ballot_sync(0xffffffffu, first);
+        if (first) shown(r.y & 0xFFFFu, k + __popc(fm & ((1u << lane) - 1u)));
+        k += __popc(fm);
+    }
+    return k;
+}
+
 // A request's clock entries [lo, hi) into clk[actor] (actors < n_actors and distinct: the host checks them).
 __device__ __forceinline__ void load_clock(uint32_t* clk, const pt_clock_entry* clock, unsigned long long lo, unsigned long long hi, uint32_t lane) {
     for (unsigned long long e = lo + lane; e < hi; e += 32) {

@@ -31,6 +31,7 @@
 #include "sync_kernel.cuh"
 #include "checkout_kernel.cuh"
 #include "attribute_kernel.cuh"
+#include "restore_kernel.cuh"
 #include "plan.h"
 
 namespace {
@@ -147,6 +148,7 @@ struct pt_batch {
     HostBuf h_add_totals, h_add_rank, h_add_aoff, h_add_amap;               // the view of the last pt_batch_add_actors
     HostBuf h_clk_off, h_clk_seq, h_clk_status;                             // the view of the last pt_batch_download_clocks
     HostBuf h_attr_status, h_attr_off, h_attr_runs;                         // the view of the last pt_batch_attribute
+    HostBuf h_rst_status, h_rst_ops, h_rst_seq;                             // the view of the last pt_batch_restore
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side = nullptr, launch_stream = nullptr;   // side: the CTA-per-log bins' own launches run beside the warp / team kernels
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -2244,6 +2246,109 @@ int pt_batch_attribute(pt_batch* b, const uint32_t* logs, uint32_t n, const uint
     }
     *out = pt_attr_view{n, (const uint32_t*)b->h_attr_status.p, hoff, (const pt_attr_run*)b->h_attr_runs.p, total};
     return PT_OK;
+}
+
+// pt_batch_restore's host checks of the requests (include/peritext_b200.h).  Returns the problem, or an empty string.
+static std::string check_restore(const pt_batch* b, const pt_restore_request* req, uint32_t n) {
+    std::vector<char> target(b->n_logs, 0);
+    for (uint32_t k = 0; k < n; k++) {
+        const pt_restore_request& q = req[k];
+        const std::string here = "request " + std::to_string(k) + ": ";
+        if (q.log >= b->n_logs || q.version >= b->n_logs)
+            return here + "log " + std::to_string(q.log >= b->n_logs ? q.log : q.version) + " is outside the batch's " + std::to_string(b->n_logs) + " logs";
+        if (target[q.log]) return here + "log " + std::to_string(q.log) + " is the log of an earlier request";
+        target[q.log] = 1;
+        const pt_log_desc& L = b->h_desc[q.log];
+        if (q.actor >= L.n_actors) return here + "actor rank " + std::to_string(q.actor) + " >= the log's " + std::to_string(L.n_actors) + " actors";
+        if (q.first_ctr <= L.max_ctr) return here + "first_ctr " + std::to_string(q.first_ctr) + " is not above the log's max_ctr " + std::to_string(L.max_ctr);
+    }
+    return std::string();
+}
+
+int pt_batch_restore(pt_batch* b, const pt_restore_request* req, uint32_t n, uint32_t mode, pt_restore_view* out) {
+    const char* fn = "pt_batch_restore: ";
+    if (!b) return PT_ERR_INVALID;
+    if (!b->have_batch) { g_last_error = "pt_batch_restore before pt_batch_upload"; return PT_ERR_STATE; }
+    if (!b->have_changes) { g_last_error = std::string(fn) + "the handle has no change table"; return PT_ERR_STATE; }
+    if (!(b->limits.flags & PT_FLAG_EMIT_SEQUENCE)) { g_last_error = std::string(fn) + "the handle was created without PT_FLAG_EMIT_SEQUENCE"; return PT_ERR_STATE; }
+    if (!b->merged) { g_last_error = std::string(fn) + "no completed merge since the last call that changed the batch"; return PT_ERR_STATE; }
+    if (!out || (n && !req)) { g_last_error = std::string(fn) + "null requests or out"; return PT_ERR_INVALID; }
+    if (mode != PT_RESTORE_TEXT && mode != PT_RESTORE_MARKS) { g_last_error = std::string(fn) + "mode " + std::to_string(mode) + " is not exactly one of PT_RESTORE_TEXT, PT_RESTORE_MARKS"; return PT_ERR_INVALID; }
+    const std::string err = check_restore(b, req, n);
+    if (!err.empty()) { g_last_error = fn + err; return PT_ERR_INVALID; }
+    int rc;
+    if ((rc = reserve_n<uint32_t>(b->h_rst_status, n)) || (rc = reserve_n<uint32_t>(b->h_rst_ops, n)) || (rc = reserve_n<uint32_t>(b->h_rst_seq, n))) return rc;
+    uint32_t *hst = (uint32_t*)b->h_rst_status.p, *hops = (uint32_t*)b->h_rst_ops.p, *hseq = (uint32_t*)b->h_rst_seq.p;
+    *out = pt_restore_view{n, hst, hops, hseq};
+    if (!n) return PT_OK;
+    const bool marks = mode == PT_RESTORE_MARKS;
+    std::vector<unsigned long long> slot((size_t)n + 1, 0), vis((size_t)n + 1, 0), open((size_t)n + 1, 0);
+    for (uint32_t k = 0; k < n; k++) {
+        slot[k + 1] = slot[k] + b->h_cdesc[req[k].log].n_changes;
+        vis[k + 1] = vis[k] + (marks ? b->h_desc[req[k].log].n_insdel : 0);   // n_visible <= n_insdel
+        open[k + 1] = open[k] + (marks ? 2ull * ((uint64_t)b->h_desc[req[k].log].n_mark + b->h_desc[req[k].version].n_mark) : 0);
+    }
+    PT_CUDA(cudaSetDevice(b->device));
+    PT_CUDA(cudaStreamSynchronize(b->stream));              // the merge is complete; the view's buffers are free
+    // ---- count: statuses, ops, deps, seq and element totals back to the host ----
+    DevBuf dreq, dslot, dpos, dvoff, dvis, dooff, dopen, dst, dops, ddeps, dseq, delems, ddesc, dcdesc, dins, dmk, dch, ddp;   // freed on return
+    if ((rc = upload_n(b, dreq, req, n)) || (rc = upload_n(b, dslot, slot.data(), (uint64_t)n + 1)) || (rc = reserve_n<uint32_t>(dpos, slot[n])) ||
+        (rc = reserve_n<uint32_t>(dst, n)) || (rc = reserve_n<uint32_t>(dops, n)) || (rc = reserve_n<uint32_t>(ddeps, n)) ||
+        (rc = reserve_n<uint32_t>(dseq, n)) || (rc = reserve_n<uint32_t>(delems, n)) || (rc = upload_n(b, dvoff, vis.data(), (uint64_t)n + 1)) ||
+        (rc = reserve_n<uint32_t>(dvis, vis[n])) || (rc = upload_n(b, dooff, open.data(), (uint64_t)n + 1)) || (rc = reserve_n<uint4>(dopen, open[n]))) return rc;
+    ptrs::RestoreParams P{};
+    P.req = (const pt_restore_request*)dreq.p; P.n = n; P.maxR = b->adm_maxR;
+    P.desc = (const pt_log_desc*)b->d_desc.p; P.cdesc = (const pt_change_desc*)b->d_cdesc.p;
+    P.changes = (const pt_change_rec*)b->d_changes.p; P.deps = (const pt_dep_rec*)b->d_deps.p;
+    P.insdel = b->dp_insdel; P.marks = b->dp_marks;
+    P.res = (const pt_log_result*)b->d_results.p; P.seq_off = (const uint64_t*)b->d_text_off.p; P.seq = (const uint32_t*)b->d_seq.p;
+    P.mode = mode;
+    P.text_off = (const uint64_t*)b->d_text_off.p; P.text = (const uint32_t*)b->d_text.p;
+    P.span_off = (const uint64_t*)b->d_span_off.p; P.spans = (const pt_span*)b->d_spans.p; P.cpool = (const uint32_t*)b->d_pool.p;
+    P.slot_off = (const unsigned long long*)dslot.p; P.pos = (uint32_t*)dpos.p;
+    P.vis_off = (const unsigned long long*)dvoff.p; P.vis = (uint32_t*)dvis.p; P.open_off = (const unsigned long long*)dooff.p; P.open = (uint4*)dopen.p;
+    P.status = (uint32_t*)dst.p; P.n_ops = (uint32_t*)dops.p; P.n_deps = (uint32_t*)ddeps.p; P.seq_out = (uint32_t*)dseq.p; P.elems = (uint32_t*)delems.p;
+    if ((rc = launch_actor_kernel(b, ptrs::restore_kernel<false>, n, P))) return rc;
+    std::vector<uint32_t> nd(n), el(n);
+    PT_CUDA(cudaMemcpyAsync(hst, dst.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(hops, dops.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(hseq, dseq.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(nd.data(), ddeps.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaMemcpyAsync(el.data(), delems.p, (size_t)n * 4, cudaMemcpyDeviceToHost, b->stream));
+    PT_CUDA(cudaStreamSynchronize(b->stream));
+    // ---- the limits that depend on the counts, and the delta's layout: records, one change record and its deps per log ----
+    const uint32_t nl = b->n_logs;
+    std::vector<pt_log_desc> dd(nl);
+    std::vector<pt_change_desc> cd(nl, pt_change_desc{0, 0, 0, 0});
+    for (uint32_t i = 0; i < nl; i++) dd[i] = pt_log_desc{0, 0, 0, 0, b->h_desc[i].n_actors, b->h_desc[i].max_ctr};
+    for (uint32_t k = 0; k < n; k++) {
+        if (!hops[k]) continue;
+        const pt_restore_request& q = req[k];
+        const std::string here = std::string(fn) + "request " + std::to_string(k) + ": ";
+        const uint64_t last = (uint64_t)q.first_ctr + hops[k] - 1;
+        if (last > 0xFFFFFFFFull) { g_last_error = here + "counters past 2^32 - 1"; return PT_ERR_INVALID; }
+        if (last * std::max<uint32_t>(1, b->h_desc[q.log].n_actors) > 0x7FFFFFFFull) { g_last_error = here + "max_ctr x n_actors would reach 2^31"; return PT_ERR_INVALID; }
+        if (el[k] >= (1u << 22)) { g_last_error = here + "the change would bring the log to 2^22 elements or more"; return PT_ERR_INVALID; }
+        (marks ? dd[q.log].n_mark : dd[q.log].n_insdel) = hops[k];
+        dd[q.log].max_ctr = (uint32_t)last;
+        cd[q.log].n_changes = 1; cd[q.log].n_deps = nd[k];
+    }
+    uint64_t n_ins = 0, n_mk = 0, n_ch = 0, n_dp = 0;
+    for (uint32_t i = 0; i < nl; i++) {
+        dd[i].insdel_off = n_ins; dd[i].mark_off = n_mk; cd[i].change_off = n_ch; cd[i].dep_off = n_dp;
+        n_ins += dd[i].n_insdel; n_mk += dd[i].n_mark; n_ch += cd[i].n_changes; n_dp += cd[i].n_deps;
+    }
+    // ---- write, then pt_batch_append's splice with the delta and its change table on the device ----
+    if ((rc = upload_n(b, ddesc, dd.data(), nl)) || (rc = upload_n(b, dcdesc, cd.data(), nl)) || (rc = reserve_n<pt_insdel_rec>(dins, n_ins)) ||
+        (rc = reserve_n<pt_mark_rec>(dmk, n_mk)) || (rc = reserve_n<pt_change_rec>(dch, n_ch)) || (rc = reserve_n<pt_dep_rec>(ddp, n_dp))) return rc;
+    if (n_ch) {
+        P.delta = (const pt_log_desc*)ddesc.p; P.delta_cdesc = (const pt_change_desc*)dcdesc.p;
+        P.out_insdel = (pt_insdel_rec*)dins.p; P.out_marks = (pt_mark_rec*)dmk.p; P.out_changes = (pt_change_rec*)dch.p; P.out_deps = (pt_dep_rec*)ddp.p;
+        if ((rc = launch_actor_kernel(b, ptrs::restore_kernel<true>, n, P))) return rc;
+    }
+    const pt_packed_ops delta{nl, dd.data(), (const pt_insdel_rec*)dins.p, n_ins, (const pt_mark_rec*)dmk.p, n_mk};
+    const pt_change_table ct{nl, cd.data(), (const pt_change_rec*)dch.p, n_ch, (const pt_dep_rec*)ddp.p, n_dp};
+    return splice_append(b, fn, &delta, true, pt_append_remap{}, &ct, true);
 }
 
 // JSON render of the spans (render_kernel.cuh).

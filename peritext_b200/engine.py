@@ -63,6 +63,7 @@ _ENTRY_POINTS = {
     "pt_batch_query_elements": ([_vp, _vp, _u32, _vp], _int),
     "pt_batch_find_elements": ([_vp, _vp, _u32, _vp], _int),
     "pt_batch_attribute": ([_vp, _vp, _u32, _vp, _vp, _vp], _int),
+    "pt_batch_restore": ([_vp, _vp, _u32, _u32, _vp], _int),
     "pt_batch_render_json": ([_vp, _vp, _vp], _int),
     "pt_batch_render_patches_json": ([_vp, _vp, _vp], _int),
     "pt_batch_render_changes_json": ([_vp, _vp, _vp], _int),
@@ -756,6 +757,45 @@ class BatchEngine:
                "pt_batch_attribute")
         o = _view(v.off, len(lg) + 1, np.uint64) if len(lg) else np.zeros(1, np.uint64)
         return _view(v.status, len(lg), np.uint32), o, _view(v.runs, v.n_runs, ATTR_RUN_DT)
+
+    def restore(self, requests, mode: int = 1):
+        """Restore resident logs to earlier versions as new local changes, on the device (pt_batch_restore), after a merge with
+        ``emit_sequence``: request k (``restore.RESTORE_REQUEST_DT`` rows, or (log, version, actor, first_ctr) tuples) appends
+        to log ``log`` the change by actor rank ``actor`` that makes its visible text (``mode`` RESTORE_TEXT = 1) or its formatting
+        (RESTORE_MARKS = 2) equal to that of log ``version`` (a checkout of it), ops counted from ``first_ctr``.  Returns (u32 status RESTORE_*, u32 n_ops, u32 seq) per request; a
+        request with no ops appends nothing.  ``restore.restore_inputs`` / ``restore_change_record`` are its host
+        specification.  The handle then needs a merge.  Needs a change table."""
+        from .restore import RESTORE_REQUEST_DT, _RestoreView
+        req = np.ascontiguousarray(np.array([tuple(int(x) for x in q) for q in requests], RESTORE_REQUEST_DT) if len(requests) else np.zeros(0, RESTORE_REQUEST_DT))
+        v = _RestoreView()
+        _check(self._L.pt_batch_restore(self._h, _ptr(req), len(req), mode, ctypes.byref(v)), "pt_batch_restore")
+        status, n_ops, seq = (_view(p, len(req), np.uint32) for p in (v.status, v.n_ops, v.seq))
+        if len(req):
+            desc = np.zeros(self.n_logs, DESC_DT)
+            desc["n_actors"] = self._log_n_actors
+            desc["n_insdel" if mode == 1 else "n_mark"][req["log"]] = n_ops
+            self._spliced(desc)
+        return status, n_ops, seq
+
+    def restore_version(self, logs, versions, actors, first_ctrs=None):
+        """The full restore of each ``logs[k]`` to ``versions[k]`` by actor rank ``actors[k]``: restore TEXT, merge, MARKS,
+        merge (MARKS compares the formatting the restored text inherits, which only a merge computes).  ``first_ctrs`` default
+        to each log's max_ctr + 1 at each step.  Returns ((status, n_ops, seq) of TEXT, the same of MARKS); the handle is
+        merged afterwards.  Needs emit_sequence and a change table."""
+        from .restore import RESTORE_MARKS, RESTORE_TEXT
+        out = []
+        for step, mode in enumerate((RESTORE_TEXT, RESTORE_MARKS)):
+            if first_ctrs is not None and step == 0:
+                ctrs = [int(c) for c in first_ctrs]
+            else:
+                d = ctypes.c_void_p()
+                _check(self._L.pt_batch_download_descs(self._h, ctypes.byref(d)), "pt_batch_download_descs")
+                desc = _view(d.value, self.n_logs, DESC_DT)
+                ctrs = [int(desc[int(i)]["max_ctr"]) + 1 for i in logs]
+            out.append(self.restore(list(zip(logs, versions, actors, ctrs)), mode))
+            self.merge()
+        self.sync()
+        return tuple(out)
 
     def resolve_cursors(self, batch: PackedBatch, logs, elem_ids) -> np.ndarray:
         """resolveCursor (reference src/micromerge.ts:475-477) for many documents in one device pass: the number of visible
