@@ -172,14 +172,15 @@ struct Arena {
     uint32_t sm_cap, sm_used;
     char* gm; unsigned long long gm_cap, gm_used;
     bool overflow;
+    // bytes in 64 bits: the id table of a key space near 2^31 is 4-8 GiB, and a 32-bit count would wrap to a size that fits
     template <class T> __device__ __forceinline__ T* alloc(uint32_t count) {
-        const uint32_t bytes = (uint32_t)((count * sizeof(T) + 15u) & ~15u);
+        const unsigned long long bytes = ((unsigned long long)count * sizeof(T) + 15ull) & ~15ull;
         if (SH) {
-            const uint32_t off = sm_used; sm_used += bytes;
-            if (sm_used > sm_cap) { overflow = true; sm_used = off; return reinterpret_cast<T*>(ptk_smem); }
+            if (sm_used + bytes > sm_cap) { overflow = true; return reinterpret_cast<T*>(ptk_smem); }
+            const uint32_t off = sm_used; sm_used += (uint32_t)bytes;
             return reinterpret_cast<T*>(ptk_smem + off);
         }
-        if (sm_used + bytes <= sm_cap) { T* p = reinterpret_cast<T*>(ptk_smem + sm_used); sm_used += bytes; return p; }
+        if (sm_used + bytes <= sm_cap) { T* p = reinterpret_cast<T*>(ptk_smem + sm_used); sm_used += (uint32_t)bytes; return p; }
         if (gm_used + bytes > gm_cap) { overflow = true; return reinterpret_cast<T*>(gm); }
         T* p = reinterpret_cast<T*>(gm + gm_used); gm_used += bytes; return p;
     }
@@ -1016,7 +1017,7 @@ __device__ int merge_one_log(const BatchParams& P, uint32_t li, BlockCtx<BLOCK>&
         if (c.status) { bail(); return 0; }
         uint32_t* pool = P.comment_pool + c.pool_base;
         // build and sort the lists in shared memory when they fit (latency of the per-span sort), else in the pool itself
-        const uint32_t slBytes = (totalC * 4u + 15u) & ~15u;
+        const unsigned long long slBytes = ((unsigned long long)totalC * 4u + 15u) & ~15ull;
         const bool staged = totalC > 0 && A.sm_used + slBytes <= A.sm_cap;
         uint32_t* SL = staged ? reinterpret_cast<uint32_t*>(ptk_smem + A.sm_used) : pool;
         for (uint32_t e = pe0; e < 2 * Mc; e += peStep) {
