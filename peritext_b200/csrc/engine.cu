@@ -409,7 +409,8 @@ int derive_key_records(pt_batch* b) {
     const uint32_t* nr = b->plan.n_route;
     if (!(nr[ptp::kPacked3] + nr[ptp::kCompact] + nr[ptp::kDirect])) { b->d_key_insdel.release(); b->d_key_marks.release(); return PT_OK; }
     int rc;
-    if ((rc = reserve_n<uint32_t>(b->d_key_insdel, b->n_insdel)) || (rc = reserve_n<uint2>(b->d_key_marks, b->n_mark))) return rc;
+    // 32 mark records of slack past the end: the warp kernel's mark pass loads one trip (32 records) ahead without a bounds clamp
+    if ((rc = reserve_n<uint32_t>(b->d_key_insdel, b->n_insdel)) || (rc = reserve_n<uint2>(b->d_key_marks, b->n_mark + 32))) return rc;
     const uint32_t threads = 256;      // one warp per log
     if (b->n_logs) {
         ptu::derive_key_records_kernel<<<warp_grid(b, b->n_logs, threads), threads, 0, b->stream>>>(

@@ -180,11 +180,11 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
     // reciprocal ceil(2^32 / R), exact for 16-bit keys (the error is below (R-1) * 2^16 / 2^32 < 1 / R)
     const uint32_t invR = compact ? 0xFFFFFFFFu / R + 1u : 0u;
     auto ctrOf = [&](uint32_t key) -> uint32_t { return packed ? (key * 0xAAABu) >> 17 : __umulhi(key, invR); };
-    // index of the insert record with opId key `key`, kNone16 if there is none; the key must be valid (< kS0)
+    // index of the insert record with opId key `key`; if there is none, kNone16 (packed3: 0xFFFFFFFF); the key must be valid (< kS0)
     auto lookup = [&](uint32_t key) -> uint32_t {
         if (!packed && !compact) return T[key];
         const uint32_t c = ctrOf(key), actor = key - c * (packed ? 3u : R);
-        if (packed) { const uint32_t f = (T32[c] >> (10u * actor)) & 1023u; return f ? f - 1u : kNone16; }
+        if (packed) return ((T32[c] >> (10u * actor)) & 1023u) - 1u;    // field 0 (none): 0xFFFFFFFF, above every index
         const uint32_t e = T[c];
         if (e == kNone16) return kNone16;                      // no insert with this counter at all
         if ((e >> 11) == actor) return e & 0x7FFu;
@@ -556,67 +556,77 @@ __device__ __forceinline__ int warp_merge_one_log(const BatchParams& P, const ui
         if (capS > m) capS = m;
         Sv = A.alloc<uint4>(capS + 1);
         if (!A.fits()) { ps.leave(); return 1; }
-        const uint32_t mm1 = m - 1u;                               // m > 0 here; past-the-end lanes load a clamped record, unused
         const uint32_t ksMax = KS ? KS - 1u : 0u;                  // boundary keys are clamped to a valid slot for the lookups
-        uint2 a = __ldg(mk + min(lane, mm1));
-        const uint32_t mkBytes = m * 8u;
-#pragma unroll 2
-        for (uint32_t kb = 0; kb < m; kb += 32) {
+        // one trip of 32 marks; `tail`: the last, partial trip (the full trips need no bounds test).  Straight-line form: both
+        // boundary chains (lookup, then EV read) are issued unconditionally, on keys clamped to a valid slot and on EV's entry n
+        // for "no insert record", so they overlap; the hit rules are selects after the loads.  A boundary element must exist AND
+        // have arrived before the mark op: the reference's walk never matches anything else (peritext.ts:236-241) — a missing
+        // start is a no-op, a missing end never ends
+        auto markTrip = [&](const uint2 a, const uint32_t kb, const bool tail) {
             const uint32_t k = kb + lane;
-            if ((kb & 511u) == 0u) {                               // every 16th trip: the 32 lines of trips t+24 .. t+39 (256 B per trip)
-                const uint32_t po = (kb + 768u) * 8u + lane * 128u;
-                if (po < mkBytes) prefetch_l2(reinterpret_cast<const char*>(mk) + po);
-            }
-            const uint2 b = __ldg(mk + min(k + 32u, mm1));         // one trip ahead (L2 hits); unrolled by 2: no moves
             // own / start / end == kS1: the id is out of range (a start or end also when its bound is above PT_BOUND_AFTER)
             const uint32_t key = a.x & 0xFFFFu, skey = a.x >> 16, ekey = a.y & 0xFFFFu, arrival = (a.y >> 16) & 0x7FFu;
             const uint32_t kind = (a.y >> 27) & 7u, sb = (a.y >> 30) & 1u, eb = a.y >> 31;
             const uint32_t type = (kind >> 1) & 3u;
-            // straight-line form: both boundary chains (lookup, then EV read) are issued unconditionally, on keys clamped to a
-            // valid slot and on EV's entry n for "no insert record", so they overlap; the hit rules are selects after the loads.
-            // A boundary element must exist AND have arrived before the mark op: the reference's walk never matches anything
-            // else (peritext.ts:236-241) — a missing start is a no-op, a missing end never ends
-            const bool inb = k < m;
-            const bool idok = inb && key != kS1;
+            const bool inb = !tail || k < m;
             const uint32_t js = lookup(min(skey, ksMax)), je = lookup(min(ekey, ksMax));
             const uint32_t es = EV[min(js, n)], ee = EV[min(je, n)];
-            bool dup = false;
-            if (idok) { const uint32_t bit = 1u << (key & 31); dup = (atomicOr(&KSeen[key >> 5], bit) & bit) != 0; }   // an insert's or an earlier mark's opId
-            if (inb && (!idok || dup)) fail(PT_LOG_BAD_OPID);
-            // kNone16 is above every arrival (11 bits)
-            const bool sHit = idok && skey != kS1 && js < arrival;
+            // st is 0 here (A+B's failures returned): any bit set in the pass is a bad opId
+            if (inb) {                                             // out of range, or an insert's or an earlier mark's opId
+                if (key == kS1) st |= 1u;
+                else { const uint32_t bit = 1u << (key & 31); st |= atomicOr(&KSeen[key >> 5], bit) & bit; }
+            }
+            // a missing boundary's index is above every arrival (11 bits).  A bad own id fails the log: its survivors are unused
+            const bool sHit = inb && skey != kS1 && js < arrival;
             // same slot: the start branch wins and the op never ends (quirk Q2)
             const bool eHit = ekey != kS1 && je < arrival && !(je == js && eb == sb);
             const uint32_t va = (es & 0x7FFFu) + (sb & (es >> 15));
             const uint32_t vb = eHit ? (ee & 0x7FFFu) + (eb & (ee >> 15)) : nvis;
             const bool surv = sHit && va < vb;
-            const bool isC = surv && type == PT_MARK_COMMENT;
-            const uint32_t bal = __ballot_sync(kFull, surv), balC = __ballot_sync(kFull, isC);
+            const uint32_t bal = __ballot_sync(kFull, surv);
             if (surv) {
                 const uint32_t idx = nS + __popc(bal & lt);
-                if (idx < capS) {
-                    // priority: LWW types compare opIds (peritext.ts:304-313) = keys; comments fold in arrival order (Q4)
-                    Sv[idx] = make_uint4(va | (vb << 16), (type == PT_MARK_COMMENT ? k : key) | (kind << 16), PT_ATTR_NONE, k);
-                    if (isC) { const uint32_t ci = nC + __popc(balC & lt); if (ci <= kMaxCommentSurvivors) CIdx[ci] = (uint16_t)idx; }
-                }
+                // priority: LWW types compare opIds (peritext.ts:304-313) = keys; comments fold in arrival order (Q4)
+                if (idx < capS) Sv[idx] = make_uint4(va | (vb << 16), (type == PT_MARK_COMMENT ? k : key) | (kind << 16), PT_ATTR_NONE, k);
                 // the attr that the batch after the loop loads: its line goes to L2 now, off the end of the pass
                 if (type == PT_MARK_LINK || type == PT_MARK_COMMENT) prefetch_l2(&P.marks[(mk + k) - P.key_marks].attr);
             }
-            nS += __popc(bal); nC += __popc(balC);
+            nS += __popc(bal);
+        };
+        // the key-record copy has 32 records of slack past its end: the one-ahead loads need no clamp
+        uint2 a = __ldg(mk + lane);
+        const uint32_t mkBytes = m * 8u, mFull = m & ~31u;
+#pragma unroll 2
+        for (uint32_t kb = 0; kb < mFull; kb += 32) {
+            if ((kb & 511u) == 0u) {                               // every 16th trip: the 32 lines of trips t+24 .. t+39 (256 B per trip)
+                const uint32_t po = (kb + 768u) * 8u + lane * 128u;
+                if (po < mkBytes) prefetch_l2(reinterpret_cast<const char*>(mk) + po);
+            }
+            const uint2 b = __ldg(mk + (kb + 32u + lane));         // one trip ahead (L2 hits); unrolled by 2: no moves
+            markTrip(a, kb, false);
             a = b;
         }
+        if (mFull < m) markTrip(a, mFull, true);
         __syncwarp();
-        st = __reduce_or_sync(kFull, st);
-        if (st) { bail(31u - __clz(st)); ps.leave(); return 0; }
+        if (__reduce_or_sync(kFull, st)) { bail(PT_LOG_BAD_OPID); ps.leave(); return 0; }
         if (nS > capS) { ps.leave(); return 1; }
         A.used = svStart + ((nS * 16u + 15u) & ~15u);               // keep only the survivors
-        // the attrs of the link and comment survivors (phase I reads no other) from the full records, all loads in flight at once
+        // the attrs of the link and comment survivors (phase I reads no other) from the full records, all loads in flight at
+        // once; the comment survivors in arrival order (Sv's order) go to CIdx
         const pt_mark_rec* __restrict__ full_mk = P.marks + (mk - P.key_marks);
 #pragma unroll 1
-        for (uint32_t s = lane; s < nS; s += 32) {
-            const uint4 sv = Sv[s];
-            const uint32_t t = (sv.y >> 17) & 3u;
-            if (t == PT_MARK_LINK || t == PT_MARK_COMMENT) Sv[s].z = __ldg(&full_mk[sv.w].attr);
+        for (uint32_t s0 = 0; s0 < nS; s0 += 32) {
+            const uint32_t s = s0 + lane;
+            uint32_t t = 0;
+            if (s < nS) {
+                const uint4 sv = Sv[s];
+                t = (sv.y >> 17) & 3u;
+                if (t == PT_MARK_LINK || t == PT_MARK_COMMENT) Sv[s].z = __ldg(&full_mk[sv.w].attr);
+            }
+            const bool isC = s < nS && t == PT_MARK_COMMENT;
+            const uint32_t balC = __ballot_sync(kFull, isC);
+            if (isC) { const uint32_t ci = nC + __popc(balC & lt); if (ci <= kMaxCommentSurvivors) CIdx[ci] = (uint16_t)s; }
+            nC += __popc(balC);
         }
         __syncwarp();
     }
